@@ -1,4 +1,4 @@
-"""audio_diffusion_b200 — B200-native (sm_100a) engine for the teticio/audio-diffusion hot path.
+"""audio_diffusion_b200 — H100-native (sm_90a) engine for the teticio/audio-diffusion hot path.
 
 Public surface mirrors the reference objects the unchanged `AudioDiffusionPipeline` drives:
 `UNet2DModel`, `AutoencoderKL`, `DDPMScheduler`, `DDIMScheduler`, `Mel`, `AudioDiffusionPipeline`.

@@ -145,7 +145,7 @@ def require_cuda():
     import torch
 
     if not torch.cuda.is_available():
-        raise B200ADError("audio_diffusion_b200 needs a CUDA device (B200, sm_100a); there is no CPU fallback")
+        raise B200ADError("audio_diffusion_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
 
 
 def stream_ptr():

@@ -1,5 +1,5 @@
 """Minimal `accelerate` surface for the UNCHANGED scripts/train_unet.py (imports :13-15; calls :45-50, :181, :199-201,
-:252-283, :285-346), on the B200 engine.
+:252-283, :285-346), on the H100 engine.
 
 What HF accelerate 0.34 does for that script, restated here ([3P-recall] accelerate==0.34.2, requirements-lock.txt:2):
   * one process per GPU (torchrun env: RANK / LOCAL_RANK / WORLD_SIZE), NCCL process group, `accelerator.device`;

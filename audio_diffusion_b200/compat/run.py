@@ -1,4 +1,4 @@
-"""Run an UNCHANGED reference script on the B200 engine:
+"""Run an UNCHANGED reference script on the H100 engine:
 
     python -m audio_diffusion_b200.compat.run /path/to/audio-diffusion/scripts/train_unet.py --dataset_name ... [args]
     torchrun --nproc-per-node 8 -m audio_diffusion_b200.compat.run .../scripts/train_unet.py ...

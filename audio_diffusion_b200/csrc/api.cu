@@ -129,7 +129,7 @@ static int conv2d_impl(const float* x, const float* w, const float* bias, const 
       }
     p.nseg = 4;
   }
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   CK(cudaGetDevice(&dev));
   CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   if (stride == -2) {  // nearest-2x upsample + 3x3 conv as four folded 2x2 convs on the low-res input
@@ -204,7 +204,7 @@ extern "C" int b200ad_conv2d_dgrad(const float* gy, const float* w, float* gx, i
   for (int k = 0; k < K * K; ++k) { s.dh[k] = (signed char)(k / K - K / 2); s.dw[k] = (signed char)(k % K - K / 2); }
   s.ss = nullptr; s.ss_stride = 0; s.silu = 0;
   p.nseg = 1;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   CK(cudaGetDevice(&dev));
   CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   CK(launch_conv_tc(p, sms, st));
@@ -228,7 +228,7 @@ extern "C" int b200ad_conv2d_wgrad(const float* gy, const float* a, float* dw, i
   CK(launch_nchw_to_pf8(gy, gyp, N, cout, H, W, st));
   CK(launch_nchw_to_pf8(a, ap, N, cin, H, W, st));
   CK(cudaMemsetAsync(dw, 0, (size_t)cout * cin * K * K * sizeof(float), st));
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   CK(cudaGetDevice(&dev));
   CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   WgradDesc d{};

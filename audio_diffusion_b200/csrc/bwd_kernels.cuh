@@ -47,7 +47,7 @@ cudaError_t launch_lin_bwd_weight(const float* g, int gstride, const float* x, i
 cudaError_t launch_silu_bwd(float* g, const float* u, int n, cudaStream_t s);
 cudaError_t launch_silu_fwd(const float* u, float* y, int n, cudaStream_t s);
 
-// Weight gradient on tcgen05 (wgrad_tc.cu):  dw[(co * cin_total + ci_off + ci) * ntaps_total + tapidx[t]] +=
+// Weight gradient on wgmma (wgrad_tc.cu):  dw[(co * cin_total + ci_off + ci) * ntaps_total + tapidx[t]] +=
 //   sum_{n, p} gy[n][co][p] * act[n][ci][p + shift[t]].   gy / act are channel views: `*_img_planes` planes per image in the
 // underlying tensors, the pointers already offset to the view's first plane.
 struct WgradDesc {

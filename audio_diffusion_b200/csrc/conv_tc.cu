@@ -1,53 +1,44 @@
-// tcgen05 implicit-GEMM convolution for the U-Net hot path (replaces the cuDNN conv2d calls that
+// wgmma implicit-GEMM convolution for the U-Net hot path (replaces the cuDNN conv2d calls that
 // diffusers' UNet2DModel.forward makes; reference call site audiodiffusion/pipeline_audio_diffusion.py:163).
 //
 // GEMM view (transposed): D^T[cout, pixel] = sum over (segment, tap, cin) W[cout, cin, tap] * X[pixel + shift(tap), cin].
-//   M = 128 output channels (weights are the A operand), N = up to 256 output pixels (activations are the B operand),
-//   K = 16 input channels per tcgen05.mma.  Why this way round: the kernel is bound by SHARED-MEMORY bandwidth - with
-//   M = N = 128 the two operand reads alone need the full 128 B/clk; N = 256 reads 12 KB per 128-cycle MMA (96 B/clk),
-//   halves the number of MMAs to issue, and the weights of one tap stay latched in the A collector (.collector::a::fill /
-//   ::lastuse) while the second pixel group is multiplied.
+//   M = 128 output channels (weights are the A operand; two consumer warpgroups take 64 rows each), N = up to 256 output
+//   pixels (activations are the B operand), K = 16 input channels per wgmma.m64nNk16.  The accumulators of an item
+//   (64 x 256 fp32 per warpgroup) live in registers, which caps an item at two 128-pixel tiles.
 // Pixel operand: the PF8 layout stores 8-channel vectors of consecutive pixels contiguously, which *is* the K-major
-//   no-swizzle UMMA core-matrix layout (8 rows x 16 B). A work item covers 4 x 128 consecutive flat pixels; per 16 input
+//   no-swizzle core-matrix layout (8 rows x 16 B). A work item covers 2 x 128 consecutive flat pixels; per 16 input
 //   channels ONE contiguous window per 8-channel plane (the run plus a halo of Wp+1 pixels on both sides) is bulk-copied
-//   (TMA engine, UBLKCP) into shared memory, and every tap is a descriptor whose start address is shifted by
-//   (dh*Wp + dw) * 16 B.  (Measured: a bulk copy costs ~130 cycles of TMA time however small it is -> few large copies.)
-// Fused GroupNorm(+SiLU): the windows hold the RAW producer output; five transform warps rewrite them in place
+//   (TMA engine) into shared memory, and every tap is a descriptor whose start address is shifted by (dh*Wp + dw) * 16 B.
+//   (Few large copies: a bulk copy has a fixed cost however small it is.)
+// Fused GroupNorm(+SiLU): the windows hold the RAW producer output; the transform warps rewrite them in place
 //   (x * scale[n][c] + shift[n][c], SiLU via one tanh.approx, zero on pad/guard positions) between the TMA landing and
-//   the MMA reading them, so the normalised tensor never exists in HBM.  The work is split 2:2:2:1:1 over the warps so
-//   that each SM sub-partition (scheduler + MUFU) carries a quarter of it.
+//   the MMA reading them, so the normalised tensor never exists in HBM.
 // Weights: pre-packed on the device into per-(cout tile, 16-channel step, tap) 4 KB blocks; a separate, finer ring
 //   (CONV_BT taps per slot) with its own producer warp.
 // Residual adds are an extra 1-tap K-segment with identity weights (exact, and no epilogue loads).
-// Accumulators: 128 lanes (cout) x 512 fp32 columns (pixels) in TMEM = all of it, handled as two 256-column HALVES with
-//   their own full/empty barriers.  The first and the last k-step of an item are issued half by half (all taps into
-//   columns 0-255, then all taps into 256-511) instead of tap by tap, so half 0 is complete one k-step's worth of MMAs
-//   before half 1, and the next item may start on half 0 while half 1 is still being drained: the epilogue of item i
-//   overlaps the tail of item i and the head of item i+1 (it was fully exposed, 7 of 34 ms per step, in round 1).
-// Epilogue (8 warps, ~2.7 instructions per element instead of ~7): TMEM -> registers (32x32b: thread = channel, 32
-//   pixels) -> +bias/temb and GroupNorm partial sums on packed fp32 pairs (FADD2/FFMA2) -> cvt.rn.bf16x2 -> four
-//   stmatrix.x4.trans per 32-pixel chunk into one of TWO staging buffers of a 128-pixel tile ([plane][pixel][8 ch] =
-//   finished PF8 runs) -> one bulk store (TMA engine, UBLKCP.G.S) per plane and tile, draining while the next tile is
-//   converted.  The packed weight rows are interleaved (conv_lane_channel) so that a transposed 8x8 store lands exactly
-//   one PF8 vector (8 channels of one pixel) per 16-byte row; pad columns and the run-off behind the image are stored as
-//   the zeros the layout requires there.
-// Small images (H * Wp + bottom halo <= 128 pixels: 8x8 and below): an item's four tiles are the first tiles of four
-//   CONSECUTIVE IMAGES, so one weight fetch and one N = 256 MMA serve several samples (ConvParams::pack).
-// Warp roles (16 warps): 0 activation producer, 1 MMA issuer (uniform datapath, one elected lane), 3 weight producer,
-//   2/8-11 transform (warp 2 also owns the TMEM allocation), 4-7 + 12-15 epilogue.
+// MMA pipeline: a consumer warpgroup issues the taps of one weight slot as one wgmma group and keeps one group in flight;
+//   a weight slot (and, after the last slot of a k-step, the activation stage) is released once its group has retired.
+// Epilogue (per consumer warpgroup, from registers): +bias/temb and GroupNorm partial sums -> cvt.rn.bf16x2 ->
+//   stmatrix.trans into a staging buffer ([plane][pixel][8 ch] = finished PF8 runs; the wgmma fragment puts the 8 channels
+//   of a plane in lanes 4 apart, which is exactly a transposed 8x8 matrix) -> one bulk store (TMA engine) per plane and
+//   tile, draining while the next item is multiplied.  Pad columns and the run-off behind the image are stored as the
+//   zeros the layout requires there.
+// Small images (H * Wp + bottom halo <= 128 pixels: 8x8 and below): an item's tiles are the first tiles of CONSECUTIVE
+//   IMAGES, so one weight fetch and one N = 256 MMA serve two samples (ConvParams::pack).
+// Warp roles (12 warps): 0 activation producer, 1 weight producer, 2-3 transform, 4-7 and 8-11 the two consumer
+//   warpgroups (MMA + epilogue).
 #include <cstdlib>
 
 #include "conv_tc.cuh"
 
 namespace b200ad {
 
-constexpr int CONV_THREADS = 512;     // 16 warps
-constexpr int CONV_XF_THREADS = 160;  // transform warps 2, 8, 9, 10, 11
-constexpr int CONV_HALF = 2 * CONV_TM;      // pixels per epilogue half (256 accumulator columns)
-// epilogue staging: two buffers of one 128-pixel tile each: the store of tile s drains while tile s + 1 is converted
-constexpr int CONV_SPLANE = CONV_TM * 16 + 32;    // bytes per 8-channel plane of a buffer (128 pixels x 16 B, +32 B bank skew)
-constexpr int CONV_STG_BUF = 16 * CONV_SPLANE;    // one tile: 16 planes (128 channels) x 128 pixels, bf16
-constexpr int CONV_STAGING = 2 * CONV_STG_BUF;
+constexpr int CONV_THREADS = 384;     // 12 warps
+constexpr int CONV_XF_THREADS = 64;   // transform warps 2, 3
+// epilogue staging, one buffer per consumer warpgroup: its 8 planes (64 channels) x 256 pixels, bf16
+constexpr int CONV_SPLANE = CONV_MAXG * CONV_TM * 16;   // bytes per 8-channel plane of a buffer
+constexpr int CONV_STG_WG = 8 * CONV_SPLANE;
+constexpr int CONV_STAGING = 2 * CONV_STG_WG;
 
 struct WorkItem {
   int n, ntile, m0, G;
@@ -99,11 +90,10 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_c
   const int a_bytes = p.a_stage;
 
   uint8_t* bring = smem + AS * a_bytes;                 // weight ring
-  uint8_t* stg = bring + BS * CONV_B_SLOT;              // epilogue staging: [16 planes][256 px][16 B] of one half item
+  uint8_t* stg = bring + BS * CONV_B_SLOT;              // epilogue staging: one buffer per consumer warpgroup
   uint8_t* ctrl = stg + CONV_STAGING;
-  // barriers: fullA[AS], readyA[AS], emptyA[AS], fullB[BS], emptyB[BS], tmem_full, tmem_empty
+  // barriers: fullA[AS], readyA[AS], emptyA[AS], fullB[BS], emptyB[BS]
   uint64_t* bars = reinterpret_cast<uint64_t*>(ctrl);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(ctrl + 504);
   const uint32_t smem_base = smem_u32(smem);
   const uint32_t bring_base = smem_u32(bring);
   const uint32_t bar_fullA = smem_u32(bars);
@@ -111,32 +101,21 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_c
   const uint32_t bar_emptyA = smem_u32(bars + 2 * ASM);
   const uint32_t bar_fullB = smem_u32(bars + 3 * ASM);
   const uint32_t bar_emptyB = smem_u32(bars + 3 * ASM + BSM);
-  const uint32_t bar_tfull = smem_u32(bars + 3 * ASM + 2 * BSM);        // [2]: accumulator half h is complete
-  const uint32_t bar_tempty = smem_u32(bars + 3 * ASM + 2 * BSM + 2);   // [2]: accumulator half h has been read out
-  static_assert((3 * ASM + 2 * BSM + 4) * 8 <= 504, "barrier block overflows");
+  static_assert((3 * ASM + 2 * BSM) * 8 <= 1024, "barrier block overflows");
 
   if (warp == 1 && lane == 0) {
     for (int s = 0; s < AS; ++s) {
       mbar_init(bar_fullA + 8 * s, 1);
-      // one arrival per transform WARP (its lanes meet on __syncwarp first); B200AD_CONV_DBG & 4096: one per thread (A/B)
-      mbar_init(bar_readyA + 8 * s, (p.dbg & 4096) ? CONV_XF_THREADS : CONV_XF_THREADS / 32);
-      mbar_init(bar_emptyA + 8 * s, 1);
+      mbar_init(bar_readyA + 8 * s, CONV_XF_THREADS / 32);   // one arrival per transform warp
+      mbar_init(bar_emptyA + 8 * s, 8);                       // one arrival per consumer warp
     }
     for (int s = 0; s < BS; ++s) {
       mbar_init(bar_fullB + 8 * s, 1);
-      mbar_init(bar_emptyB + 8 * s, 1);
-    }
-    for (int h = 0; h < 2; ++h) {
-      mbar_init(bar_tfull + 8 * h, 1);
-      mbar_init(bar_tempty + 8 * h, (p.dbg & 4096) ? 256 : 8);   // one arrival per epilogue warp
+      mbar_init(bar_emptyB + 8 * s, 8);
     }
     mbar_fence_init();
   }
-  if (warp == 2) tmem_alloc(smem_u32(tmem_slot), 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   // Programmatic dependent launch: this grid may have been started while the previous kernel of the stream was still
   // draining (its last wave, its last-CTA GroupNorm finalize).  Everything above, and the weight producer's prefetch below,
@@ -144,7 +123,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_c
   // launch is released at once - it parks at this same point.
   if (p.pdl) {
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-    if (warp != 3) asm volatile("griddepcontrol.wait;" ::: "memory");
+    if (warp != 1) asm volatile("griddepcontrol.wait;" ::: "memory");
   }
 
   if (warp == 0) {
@@ -189,7 +168,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_c
         if (++stage == AS) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 3) {
+  } else if (warp == 1) {
     // ================================ weight producer: slots of up to CONV_BT taps (12 KB), one bulk copy each
     if (lane == 0) {
       int stage = 0;
@@ -216,272 +195,167 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_c
         }
       }
     }
-  } else if (warp == 1) {
-    // ================================ MMA issuer. The warp runs convergently (all operands live in uniform registers);
-    // one elected lane issues. Per tap: weights (A, M = 128 cout) x pixel window (B, N = 256 then the remaining pixels).
-    constexpr uint32_t idesc256 = make_idesc_bf16(CONV_NT, 256);
-    constexpr uint32_t wdesc_lo_hi = ((CONV_NT / 8) * 128 >> 4) << 16;       // LBO of the weight blocks
-    constexpr uint64_t desc_hi = (uint64_t)((128u >> 4) | (1u << 14)) << 32;  // SBO = 128 B, descriptor version 1
-    int sa = 0, sb = 0;
-    uint32_t pa = 0, pb = 0;
-    uint32_t item = 0;
-    for (int w = blockIdx.x; w < p.total_work; w += gridDim.x, ++item) {
-      const WorkItem wi = decode_work(p, w);
-      const uint32_t d0 = tmem_base;
-      // pixel groups: [0, n0) with one MMA of N = n0 (<= 256) and, if the item has more than two tiles, [256, 256 + n1)
-      const int n0 = min(wi.G, 2) * CONV_TM, n1 = (wi.G - 2) * CONV_TM;
-      const uint32_t idesc0 = (n0 == 256) ? idesc256 : make_idesc_bf16(CONV_NT, CONV_TM);
-      const uint32_t idesc1 = (n1 == 256) ? idesc256 : make_idesc_bf16(CONV_NT, CONV_TM);
-      const bool two = n1 > 0 && !(p.dbg & 16);   // both accumulator halves in use: split the boundary k-steps
-      const uint32_t epar = (item & 1) ^ 1;
-      if (!two) {  // the epilogue has moved the previous item out of TMEM
-        mbar_wait_warp(bar_tempty, epar);
-        mbar_wait_warp(bar_tempty + 8, epar);
-        tc_fence_after();
-      }
-      for (int kidx = 0; kidx < p.ktotal; ++kidx) {
-        {
-          const ConvSeg& sg = p.seg[p.sched[kidx] >> 8];
-          const int npix = wi.G * CONV_TM + (sg.ht + sg.hb) * p.Wp + sg.hl + sg.hr;
-          const uint32_t xdesc_lo_hi = ((uint32_t)npix & 0x3FFF) << 16;  // LBO of the pixel windows = npix * 16 B
-          const int ntaps = sg.ntaps;
-          const bool first = kidx == 0, last = kidx == p.ktotal - 1;
-          mbar_wait_warp(bar_readyA + 8 * sa, pa);   // windows landed and (if asked) normalised in place
-          const uint32_t abase16 = (smem_base + sa * a_bytes) >> 4;
-          if (two && (first || last)) {
-            // Boundary k-step, half by half: all taps into columns 0-255, then all taps into 256-511 (the weights are read
-            // from shared memory twice instead of being latched).  Half 0 of the LAST k-step is complete one k-step's worth
-            // of MMAs before half 1, and half 0 of the next item's FIRST k-step only needs half 0 drained: the epilogue of
-            // either half runs under the other half's MMAs.
-            const int sb0 = sb;
-            const uint32_t pb0 = pb;
-            for (int h = 0; h < 2; ++h) {
-              if (first) {
-                mbar_wait_warp(bar_tempty + 8 * h, epar);
-                tc_fence_after();
-              }
-              sb = sb0; pb = pb0;
-              const uint32_t dh = d0 + (uint32_t)(h * CONV_HALF);
-              const uint32_t xoff = (uint32_t)(h * (CONV_HALF * 16 >> 4));
-              const uint32_t idesc = h ? idesc1 : idesc0;
-              for (int t0 = 0; t0 < ntaps; t0 += CONV_BT) {
-                if (h == 0) {
-                  mbar_wait_warp(bar_fullB + 8 * sb, pb);  // this slot's taps landed (still resident in the second pass)
-                  tc_fence_after();
-                }
-                const uint32_t bbase16 = (bring_base + sb * CONV_B_SLOT) >> 4;
-                const int nt = min(CONV_BT, ntaps - t0);
-                if (elect_one()) {
-                  for (int t = 0; t < nt; ++t) {
-                    const uint64_t wdesc = desc_hi | (uint64_t)((bbase16 + (uint32_t)t * (CONV_B_TAP >> 4)) | wdesc_lo_hi);
-                    const uint32_t x_lo = (abase16 + (uint32_t)sg.aoff[t0 + t] + xoff) | xdesc_lo_hi;
-                    umma_bf16(dh, wdesc, desc_hi | (uint64_t)x_lo, idesc, (first && t0 + t == 0) ? 0u : 1u);
-                  }
-                }
-                __syncwarp();
-                if (h == 1) umma_commit_elect(bar_emptyB + 8 * sb);  // frees the weight slot when these MMAs retire
-                if (++sb == BS) { sb = 0; pb ^= 1; }
-              }
-              if (last) umma_commit_elect(bar_tfull + 8 * h);
-            }
-          } else {
-            for (int t0 = 0; t0 < ntaps; t0 += CONV_BT) {
-              mbar_wait_warp(bar_fullB + 8 * sb, pb);  // this slot's taps landed
-              tc_fence_after();
-              const uint32_t bbase16 = (bring_base + sb * CONV_B_SLOT) >> 4;
-              const int nt = min(CONV_BT, ntaps - t0);
-              if (elect_one()) {
-                for (int t = 0; t < nt; ++t) {
-                  const uint64_t wdesc = desc_hi | (uint64_t)((bbase16 + (uint32_t)t * (CONV_B_TAP >> 4)) | wdesc_lo_hi);
-                  const uint32_t x_lo = (abase16 + (uint32_t)sg.aoff[t0 + t]) | xdesc_lo_hi;
-                  const uint32_t accum = (first && t0 + t == 0) ? 0u : 1u;
-                  if (n1 > 0) {  // two pixel groups share the weights: latch them in the A collector
-                    umma_bf16_afill(d0, wdesc, desc_hi | (uint64_t)x_lo, idesc0, accum);
-                    umma_bf16_alast(d0 + CONV_HALF, wdesc, desc_hi | (uint64_t)(x_lo + (CONV_HALF * 16 >> 4)), idesc1, accum);
-                  } else {
-                    umma_bf16(d0, wdesc, desc_hi | (uint64_t)x_lo, idesc0, accum);
-                  }
-                }
-              }
-              __syncwarp();
-              umma_commit_elect(bar_emptyB + 8 * sb);  // frees the weight slot when these MMAs retire
-              if (++sb == BS) { sb = 0; pb ^= 1; }
-            }
-          }
-          umma_commit_elect(bar_emptyA + 8 * sa);    // frees the activation slot
-          if (++sa == AS) { sa = 0; pa ^= 1; }
-        }
-      }
-      if (!two) {
-        umma_commit_elect(bar_tfull);
-        umma_commit_elect(bar_tfull + 8);
-      }
-    }
-  } else if ((warp >= 4 && warp < 8) || warp >= 12) {
-    // ================================ epilogue (8 warps). TMEM lane = output channel (interleaved, conv_lane_channel),
-    // column = pixel. The item leaves TMEM in two halves of 256 pixels: registers -> bf16 -> transposed into the 64 KB
-    // staging buffer as finished PF8 runs ([plane][pixel][8 ch]) -> ONE bulk store (TMA engine) per plane and half.
-    // The accumulators are released as soon as the last TMEM load has landed; the global stores (4.9 of the 6.8 ms/step the
-    // round-1 epilogue exposed: st.global from 8 warps moves ~20 B/clk/SM) drain behind the next item's MMAs.
-    // Two warps share a TMEM lane quarter (= 4 planes) and take alternate 32-pixel chunks; they meet on a named barrier.
-    const int q = warp & 3;                  // TMEM lane quarter = channels [32q, 32q + 32) of this cout tile
-    const int par = warp >> 3;               // 0: warps 4-7 (even chunks), 1: warps 12-15 (odd chunks)
-    const uint32_t stg_q = smem_u32(stg) + (uint32_t)(4 * q * CONV_SPLANE);    // this quarter's 4 planes
-    // stmatrix row address of this lane: matrix m = lane >> 3 holds pixel pair m of a group of 8 pixels, row r = lane & 7
-    // is (pixel 2m + (r & 1), plane r >> 1)
-    const uint32_t st_addr = stg_q + (uint32_t)(((lane & 7) >> 1) * CONV_SPLANE + (2 * (lane >> 3) + (lane & 1)) * 16);
+  } else if (warp >= 4) {
+    // ================================ consumer warpgroup cw: output channels [64 cw, 64 cw + 64) of the item's cout tile.
+    // Accumulator fragment: warp wq, lane l holds channels 64 cw + 16 wq + l/4 (h = 0) and +8 (h = 1) for pixels
+    // 8j + 2 (l % 4) + {0, 1} in acc[4j + 2h + {0, 1}].
+    const int cw = (warp - 4) >> 2, wq = warp & 3, tid = threadIdx.x & 127;
+    const uint32_t stg_w = smem_u32(stg) + (uint32_t)(cw * CONV_STG_WG);
+    // stmatrix.x4.trans row address of this lane: matrix m = lane >> 3 is (8-pixel group 2k + (m >> 1), plane 2 wq + (m & 1)),
+    // row r = lane & 7 is pixel r of that group; element c of the row comes from lane 4c + r / 2
+    const uint32_t st_addr = stg_w + (uint32_t)((2 * wq + ((lane >> 3) & 1)) * CONV_SPLANE + (8 * (lane >> 4) + (lane & 7)) * 16);
     const Geom og = make_geom(p.N, p.up2 ? 2 * p.H : p.H, p.up2 ? 2 * p.W : p.W);   // geometry of the output tensor
     const long long out_img_stride = (long long)(p.cout >> 3) * og.PL * 8;
     const int hw_end = p.H * p.Wp;
     const bool do_stats = p.stats != nullptr;
-    const bool issuer = par == 0 && lane < 4;         // lane g of warp (q, 0) stores plane 4q + g
-    const int cw = ((lane & 3) << 3) | (lane >> 2);   // this lane's channel within the warp's 32 (conv_lane_channel)
-    uint32_t item = 0;
-    for (int w = blockIdx.x; w < p.total_work; w += gridDim.x, ++item) {
+    const bool issuer = tid < 8 * CONV_MAXG;   // thread (tile g, plane pl) = (tid >> 3, tid & 7) bulk-stores one run
+    float acc[CONV_MAXG * CONV_TM / 2];
+    int sa = 0, sb = 0;
+    uint32_t pa = 0, pb = 0;
+    for (int w = blockIdx.x; w < p.total_work; w += gridDim.x) {
       const WorkItem wi = decode_work(p, w);
-      const int c = wi.ntile * CONV_NT + q * 32 + cw;   // this thread's output channel
-      const float bias0 = p.bias ? __ldg(p.bias + c) : 0.f;
-      f32x2_t bias2;
-      __nv_bfloat16* out_pl;     // the four 8-channel planes this warp pair writes
-      // per-sample state (bias + time-embedding row, output image): the item's sample, or - packed small images - tile g's
-      auto set_sample = [&](int n) {
-        float b = bias0;
-        if (p.temb) b += __ldg(p.temb + (long long)n * p.temb_stride + c);
-        bias2 = f2_pack(b, b);
-        out_pl = p.out + (long long)n * out_img_stride + (long long)(wi.ntile * 16 + q * 4) * og.PL * 8;
+#pragma unroll
+      for (int i = 0; i < CONV_MAXG * CONV_TM / 2; ++i) acc[i] = 0.f;
+      // MMA groups: one per weight slot, one group in flight; pend_* = the slots of the group before the current one
+      int pend_b = -1, pend_a = -1;
+      auto release = [&]() {
+        __syncwarp();
+        if (lane == 0) {
+          if (pend_b >= 0) mbar_arrive(bar_emptyB + 8 * pend_b);
+          if (pend_a >= 0) mbar_arrive(bar_emptyA + 8 * pend_a);
+        }
       };
-      set_sample(wi.n);
+      for (int kidx = 0; kidx < p.ktotal; ++kidx) {
+        const ConvSeg& sg = p.seg[p.sched[kidx] >> 8];
+        const int npix = wi.G * CONV_TM + (sg.ht + sg.hb) * p.Wp + sg.hl + sg.hr;
+        const uint32_t xlbo = (uint32_t)npix * 16u;   // the second 8-channel plane of the window
+        const int ntaps = sg.ntaps;
+        mbar_wait(bar_readyA + 8 * sa, pa);   // windows landed and (if asked) normalised in place
+        const uint32_t abase = smem_base + sa * a_bytes;
+        for (int t0 = 0; t0 < ntaps; t0 += CONV_BT) {
+          mbar_wait(bar_fullB + 8 * sb, pb);  // this slot's taps landed
+          const uint32_t bbase = bring_base + sb * CONV_B_SLOT + (uint32_t)(cw * 1024);   // rows 64 cw .. 64 cw + 63
+          const int nt = min(CONV_BT, ntaps - t0);
+          wgmma_fence();
+          for (int t = 0; t < nt; ++t) {
+            const uint64_t wdesc = gmma_desc(bbase + (uint32_t)t * CONV_B_TAP, (CONV_NT / 8) * 128, 128);
+            const uint64_t xdesc = gmma_desc(abase + (uint32_t)sg.aoff[t0 + t] * 16u, xlbo, 128);
+            if (wi.G == 2) wgmma_m64n256k16<0, 0>(acc, wdesc, xdesc);
+            else           wgmma_m64n128k16<0, 0>(acc, wdesc, xdesc);
+          }
+          wgmma_commit();
+          wgmma_wait<1>();   // the previous group has retired: its slots are free
+          release();
+          pend_b = sb;
+          pend_a = (t0 + CONV_BT >= ntaps) ? sa : -1;
+          if (++sb == BS) { sb = 0; pb ^= 1; }
+        }
+        if (++sa == AS) { sa = 0; pa ^= 1; }
+      }
+      wgmma_wait<0>();
+      release();
 
-      f32x2_t ssum2 = 0ull, ssq2 = 0ull;     // (even pixel, odd pixel) partial sums of this thread's channel
-      // quad (4-channel) partial sums: channels 4k..4k+3 of a plane sit in lanes 4 apart; fp64 atomics into sample n
-      auto flush_stats = [&](int n) {
-        const float2 s2 = f2_unpack(ssum2), q2 = f2_unpack(ssq2);
-        float ssum = s2.x + s2.y, ssq = q2.x + q2.y;
-        ssum += __shfl_xor_sync(0xffffffffu, ssum, 4);
-        ssq += __shfl_xor_sync(0xffffffffu, ssq, 4);
-        ssum += __shfl_xor_sync(0xffffffffu, ssum, 8);
-        ssq += __shfl_xor_sync(0xffffffffu, ssq, 8);
-        if ((lane & 12) == 0) {
-          stat_t* sdst = p.stats + ((long long)n * (p.cout >> 2) + (c >> 2)) * 2;
-          atomicAdd(sdst, (stat_t)ssum);
-          atomicAdd(sdst + 1, (stat_t)ssq);
-        }
-        ssum2 = 0ull;
-        ssq2 = 0ull;
-      };
-      const int nchunk = (p.dbg & 8) ? 0 : wi.G * (CONV_TM / 32);
-      const uint32_t tsrc = tmem_base + ((uint32_t)(q * 32) << 16);
-      // one 32-pixel chunk: +bias, statistics, bf16, transposed store into the staging buffer at pixel offset `spx`
-      auto process = [&](const uint32_t (&r)[32], int jc, uint32_t boff, int spx) {
-        const int mc = p.pack ? (jc & 3) * 32 : wi.m0 + jc * 32;   // first pixel of the chunk within its image
-        // validity mask of the chunk's 32 pixels: pad columns and the run-off behind the image are written as ZEROS (they
-        // are zero guards of the layout) and do not count for the statistics
-        uint32_t mask;
-        {
-          const int nvalid = min(32, max(0, hw_end - mc));
-          mask = (nvalid == 32) ? 0xffffffffu : ((1u << nvalid) - 1u);
-          int cc = mc % p.Wp;
-          if (p.Wp > 32) {            // at most one pad column per chunk
-            const int pe = p.W - cc;
-            if (pe >= 0 && pe < 32) mask &= ~(1u << pe);
-          } else {
-            for (int e = 0; e < 32; ++e) {
-              if (cc == p.W) mask &= ~(1u << e);
-              if (++cc == p.Wp) cc = 0;
+      // ---- epilogue. The staging buffer is free once this warpgroup's bulk stores of the previous item have read it.
+      if (issuer) bulk_wait_read_all();
+      named_bar_sync(1 + cw, 128);
+      if (!(p.dbg & 8)) {
+        float ssum[2] = {0.f, 0.f}, ssq[2] = {0.f, 0.f};   // partial sums of this thread's two channels
+#pragma unroll
+        for (int g = 0; g < CONV_MAXG; ++g) {
+          if (g < wi.G) {
+            const int n = p.pack ? wi.n + g : wi.n;
+            float bias[2];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int c = wi.ntile * CONV_NT + cw * 64 + wq * 16 + 8 * h + (lane >> 2);
+              bias[h] = p.bias ? __ldg(p.bias + c) : 0.f;
+              if (p.temb) bias[h] += __ldg(p.temb + (long long)n * p.temb_stride + c);
             }
-          }
-        }
-        uint32_t pk[16];
-        if (mask == 0xffffffffu) {   // common case: no per-element predicate
+            // first pixel of this thread within its image, and its column
+            int m = (p.pack ? 0 : wi.m0 + g * CONV_TM) + 2 * (lane & 3);
+            int col = m % p.Wp;
 #pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const f32x2_t v = f2_add(f2_pack(__uint_as_float(r[2 * j]), __uint_as_float(r[2 * j + 1])), bias2);
-            ssum2 = f2_add(ssum2, v);
-            ssq2 = f2_fma(v, v, ssq2);
-            pk[j] = f2_to_bf16x2(v);
-          }
-        } else {
+            for (int k = 0; k < CONV_TM / 16; ++k) {   // two 8-pixel groups per stmatrix.x4
+              uint32_t pk[4];
 #pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const f32x2_t v = f2_add(f2_pack(__uint_as_float(r[2 * j]), __uint_as_float(r[2 * j + 1])), bias2);
-            const float2 f = f2_unpack(v);
-            const f32x2_t vm = f2_pack(((mask >> (2 * j)) & 1) ? f.x : 0.f, ((mask >> (2 * j + 1)) & 1) ? f.y : 0.f);
-            ssum2 = f2_add(ssum2, vm);
-            ssq2 = f2_fma(vm, vm, ssq2);
-            pk[j] = f2_to_bf16x2(vm);
-          }
-        }
-        const uint32_t sa = st_addr + boff + (uint32_t)spx * 16u;
+              for (int u = 0; u < 2; ++u) {
+                // pad columns and the run-off behind the image are written as ZEROS (they are zero guards of the layout)
+                // and do not count for the statistics
+                const int col1 = (col + 1 == p.Wp) ? 0 : col + 1;
+                const bool v0 = m < hw_end && col < p.W, v1 = m + 1 < hw_end && col1 < p.W;
 #pragma unroll
-        for (int k = 0; k < 4; ++k) stmatrix_x4_trans(sa + 128u * k, pk[4 * k], pk[4 * k + 1], pk[4 * k + 2], pk[4 * k + 3]);
-        if (p.up2) {   // folded upsample: scatter into the 2x tensor at this launch's parity, straight from the staging rows
-          __syncwarp();
-          if (((mask >> lane) & 1) && !(p.dbg & 2)) {
-            const int m = mc + lane, hh = m / p.Wp, ww = m - hh * p.Wp;
-            const long long pix = (long long)(og.lead + (2 * hh + p.oy) * og.Wp + 2 * ww + p.ox) * 8;
-#pragma unroll
-            for (int g = 0; g < 4; ++g) {
-              const uint4 o = *reinterpret_cast<const uint4*>(stg + (4 * q + g) * CONV_SPLANE + (spx + lane) * 16);
-              *reinterpret_cast<uint4*>(out_pl + (long long)g * og.PL * 8 + pix) = o;
+                for (int h = 0; h < 2; ++h) {
+                  const int j = g * (CONV_TM / 8) + 2 * k + u;
+                  const float a0 = v0 ? acc[4 * j + 2 * h] + bias[h] : 0.f;
+                  const float a1 = v1 ? acc[4 * j + 2 * h + 1] + bias[h] : 0.f;
+                  ssum[h] += a0 + a1;
+                  ssq[h] = fmaf(a0, a0, fmaf(a1, a1, ssq[h]));
+                  pk[2 * u + h] = pack_bf16x2(a0, a1);
+                }
+                m += 8;
+                col += 8;
+                while (col >= p.Wp) col -= p.Wp;
+              }
+              stmatrix_x4_trans(st_addr + (uint32_t)((g * CONV_TM + 16 * k) * 16), pk[0], pk[1], pk[2], pk[3]);
             }
-          }
-          __syncwarp();
-        }
-      };
-      // The item leaves TMEM tile by tile (128 pixels = 4 chunks; the two warps of a pair take two chunks each) through two
-      // staging buffers: while the TMA engine reads tile s out of one buffer, tile s + 1 is converted into the other one.
-      // One named barrier per tile: it publishes the tile's staging rows and, because the issuer first waits for its
-      // earlier stores to have been read, tells both warps that the other buffer is free again.
-#pragma unroll 1
-      for (int sblk = 0; sblk < CONV_MAXG; ++sblk) {
-        const int h = sblk >> 1;
-        if ((sblk & 1) == 0) {
-          mbar_wait(bar_tfull + 8 * h, item & 1);   // the MMAs into this half have retired
-          tc_fence_after();
-        }
-        const bool live = sblk < wi.G && nchunk > 0;
-        const uint32_t boff = p.up2 ? 0u : (uint32_t)((sblk & 1) * CONV_STG_BUF);
-        if (p.pack && live && sblk > 0) set_sample(wi.n + sblk);   // packed small images: tile g is image n + g
-        if (live) {
-          uint32_t ra[32], rb[32];
-          const int j0 = 4 * sblk + par;
-          tmem_ld32(tsrc + (uint32_t)(j0 * 32), ra);
-          tmem_ld32(tsrc + (uint32_t)((j0 + 2) * 32), rb);
-          tmem_ld_wait();
-          process(ra, j0, boff, par * 32);
-          process(rb, j0 + 2, boff, p.up2 ? par * 32 : (par + 2) * 32);
-          if (p.pack && do_stats) flush_stats(wi.n + sblk);
-        }
-        if (sblk & 1) {   // every TMEM load of this thread from this half has landed: the MMA warp may overwrite it
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0 || (p.dbg & 4096)) mbar_arrive(bar_tempty + 8 * h);
-        }
-        if (!p.up2) {
-          if (live) fence_proxy_async_smem();   // staging rows written through the generic proxy -> visible to the TMA engine
-          if (issuer) bulk_wait_read_all();     // this thread's earlier stores (the other buffer) have been read out
-          __syncwarp();
-          named_bar_sync(1 + q, 64);
-          if (live && issuer && !(p.dbg & 2)) {
-            bulk_s2g(out_pl + (long long)lane * og.PL * 8 + (long long)(p.lead + (p.pack ? 0 : wi.m0 + CONV_TM * sblk)) * 8,
-                     stg_q + boff + (uint32_t)(lane * CONV_SPLANE), (uint32_t)CONV_TM * 16u);
-            bulk_commit();
+            if (do_stats && (p.pack || g == wi.G - 1)) {
+              // quad (4-channel) sums: the 4 lanes of a channel and the 4 channels of a quad are the lanes of a half-warp
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                float s1 = ssum[h], s2 = ssq[h];
+#pragma unroll
+                for (int o = 1; o < 16; o <<= 1) {
+                  s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+                  s2 += __shfl_xor_sync(0xffffffffu, s2, o);
+                }
+                if ((lane & 15) == 0) {
+                  const int c = wi.ntile * CONV_NT + cw * 64 + wq * 16 + 8 * h + (lane >> 2);
+                  stat_t* sdst = p.stats + ((long long)n * (p.cout >> 2) + (c >> 2)) * 2;
+                  atomicAdd(sdst, (stat_t)s1);
+                  atomicAdd(sdst + 1, (stat_t)s2);
+                }
+                ssum[h] = 0.f;
+                ssq[h] = 0.f;
+              }
+            }
           }
         }
       }
-
-      if (do_stats && !p.pack) flush_stats(wi.n);
+      if (!p.up2) {
+        fence_proxy_async_smem();   // staging rows written through the generic proxy -> visible to the TMA engine
+        named_bar_sync(1 + cw, 128);
+        const int g = tid >> 3, pl = tid & 7;
+        if (issuer && g < wi.G && !(p.dbg & 2)) {
+          const int n = p.pack ? wi.n + g : wi.n;
+          bulk_s2g(p.out + (long long)n * out_img_stride + (long long)(wi.ntile * 16 + cw * 8 + pl) * og.PL * 8 +
+                       (long long)(p.lead + (p.pack ? 0 : wi.m0 + CONV_TM * g)) * 8,
+                   stg_w + (uint32_t)(pl * CONV_SPLANE + g * CONV_TM * 16), (uint32_t)CONV_TM * 16u);
+          bulk_commit();
+        }
+      } else {
+        // folded upsample: scatter into the 2x tensor at this launch's parity, straight from the staging rows
+        named_bar_sync(1 + cw, 128);
+        const int npx = wi.G * CONV_TM;
+        for (int i = tid; i < 8 * npx && !(p.dbg & 2); i += 128) {
+          const int pl = i / npx, px = i - pl * npx, g = px >> 7;
+          const int m = p.pack ? px & (CONV_TM - 1) : wi.m0 + px;
+          const int hh = m / p.Wp, ww = m - hh * p.Wp;
+          if (m < hw_end && ww < p.W) {
+            const int n = p.pack ? wi.n + g : wi.n;
+            const uint4 o = *reinterpret_cast<const uint4*>(stg + cw * CONV_STG_WG + pl * CONV_SPLANE + px * 16);
+            *reinterpret_cast<uint4*>(p.out + (long long)n * out_img_stride + (long long)(wi.ntile * 16 + cw * 8 + pl) * og.PL * 8 +
+                                      (long long)(og.lead + (2 * hh + p.oy) * og.Wp + 2 * ww + p.ox) * 8) = o;
+          }
+        }
+      }
     }
     if (issuer) bulk_wait_all();   // shared memory must outlive the engine's reads; the stores complete before the CTA exits
   } else {
-    // ================================ transform warps (2, 8..11): GroupNorm(+SiLU) of the landed windows, in place.
-    // Every 160-pixel sweep of a window is five groups of 32 pixels, one per transform warp.  (Weighting the shares so that
-    // the sub-partition hosting two transform warps, 2 and 10, gets a quarter of the work like the others - 2:2:2:1:1 over a
-    // 256-pixel sweep - measured 2.4 ms / step SLOWER in the in-process A/B of round 2: the longest warp, not the busiest
-    // sub-partition, sets the stage latency.)
-    const int xg0 = (warp == 2) ? 0 : (warp - 7);
+    // ================================ transform warps (2, 3): GroupNorm(+SiLU) of the landed windows, in place.
+    // Every 64-pixel sweep of a window is two groups of 32 pixels, one per transform warp.
+    const int xg0 = warp - 2;
     constexpr int xng = 1;
-    constexpr int XSWEEP = 160;
+    constexpr int XSWEEP = CONV_XF_THREADS;
     int stage = 0;
     uint32_t phase = 0;
     for (int w = blockIdx.x; w < p.total_work; w += gridDim.x) {
@@ -526,7 +400,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_c
             // touched - everything else in the window is zero guard from global memory and stays zero
             uint4* base = reinterpret_cast<uint4*>(smem + stage * a_bytes);
             const int lead_px = sg.ht * p.Wp + sg.hl, hw = p.H * p.Wp;
-            const int tidx = ((warp == 2) ? 0 : (warp - 7)) * 32 + lane;
+            const int tidx = (warp - 2) * 32 + lane;
             const float hs = silu ? 0.5f : 1.0f;
             for (int g = 0; g < wi.G; ++g) {
               const float4* sp = reinterpret_cast<const float4*>(ssn + (long long)g * sg.ss_stride + ks * 16);
@@ -581,7 +455,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_c
           // every lane has fenced its own writes towards the async proxy; the warp then arrives ONCE (32 same-address
           // shared-memory atomics per warp and k-step were ~7 % of the kernel's shared-memory wavefronts)
           __syncwarp();
-          if (lane == 0 || (p.dbg & 4096)) mbar_arrive(bar_readyA + 8 * stage);
+          if (lane == 0) mbar_arrive(bar_readyA + 8 * stage);
           if (++stage == AS) { stage = 0; phase ^= 1; }
         }
       }
@@ -589,9 +463,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_c
   }
 
   if (p.fin.ss) __threadfence();   // this thread's statistics atomics are ordered before the CTA's arrival below
-  tc_fence_before();
   __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem_base, 512);
 
   // ---- GroupNorm finalize of the consumer, by the last CTA to arrive (replaces a launch per GroupNorm)
   if (p.fin.ss) {
@@ -665,9 +537,8 @@ cudaError_t launch_conv_tc(const ConvParams& p_in, int num_sms, cudaStream_t str
   for (int s = 0; s < p.nseg; ++s)
     if (p.seg[s].wtile_stride == 0) p.seg[s].wtile_stride = (long long)p.seg[s].ksteps * p.seg[s].ntaps * (CONV_B_TAP / 2);
   // Experiment (B200AD_CONV_DBG & 128, off by default): move trailing 1-tap segments (shortcut / residual) in front of the
-  // main segment's last k-step so that a 9-tap k-step closes the K loop and the half-by-half overlap of the epilogue gets a
-  // full k-step at both ends.  Measured slower (+0.3 ms / step, in-process A/B): the 1-tap k-steps are load-bound (a 16 KB
-  // window per 256 MMA cycles) and stall the 3-deep ring in the middle of the item instead of next to the epilogue.
+  // main segment's last k-step so that a many-tap k-step closes the K loop.  The 1-tap k-steps are load-bound (a 16 KB
+  // window per k-step of MMAs) and would stall the ring in the middle of the item instead of next to the epilogue.
   if ((dbg & 128) && p.nseg >= 2 && p.nseg < CONV_MAXSEG && p.seg[0].ksteps >= 2 && p.seg[p.nseg - 1].ntaps < p.seg[0].ntaps) {
     ConvSeg tail = p.seg[0];
     const int ka = tail.ksteps - 1;
@@ -690,8 +561,7 @@ cudaError_t launch_conv_tc(const ConvParams& p_in, int num_sms, cudaStream_t str
     int nh = 0, nl = 0;
     for (int s = 0; s < p.nseg; ++s) (p.seg[s].ntaps > 1 ? nh : nl) += p.seg[s].ksteps;
     int n = 0;
-    // (measured: interleaving is 1.6 ms / step SLOWER than segment-by-segment order - in-process A/B, profiles/ab_conv_r02.txt -
-    //  so it is an experiment switch, B200AD_CONV_DBG & 2048, not the default)
+    // (interleaving is an experiment switch, B200AD_CONV_DBG & 2048, not the default)
     if (!(dbg & 2048) || nh < 2 || nl == 0) {
       for (int s = 0; s < p.nseg; ++s)
         for (int ks = 0; ks < p.seg[s].ksteps; ++ks) p.sched[n++] = (unsigned short)((s << 8) | ks);
@@ -806,7 +676,7 @@ __global__ void pack_identity_kernel(int channels, __nv_bfloat16* __restrict__ d
   const long long rest = id >> 8;
   const int ksteps = channels / 16;
   const int ks = (int)(rest % ksteps), ntile = (int)(rest / ksteps);
-  const int co = ntile * 128 + conv_lane_channel(n8 * 8 + r);
+  const int co = ntile * 128 + n8 * 8 + r;
   const int ci0 = ks * 16 + k8 * 8;
   uint32_t o[4];
 #pragma unroll

@@ -1,12 +1,12 @@
-// Parameter block of the tcgen05 implicit-GEMM convolution (conv_tc.cu). Host + device.
+// Parameter block of the wgmma implicit-GEMM convolution (conv_tc.cu). Host + device.
 #pragma once
 #include "common.cuh"
 
 namespace b200ad {
 
-constexpr int CONV_NT = 128;        // output-channel tile = MMA M (TMEM lanes)
+constexpr int CONV_NT = 128;        // output-channel tile = 2 x MMA M (one 64-row half per consumer warpgroup)
 constexpr int CONV_TM = 128;        // pixels per tile; an MMA covers up to two tiles (N = 256)
-constexpr int CONV_MAXG = 4;        // pixel tiles per work item: 4 x 128 fp32 columns = all of TMEM
+constexpr int CONV_MAXG = 2;        // pixel tiles per work item: 64 x 256 fp32 accumulators = 128 registers per thread
 constexpr int CONV_MAXSEG = 6;      // K-segments per launch (callers use up to 4; the launcher may split one, see below)
 constexpr int CONV_MAXTAPS = 9;
 constexpr int CONV_MAXSCHED = 256;  // k-steps of one item (all segments); a k-step index within its segment is 8 bits
@@ -19,7 +19,7 @@ constexpr int CONV_SMEM_MAX = 227 * 1024;
 constexpr int CONV_BT = 3;                       // taps per weight slot
 constexpr int CONV_B_SLOT = CONV_BT * CONV_B_TAP;
 constexpr int CONV_AS_MAX = 8;    // launches with small windows use more activation stages (see launch_conv_tc)
-constexpr int CONV_AS = 3;   // (4 / 6 measured the same as 3 / 5 in round 1; the bytes now buy the epilogue staging buffer)
+constexpr int CONV_AS = 3;        // minimum activation-ring depth
 constexpr int CONV_BS = 5;        // minimum weight-ring depth (W = 256: shared memory is full)
 constexpr int CONV_BS_MAX = 10;   // launches with smaller activation stages use the rest for a deeper weight ring
 
@@ -28,7 +28,7 @@ constexpr int CONV_BS_MAX = 10;   // launches with smaller activation stages use
 // conv is four segments (one per input parity plane).
 struct ConvSeg {
   const __nv_bfloat16* src;    // PF8 activations, same geometry as the output
-  const __nv_bfloat16* wpack;  // [cout/128][ksteps][ntaps][2 k8][16 lanes8][8][8] bf16, rows in conv_lane_channel order
+  const __nv_bfloat16* wpack;  // [cout/128][ksteps][ntaps][2 k8][16 rows8][8][8] bf16, rows in channel order
   long long img_stride;        // elements between images of src (= C/8 * PL * 8)
   long long wtile_stride;      // elements between cout tiles of wpack (0: ksteps * ntaps * 2048; set by the launcher)
   int ksteps;                  // input channels / 16
@@ -64,9 +64,8 @@ struct ConvParams {
   int N, H, W, Wp, lead, PL;
   int ktotal;           // sum of the segments' k-steps (set by the launcher)
   // Order of the k-steps of an item, (segment << 8) | k-step (set by the launcher): segment by segment.  Experiment
-  // (B200AD_CONV_DBG & 2048): many-tap and 1-tap k-steps (shortcut, residual) interleaved - a 1-tap k-step needs a 16 KB
-  // window for 256 MMA cycles (80 B/clk against ~42 B/clk of L2 -> SM throughput), so spreading them between 9-tap k-steps
-  // should hide their loads; measured 1.6 ms / step slower.
+  // (B200AD_CONV_DBG & 2048): many-tap and 1-tap k-steps (shortcut, residual) interleaved, to spread the 1-tap k-steps'
+  // window loads between many-tap k-steps.
   unsigned short sched[CONV_MAXSCHED];
   int a_stage;          // bytes reserved for the A strips of one stage (set by the launcher)
   int groups_per_img;
@@ -86,7 +85,7 @@ struct ConvParams {
   // (2h + oy, 2w + ox) of the (2H, 2W) output tensor. One launch per output parity (oy, ox) with pre-summed 2x2 weights.
   int up2, oy, ox;
   ConvGnFin fin;
-  int dbg;                      // B200AD_CONV_DBG bit flags (timing experiments only): 2 no stores, 4 CTAs out of phase, 8 no epilogue work, 16 no half-by-half boundary k-steps, 32 no weight loads, 64 no transform, 128 reorder 1-tap segments before the last main k-step, 256 no small-image packing, 512 rings fixed at CONV_AS stages / CONV_BS slots, 1024 no programmatic dependent launch, 2048 interleave 1-tap k-steps between many-tap ones, 4096 per-thread (not per-warp) mbarrier arrivals
+  int dbg;                      // B200AD_CONV_DBG bit flags (timing experiments only): 2 no stores, 4 CTAs out of phase, 8 no epilogue work, 32 no weight loads, 64 no transform, 128 reorder 1-tap segments before the last main k-step, 256 no small-image packing, 512 rings fixed at CONV_AS stages / CONV_BS slots, 1024 no programmatic dependent launch, 2048 interleave 1-tap k-steps between many-tap ones
 };
 
 cudaError_t launch_conv_tc(const ConvParams& p, int num_sms, cudaStream_t stream);

@@ -21,7 +21,7 @@ __device__ __forceinline__ void pack_one_vector(const float* __restrict__ w, int
   rest /= taps.ntaps;
   const int ks = (int)(rest % ksteps);
   const int ntile = (int)(rest / ksteps);
-  const int co = ntile * 128 + conv_lane_channel(n8 * 8 + r);   // TMEM lane -> channel interleave (conv_tc.cuh)
+  const int co = ntile * 128 + n8 * 8 + r;
   const int ci0 = cin_off + ks * 16 + k8 * 8;
   float v[8];
 #pragma unroll

@@ -2,7 +2,7 @@
 // and uint8 -> dB -> power -> inverse mel -> 32-iteration Griffin-Lim (Mel.image_to_audio, audiodiffusion/mel.py:153-168).
 // The librosa 0.10.2 arithmetic these follow is restated in oracle/mel_oracle.py.
 //
-// All FFTs run in fp64 (B200 has the fp64 rate to spare; the reference mixes fp64 FFTs with fp32 storage), one frame per
+// All FFTs run in fp64 (H100 has the fp64 rate to spare; the reference mixes fp64 FFTs with fp32 storage), one frame per
 // CTA.  A real n_fft-point transform is ONE complex transform of n_fft / 2 points (even samples = real parts, odd samples =
 // imaginary parts) plus an O(n_fft) split / merge step, and the complex transform is a Stockham autosort with radix-4
 // passes in shared memory (one radix-2 pass first when log2 is odd): 5 passes over 1024 points for n_fft = 2048 where the

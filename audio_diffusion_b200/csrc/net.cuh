@@ -108,7 +108,7 @@ struct NetBase {
   float* temb_emb = nullptr;        // [N][dim0]      sinusoid
   float* temb_u1 = nullptr;         // [N][4 dim0]    linear_1 output before SiLU
   float* temb_u2 = nullptr;         // [N][4 dim0]    linear_2 output before SiLU
-  int num_sms = 148;
+  int num_sms = 132;
   const float* enc = nullptr;       // conditional U-Net: encoder_hidden_states [N][enc_S][X] of the next forward
   int enc_S = 0;
   int last_launches = 0;

@@ -3,7 +3,7 @@
 // the gradients of all parameters.
 //   * data gradients of every convolution run on conv_tc_kernel with transposed / mirrored weight packing (stride-2 convs
 //     as four scatter launches, the folded upsampling convs as one gather launch over the parity planes of the gradient);
-//   * weight gradients run on wgrad_tc_kernel (tcgen05, pixels as the reduction dimension, MN-major operands);
+//   * weight gradients run on wgrad_tc_kernel (wgmma, pixels as the reduction dimension, MN-major operands);
 //   * GroupNorm(+SiLU), attention core, biases / time embedding, conv_in / conv_out are memory-bound kernels (bwd_kernels.cu).
 // This first version materialises the normalised activations for the weight gradients (no fusion yet) — DESIGN.md §6.
 #include "bwd_kernels.cuh"

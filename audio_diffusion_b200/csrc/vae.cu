@@ -3,7 +3,7 @@
 //   audiodiffusion/pipeline_audio_diffusion.py:143-147   vqvae.encode(x).latent_dist.sample(generator) * scaling_factor
 //   audiodiffusion/pipeline_audio_diffusion.py:187-190   vqvae.decode(1 / scaling_factor * z)["sample"]
 // Parameter names are the diffusers state-dict keys that audiodiffusion/utils.py:156-303 (convert_ldm_to_hf_vae) emits.
-// The resnets, attention and up/down-samplers run on the same tcgen05 implicit-GEMM kernel as the U-Net (net.cuh).
+// The resnets, attention and up/down-samplers run on the same wgmma implicit-GEMM kernel as the U-Net (net.cuh).
 #include "net.cuh"
 
 using namespace b200ad;

@@ -1,14 +1,14 @@
-// Weight gradient of a convolution on tcgen05 (DESIGN.md §3 "Training step").
+// Weight gradient of a convolution on wgmma.
 //   dW[co][ci][tap] = sum over samples and flat pixels p of  gY[co][p] * A[ci][p + shift(tap)]
 // GEMM view per tap: D[M = 128 co][N = NCI ci] += sum_K gY[co][K = pixel] * A[ci][K = pixel + shift]: the reduction runs over
 // PIXELS, so both operands are "MN-major": in PF8 the 8 channels of a pixel are contiguous (MN) and consecutive pixels are
 // 16 B apart (K) — a run of 8 pixels of one 8-channel plane IS the 8x8 MN-major core matrix (128 B): LBO (next 8 pixels) =
-// 128 B, SBO (next 8 channels) = the plane pitch of the staged window (verified on hardware: tools/wgrad_probe.py).
+// 128 B, SBO (next 8 channels) = the plane pitch of the staged window.
 // Work decomposition: one CTA = (128-co tile, NCI-ci tile, ONE ROW of taps (same dh, dw in {-1,0,+1}), a share of the pixel
-// blocks).  A tap row needs only a 1-pixel halo (the row offset dh*Wp moves the window start), its <= 3 taps are shifted
-// descriptors of one activation window, and N = 128 keeps the per-MMA fixed cost small (measured: N = 32 MMAs cost ~110
-// cycles each, 7x their tensor time).  The gY block (A operand) is latched in the A collector across the taps of a row.
-// TMEM: 3 taps x NCI fp32 columns.  Partial dW is added to global memory with fp32 atomics (split-K over pixels and CTAs).
+// blocks).  A tap row needs only a 1-pixel halo (the row offset dh*Wp moves the window start), and its <= 3 taps are shifted
+// descriptors of one activation window.  Two consumer warpgroups take 64 output channels each and keep 3 taps x NCI fp32
+// accumulators in registers across all of the CTA's pixel blocks.  Partial dW is added to global memory with fp32 atomics
+// (split-K over pixels and CTAs).
 #include <cstdlib>
 
 #include "bwd_kernels.cuh"
@@ -31,7 +31,7 @@ struct WgradParams {
   int nblk;                   // blocks per image
 };
 
-constexpr int WG_THREADS = 192;   // warp 0 producer, warp 1 MMA, warps 2-5 epilogue
+constexpr int WG_THREADS = 288;   // warps 0-3 and 4-7: consumer warpgroups (MMA + epilogue), warp 8: producer
 
 template <int NCI, int STAGES>
 __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_tc_kernel(const __grid_constant__ WgradParams p) {
@@ -42,25 +42,19 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_tc_kernel(const __grid_co
   const int act_bytes = (NCI / 8) * act_pix * 16;
   const int stage_bytes = (gy_bytes + act_bytes + 127) & ~127;
   uint8_t* ctrl = smem + STAGES * stage_bytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(ctrl);         // full[S], empty[S], done
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(ctrl + 128);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(ctrl);         // full[S], empty[S]
   const uint32_t smem_base = smem_u32(smem);
-  const uint32_t bar_full = smem_u32(bars), bar_empty = smem_u32(bars + STAGES), bar_done = smem_u32(bars + 2 * STAGES);
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 1); }
-    mbar_init(bar_done, 1);
+  const uint32_t bar_full = smem_u32(bars), bar_empty = smem_u32(bars + STAGES);
+  if (warp == 8 && lane == 0) {
+    for (int s = 0; s < STAGES; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 8); }
     mbar_fence_init();
   }
-  if (warp == 2) tmem_alloc(smem_u32(tmem_slot), 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const int row = blockIdx.y % p.nrows, cj = blockIdx.y / p.nrows, ct = blockIdx.z;
   const int total_blocks = p.N * p.nblk;
   const int ntaps = p.row_ntaps[row];
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -82,72 +76,65 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_tc_kernel(const __grid_co
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    // MMA issuer: the warp runs convergently (operands in uniform registers, waits exit on a vote), one elected lane issues.
-    constexpr uint32_t idesc = make_idesc_bf16(128, NCI) | (1u << 15) | (1u << 16);   // A and B MN-major
-    const uint64_t a_hi = (uint64_t)(((uint32_t)p.P & 0x3FFF) | (1u << 14)) << 32;    // SBO = P * 16 B, descriptor version 1
-    const uint64_t b_hi = (uint64_t)(((uint32_t)act_pix & 0x3FFF) | (1u << 14)) << 32;
-    constexpr uint32_t lbo = (128u >> 4) << 16;
-    const int dw0 = p.row_dw[row][0] + 1, dw1 = p.row_dw[row][1] + 1, dw2 = p.row_dw[row][2] + 1;   // + halo
+  } else {
+    // consumer warpgroup cw: output channels [64 cw, 64 cw + 64) of the co tile.  Accumulator fragment of tap t: warp wq,
+    // lane l holds co 16 wq + l/4 (+8) and ci 8j + 2 (l % 4) (+1) in acc[t][4j + {0, 1}] (co + 8: acc[t][4j + {2, 3}]).
+    const int cw = warp >> 2, wq = warp & 3;
+    float acc[3][NCI / 2];
+#pragma unroll
+    for (int t = 0; t < 3; ++t)
+#pragma unroll
+      for (int i = 0; i < NCI / 2; ++i) acc[t][i] = 0.f;
+    const uint32_t a_sbo = (uint32_t)p.P * 16u, b_sbo = (uint32_t)act_pix * 16u;
+    const uint32_t dw0 = (uint32_t)(p.row_dw[row][0] + 1) * 16u, dw1 = (uint32_t)(p.row_dw[row][1] + 1) * 16u,
+                   dw2 = (uint32_t)(p.row_dw[row][2] + 1) * 16u;   // + halo
     int stage = 0;
     uint32_t phase = 0;
-    uint32_t first = 1;
     for (int b = blockIdx.x; b < total_blocks; b += gridDim.x) {
-      mbar_wait_warp(bar_full + 8 * stage, phase);
-      tc_fence_after();
-      const uint32_t a16 = (smem_base + stage * stage_bytes) >> 4;
-      const uint32_t b16 = a16 + ((uint32_t)gy_bytes >> 4);
+      mbar_wait(bar_full + 8 * stage, phase);
+      const uint32_t a0 = smem_base + stage * stage_bytes + (uint32_t)cw * 8u * a_sbo;   // planes 8 cw .. 8 cw + 7 of gY
+      const uint32_t b0 = smem_base + stage * stage_bytes + (uint32_t)gy_bytes;
       const int ksteps = p.P / 16;
-      if (elect_one()) {
-        for (int k = 0; k < ksteps; ++k) {
-          const uint64_t adesc = a_hi | (uint64_t)((a16 + (uint32_t)k * 16u) | lbo);
-          const uint32_t acc = (first && k == 0) ? 0u : 1u;
-          const uint32_t bk = b16 + (uint32_t)k * 16u;
-          const uint64_t bd0 = b_hi | (uint64_t)((bk + (uint32_t)dw0) | lbo);
-          if (ntaps == 1) {
-            umma_bf16(tmem_base, adesc, bd0, idesc, acc);
-          } else {
-            umma_bf16_afill(tmem_base, adesc, bd0, idesc, acc);
-            const uint64_t bd1 = b_hi | (uint64_t)((bk + (uint32_t)dw1) | lbo);
-            if (ntaps == 2) {
-              umma_bf16_alast(tmem_base + NCI, adesc, bd1, idesc, acc);
-            } else {
-              umma_bf16_ause(tmem_base + NCI, adesc, bd1, idesc, acc);
-              const uint64_t bd2 = b_hi | (uint64_t)((bk + (uint32_t)dw2) | lbo);
-              umma_bf16_alast(tmem_base + 2 * NCI, adesc, bd2, idesc, acc);
-            }
-          }
+      wgmma_fence();
+      for (int k = 0; k < ksteps; ++k) {
+        const uint64_t adesc = gmma_desc(a0 + (uint32_t)k * 256u, 128, a_sbo);
+        const uint32_t bk = b0 + (uint32_t)k * 256u;
+        if (NCI == 64) wgmma_m64n64k16<1, 1>(acc[0], adesc, gmma_desc(bk + dw0, 128, b_sbo));
+        else           wgmma_m64n32k16<1, 1>(acc[0], adesc, gmma_desc(bk + dw0, 128, b_sbo));
+        if (ntaps > 1) {
+          if (NCI == 64) wgmma_m64n64k16<1, 1>(acc[1], adesc, gmma_desc(bk + dw1, 128, b_sbo));
+          else           wgmma_m64n32k16<1, 1>(acc[1], adesc, gmma_desc(bk + dw1, 128, b_sbo));
+        }
+        if (ntaps > 2) {
+          if (NCI == 64) wgmma_m64n64k16<1, 1>(acc[2], adesc, gmma_desc(bk + dw2, 128, b_sbo));
+          else           wgmma_m64n32k16<1, 1>(acc[2], adesc, gmma_desc(bk + dw2, 128, b_sbo));
         }
       }
+      wgmma_commit();
+      wgmma_wait<0>();
       __syncwarp();
-      first = 0;
-      umma_commit_elect(bar_empty + 8 * stage);
+      if (lane == 0) mbar_arrive(bar_empty + 8 * stage);
       if (++stage == STAGES) { stage = 0; phase ^= 1; }
     }
-    umma_commit_elect(bar_done);
-  } else {
-    // epilogue: warp w owns TMEM lanes 32 (w % 4) .. +31 = output channels; columns = the CTA's input channels per tap
-    const int q = warp & 3;
     if (blockIdx.x < total_blocks) {
-      mbar_wait(bar_done, 0);
-      tc_fence_after();
-      const int co = ct * 128 + q * 32 + lane;
-      for (int t = 0; t < ntaps; ++t) {
-        const int tapidx = p.row_tapidx[row][t];
-        for (int c0 = 0; c0 < NCI; c0 += 32) {
-          uint32_t r[32];
-          tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(t * NCI + c0), r);
-          tmem_ld_wait();
-          float* dst = p.dw + ((long long)co * p.cin_total + p.ci_off + cj * NCI + c0) * p.ntaps_total + tapidx;
 #pragma unroll
-          for (int e = 0; e < 32; ++e) atomicAdd(dst + (long long)e * p.ntaps_total, __uint_as_float(r[e]));
+      for (int t = 0; t < 3; ++t) {
+        if (t < ntaps) {
+          const int tapidx = p.row_tapidx[row][t];
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int co = ct * 128 + cw * 64 + wq * 16 + 8 * h + (lane >> 2);
+            float* dst = p.dw + ((long long)co * p.cin_total + p.ci_off + cj * NCI + 2 * (lane & 3)) * p.ntaps_total + tapidx;
+#pragma unroll
+            for (int j = 0; j < NCI / 8; ++j)
+#pragma unroll
+              for (int e = 0; e < 2; ++e)
+                atomicAdd(dst + (long long)(8 * j + e) * p.ntaps_total, acc[t][4 * j + 2 * h + e]);
+          }
         }
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem_base, 512);
 }
 
 template <int NCI, int STAGES>
@@ -199,11 +186,11 @@ cudaError_t launch_wgrad_tc(const WgradDesc& d, int num_sms, cudaStream_t s) {
     ++p.row_ntaps[r];
   }
   const int flat = d.H * g.Wp;
-  if (d.cin % 128 == 0) {
-    // 128-wide ci tiles: 192-pixel stages, two of them (2 x 97 KB)
+  if (d.cin % 64 == 0) {
+    // 64-wide ci tiles (3 taps x 32 accumulator registers per ci tile and thread): 192-pixel stages, two of them (2 x 73 KB)
     p.P = flat <= 128 ? 128 : 192;
     p.nblk = (flat + p.P - 1) / p.P;
-    return launch_wg<128, 2>(p, num_sms, s);
+    return launch_wg<64, 2>(p, num_sms, s);
   }
   p.P = flat <= 128 ? 128 : 256;
   p.nblk = (flat + p.P - 1) / p.P;

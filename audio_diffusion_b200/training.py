@@ -1,4 +1,4 @@
-"""Optimizer side of `scripts/train_unet.py`'s training step on the B200 engine (SURVEY §8 row T-step).
+"""Optimizer side of `scripts/train_unet.py`'s training step on the H100 engine (SURVEY §8 row T-step).
 
 `FusedAdamW` has the `torch.optim.AdamW` constructor the reference uses (train_unet.py:166-172) and folds
 `accelerator.clip_grad_norm_(model.parameters(), 1.0)` (:262), the AdamW update (:263) and `EMAModel.step` (:265-266)

@@ -5,7 +5,7 @@ A "step" is one denoising step (per-step noise draw + U-Net forward + fused DDPM
 input: config C2 of BASELINE.json — audio-diffusion-256 architecture (scripts/train_unet.py:115-137), 256x256x1, batch 64
 per GPU, DDPM with 1000 steps per mel-spectrogram.  value = (batch * n_gpus) / (1000 * step time).
 
-    python bench.py --gpus N --steps K --warmup W            # B200 arm (libb200ad.so)
+    python bench.py --gpus N --steps K --warmup W            # GPU arm (libb200ad.so)
     python bench.py --impl reference --gpus N ...            # CPU arm: oracle port of diffusers, host cores
     python bench.py --mode train ...                         # only the train_unet.py iteration (config C5)
 
@@ -46,19 +46,18 @@ VAE_ARCH = dict(   # config/ldm_autoencoder_kl.yaml:18-28 as an AutoencoderKL: 1
 GFLOP_PER_SAMPLE_FWD = 496.415145984   # analytic, oracle.unet_oracle.unet_flops(256, 256); SURVEY §8(d)
 GFLOP_PER_LATENT_FWD = 7.76            # same architecture at 32x32 (SURVEY §8a)
 DDPM_STEPS = 1000
-TRAFFIC_FILE = "traffic_r02.json"      # profiles/: ncu dram bytes per conv_tc launch of this same command (round tag)
 
 
 def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("bf16_tflops_sustained", 1439.1), d.get("hbm_gbs", 6572.5), "measured"
-    return 1400.0, 6650.0, "fallback"
+        return d.get("bf16_tflops_sustained", 989.0), d.get("hbm_gbs", 3350.0), "measured"
+    return 989.0, 3350.0, "fallback (H100 SXM data sheet, dense bf16 / HBM3)"
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     def __init__(self, index: int):
         super().__init__(daemon=True)
@@ -127,9 +126,8 @@ def cpu_step_rate(batch: int, hw: int, steps: int, warmup: int):
 
 
 def _cpu_threads():
-    """Threads of the CPU arm.  The oracle port (torch CPU convolutions) stops scaling early: on the pool's 128-cpu hosts a
-    denoise step at batch 4 takes 4.8 s with 16 or 32 threads, 6.6 s with torch's default 64 and 55 s with 128
-    (profiles/cpu_threads_r02.txt), so the baseline runs on the count that is FASTEST for it, not on the largest."""
+    """Threads of the CPU arm.  The oracle port (torch CPU convolutions) stops scaling early on many-core hosts, so the
+    baseline runs on at most 32 threads rather than on every core."""
     want = max(1, min(32, os.cpu_count() or 1))
     if torch.get_num_threads() != want:
         torch.set_num_threads(want)
@@ -163,7 +161,7 @@ def run_reference(args):
     print(json.dumps(line), flush=True)
 
 
-# ------------------------------------------------------------------------------------------------ helpers (B200 arm)
+# ------------------------------------------------------------------------------------------------ helpers (GPU arm)
 def _sync(dist_on):
     if dist_on:
         import torch.distributed as dist
@@ -208,7 +206,7 @@ def whole_call(pipe, batch, steps_a, steps_b, dev, dist_on, latent_hw=None):
             "h2d_bytes_per_call": noise.numel() * 4, "d2h_bytes_per_call": int(d2h)}
 
 
-# ------------------------------------------------------------------------------------------------ B200 arm
+# ------------------------------------------------------------------------------------------------ GPU arm
 def run_b200(args):
     rank, world, local = dist_env()
     from audio_diffusion_b200 import _lib
@@ -257,6 +255,11 @@ def run_b200(args):
         ms = e0.elapsed_time(e1) / K
         clocks = sampler.stop()
         launches = model.last_launch_count * K
+        if args.dump_outputs and rank == 0:
+            # the denoised batch after the last timed step: what forward_step hands back to its caller
+            import numpy as np
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            np.save(os.path.join(args.dump_outputs, "sample.npy"), x.float().cpu().numpy())
 
         # ---- e2e: AudioDiffusionPipeline.__call__ — pinned host noise in (H2D inside), K denoise steps incl. the per-step
         # noise draw, float->uint8, D2H, PIL, batched Griffin-Lim, audio D2H.  Two step counts separate the per-step cost
@@ -331,18 +334,7 @@ def run_b200(args):
     conv = prof["by_kind"].get(3, [0.0, 0.0, 0])
     step_prof_ms = sum(v[0] for v in prof["by_kind"].values())
     conv_tf = conv[1] / (conv[0] * 1e-3) / 1e12 if conv[0] > 0 else 0.0
-    # DRAM bytes per conv_tc launch: ncu launch list of this same command, committed under profiles/ with the round tag;
-    # valid for the default workload only (batch 64, 256x256), null otherwise
-    traffic, traffic_src = None, None
-    tpath = os.path.join(ROOT, "profiles", TRAFFIC_FILE)
-    if os.path.exists(tpath) and HW == 256 and B == 64:
-        with open(tpath) as f:
-            tj = json.load(f)
-        tk = tj["kernels"].get("conv_tc_kernel")
-        if tk:
-            traffic = tk["dram_read_bytes_per_launch"] + tk["dram_write_bytes_per_launch"]
-            traffic_src = (f"profiles/{TRAFFIC_FILE} (ncu dram__bytes_read.sum + dram__bytes_write.sum, mean over "
-                           f"{tk.get('launches', '?')} launches)")
+    traffic, traffic_src = None, "not measured"
     roof = {"bound": "tensor", "kernel": "conv_tc_kernel", "achieved": conv_tf, "peak": peak_tf, "unit": "TFLOP/s",
             "frac": conv_tf / peak_tf, "peak_source": f"{how} bf16 sustained (MEASURED_PEAKS.json)",
             "traffic": traffic, "traffic_source": traffic_src,
@@ -366,9 +358,9 @@ def run_b200(args):
         "n_gpus": world, "steps": K, "warmup": W, "ms_per_step": ms, "higher_is_better": True, "scaling": "weak",
         "vs_baseline": None, "dtype": "bf16 operands, fp32 accumulate (fp32 master weights, fp64 GroupNorm sums)",
         "data": "synthetic (random-init weights seed 0, noise seed 42)",
-        "config": {"workload": f"audio-diffusion-256 DDPM 1000-step, batch={B} per GPU, {HW}x{HW}x1, {world}xB200",
+        "config": {"workload": f"audio-diffusion-256 DDPM 1000-step, batch={B} per GPU, {HW}x{HW}x1, {world}x{torch.cuda.get_device_name(dev)}",
                    "global_batch": B * world, "parallelism": f"dp{world} (batch sharded, weights broadcast once)",
-                   "l2": "activations per step (>10 GB) far exceed the 126 MB L2; no explicit flush",
+                   "l2": "activations per step (>10 GB) far exceed the 50 MB L2; no explicit flush",
                    "step": "one denoise step = per-step randn + UNet2DModel forward + fused DDPMScheduler.step"},
         "clocks": clocks, "gpu_launches": launches,
         "e2e": {"value": (sustained["value"] if sustained else B * world / e2e_call_s), "unit": "mel-spectrograms/s",
@@ -605,7 +597,7 @@ def format_extras(ex, world, peak_tf, peak_hbm):
                        "exposed_allreduce_ms": max(ex["c5_step_s"] - ex["c5_step_nosync_s"], 0.0) * 1e3,
                        "tflops_per_gpu": tf, "frac_of_peak": tf / peak_tf, "flops_model": "3 x 496.42 GFLOP per sample",
                        "gpu_launches_per_step": int(ex["c5_launches"])}
-    # Mel codec: algorithmic bytes (DESIGN.md §3, Mel codec): encode reads the slice (fp32) and writes the image;
+    # Mel codec: algorithmic bytes: encode reads the slice (fp32) and writes the image;
     # decode per Griffin-Lim iteration reads + writes the complex128 spectrum (1025 x 256 x 16 B) and the fp64 audio twice
     n, L, F, T = 64, 131071, 1025, 256
     enc_bytes = n * (L * 4 + 256 * 256)
@@ -679,7 +671,7 @@ def run_train(args):
             "ms_per_step": ms, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
             "dtype": "bf16 activations and activation gradients, fp32 parameters / parameter gradients / optimizer",
             "data": "synthetic (uint8 images -> [-1,1], random-init weights seed 0)",
-            "config": {"workload": f"train_unet.py iteration, batch={B} per GPU, {HW}x{HW}x1, {world}xB200",
+            "config": {"workload": f"train_unet.py iteration, batch={B} per GPU, {HW}x{HW}x1, {world}x{torch.cuda.get_device_name(dev)}",
                        "global_batch": B * world, "parallelism": f"dp{world} (one all-reduce of the flat gradient buffer per step)"},
             "clocks": clocks, "gpu_launches": (model.last_launch_count + model.last_backward_launch_count + 4) * args.steps,
             "roofline": {"bound": "tensor", "achieved": tf, "peak": peak_tf, "unit": "TFLOP/s",
@@ -703,6 +695,8 @@ def main():
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline and parity_check legs (both run the CPU oracle)")
     ap.add_argument("--no-extras", action="store_true", help="skip the C3/C4/C5/Mel sub-benchmarks and the sustained call")
     ap.add_argument("--dump-ops", default=None, help="write the per-launch profile (kind, ms, flops) to this JSON")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="sample mode: write the batch the last timed step produced to DIR/sample.npy (float32)")
     args = ap.parse_args()
     if os.environ.get("NCCL_DEBUG", "").upper() == "VERSION":
         os.environ["NCCL_DEBUG"] = "WARN"      # keep stdout to the one JSON line (NCCL prints its version banner to stdout)

@@ -1,4 +1,4 @@
-/* libb200ad — C ABI of the B200-native audio-diffusion hot path.
+/* libb200ad — C ABI of the H100-native audio-diffusion hot path.
  *
  * The reference (teticio/audio-diffusion) has no FFI: its boundary is Python duck-typing on the objects that
  * `AudioDiffusionPipeline.__call__` drives (audiodiffusion/pipeline_audio_diffusion.py:71-205) and on
@@ -194,7 +194,7 @@ int b200ad_mse_loss_grad(const float* pred, const float* target, size_t n, float
                          double* scratch, void* stream);
 
 /* ---- Op-level entry points (parity tests call the kernels in isolation) ------------------------------- */
-/* conv2d (KHxKW in {1x1, 3x3}, stride 1 or 2, padding KH/2) on fp32 NCHW tensors through the tcgen05
+/* conv2d (KHxKW in {1x1, 3x3}, stride 1 or 2, padding KH/2) on fp32 NCHW tensors through the wgmma
  * implicit-GEMM kernel; optional residual (fp32 NCHW, cout channels) and per-sample additive vector
  * temb [N][cout]; stats_out (optional) receives [N][cout/4][2] (sum, sumsq). scratch >= b200ad_conv2d_scratch_bytes. */
 size_t b200ad_conv2d_scratch_bytes(int N, int cin, int cout, int H, int W, int K, int stride);
@@ -208,12 +208,12 @@ int b200ad_gn_conv2d(const float* x, const float* gamma, const float* beta, int 
                      void* scratch, size_t scratch_bytes, void* stream);
 /* Data gradient of the stride-1 conv above (what autograd's conv2d backward returns for the input; first piece of the
  * U-Net backward, scripts/train_unet.py:259): gy [N, cout, H, W], w [cout, cin, K, K] -> gx [N, cin, H, W]. Runs on the
- * same tcgen05 kernel with transposed / mirrored weight packing. cin % 128 == 0, cout % 16 == 0;
+ * same wgmma kernel with transposed / mirrored weight packing. cin % 128 == 0, cout % 16 == 0;
  * scratch >= b200ad_conv2d_scratch_bytes(N, cout, cin, H, W, K, 1). */
 int b200ad_conv2d_dgrad(const float* gy, const float* w, float* gx, int N, int cin, int cout, int H, int W, int K,
                         void* scratch, size_t scratch_bytes, void* stream);
 /* Weight gradient of the same conv (autograd's conv2d backward for the weight): gy [N, cout, H, W], a [N, cin, H, W] (the
- * conv's input) -> dw fp32 [cout, cin, K, K] (overwritten). tcgen05 with pixels as the reduction dimension (both operands
+ * conv's input) -> dw fp32 [cout, cin, K, K] (overwritten). wgmma with pixels as the reduction dimension (both operands
  * MN-major); cout % 128 == 0, cin % 32 == 0. */
 size_t b200ad_conv2d_wgrad_scratch_bytes(int N, int cin, int cout, int H, int W);
 int b200ad_conv2d_wgrad(const float* gy, const float* a, float* dw, int N, int cin, int cout, int H, int W, int K,

@@ -1,5 +1,5 @@
-"""Generates tests/golden/* by running the reference's OWN Python files (read from /root/reference, unchanged) in this
-container.  Run from the repo root:  python tests/golden/make_golden.py
+"""Generates tests/golden/* by running the reference's OWN Python files (read unchanged from a checkout of
+teticio/audio-diffusion).  Run from the repo root:  python tests/golden/make_golden.py <reference checkout>
 
  * vae_key_map.json — output of audiodiffusion/utils.py::convert_ldm_vae_checkpoint on an ldm-format checkpoint of the
    config/ldm_autoencoder_kl.yaml shape: [hf key, shape] in the order the reference writes them.  Pins the parameter
@@ -10,6 +10,9 @@ container.  Run from the repo root:  python tests/golden/make_golden.py
    product's own scheduler gives bit-identical images, which the generator asserts) for 6 steps from a given noise tensor
    with a CPU step generator: the uint8 images it returns.
    The GPU pipeline must reproduce them within the stated tolerance (tests/test_gpu_pipeline.py).
+ * dropin_ref.npz — what tests/test_cpu_dropin.py compares the product against: the reference pipeline's images on the
+   import shim, its audio-conditioned / in-painting images, DDIM inversion and slerp, the ldm -> diffusers VAE key mapping
+   of its converter, and its Mel class's slicing bookkeeping (SHA-256 of the audio and of the slices).
 The numerical content is the oracle's (diffusers cannot be imported here); what the fixtures pin is the reference
 files' own logic: key mapping, loop order, noise draws, float->uint8 conversion.
 """
@@ -18,7 +21,7 @@ import os
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-REF = "/root/reference"
+REF = sys.argv[1] if len(sys.argv) > 1 else sys.exit("usage: make_golden.py <reference checkout>")
 sys.path[:0] = [ROOT, os.path.join(ROOT, "audio_diffusion_b200", "compat"), REF, os.path.join(ROOT, "tests")]
 
 import numpy as np  # noqa: E402
@@ -81,6 +84,66 @@ def pipeline_small():
     print("pipeline_ddpm_small.npz", arr.shape, arr.mean())
 
 
+def dropin():
+    import hashlib
+
+    from audiodiffusion.mel import Mel as RefMel
+    from audiodiffusion.pipeline_audio_diffusion import AudioDiffusionPipeline as RefPipe
+    from audiodiffusion.utils import convert_ldm_vae_checkpoint
+    from diffusers import DDIMScheduler, DDPMScheduler
+    from oracle.vae_oracle import VAEConfig, init_weights
+    from PIL import Image
+    from test_cpu_dropin import FakeMel, OracleUNet, ScriptedMel, _hf_to_ldm_vae
+    out = {}
+    for sched in ("ddpm", "ddim"):
+        is_ddim = sched == "ddim"
+        pipe = RefPipe(vqvae=None, unet=OracleUNet(), mel=FakeMel(), scheduler=DDIMScheduler() if is_ddim else DDPMScheduler())
+        pipe.set_progress_bar_config(disable=True)
+        assert pipe.get_default_steps() == (50 if is_ddim else 1000)
+        r = pipe(batch_size=2, steps=4, generator=torch.Generator().manual_seed(42))
+        assert len(r.images) == 2 and r.audios.shape == (2, 1, 15 * 512)
+        out[f"shim_{sched}"] = np.stack([np.asarray(im) for im in r.images])
+        pipe = RefPipe(vqvae=None, unet=OracleUNet(), mel=ScriptedMel(), scheduler=DDIMScheduler() if is_ddim else DDPMScheduler())
+        pipe.set_progress_bar_config(disable=True)
+        images, (sr, audios) = pipe(**mirror_kwargs(is_ddim))
+        assert sr == 22050 and len(audios) == 1
+        out[f"mirror_{sched}"] = np.stack([np.asarray(im) for im in images])
+    rng = np.random.default_rng(9)
+    pil = [Image.fromarray(rng.integers(0, 256, (16, 16), dtype=np.uint8)) for _ in range(2)]
+    pipe = RefPipe(vqvae=None, unet=OracleUNet(), mel=ScriptedMel(), scheduler=DDIMScheduler())
+    pipe.set_progress_bar_config(disable=True)
+    out["encode_ddim"] = pipe.encode(pil, steps=5).numpy()
+    a, b = torch.randn(4, 4, generator=torch.Generator().manual_seed(1)), torch.randn(4, 4, generator=torch.Generator().manual_seed(2))
+    out["slerp"] = RefPipe.slerp(a, b, 0.3).numpy()
+    ldm = _hf_to_ldm_vae(init_weights(VAEConfig(), seed=3))
+    tagged = {k: torch.tensor([float(i)]) for i, k in enumerate(ldm)}        # which ldm tensor lands under which key
+    for k, v in ldm.items():
+        if v.dim() == 4 and v.shape[2:] == (1, 1) and ".attn_1." in k:
+            tagged[k] = tagged[k].reshape(1, 1, 1, 1).expand(v.shape[0], v.shape[1], 1, 1)
+    conv = convert_ldm_vae_checkpoint(dict(tagged), None)
+    out["vae_ldm_keys"] = np.array([list(ldm)[int(v.flatten()[0])] for v in conv.values()])
+    out["vae_hf_keys"] = np.array(list(conv))
+    out["vae_squeezed"] = np.array([v.dim() == 2 for v in conv.values()])
+    mel = []
+    rng = np.random.default_rng(0)
+    for (x_res, y_res, hop) in MEL_CASES:
+        for n in (10, x_res * hop - 1, x_res * hop, 3 * x_res * hop + 17):
+            m = RefMel(x_res=x_res, y_res=y_res, hop_length=hop)
+            m.load_audio(raw_audio=rng.standard_normal(n).astype(np.float32))
+            h = hashlib.sha256(m.audio.tobytes())
+            for i in range(m.get_number_of_slices()):
+                h.update(m.get_audio_slice(i).tobytes())
+            mel.append([m.slice_size, m.n_mels, m.get_sample_rate(), m.get_number_of_slices(), len(m.audio), str(m.audio.dtype),
+                        h.hexdigest()])
+        m.set_resolution(32, 16)
+        mel.append([m.x_res, m.y_res, m.n_mels, m.slice_size])
+    out["mel"] = np.array(json.dumps(mel))
+    np.savez_compressed(os.path.join(ROOT, "tests", "golden", "dropin_ref.npz"), **out)
+    print("dropin_ref.npz", sorted(out))
+
+
 if __name__ == "__main__":
+    from test_cpu_dropin import MEL_CASES, mirror_kwargs
     vae_key_map()
     pipeline_small()
+    dropin()

@@ -1,8 +1,7 @@
-"""CPU tests of the drop-in boundary: the UNCHANGED reference pipeline file runs on top of the import shim
-(`audio_diffusion_b200/compat`) with the product's schedulers / pipeline base, and the N>1 path's host logic
-(weight broadcast + batch sharding) works over gloo with world_size 2.
-
-The reference sources are read from /root/reference when present (this container); on the GPU box the test skips.
+"""CPU tests of the drop-in boundary: the product's pipeline, schedulers, VAE parameter table and Mel bookkeeping against
+what the UNCHANGED reference files computed on top of the import shim (`audio_diffusion_b200/compat`), stored in
+tests/golden/dropin_ref.npz by tests/golden/make_golden.py; and the N>1 path's host logic (weight broadcast + batch
+sharding) over gloo with world_size 2.
 """
 import os
 import subprocess
@@ -13,7 +12,22 @@ import pytest
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference"
+MEL_CASES = [(256, 256, 512), (64, 64, 1024), (96, 32, 256)]
+
+
+def golden():
+    return np.load(os.path.join(ROOT, "tests", "golden", "dropin_ref.npz"))
+
+
+def mirror_kwargs(is_ddim):
+    """Arguments of the audio-conditioned / in-painting call (`raw_audio`, `start_step`, `mask_start_secs`,
+    `mask_end_secs`, pipeline_audio_diffusion.py:133-185); the reference's start_step path is batch-1 only (:150)."""
+    noise = torch.randn(1, 1, 16, 16, generator=torch.Generator().manual_seed(3))
+    kw = dict(batch_size=1, raw_audio=np.zeros(16 * 512 * 2, dtype=np.float32), slice=0, start_step=2, steps=6, noise=noise,
+              step_generator=torch.Generator().manual_seed(4), mask_start_secs=0.05, mask_end_secs=0.05, return_dict=False)
+    if is_ddim:
+        kw["eta"] = 0.5
+    return kw
 
 
 class OracleUNet:
@@ -43,40 +57,24 @@ class FakeMel:
         return np.zeros((self.x_res - 1) * self.hop_length, dtype=np.float32)
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference sources not present (GPU box)")
 @pytest.mark.parametrize("sched", ["ddpm", "ddim"])
 def test_unchanged_reference_pipeline_runs_on_the_shim(sched):
-    code = f"""
-import sys
-sys.path[:0] = [{ROOT!r}, {os.path.join(ROOT, 'audio_diffusion_b200', 'compat')!r}, {REF!r}, {os.path.join(ROOT, 'tests')!r}]
-import torch, numpy as np
-from audiodiffusion.pipeline_audio_diffusion import AudioDiffusionPipeline as RefPipe   # byte-identical reference file
-from diffusers import DDPMScheduler, DDIMScheduler
-from test_cpu_dropin import OracleUNet, FakeMel
-from oracle.schedulers_oracle import OracleDDPM, OracleDDIM
-from oracle.unet_oracle import unet_forward
-is_ddim = {sched!r} == 'ddim'
-unet = OracleUNet()
-pipe = RefPipe(vqvae=None, unet=unet, mel=FakeMel(), scheduler=(DDIMScheduler() if is_ddim else DDPMScheduler()))
-assert pipe.get_default_steps() == (50 if is_ddim else 1000)
-pipe.set_progress_bar_config(disable=True)
-out = pipe(batch_size=2, steps=4, generator=torch.Generator().manual_seed(42))
-assert len(out.images) == 2 and out.images[0].size == (16, 16) and out.audios.shape == (2, 1, 15 * 512)
-# same loop by hand with the oracle schedulers -> identical uint8 images
-g = torch.Generator().manual_seed(42)
-x = torch.randn((2, 1, 16, 16), generator=g)
-o = OracleDDIM() if is_ddim else OracleDDPM()
-o.set_timesteps(4)
-for t in o.timesteps:
-    eps = unet_forward(unet.w, unet.cfg, x, t)
-    x = (o.step(eps, t, x, eta=0, generator=g) if is_ddim else o.step(eps, t, x, generator=g))['prev_sample']
-ref = ((x / 2 + 0.5).clamp(0, 1).permute(0, 2, 3, 1).numpy() * 255).round().astype('uint8')[..., 0]
-got = np.stack([np.asarray(im) for im in out.images])
-assert np.array_equal(got, ref), np.abs(got.astype(int) - ref.astype(int)).max()
-print('ok')
-"""
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=300)
-    assert r.returncode == 0 and "ok" in r.stdout, r.stderr[-2000:]
+    """The reference pipeline file on the shim's schedulers (stored uint8 images) == the same loop by hand with the oracle
+    schedulers and the oracle U-Net."""
+    from oracle.schedulers_oracle import OracleDDIM, OracleDDPM
+    from oracle.unet_oracle import unet_forward
+    is_ddim = sched == "ddim"
+    unet = OracleUNet()
+    g = torch.Generator().manual_seed(42)
+    x = torch.randn((2, 1, 16, 16), generator=g)
+    o = OracleDDIM() if is_ddim else OracleDDPM()
+    o.set_timesteps(4)
+    for t in o.timesteps:
+        eps = unet_forward(unet.w, unet.cfg, x, t)
+        x = (o.step(eps, t, x, eta=0, generator=g) if is_ddim else o.step(eps, t, x, generator=g))["prev_sample"]
+    ref = ((x / 2 + 0.5).clamp(0, 1).permute(0, 2, 3, 1).numpy() * 255).round().astype("uint8")[..., 0]
+    got = golden()[f"shim_{sched}"]
+    assert np.array_equal(got, ref), np.abs(got.astype(int) - ref.astype(int)).max()
 
 
 def _worker(rank, world, port, q):
@@ -89,7 +87,8 @@ def _worker(rank, world, port, q):
     broadcast_parameters(params, src=0)
     full = torch.randn(8, 1, 4, 4, generator=torch.Generator().manual_seed(42))
     mine = shard_noise((8, 1, 4, 4), torch.Generator().manual_seed(42), rank, world, device="cpu")
-    q.put((rank, [p.detach().clone() for p in params], mine, full))
+    # numpy, not tensors: a tensor sent through the queue is fetched from this process, which may have exited by then
+    q.put((rank, [p.detach().numpy().copy() for p in params], mine.numpy(), full.numpy()))
     dist.barrier()
     dist.destroy_process_group()
 
@@ -108,7 +107,8 @@ def test_weight_broadcast_and_noise_sharding_gloo_world2():
     for p in procs:
         p.join(timeout=60)
         assert p.exitcode == 0
-    (r0, p0, m0, full), (r1, p1, m1, _) = res
+    (r0, p0, m0, full), (r1, p1, m1, _) = [(r, [torch.from_numpy(a) for a in p], torch.from_numpy(m), torch.from_numpy(f))
+                                          for r, p, m, f in res]
     assert all(torch.equal(a, b) for a, b in zip(p0, p1))            # weights identical after the broadcast
     assert torch.equal(torch.cat([m0, m1]), full)                    # shards tile the global noise stream
 
@@ -139,36 +139,28 @@ def _hf_to_ldm_vae(w, num_blocks=4):
     return out
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference sources not present (GPU box)")
 def test_reference_vae_converter_feeds_the_b200_autoencoder():
-    """audiodiffusion/utils.py:156-291 (`convert_ldm_vae_checkpoint`, UNCHANGED, imported through the shim) turns an
-    ldm-format checkpoint into exactly the state dict the B200 `AutoencoderKL` loads: the library's parameter table
-    (names and shapes) is pinned against the reference's own converter."""
-    code = f"""
-import sys
-sys.path[:0] = [{ROOT!r}, {os.path.join(ROOT, 'audio_diffusion_b200', 'compat')!r}, {REF!r}, {os.path.join(ROOT, 'tests')!r}]
-import torch
-from audiodiffusion.utils import convert_ldm_vae_checkpoint            # byte-identical reference file
-from diffusers import AutoencoderKL                                     # -> audio_diffusion_b200.vae.AutoencoderKL
-from oracle.vae_oracle import VAEConfig, init_weights
-from test_cpu_dropin import _hf_to_ldm_vae
-w = init_weights(VAEConfig(), seed=3)
-ldm = _hf_to_ldm_vae(w)
-assert any(k.startswith('encoder.down.0.block.0.') for k in ldm) and 'decoder.mid.attn_1.q.weight' in ldm
-assert ldm['decoder.mid.attn_1.q.weight'].dim() == 4
-conv = convert_ldm_vae_checkpoint(dict(ldm), None)
-vae = AutoencoderKL(in_channels=1, out_channels=1, down_block_types=('DownEncoderBlock2D',) * 4,
-                    up_block_types=('UpDecoderBlock2D',) * 4, block_out_channels=(128, 256, 512, 512),
-                    layers_per_block=2, latent_channels=1)
-vae.load_state_dict(conv)                                               # strict: every key must land
-sd = vae.state_dict()
-assert set(sd) == set(w)
-for k in w:
-    assert torch.equal(sd[k], w[k]), k
-print('OK', len(sd))
-"""
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0 and "OK 248" in r.stdout, r.stdout + r.stderr
+    """audiodiffusion/utils.py:156-291 (`convert_ldm_vae_checkpoint`, its stored key mapping) turns an ldm-format
+    checkpoint into exactly the state dict the product's `AutoencoderKL` loads: the library's parameter table (names and
+    shapes) is pinned against the reference's own converter."""
+    from audio_diffusion_b200.vae import AutoencoderKL
+    from oracle.vae_oracle import VAEConfig, init_weights
+    w = init_weights(VAEConfig(), seed=3)
+    ldm = _hf_to_ldm_vae(w)
+    assert any(k.startswith("encoder.down.0.block.0.") for k in ldm) and "decoder.mid.attn_1.q.weight" in ldm
+    assert ldm["decoder.mid.attn_1.q.weight"].dim() == 4
+    z = golden()
+    conv = {}
+    for hf, lk, sq in zip(z["vae_hf_keys"], z["vae_ldm_keys"], z["vae_squeezed"]):
+        conv[str(hf)] = ldm[str(lk)][:, :, 0, 0] if sq and ldm[str(lk)].dim() == 4 else ldm[str(lk)]
+    vae = AutoencoderKL(in_channels=1, out_channels=1, down_block_types=("DownEncoderBlock2D",) * 4,
+                        up_block_types=("UpDecoderBlock2D",) * 4, block_out_channels=(128, 256, 512, 512),
+                        layers_per_block=2, latent_channels=1)
+    vae.load_state_dict(conv)                                               # strict: every key must land
+    sd = vae.state_dict()
+    assert set(sd) == set(w) and len(sd) == 248
+    for k in w:
+        assert torch.equal(sd[k], w[k]), k
 
 
 def test_gradient_allreduce_gloo_world2():
@@ -253,103 +245,75 @@ class ScriptedMel(FakeMel):
         return Image.fromarray(rng.integers(0, 256, (self.y_res, self.x_res), dtype=np.uint8))
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference sources not present (GPU box)")
 @pytest.mark.parametrize("sched", ["ddpm", "ddim"])
 def test_mirrored_pipeline_equals_reference_pipeline_on_cpu(sched):
     """The product's own `AudioDiffusionPipeline.__call__` (audio_diffusion_b200/pipeline.py) against the reference's
-    unchanged file for the audio-conditioned / in-painting path (`raw_audio`, `start_step`, `mask_start_secs`,
-    `mask_end_secs`, pipeline_audio_diffusion.py:133-185): identical uint8 images. Both drive the CPU oracle U-Net (the mirror
-    then takes its unfused branch); only the mirror's float->uint8 CUDA kernel is replaced by the same torch expression."""
-    code = f"""
-import sys
-sys.path[:0] = [{ROOT!r}, {os.path.join(ROOT, 'audio_diffusion_b200', 'compat')!r}, {REF!r}, {os.path.join(ROOT, 'tests')!r}]
-import torch, numpy as np
-from audiodiffusion.pipeline_audio_diffusion import AudioDiffusionPipeline as RefPipe   # byte-identical reference file
-from audio_diffusion_b200.pipeline import AudioDiffusionPipeline as Mirror
-from diffusers import DDPMScheduler, DDIMScheduler
-from test_cpu_dropin import OracleUNet, ScriptedMel
-Mirror.images_to_u8 = staticmethod(lambda x: ((x / 2 + 0.5).clamp(0, 1) * 255).round().to(torch.uint8))
-is_ddim = {sched!r} == 'ddim'
-outs = []
-for cls in (RefPipe, Mirror):
-    pipe = cls(vqvae=None, unet=OracleUNet(), mel=ScriptedMel(), scheduler=(DDIMScheduler() if is_ddim else DDPMScheduler()))
-    pipe.set_progress_bar_config(disable=True)
-    noise = torch.randn(1, 1, 16, 16, generator=torch.Generator().manual_seed(3))   # the reference's start_step path is batch-1 only (:150)
-    kw = dict(batch_size=1, raw_audio=np.zeros(16 * 512 * 2, dtype=np.float32), slice=0, start_step=2, steps=6, noise=noise,
-              step_generator=torch.Generator().manual_seed(4), mask_start_secs=0.05, mask_end_secs=0.05, return_dict=False)
-    if is_ddim:
-        kw['eta'] = 0.5
-    images, (sr, audios) = pipe(**kw)
-    outs.append(np.stack([np.asarray(im) for im in images]))
-    assert sr == 22050 and len(audios) == 1
-assert outs[0].shape == (1, 16, 16) and np.array_equal(outs[0], outs[1]), np.abs(outs[0].astype(int) - outs[1].astype(int)).max()
-if is_ddim:   # DDIM inversion (`encode`, :207-242) and `slerp` (:244-263): same numbers from both files
+    unchanged file for the audio-conditioned / in-painting path: identical uint8 images; for DDIM also inversion (`encode`,
+    :207-242) and `slerp` (:244-263). Both drove the CPU oracle U-Net (the mirror then takes its unfused branch); only the
+    mirror's float->uint8 CUDA kernel is replaced by the same torch expression."""
     from PIL import Image
-    rng = np.random.default_rng(9)
-    pil = [Image.fromarray(rng.integers(0, 256, (16, 16), dtype=np.uint8)) for _ in range(2)]
-    encs = []
-    for cls in (RefPipe, Mirror):
-        pipe = cls(vqvae=None, unet=OracleUNet(), mel=ScriptedMel(), scheduler=DDIMScheduler())
+
+    from audio_diffusion_b200.pipeline import AudioDiffusionPipeline as Mirror
+    from audio_diffusion_b200.schedulers import DDIMScheduler, DDPMScheduler
+    is_ddim = sched == "ddim"
+    z = golden()
+    u8 = Mirror.__dict__["images_to_u8"]
+    Mirror.images_to_u8 = staticmethod(lambda x: ((x / 2 + 0.5).clamp(0, 1) * 255).round().to(torch.uint8))
+    try:
+        pipe = Mirror(vqvae=None, unet=OracleUNet(), mel=ScriptedMel(), scheduler=(DDIMScheduler() if is_ddim else DDPMScheduler()))
         pipe.set_progress_bar_config(disable=True)
-        encs.append(pipe.encode(pil, steps=5))
-    assert encs[0].shape == (2, 1, 16, 16) and torch.equal(encs[0], encs[1])
-    a, b = torch.randn(4, 4, generator=torch.Generator().manual_seed(1)), torch.randn(4, 4, generator=torch.Generator().manual_seed(2))
-    assert torch.equal(RefPipe.slerp(a, b, 0.3), Mirror.slerp(a, b, 0.3))
-print('ok')
-"""
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=300)
-    assert r.returncode == 0 and "ok" in r.stdout, (r.stdout + r.stderr)[-3000:]
+        images, (sr, audios) = pipe(**mirror_kwargs(is_ddim))
+        got = np.stack([np.asarray(im) for im in images])
+        assert sr == 22050 and len(audios) == 1
+        ref = z[f"mirror_{sched}"]
+        assert ref.shape == (1, 16, 16) and np.array_equal(got, ref), np.abs(got.astype(int) - ref.astype(int)).max()
+        if is_ddim:
+            rng = np.random.default_rng(9)
+            pil = [Image.fromarray(rng.integers(0, 256, (16, 16), dtype=np.uint8)) for _ in range(2)]
+            pipe = Mirror(vqvae=None, unet=OracleUNet(), mel=ScriptedMel(), scheduler=DDIMScheduler())
+            pipe.set_progress_bar_config(disable=True)
+            enc = pipe.encode(pil, steps=5)
+            assert enc.shape == (2, 1, 16, 16) and torch.equal(enc, torch.from_numpy(z["encode_ddim"]))
+            a = torch.randn(4, 4, generator=torch.Generator().manual_seed(1))
+            b = torch.randn(4, 4, generator=torch.Generator().manual_seed(2))
+            assert torch.equal(Mirror.slerp(a, b, 0.3), torch.from_numpy(z["slerp"]))
+    finally:
+        Mirror.images_to_u8 = u8
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference sources not present (GPU box)")
 def test_mel_host_logic_equals_reference_mel():
     """Slicing / padding / resolution bookkeeping of the engine's `Mel` against the reference's own `audiodiffusion/mel.py`
-    class (imported unchanged through the shim; its librosa-backed transforms are not called): mel.py:80-133."""
+    class (stored sizes and SHA-256 of the audio and its slices; its librosa-backed transforms are not called): mel.py:80-133."""
+    import hashlib
+    import json
+
+    from audio_diffusion_b200.mel import Mel
+    ref = json.loads(str(golden()["mel"]))
+    got = []
+    rng = np.random.default_rng(0)
+    for (x_res, y_res, hop) in MEL_CASES:
+        for n in (10, x_res * hop - 1, x_res * hop, 3 * x_res * hop + 17):
+            m = Mel(x_res=x_res, y_res=y_res, hop_length=hop)
+            m.load_audio(raw_audio=rng.standard_normal(n).astype(np.float32))
+            h = hashlib.sha256(m.audio.tobytes())
+            for i in range(m.get_number_of_slices()):
+                h.update(m.get_audio_slice(i).tobytes())
+            got.append([m.slice_size, m.n_mels, m.get_sample_rate(), m.get_number_of_slices(), len(m.audio), str(m.audio.dtype),
+                        h.hexdigest()])
+        m.set_resolution(32, 16)
+        got.append([m.x_res, m.y_res, m.n_mels, m.slice_size])
+    assert got == ref
+
+
+def test_conditional_unet_surface():
+    """SURVEY §8 f3 boundary: `diffusers.UNet2DConditionModel` of the import shim resolves to the engine's class with
+    exactly the diffusers state-dict keys / shapes of the architecture scripts/train_unet.py:139-159 builds."""
     code = f"""
 import sys
-sys.path[:0] = [{ROOT!r}, {os.path.join(ROOT, 'audio_diffusion_b200', 'compat')!r}, {REF!r}]
-import numpy as np
-from audiodiffusion.mel import Mel as RefMel          # byte-identical reference file
-from audio_diffusion_b200.mel import Mel
-rng = np.random.default_rng(0)
-for (x_res, y_res, hop) in [(256, 256, 512), (64, 64, 1024), (96, 32, 256)]:
-    for n in [10, x_res * hop - 1, x_res * hop, 3 * x_res * hop + 17]:
-        a, b = RefMel(x_res=x_res, y_res=y_res, hop_length=hop), Mel(x_res=x_res, y_res=y_res, hop_length=hop)
-        audio = rng.standard_normal(n).astype(np.float32)
-        a.load_audio(raw_audio=audio.copy()); b.load_audio(raw_audio=audio.copy())
-        assert a.slice_size == b.slice_size and a.n_mels == b.n_mels and a.get_sample_rate() == b.get_sample_rate()
-        assert a.get_number_of_slices() == b.get_number_of_slices(), (x_res, n)
-        assert len(a.audio) == len(b.audio) and a.audio.dtype == b.audio.dtype and np.array_equal(a.audio, b.audio)
-        for s in range(a.get_number_of_slices()):
-            assert np.array_equal(a.get_audio_slice(s), b.get_audio_slice(s))
-    a.set_resolution(32, 16); b.set_resolution(32, 16)
-    assert (a.x_res, a.y_res, a.n_mels, a.slice_size) == (b.x_res, b.y_res, b.n_mels, b.slice_size)
-print('ok')
-"""
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=300)
-    assert r.returncode == 0 and "ok" in r.stdout, (r.stdout + r.stderr)[-3000:]
-
-
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference sources not present (GPU box)")
-def test_reference_audio_encoder_and_conditional_unet_surface():
-    """SURVEY §8 f3 boundary: the reference's own audiodiffusion/audio_encoder.py runs on the shim's ModelMixin / Mel (a
-    small CNN that is not part of the denoising loop), and `diffusers.UNet2DConditionModel` resolves to the engine's class
-    with exactly the diffusers state-dict keys / shapes of the architecture scripts/train_unet.py:139-159 builds."""
-    code = f"""
-import sys, tempfile
-sys.path[:0] = [{ROOT!r}, {os.path.join(ROOT, 'audio_diffusion_b200', 'compat')!r}, {REF!r}]
-import torch
-from audiodiffusion.audio_encoder import AudioEncoder          # byte-identical reference file
-enc = AudioEncoder().eval()
-y = enc(torch.rand(2, 1, 96, 216))
-assert y.shape == (2, 100)
-d = tempfile.mkdtemp()
-enc.save_pretrained(d)
-again = AudioEncoder.from_pretrained(d).eval()
-assert torch.equal(again(torch.ones(1, 1, 96, 216)), enc(torch.ones(1, 1, 96, 216)))
+sys.path[:0] = [{ROOT!r}, {os.path.join(ROOT, 'audio_diffusion_b200', 'compat')!r}]
 from diffusers import UNet2DConditionModel
-from audiodiffusion.pipeline_audio_diffusion import UNet2DConditionModel as seen_by_pipeline
-assert seen_by_pipeline is UNet2DConditionModel
+from audio_diffusion_b200.unet_cond import UNet2DConditionModel as engine_cls
+assert UNet2DConditionModel is engine_cls
 u = UNet2DConditionModel(sample_size=(32, 32), in_channels=1, out_channels=1, layers_per_block=2,
                          block_out_channels=(128, 256, 512, 512),
                          down_block_types=("CrossAttnDownBlock2D",) * 3 + ("DownBlock2D",),

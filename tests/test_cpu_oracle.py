@@ -245,7 +245,7 @@ def test_unet_handle_param_table_matches_oracle_without_gpu():
     assert all(tuple(sd[k].shape) == ref[k] for k in ref)
     from audio_diffusion_b200 import _lib
     need = _lib.lib().b200ad_unet_workspace_bytes(m._h, 64, 256, 256)
-    assert 5e9 < need < 60e9  # activations for config C2 fit a 180 GB B200 many times over
+    assert 5e9 < need < 60e9  # activations for config C2 fit an 80 GB H100
 
 
 def test_product_fails_loudly_without_cuda():

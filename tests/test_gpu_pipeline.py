@@ -220,7 +220,7 @@ def test_latent_pipeline_audio_conditioning(cuda):
 
 def test_golden_reference_driven_images(cuda):
     """tests/golden/pipeline_ddpm_small.npz: uint8 images returned by the REFERENCE's own pipeline file (driving the fp32
-    oracle U-Net, tests/golden/make_golden.py). The B200 pipeline on the same noise, weights and CPU step generator reproduces
+    oracle U-Net, tests/golden/make_golden.py). The product pipeline on the same noise, weights and CPU step generator reproduces
     them to the stated trajectory tolerance (>= 90 % of pixels within 2 grey levels)."""
     import os
     from audio_diffusion_b200.mel import Mel

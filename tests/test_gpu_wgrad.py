@@ -1,4 +1,4 @@
-"""tcgen05 weight-gradient kernel (b200ad_conv2d_wgrad) against torch autograd (bf16-rounded operands, fp32 reference).
+"""wgmma weight-gradient kernel (b200ad_conv2d_wgrad) against torch autograd (bf16-rounded operands, fp32 reference).
 Tolerance: products of bf16 values accumulated in fp32 in a different order: 2e-3 of max|ref|."""
 import pytest
 import torch
