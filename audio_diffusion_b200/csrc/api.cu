@@ -3,9 +3,8 @@
 #include <cstring>
 
 #include "../../include/b200ad.h"
-#include "conv_tc.cuh"
 #include "bwd_kernels.cuh"
-#include "kernels.cuh"
+#include "taps.cuh"
 
 namespace b200ad {
 int set_err(const char* fmt, ...);
@@ -76,19 +75,11 @@ static int conv2d_impl(const float* x, const float* w, const float* bias, const 
   p.cout = cout;
   p.out = op; p.bias = bias; p.temb = temb; p.temb_stride = cout;
   p.stats = stats_out ? stp : nullptr;
-  const long long img_stride = (long long)(cin / 8) * go.PL * 8;
-  if (stride == -2) {
-    // segments are built per output parity below
-  } else if (stride == 1) {
-    PackTaps t{};
-    t.ntaps = K * K;
-    for (int k = 0; k < K * K; ++k) { t.kh[k] = k / K; t.kw[k] = k % K; }
-    CK(launch_pack_weights(w, cout, cin, K, K, 0, cin / 16, t, wp, st));
+  if (stride == 1) {
+    const TapSet t = taps_conv(K);
+    CK(launch_pack_weights(w, cout, cin, K, K, 0, cin / 16, t.pack, wp, st));
     ConvSeg& s = p.seg[0];
-    s.src = xp; s.wpack = wp; s.img_stride = img_stride; s.ksteps = cin / 16; s.ntaps = K * K;
-    s.ht = s.hb = s.hl = s.hr = (K == 3) ? 1 : 0;
-    for (int k = 0; k < K * K; ++k) { s.dh[k] = (signed char)(k / K - K / 2); s.dw[k] = (signed char)(k % K - K / 2); }
-    s.ss = nullptr; s.ss_stride = 0; s.silu = 0;
+    set_seg(s, xp, cin / 8, cin, H, W, wp, t);
     p.nseg = 1;
     if (gn_gamma) {  // GroupNorm(+SiLU) of x fused into the conv's A staging
       stat_t* ist = (stat_t*)(sb + L.instats);
@@ -103,29 +94,20 @@ static int conv2d_impl(const float* x, const float* w, const float* bias, const 
     if (residual) {  // residual add = 1-tap identity-weight segment over the raw residual tensor
       __nv_bfloat16* ident = (__nv_bfloat16*)(sb + L.ident);
       CK(launch_pack_identity(cout, ident, st));
-      ConvSeg& r = p.seg[1];
-      r.src = rp; r.wpack = ident; r.img_stride = (long long)(cout / 8) * go.PL * 8; r.ksteps = cout / 16; r.ntaps = 1;
-      r.ht = r.hb = r.hl = r.hr = 0; r.dh[0] = 0; r.dw[0] = 0; r.ss = nullptr; r.ss_stride = 0; r.silu = 0;
+      set_seg(p.seg[1], rp, cout / 8, cout, Ho, Wo, ident, taps_conv(1));
       p.nseg = 2;
     }
-  } else {
+  } else if (stride == 2) {
     CK(launch_parity_split(xp, par, N, cin, H, W, st));
     const size_t tsz = (size_t)N * (cin / 8) * go.PL * 8;
     size_t woff = 0;
     for (int a = 0; a < 2; ++a)
       for (int b = 0; b < 2; ++b) {
-        PackTaps t{};
-        for (int kh = 0; kh < 3; ++kh)
-          for (int kw = 0; kw < 3; ++kw)
-            if (((kh == 1) ? 0 : 1) == a && ((kw == 1) ? 0 : 1) == b) { t.kh[t.ntaps] = kh; t.kw[t.ntaps] = kw; ++t.ntaps; }
+        const TapSet t = taps_parity(a, b);
         __nv_bfloat16* wseg = wp + woff / 2;
-        CK(launch_pack_weights(w, cout, cin, 3, 3, 0, cin / 16, t, wseg, st));
-        woff += (size_t)(cout / 128) * (cin / 16) * t.ntaps * CONV_B_TAP;
-        ConvSeg& s = p.seg[a * 2 + b];
-        s.src = par + (size_t)(a * 2 + b) * tsz; s.wpack = wseg; s.img_stride = img_stride; s.ksteps = cin / 16;
-        s.ntaps = t.ntaps;
-        s.ht = a; s.hb = 0; s.hl = b; s.hr = 0; s.ss = nullptr; s.ss_stride = 0; s.silu = 0;
-        for (int k = 0; k < t.ntaps; ++k) { s.dh[k] = (t.kh[k] == 0) ? -1 : 0; s.dw[k] = (t.kw[k] == 0) ? -1 : 0; }
+        CK(launch_pack_weights(w, cout, cin, 3, 3, 0, cin / 16, t.pack, wseg, st));
+        woff += (size_t)(cout / 128) * (cin / 16) * t.pack.ntaps * CONV_B_TAP;
+        set_seg(p.seg[a * 2 + b], par + (size_t)(a * 2 + b) * tsz, cin / 8, cin, Ho, Wo, wseg, t);
       }
     p.nseg = 4;
   }
@@ -140,20 +122,11 @@ static int conv2d_impl(const float* x, const float* w, const float* bias, const 
     size_t woff = 0;
     for (int pa = 0; pa < 2; ++pa)
       for (int pb = 0; pb < 2; ++pb) {
-        const UpTaps ut = taps_up2(pa, pb);
+        const TapSet t = taps_up2(pa, pb);
         __nv_bfloat16* wseg = wp + woff / 2;
-        CK(launch_pack_weights(w, cout, cin, 3, 3, 0, cin / 16, ut.pack, wseg, st));
+        CK(launch_pack_weights(w, cout, cin, 3, 3, 0, cin / 16, t.pack, wseg, st));
         woff += (size_t)(cout / 128) * (cin / 16) * 4 * CONV_B_TAP;
-        ConvSeg& s = p.seg[0];
-        s.src = xp; s.wpack = wseg; s.img_stride = (long long)(cin / 8) * gi.PL * 8; s.ksteps = cin / 16; s.ntaps = 4;
-        s.ht = s.hb = s.hl = s.hr = 0; s.ss = nullptr; s.ss_stride = 0; s.silu = 0;
-        for (int t = 0; t < 4; ++t) {
-          s.dh[t] = ut.dh[t]; s.dw[t] = ut.dw[t];
-          if (ut.dh[t] < 0) s.ht = 1;
-          if (ut.dh[t] > 0) s.hb = 1;
-          if (ut.dw[t] < 0) s.hl = 1;
-          if (ut.dw[t] > 0) s.hr = 1;
-        }
+        set_seg(p.seg[0], xp, cin / 8, cin, H, W, wseg, t);
         p.oy = pa; p.ox = pb;
         CK(launch_conv_tc(p, sms, st));
       }
@@ -189,20 +162,13 @@ extern "C" int b200ad_conv2d_dgrad(const float* gy, const float* w, float* gx, i
   __nv_bfloat16* gxp = (__nv_bfloat16*)(sb + L.out);
   __nv_bfloat16* wp = (__nv_bfloat16*)(sb + L.wpack);
   CK(launch_nchw_to_pf8(gy, gyp, N, cout, H, W, st));
-  PackTaps t{};
-  t.ntaps = K * K;
-  t.transpose = 1;
-  for (int k = 0; k < K * K; ++k) { t.kh[k] = K - 1 - k / K; t.kw[k] = K - 1 - k % K; }   // mirrored taps
-  CK(launch_pack_weights(w, cin, cin, K, K, 0, cout / 16, t, wp, st, cin));
+  const TapSet t = taps_mirrored(K);
+  CK(launch_pack_weights(w, cin, cin, K, K, 0, cout / 16, t.pack, wp, st, cin));
   ConvParams p{};
   p.N = N; p.H = H; p.W = W; p.Wp = g.Wp; p.lead = g.lead; p.PL = g.PL;
   p.cout = cin;
   p.out = gxp; p.bias = nullptr; p.temb = nullptr; p.temb_stride = 0; p.stats = nullptr;
-  ConvSeg& s = p.seg[0];
-  s.src = gyp; s.wpack = wp; s.img_stride = (long long)(cout / 8) * g.PL * 8; s.ksteps = cout / 16; s.ntaps = K * K;
-  s.ht = s.hb = s.hl = s.hr = (K == 3) ? 1 : 0;
-  for (int k = 0; k < K * K; ++k) { s.dh[k] = (signed char)(k / K - K / 2); s.dw[k] = (signed char)(k % K - K / 2); }
-  s.ss = nullptr; s.ss_stride = 0; s.silu = 0;
+  set_seg(p.seg[0], gyp, cout / 8, cout, H, W, wp, t);
   p.nseg = 1;
   int dev = 0, sms = 132;
   CK(cudaGetDevice(&dev));
@@ -234,8 +200,9 @@ extern "C" int b200ad_conv2d_wgrad(const float* gy, const float* a, float* dw, i
   WgradDesc d{};
   d.gy = gyp; d.act = ap; d.dw = dw; d.N = N; d.H = H; d.W = W; d.cout = cout; d.cin = cin;
   d.gy_img_planes = cout / 8; d.act_img_planes = cin / 8; d.cin_total = cin; d.ci_off = 0; d.ntaps_total = K * K;
+  const TapSet t = taps_conv(K);
   d.ntaps = K * K;
-  for (int t = 0; t < K * K; ++t) { d.dh[t] = t / K - K / 2; d.dw_[t] = t % K - K / 2; d.tapidx[t] = t; }
+  for (int k = 0; k < K * K; ++k) { d.dh[k] = t.dh[k]; d.dw_[k] = t.dw[k]; d.tapidx[k] = t.wtap[k]; }
   CK(launch_wgrad_tc(d, sms, st));
   return 0;
 }

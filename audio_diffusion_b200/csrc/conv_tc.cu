@@ -534,8 +534,16 @@ cudaError_t launch_conv_tc(const ConvParams& p_in, int num_sms, cudaStream_t str
   if (p_in.nseg < 1 || p_in.nseg > CONV_MAXSEG) return cudaErrorInvalidValue;
   ConvParams p = p_in;
   p.dbg = dbg;
-  for (int s = 0; s < p.nseg; ++s)
-    if (p.seg[s].wtile_stride == 0) p.seg[s].wtile_stride = (long long)p.seg[s].ksteps * p.seg[s].ntaps * (CONV_B_TAP / 2);
+  for (int s = 0; s < p.nseg; ++s) {
+    ConvSeg& sg = p.seg[s];
+    if (sg.ntaps > CONV_MAXTAPS) return cudaErrorInvalidValue;
+    if (sg.wtile_stride == 0) sg.wtile_stride = (long long)sg.ksteps * sg.ntaps * (CONV_B_TAP / 2);
+    sg.ht = sg.hb = sg.hl = sg.hr = 0;
+    for (int t = 0; t < sg.ntaps; ++t) {
+      sg.ht |= sg.dh[t] < 0; sg.hb |= sg.dh[t] > 0;
+      sg.hl |= sg.dw[t] < 0; sg.hr |= sg.dw[t] > 0;
+    }
+  }
   // Experiment (B200AD_CONV_DBG & 128, off by default): move trailing 1-tap segments (shortcut / residual) in front of the
   // main segment's last k-step so that a many-tap k-step closes the K loop.  The 1-tap k-steps are load-bound (a 16 KB
   // window per k-step of MMAs) and would stall the ring in the middle of the item instead of next to the epilogue.

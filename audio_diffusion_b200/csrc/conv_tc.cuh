@@ -33,7 +33,7 @@ struct ConvSeg {
   long long wtile_stride;      // elements between cout tiles of wpack (0: ksteps * ntaps * 2048; set by the launcher)
   int ksteps;                  // input channels / 16
   int ntaps;
-  int ht, hb, hl, hr;          // halo rows above / below, pixels left / right
+  int ht, hb, hl, hr;          // halo rows above / below, pixels left / right, filled in by launch_conv_tc from dh / dw
   signed char dh[CONV_MAXTAPS];
   signed char dw[CONV_MAXTAPS];
   int aoff[CONV_MAXTAPS];      // (dh + ht) * Wp + dw + hl, filled in by launch_conv_tc: window offset of each tap

@@ -590,22 +590,6 @@ cudaError_t launch_conv_out(const ConvOutParams& p, cudaStream_t s) {
 }
 
 // ------------------------------------------------------------------------------------ resampling
-__global__ void upsample2x_kernel(const __nv_bfloat16* __restrict__ src, __nv_bfloat16* __restrict__ dst, int N, int C,
-                                  int H, int W) {
-  const Geom gi = make_geom(N, H, W), go = make_geom(N, 2 * H, 2 * W);
-  const int pidx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (pidx >= 4 * H * W) return;
-  const int ho = pidx / (2 * W), wo = pidx - ho * 2 * W;
-  const long long plane = (long long)blockIdx.z * (C >> 3) + blockIdx.y;
-  const uint4 v = *reinterpret_cast<const uint4*>(src + (plane * gi.PL + gi.lead + (ho >> 1) * gi.Wp + (wo >> 1)) * 8);
-  *reinterpret_cast<uint4*>(dst + (plane * go.PL + go.lead + ho * go.Wp + wo) * 8) = v;
-}
-cudaError_t launch_upsample2x(const __nv_bfloat16* src, __nv_bfloat16* dst, int N, int C, int H, int W, cudaStream_t s) {
-  dim3 grid((4 * H * W + 255) / 256, C >> 3, N);
-  upsample2x_kernel<<<grid, 256, 0, s>>>(src, dst, N, C, H, W);
-  return cudaGetLastError();
-}
-
 // dst4: four PF8 tensors (N, C, H/2, W/2) back to back, index a*2+b holds x[2h'+a, 2w'+b]
 __global__ void parity_split_kernel(const __nv_bfloat16* __restrict__ src, __nv_bfloat16* __restrict__ dst4, int N,
                                     int C, int H, int W) {

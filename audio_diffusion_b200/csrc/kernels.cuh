@@ -42,30 +42,6 @@ struct PackBatch {
 };
 cudaError_t launch_pack_batch(PackBatch& pb, const std::vector<PackItem>& items, cudaStream_t s);
 
-// nearest-2x upsample + 3x3 conv, output parity (a, b): a 2x2 conv on the low-res input whose taps are sums of the 3x3
-// taps that read the same low-res pixel. Row taps: a = 0 -> dh = -1 (kh 0), dh = 0 (kh 1,2); a = 1 -> dh = 0 (kh 0,1), +1 (kh 2).
-struct UpTaps { PackTaps pack; signed char dh[4], dw[4]; };
-inline UpTaps taps_up2(int a, int b) {
-  UpTaps u{};
-  u.pack.fold = 1;
-  u.pack.ntaps = 4;
-  for (int ri = 0; ri < 2; ++ri)
-    for (int ci = 0; ci < 2; ++ci) {
-      const int t = ri * 2 + ci;
-      const int dh = (a == 0) ? ri - 1 : ri, dw = (b == 0) ? ci - 1 : ci;
-      u.dh[t] = (signed char)dh; u.dw[t] = (signed char)dw;
-      unsigned mask = 0;
-      for (int kh = 0; kh < 3; ++kh)
-        for (int kw = 0; kw < 3; ++kw) {
-          const int rdh = (a == 0) ? (kh == 0 ? -1 : 0) : (kh == 2 ? 1 : 0);
-          const int rdw = (b == 0) ? (kw == 0 ? -1 : 0) : (kw == 2 ? 1 : 0);
-          if (rdh == dh && rdw == dw) mask |= 1u << (kh * 3 + kw);
-        }
-      u.pack.fold_mask[t] = mask;
-    }
-  return u;
-}
-
 // GroupNorm (+ optional SiLU) apply over the channel concatenation of up to two raw PF8 sources.
 // stats: running (sum, sumsq) per (n, 4-channel quad) written by the producers' epilogues.
 struct GnApplyParams {
@@ -116,8 +92,7 @@ struct ConvOutParams {
 };
 cudaError_t launch_conv_out(const ConvOutParams& p, cudaStream_t s);
 
-// nearest 2x upsample PF8 (H, W) -> PF8 (2H, 2W); stride-2 parity split PF8 (H, W) -> 4 x PF8 (H/2, W/2)
-cudaError_t launch_upsample2x(const __nv_bfloat16* src, __nv_bfloat16* dst, int N, int C, int H, int W, cudaStream_t s);
+// stride-2 parity split PF8 (H, W) -> 4 x PF8 (H/2, W/2)
 cudaError_t launch_parity_split(const __nv_bfloat16* src, __nv_bfloat16* dst4, int N, int C, int H, int W, cudaStream_t s);
 
 cudaError_t launch_quad_stats(const __nv_bfloat16* src, stat_t* stats, int N, int C, int H, int W, cudaStream_t s);

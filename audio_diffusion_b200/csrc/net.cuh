@@ -1,5 +1,6 @@
-// Shared host-side machinery of the model handles: parameter table, packed-weight arena, activation workspace and the
-// launch-plan builder (ResnetBlock2D / attention with the GroupNorm apply fused into the consuming conv).
+// Shared host-side machinery of the model handles.  An architecture is one list of blocks (Block); the parameter table,
+// the packed-weight arena layout and the launch plan (ResnetBlock2D / attention with the GroupNorm apply fused into the
+// consuming conv) are each one loop over it, and one executor runs the plans of both models.
 #pragma once
 #include <cstdarg>
 #include <cstdio>
@@ -10,8 +11,7 @@
 #include <vector>
 
 #include "../../include/b200ad.h"
-#include "conv_tc.cuh"
-#include "kernels.cuh"
+#include "taps.cuh"
 
 namespace b200ad {
 
@@ -33,11 +33,12 @@ struct Act {  // PF8 activation tensor
   stat_t* stats = nullptr;
 };
 
-enum OpKind { OP_TEMB, OP_CONV_IN, OP_GN, OP_CONV, OP_UPSAMPLE, OP_PARITY, OP_ATTN, OP_CONV_OUT,
-              OP_ATTN1 /* single head of dim C */, OP_VAE_SAMPLE, OP_MIX1X1,
-              OP_LN /* LayerNorm over channels */, OP_GEGLU, OP_MHA /* multi-head attention, head_dim 16/32/64 */,
-              OP_XVEC /* cross-attention against a one-token encoding = per-sample vector */,
-              OP_GNAPPLY /* materialised GroupNorm (attention input: the q/k/v projection has 12 cout tiles) */ };
+// The values are reported per launch by b200ad_unet_profile_step (4 was the unfolded nearest-2x upsample).
+enum OpKind { OP_TEMB = 0, OP_CONV_IN = 1, OP_GN = 2, OP_CONV = 3, OP_PARITY = 5, OP_ATTN = 6, OP_CONV_OUT = 7,
+              OP_ATTN1 = 8 /* single head of dim C */, OP_VAE_SAMPLE = 9, OP_MIX1X1 = 10,
+              OP_LN = 11 /* LayerNorm over channels */, OP_GEGLU = 12, OP_MHA = 13 /* multi-head attention, head_dim 16/32/64 */,
+              OP_XVEC = 14 /* cross-attention against a one-token encoding = per-sample vector */,
+              OP_GNAPPLY = 15 /* materialised GroupNorm (attention input: the q/k/v projection has 12 cout tiles) */ };
 struct Op {
   OpKind kind;
   ConvParams conv;
@@ -48,12 +49,12 @@ struct Op {
   int C = 0, H = 0, W = 0;
   ConvOutParams co;
   float2* ss = nullptr;  // OP_GN: output of gn_finalize
-  float* f0 = nullptr;   // OP_ATTN1: score scratch; OP_MIX1X1: fp32 destination
-  const float* fw = nullptr;  // OP_CONV_IN / OP_VAE_SAMPLE / OP_MIX1X1: fp32 weight and bias
+  float* f0 = nullptr;   // OP_ATTN1: score scratch; OP_MIX1X1: fp32 destination; OP_CONV_IN: fp32 source (null: the caller's)
+  const float* fw = nullptr;  // OP_CONV_IN / OP_VAE_SAMPLE / OP_MIX1X1 / OP_LN: fp32 weight and bias
   const float* fb = nullptr;
   const float* fc = nullptr;  // OP_XVEC: to_out bias
   float* f1 = nullptr;        // OP_XVEC: destination [N][C]
-  int cin = 0;
+  int cin = 0;                // OP_CONV_IN / OP_XVEC: input channels; OP_MHA: heads; OP_VAE_SAMPLE: latent channels
   float eps = 0.f;            // OP_LN
 };
 
@@ -67,6 +68,12 @@ struct Bump {  // two-pass bump allocator: base == nullptr computes sizes only
     return r;
   }
 };
+static size_t take_off(Bump& b, size_t bytes) {  // size-only pass: returns the aligned offset
+  b.take(0);
+  const size_t o = (b.off + 255) & ~(size_t)255;
+  b.take(bytes);
+  return o;
+}
 
 struct PackJob {  // one K-segment's packed weights
   int w_param;      // index of the fp32 weight in the table
@@ -74,6 +81,73 @@ struct PackJob {  // one K-segment's packed weights
   PackTaps taps;
   size_t off;       // byte offset in the packed arena
   int cout_real = -1;  // < cout when the output channels are zero-padded up to the 128-channel tile
+};
+
+struct FusedBias {  // a bias vector of the packed arena made from one or more parameters
+  enum Kind { SUM2,     // conv2.bias + conv_shortcut.bias
+              QKV,      // to_q | to_k | to_v biases
+              PAD128 }  // bias zero-padded to 128 output channels
+    kind;
+  int p[3];         // parameter indices (-1: unused)
+  size_t off;       // byte offset in the packed arena
+};
+
+// One block of an architecture, in forward order.  Every block reads the output of the block before it (`in`); a U-Net
+// up-block resnet also reads the output of a down block (`skip`).
+enum BlockKind {
+  BK_UNET_HEAD,    // conv_in + the timestep-embedding MLP
+  BK_CONV_IN,      // conv_in on the caller's image (autoencoder encoder)
+  BK_LATENT_IN,    // post_quant_conv + conv_in on the caller's latents (autoencoder decoder)
+  BK_RESNET,       // ResnetBlock2D over cat(input, skip)
+  BK_ATTN,         // self-attention block (head_dim 8; the autoencoder: one head)
+  BK_TRANSFORMER,  // Transformer2DModel with one BasicTransformerBlock (conditional U-Net)
+  BK_DOWN,         // Downsample2D, padding 1
+  BK_DOWN_ASYM,    // Downsample2D, padding (0, 1, 0, 1) (autoencoder encoder)
+  BK_UP,           // Upsample2D: nearest 2x + 3x3 conv
+  BK_CONV_OUT,     // conv_norm_out + SiLU + conv_out (U-Net: + the scheduler update)
+  BK_LATENT_OUT,   // conv_norm_out + SiLU + conv_out + quant_conv + latent sampling (autoencoder encoder)
+};
+struct Block {
+  BlockKind kind;
+  std::string name;        // diffusers name prefix (heads and tails: of the model part, "", "encoder." or "decoder.")
+  int in = -1, skip = -1;  // indices of the blocks whose outputs are the input and the skip connection (-1: none)
+  int cin = 0, cskip = 0, cout = 0;
+  int temb = 0;            // U-Net head and resnets: width of the time embedding
+  int cross = 0;           // transformer: width of the cross-attention encoding
+  std::string pool;        // output buffer: pooled under this tag ("": a buffer of its own)
+  // byte offsets in the packed arena, assigned by the layout pass
+  size_t conv1[2] = {}, conv2 = 0, shortcut[2] = {};    // resnet K-segments: conv1 over (input, skip), conv2, 1x1 shortcut
+  size_t qkv = 0, out = 0;                              // attention / attn1: q | k | v projection, to_out
+  size_t proj_in = 0, ff1 = 0, ff2 = 0, proj_out = 0;   // transformer
+  size_t seg[4] = {};                                   // down / up: one K-segment per parity; latent out: conv_out
+  size_t ident = 0;                                     // identity block of the residual K-segment
+  size_t bias = 0;                                      // fused bias vector
+  int temb_row = -1;                                    // resnet: its rows in the concatenated time_emb_proj
+};
+static Block& add_block(std::vector<Block>& bl, BlockKind kind, const std::string& name, int cin, int cout,
+                        const char* pool) {
+  Block b;
+  b.kind = kind; b.name = name; b.in = (int)bl.size() - 1; b.cin = cin; b.cout = cout; b.pool = pool;
+  bl.push_back(b);
+  return bl.back();
+}
+
+struct OpList {  // one launch sequence and the GroupNorm statistics it accumulates (zeroed before every run)
+  std::vector<Op> ops;
+  stat_t* stats = nullptr;
+  size_t stats_bytes = 0;
+};
+struct Plan {    // everything a plan builder derives from the workspace and (N, H, W)
+  std::vector<OpList> lists;         // U-Net: the forward; autoencoder: encoder, decoder
+  std::map<std::string, Act> taps;   // activations by name (debug_tensor; the U-Net backward reads its inputs here)
+  float* temb_act = nullptr;
+  float* temb_proj = nullptr;
+  int* temb_lead = nullptr;          // [N] first sample with the same timestep (inference only)
+  float* temb_emb = nullptr;         // training: [N][dim0]   sinusoid
+  float* temb_u1 = nullptr;          // training: [N][4 dim0] linear_1 output before SiLU
+  float* temb_u2 = nullptr;          // training: [N][4 dim0] linear_2 output before SiLU
+  float* zq = nullptr;               // autoencoder: post_quant_conv(z), [N][L][h][w]
+  size_t ws_bytes = 0;
 };
 
 // State shared by the model handles (U-Net, VAE): parameter table, packed-weight arena layout, workspace plan.
@@ -85,29 +159,18 @@ struct NetBase {
   std::vector<const float*> pptr;
   // packed arena layout
   std::vector<PackJob> jobs;
-  std::map<std::string, size_t> seg_off;  // "<conv name>#<seg>" -> byte offset
-  size_t packed_bytes = 0;
-  size_t off_wcat = 0, off_bcat = 0, off_misc = 0;
-  std::map<std::string, size_t> misc_off;  // fused bias vectors (floats)
   std::map<int, size_t> ident_off;         // channels -> identity weight blocks
+  std::vector<FusedBias> fused;
+  size_t packed_bytes = 0;
+  size_t off_wcat = 0, off_bcat = 0;       // U-Net: concatenated time_emb_proj weights / biases
   int temb_rows = 0;
-  std::map<std::string, int> temb_row_off;
   uint8_t* packed = nullptr;
   // workspace / plan
   int N = 0, H = 0, W = 0;
   uint8_t* ws = nullptr;
   size_t ws_bytes = 0;
-  std::vector<Op> plan;
-  std::map<std::string, Act> taps;
-  stat_t* stats_arena = nullptr;
-  size_t stats_bytes = 0;
-  float* temb_act = nullptr;
-  float* temb_proj = nullptr;
-  int* temb_lead = nullptr;         // [N] first sample with the same timestep (inference only)
+  Plan plan;
   bool training = false;            // keep every activation (no pooling) and the timestep-MLP pre-activations for backward
-  float* temb_emb = nullptr;        // [N][dim0]      sinusoid
-  float* temb_u1 = nullptr;         // [N][4 dim0]    linear_1 output before SiLU
-  float* temb_u2 = nullptr;         // [N][4 dim0]    linear_2 output before SiLU
   int num_sms = 132;
   const float* enc = nullptr;       // conditional U-Net: encoder_hidden_states [N][enc_S][X] of the next forward
   int enc_S = 0;
@@ -134,6 +197,16 @@ static const char* check_groups(const int* ch, int n, int groups) {
   return nullptr;
 }
 
+static std::string S(const char* fmt, ...) {
+  char buf[256];
+  va_list ap;
+  va_start(ap, fmt);
+  vsnprintf(buf, sizeof(buf), fmt, ap);
+  va_end(ap);
+  return buf;
+}
+
+// ================================================================================= parameter table
 static void add_param(NetBase* h, const std::string& name, std::vector<int64_t> shape) {
   h->pidx[name] = (int)h->params.size();
   h->params.push_back({name, std::move(shape)});
@@ -165,92 +238,7 @@ static void p_attn(NetBase* h, const std::string& n, int c) {
   p_lin(h, n + ".to_v", c, c);
   p_lin(h, n + ".to_out.0", c, c);
 }
-
-static std::string S(const char* fmt, ...) {
-  char buf[256];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  return buf;
-}
-
-static PackTaps taps_3x3() {
-  PackTaps t{};
-  t.ntaps = 9;
-  for (int k = 0; k < 9; ++k) { t.kh[k] = k / 3; t.kw[k] = k % 3; }
-  return t;
-}
-static PackTaps taps_1x1() {
-  PackTaps t{};
-  t.ntaps = 1;
-  t.kh[0] = 0; t.kw[0] = 0;
-  return t;
-}
-// stride-2 3x3 conv on parity plane (a, b): the taps that read input rows of parity a and columns of parity b
-static PackTaps taps_parity(int a, int b) {
-  PackTaps t{};
-  t.ntaps = 0;
-  for (int kh = 0; kh < 3; ++kh)
-    for (int kw = 0; kw < 3; ++kw) {
-      const int pa = (kh == 1) ? 0 : 1, pb = (kw == 1) ? 0 : 1;
-      if (pa == a && pb == b) { t.kh[t.ntaps] = kh; t.kw[t.ntaps] = kw; ++t.ntaps; }
-    }
-  return t;
-}
-
-static void add_job(NetBase* h, Bump& b, const std::string& key, const std::string& wname, int cout, int cin_total,
-                    int K, int cin_off, int cin_cnt, const PackTaps& taps) {
-  PackJob j;
-  j.w_param = h->pidx.at(wname);
-  j.cout = cout; j.cin_total = cin_total; j.KH = K; j.KW = K; j.cin_off = cin_off; j.ksteps = cin_cnt / 16;
-  j.taps = taps;
-  j.cout_real = -1;
-  const size_t bytes = (size_t)(cout / 128) * j.ksteps * taps.ntaps * CONV_B_TAP;
-  b.take(0);
-  j.off = (b.off + 255) & ~(size_t)255;
-  b.take(bytes);
-  h->seg_off[key] = j.off;
-  h->jobs.push_back(j);
-}
-
-static size_t take_off(Bump& b, size_t bytes) {  // size-only pass: returns the aligned offset
-  b.take(0);
-  const size_t o = (b.off + 255) & ~(size_t)255;
-  b.take(bytes);
-  return o;
-}
-static void need_ident(NetBase* h, Bump& b, int ch) {  // identity weight blocks for residual-as-K-segment
-  if (!h->ident_off.count(ch)) h->ident_off[ch] = take_off(b, (size_t)(ch / 128) * (ch / 16) * CONV_B_TAP);
-}
-// ResnetBlock2D over cat(a, b): conv1 is one K-segment per source (each with its own fused GroupNorm scale/shift slice),
-// conv2 carries the shortcut (1x1 conv or identity) as extra K-segments.
-static void layout_resnet(NetBase* h, Bump& b, const std::string& n, int ca, int cb, int co, bool temb) {
-  const int cin = ca + cb;
-  add_job(h, b, n + ".conv1#0", n + ".conv1.weight", co, cin, 3, 0, ca, taps_3x3());
-  if (cb) add_job(h, b, n + ".conv1#1", n + ".conv1.weight", co, cin, 3, ca, cb, taps_3x3());
-  add_job(h, b, n + ".conv2#0", n + ".conv2.weight", co, co, 3, 0, co, taps_3x3());
-  if (cin == co) need_ident(h, b, co);
-  if (cin != co) {
-    add_job(h, b, n + ".conv2#1", n + ".conv_shortcut.weight", co, cin, 1, 0, ca, taps_1x1());
-    if (cb) add_job(h, b, n + ".conv2#2", n + ".conv_shortcut.weight", co, cin, 1, ca, cb, taps_1x1());
-    h->misc_off[n + ".bias2"] = take_off(b, (size_t)co * 4);
-  }
-  if (temb) {
-    h->temb_row_off[n] = h->temb_rows;
-    h->temb_rows += co;
-  }
-}
-static void layout_attn(NetBase* h, Bump& b, const std::string& n, int ch) {
-  add_job(h, b, n + ".qkv#q", n + ".to_q.weight", ch, ch, 1, 0, ch, taps_1x1());
-  add_job(h, b, n + ".qkv#k", n + ".to_k.weight", ch, ch, 1, 0, ch, taps_1x1());
-  add_job(h, b, n + ".qkv#v", n + ".to_v.weight", ch, ch, 1, 0, ch, taps_1x1());
-  add_job(h, b, n + ".out#0", n + ".to_out.0.weight", ch, ch, 1, 0, ch, taps_1x1());
-  h->misc_off[n + ".bias_qkv"] = take_off(b, (size_t)3 * ch * 4);
-  need_ident(h, b, ch);
-}
-
-// Transformer2DModel + BasicTransformerBlock of the conditional U-Net (diffusers naming): packed 1x1 projections
+// Transformer2DModel + BasicTransformerBlock of the conditional U-Net (diffusers naming)
 static void p_transformer(NetBase* h, const std::string& n, int c, int X) {
   p_gn(h, n + ".norm", c);
   p_conv(h, n + ".proj_in", c, c, 1);
@@ -270,27 +258,136 @@ static void p_transformer(NetBase* h, const std::string& n, int c, int X) {
   p_lin(h, b + ".ff.net.2", 4 * c, c);
   p_conv(h, n + ".proj_out", c, c, 1);
 }
-static void layout_transformer(NetBase* h, Bump& b, const std::string& n, int c) {
+static void p_block(NetBase* h, const Block& k) {
+  const std::string& n = k.name;
+  switch (k.kind) {
+    case BK_UNET_HEAD:
+      p_conv(h, n + "conv_in", k.cin, k.cout, 3);
+      p_lin(h, "time_embedding.linear_1", k.cout, k.temb);
+      p_lin(h, "time_embedding.linear_2", k.temb, k.temb);
+      break;
+    case BK_CONV_IN: p_conv(h, n + "conv_in", k.cin, k.cout, 3); break;
+    case BK_LATENT_IN:
+      p_conv(h, "post_quant_conv", k.cin, k.cin, 1);
+      p_conv(h, n + "conv_in", k.cin, k.cout, 3);
+      break;
+    case BK_RESNET: p_resnet(h, n, k.cin + k.cskip, k.cout, k.temb); break;
+    case BK_ATTN: p_attn(h, n, k.cout); break;
+    case BK_TRANSFORMER: p_transformer(h, n, k.cout, k.cross); break;
+    case BK_DOWN: case BK_DOWN_ASYM: case BK_UP: p_conv(h, n, k.cout, k.cout, 3); break;
+    case BK_CONV_OUT:
+      p_gn(h, n + "conv_norm_out", k.cin);
+      p_conv(h, n + "conv_out", k.cin, k.cout, 3);
+      break;
+    case BK_LATENT_OUT:
+      p_gn(h, n + "conv_norm_out", k.cin);
+      p_conv(h, n + "conv_out", k.cin, k.cout, 3);
+      p_conv(h, "quant_conv", k.cout, k.cout, 1);
+      break;
+  }
+}
+
+// ================================================================================= packed-weight arena layout
+static size_t add_job(NetBase* h, Bump& b, const std::string& wname, int cout, int cin_total, int K, int cin_off,
+                      int cin_cnt, const TapSet& taps, int cout_real = -1) {
+  PackJob j;
+  j.w_param = h->pidx.at(wname);
+  j.cout = cout; j.cin_total = cin_total; j.KH = K; j.KW = K; j.cin_off = cin_off; j.ksteps = cin_cnt / 16;
+  j.taps = taps.pack;
+  j.cout_real = cout_real;
+  j.off = take_off(b, (size_t)(cout / 128) * j.ksteps * taps.pack.ntaps * CONV_B_TAP);
+  h->jobs.push_back(j);
+  return j.off;
+}
+static size_t add_ident(NetBase* h, Bump& b, int ch) {  // identity weight blocks for residual-as-K-segment
+  auto it = h->ident_off.find(ch);
+  if (it == h->ident_off.end()) it = h->ident_off.emplace(ch, take_off(b, (size_t)(ch / 128) * (ch / 16) * CONV_B_TAP)).first;
+  return it->second;
+}
+static size_t add_bias(NetBase* h, Bump& b, FusedBias::Kind kind, size_t floats, const std::string& p0,
+                       const std::string& p1 = "", const std::string& p2 = "") {
+  FusedBias f;
+  f.kind = kind;
+  f.p[0] = h->pidx.at(p0);
+  f.p[1] = p1.empty() ? -1 : h->pidx.at(p1);
+  f.p[2] = p2.empty() ? -1 : h->pidx.at(p2);
+  f.off = take_off(b, floats * 4);
+  h->fused.push_back(f);
+  return f.off;
+}
+static TapSet down_taps(const Block& k, int a, int b) {
+  return k.kind == BK_DOWN ? taps_parity(a, b) : taps_parity_asym(a, b);
+}
+// ResnetBlock2D over cat(a, b): conv1 is one K-segment per source (each with its own fused GroupNorm scale/shift slice),
+// conv2 carries the shortcut (1x1 conv or identity) as extra K-segments.
+static void layout_resnet(NetBase* h, Bump& b, Block& k) {
+  const std::string& n = k.name;
+  const int ca = k.cin, cb = k.cskip, co = k.cout, cin = ca + cb;
+  k.conv1[0] = add_job(h, b, n + ".conv1.weight", co, cin, 3, 0, ca, taps_conv(3));
+  if (cb) k.conv1[1] = add_job(h, b, n + ".conv1.weight", co, cin, 3, ca, cb, taps_conv(3));
+  k.conv2 = add_job(h, b, n + ".conv2.weight", co, co, 3, 0, co, taps_conv(3));
+  if (cin == co) {
+    k.ident = add_ident(h, b, co);
+  } else {
+    k.shortcut[0] = add_job(h, b, n + ".conv_shortcut.weight", co, cin, 1, 0, ca, taps_conv(1));
+    if (cb) k.shortcut[1] = add_job(h, b, n + ".conv_shortcut.weight", co, cin, 1, ca, cb, taps_conv(1));
+    k.bias = add_bias(h, b, FusedBias::SUM2, co, n + ".conv2.bias", n + ".conv_shortcut.bias");
+  }
+  if (k.temb) {
+    k.temb_row = h->temb_rows;
+    h->temb_rows += co;
+  }
+}
+static void layout_attn(NetBase* h, Bump& b, Block& k) {
+  const std::string& n = k.name;
+  const int ch = k.cout;
+  k.qkv = add_job(h, b, n + ".to_q.weight", ch, ch, 1, 0, ch, taps_conv(1));   // q | k | v blocks are contiguous
+  add_job(h, b, n + ".to_k.weight", ch, ch, 1, 0, ch, taps_conv(1));
+  add_job(h, b, n + ".to_v.weight", ch, ch, 1, 0, ch, taps_conv(1));
+  k.out = add_job(h, b, n + ".to_out.0.weight", ch, ch, 1, 0, ch, taps_conv(1));
+  k.bias = add_bias(h, b, FusedBias::QKV, (size_t)3 * ch, n + ".to_q.bias", n + ".to_k.bias", n + ".to_v.bias");
+  k.ident = add_ident(h, b, ch);
+}
+static void layout_transformer(NetBase* h, Bump& b, Block& k) {
+  const std::string& n = k.name;
   const std::string t = n + ".transformer_blocks.0";
-  add_job(h, b, n + ".proj_in#0", n + ".proj_in.weight", c, c, 1, 0, c, taps_1x1());
-  add_job(h, b, t + ".qkv#q", t + ".attn1.to_q.weight", c, c, 1, 0, c, taps_1x1());   // q | k | v blocks are contiguous
-  add_job(h, b, t + ".qkv#k", t + ".attn1.to_k.weight", c, c, 1, 0, c, taps_1x1());
-  add_job(h, b, t + ".qkv#v", t + ".attn1.to_v.weight", c, c, 1, 0, c, taps_1x1());
-  add_job(h, b, t + ".attn1.out#0", t + ".attn1.to_out.0.weight", c, c, 1, 0, c, taps_1x1());
-  add_job(h, b, t + ".ff1#0", t + ".ff.net.0.proj.weight", 8 * c, c, 1, 0, c, taps_1x1());
-  add_job(h, b, t + ".ff2#0", t + ".ff.net.2.weight", c, 4 * c, 1, 0, 4 * c, taps_1x1());
-  add_job(h, b, n + ".proj_out#0", n + ".proj_out.weight", c, c, 1, 0, c, taps_1x1());
-  need_ident(h, b, c);
+  const int c = k.cout;
+  k.proj_in = add_job(h, b, n + ".proj_in.weight", c, c, 1, 0, c, taps_conv(1));
+  k.qkv = add_job(h, b, t + ".attn1.to_q.weight", c, c, 1, 0, c, taps_conv(1));   // q | k | v blocks are contiguous
+  add_job(h, b, t + ".attn1.to_k.weight", c, c, 1, 0, c, taps_conv(1));
+  add_job(h, b, t + ".attn1.to_v.weight", c, c, 1, 0, c, taps_conv(1));
+  k.out = add_job(h, b, t + ".attn1.to_out.0.weight", c, c, 1, 0, c, taps_conv(1));
+  k.ff1 = add_job(h, b, t + ".ff.net.0.proj.weight", 8 * c, c, 1, 0, c, taps_conv(1));
+  k.ff2 = add_job(h, b, t + ".ff.net.2.weight", c, 4 * c, 1, 0, 4 * c, taps_conv(1));
+  k.proj_out = add_job(h, b, n + ".proj_out.weight", c, c, 1, 0, c, taps_conv(1));
+  k.ident = add_ident(h, b, c);
+}
+static void layout_block(NetBase* h, Bump& b, Block& k) {
+  switch (k.kind) {
+    case BK_RESNET: layout_resnet(h, b, k); break;
+    case BK_ATTN: layout_attn(h, b, k); break;
+    case BK_TRANSFORMER: layout_transformer(h, b, k); break;
+    case BK_DOWN: case BK_DOWN_ASYM:   // one K-segment per parity plane of the input
+      for (int a = 0; a < 2; ++a)
+        for (int c = 0; c < 2; ++c)
+          k.seg[a * 2 + c] = add_job(h, b, k.name + ".weight", k.cout, k.cout, 3, 0, k.cout, down_taps(k, a, c));
+      break;
+    case BK_UP:                        // one folded 2x2 conv per output parity
+      for (int a = 0; a < 2; ++a)
+        for (int c = 0; c < 2; ++c)
+          k.seg[a * 2 + c] = add_job(h, b, k.name + ".weight", k.cout, k.cout, 3, 0, k.cout, taps_up2(a, c));
+      break;
+    case BK_LATENT_OUT:                // conv_out: 2L output channels zero-padded to one 128-channel tile
+      k.seg[0] = add_job(h, b, k.name + "conv_out.weight", 128, k.cin, 3, 0, k.cin, taps_conv(3), k.cout);
+      k.bias = add_bias(h, b, FusedBias::PAD128, 128, k.name + "conv_out.bias");
+      break;
+    default: break;                    // fp32 weights read as they are
+  }
 }
 
 static __global__ void add_vec_kernel(const float* a, const float* b, float* o, int n) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) o[i] = a[i] + (b ? b[i] : 0.f);
-}
-
-static bool ends_with(const std::string& s, const char* suf) {
-  const size_t n = strlen(suf);
-  return s.size() > n && s.compare(s.size() - n, n, suf) == 0;
 }
 
 // Pack every conv K-segment, the identity blocks and the fused bias vectors into the arena (after pptr/packed are set).
@@ -302,40 +399,37 @@ static int pack_common(NetBase* h, cudaStream_t st) {
     CK(launch_pack_batch(h->pack_batch, items, st));
   }
   for (const auto& kv : h->ident_off) CK(launch_pack_identity(kv.first, (__nv_bfloat16*)(h->packed + kv.second), st));
-  for (const auto& kv : h->misc_off) {
-    const std::string& key = kv.first;
-    float* dst = (float*)(h->packed + kv.second);
-    if (ends_with(key, ".bias2")) {            // conv2.bias + conv_shortcut.bias
-      const std::string n = key.substr(0, key.size() - 6);
-      const int co = (int)h->params[h->pidx.at(n + ".conv2.bias")].shape[0];
-      add_vec_kernel<<<(co + 255) / 256, 256, 0, st>>>(h->pptr[h->pidx.at(n + ".conv2.bias")],
-                                                       h->pptr[h->pidx.at(n + ".conv_shortcut.bias")], dst, co);
-      CK(cudaGetLastError());
-    } else if (ends_with(key, ".bias_qkv")) {  // to_q | to_k | to_v biases
-      const std::string n = key.substr(0, key.size() - 9);
-      const int c = (int)h->params[h->pidx.at(n + ".to_q.bias")].shape[0];
-      CK(cudaMemcpyAsync(dst, h->pptr[h->pidx.at(n + ".to_q.bias")], c * 4, cudaMemcpyDeviceToDevice, st));
-      CK(cudaMemcpyAsync(dst + c, h->pptr[h->pidx.at(n + ".to_k.bias")], c * 4, cudaMemcpyDeviceToDevice, st));
-      CK(cudaMemcpyAsync(dst + 2 * c, h->pptr[h->pidx.at(n + ".to_v.bias")], c * 4, cudaMemcpyDeviceToDevice, st));
-    } else if (ends_with(key, ".bias_pad")) {  // bias zero-padded to 128 output channels
-      const std::string n = key.substr(0, key.size() - 9);
-      const int co = (int)h->params[h->pidx.at(n + ".bias")].shape[0];
-      CK(cudaMemsetAsync(dst, 0, 128 * 4, st));
-      CK(cudaMemcpyAsync(dst, h->pptr[h->pidx.at(n + ".bias")], co * 4, cudaMemcpyDeviceToDevice, st));
-    } else {
-      return set_err("unknown fused-bias key %s", key.c_str());
+  for (const FusedBias& f : h->fused) {
+    float* dst = (float*)(h->packed + f.off);
+    const int c = (int)h->params[f.p[0]].shape[0];
+    const float* const* src = h->pptr.data();
+    switch (f.kind) {
+      case FusedBias::SUM2:
+        add_vec_kernel<<<(c + 255) / 256, 256, 0, st>>>(src[f.p[0]], src[f.p[1]], dst, c);
+        CK(cudaGetLastError());
+        break;
+      case FusedBias::QKV:
+        for (int i = 0; i < 3; ++i) CK(cudaMemcpyAsync(dst + i * c, src[f.p[i]], c * 4, cudaMemcpyDeviceToDevice, st));
+        break;
+      case FusedBias::PAD128:
+        CK(cudaMemsetAsync(dst, 0, 128 * 4, st));
+        CK(cudaMemcpyAsync(dst, src[f.p[0]], c * 4, cudaMemcpyDeviceToDevice, st));
+        break;
     }
   }
   return 0;
 }
 
+// ================================================================================= launch plan
 struct Builder {
-  NetBase* h;
+  const NetBase* h;
+  Plan* built;
   Bump ws;
   Bump st;  // stats arena (floats, offsets in bytes)
-  std::vector<Op>* plan;
+  std::vector<Op>* ops;
   std::map<std::string, Act> pool;  // reusable transient buffers keyed by tag
-  int N;
+  int N, H = 0, W = 0;              // H, W: input size of the block list being planned
+  int heads = 8;                    // transformer: attention heads
   bool nopool = false;  // B200AD_DEBUG_NOPOOL=1: every activation gets its own buffer (per-layer parity taps)
   bool single_head = false;  // attention with one head of dim C (AutoencoderKL mid block) instead of head_dim 8
 
@@ -356,11 +450,11 @@ struct Builder {
     if (stats) a.stats = (stat_t*)st.take((size_t)N * (C / 4) * 2 * sizeof(stat_t));
     return a;
   }
-  const float* P(const std::string& name) const { return h->pptr[h->pidx.at(name)]; }
-  const __nv_bfloat16* WP(const std::string& key) const {
-    return h->packed ? (const __nv_bfloat16*)(h->packed + h->seg_off.at(key)) : nullptr;
+  Act output(const Block& k, int C, int H, int W) {  // a block's output (raw + stats)
+    return k.pool.empty() ? alloc(C, H, W, true) : pooled(k.pool, C, H, W, true);
   }
-  const float* MISC(const std::string& key) const { return h->packed ? (const float*)(h->packed + h->misc_off.at(key)) : nullptr; }
+  const float* P(const std::string& name) const { return h->pptr[h->pidx.at(name)]; }
+  template <class T> const T* PK(size_t off) const { return h->packed ? (const T*)(h->packed + off) : nullptr; }
 
   void conv_common(ConvParams& p, const Act& out) {
     const Geom g = make_geom(N, out.H, out.W);
@@ -369,51 +463,21 @@ struct Builder {
     p.out = out.p;
     p.stats = out.stats;
   }
-  static void seg_taps(ConvSeg& s, const PackTaps& t, bool parity, int a, int b) {
-    s.ntaps = t.ntaps;
-    s.ht = s.hb = s.hl = s.hr = 0;
-    for (int k = 0; k < t.ntaps; ++k) {
-      if (parity) {
-        s.dh[k] = (t.kh[k] == 0) ? -1 : 0;
-        s.dw[k] = (t.kw[k] == 0) ? -1 : 0;
-      } else if (t.ntaps == 9) {
-        s.dh[k] = (signed char)(t.kh[k] - 1);
-        s.dw[k] = (signed char)(t.kw[k] - 1);
-      } else {
-        s.dh[k] = 0; s.dw[k] = 0;
-      }
-      if (s.dh[k] < 0) s.ht = 1;
-      if (s.dh[k] > 0) s.hb = 1;
-      if (s.dw[k] < 0) s.hl = 1;
-      if (s.dw[k] > 0) s.hr = 1;
-    }
-    (void)a; (void)b;
+  void seg(ConvSeg& s, const __nv_bfloat16* src, int C, int H, int W, size_t woff, const TapSet& t) {
+    set_seg(s, src, C / 8, C, H, W, PK<__nv_bfloat16>(woff), t);
   }
-  void set_seg(ConvSeg& s, const __nv_bfloat16* src, int C, int H, int W, const __nv_bfloat16* wpack, const PackTaps& t,
-               bool parity = false) {
-    const Geom g = make_geom(N, H, W);
-    s.src = src;
-    s.wpack = wpack;
-    s.img_stride = (long long)(C / 8) * g.PL * 8;
-    s.ksteps = C / 16;
-    s.ss = nullptr; s.ss_stride = 0; s.silu = 0;
-    seg_taps(s, t, parity, 0, 0);
-  }
+  void seg(ConvSeg& s, const Act& a, size_t woff, const TapSet& t) { seg(s, a.p, a.C, a.H, a.W, woff, t); }
 
-  // GroupNorm over cat(a, b): statistics -> per-(sample, channel) scale/shift; the apply itself is fused into the consumer
-  // conv's transform warps. Returns the [N][Ca + Cb] scale/shift array.
   // Let the launch just planned (the producer of `a`; `b`, a skip connection, is older) finalize the GroupNorm over
   // cat(a, b) in its last CTA.  Returns the [N][Ca + Cb] (scale, shift) array, or nullptr if the last op cannot do it
   // (conv_in, an op of another kind, a batch too large for the scratch).
   float2* gn_attach(const Act& a, const Act* b, const std::string& norm, float2* ss = nullptr, float eps = -1.f) {
     const int Ct = a.C + (b ? b->C : 0);
-    static const bool off = [] { const char* e = getenv("B200AD_NO_GNFOLD"); return e && e[0] == '1'; }();   // A/B switch
-    if (off) return nullptr;
-    if (plan->empty() || plan->back().kind != OP_CONV || plan->back().conv.out != a.p || plan->back().conv.fin.ss ||
+    if (ops->empty() || ops->back().kind != OP_CONV || ops->back().conv.out != a.p || ops->back().conv.fin.ss ||
         (size_t)N * h->norm_groups * 2 * sizeof(float) > 32768)
       return nullptr;
     if (!ss) ss = (float2*)ws.take((size_t)N * Ct * sizeof(float2));
-    ConvGnFin& f = plan->back().conv.fin;
+    ConvGnFin& f = ops->back().conv.fin;
     f.stats[0] = a.stats; f.C[0] = a.C;
     f.stats[1] = b ? b->stats : nullptr; f.C[1] = b ? b->C : 0;
     f.gamma = P(norm + ".weight"); f.beta = P(norm + ".bias");
@@ -422,8 +486,9 @@ struct Builder {
     f.groups = h->norm_groups; f.HW = a.H * a.W; f.eps = eps < 0.f ? h->norm_eps : eps;
     return ss;
   }
-  float2* gn_attach(const Act& a, const std::string& norm) { return gn_attach(a, nullptr, norm); }
 
+  // GroupNorm over cat(a, b): statistics -> per-(sample, channel) scale/shift; the apply itself is fused into the consumer
+  // conv's transform warps. Returns the [N][Ca + Cb] scale/shift array.
   float2* gn_finalize(const Act& a, const Act* b, const std::string& norm, float eps = -1.f) {
     const int Ct = a.C + (b ? b->C : 0);
     float2* ss = (float2*)ws.take((size_t)N * Ct * sizeof(float2));
@@ -437,19 +502,59 @@ struct Builder {
     p.dst = nullptr;
     p.N = N; p.H = a.H; p.W = a.W; p.groups = h->norm_groups; p.eps = eps < 0.f ? h->norm_eps : eps; p.silu = 0;
     op.ss = ss;
-    plan->push_back(op);
+    ops->push_back(op);
     return ss;
   }
   static void seg_norm(ConvSeg& s, const float2* ss, int stride, bool silu) {
     s.ss = ss; s.ss_stride = stride; s.silu = silu ? 1 : 0;
   }
-  const __nv_bfloat16* IDENT(int ch) const {
-    return h->packed ? (const __nv_bfloat16*)(h->packed + h->ident_off.at(ch)) : nullptr;
+
+  // conv_in of a model part, on the caller's fp32 input or on `src`
+  Act conv_in(const Block& k, float* src) {
+    Act x = output(k, k.cout, H, W);
+    Op op{};
+    op.kind = OP_CONV_IN;
+    op.dst = x.p; op.C = k.cout; op.H = H; op.W = W; op.cin = k.cin;
+    op.f0 = src;
+    op.fw = P(k.name + "conv_in.weight"); op.fb = P(k.name + "conv_in.bias");
+    op.conv.stats = x.stats;
+    ops->push_back(op);
+    built->taps[k.name + "conv_in"] = x;
+    return x;
+  }
+
+  // timestep embedding (one op for the MLP and every resnet's projection), then conv_in
+  Act unet_head(const Block& k) {
+    built->temb_act = (float*)ws.take((size_t)N * k.temb * 4);
+    built->temb_proj = (float*)ws.take((size_t)N * h->temb_rows * 4);
+    built->temb_lead = (int*)ws.take((size_t)N * 4);
+    if (h->training) {
+      built->temb_emb = (float*)ws.take((size_t)N * k.cout * 4);
+      built->temb_u1 = (float*)ws.take((size_t)N * k.temb * 4);
+      built->temb_u2 = (float*)ws.take((size_t)N * k.temb * 4);
+    }
+    Op op{};
+    op.kind = OP_TEMB;
+    op.C = k.cout;
+    ops->push_back(op);
+    return conv_in(k, nullptr);
+  }
+
+  // post_quant_conv on the caller's latents, then conv_in
+  Act latent_in(const Block& k) {
+    built->zq = (float*)ws.take((size_t)N * k.cin * H * W * 4);
+    Op op{};
+    op.kind = OP_MIX1X1;
+    op.f0 = built->zq; op.C = k.cin; op.H = H; op.W = W;
+    op.fw = P("post_quant_conv.weight"); op.fb = P("post_quant_conv.bias");
+    ops->push_back(op);
+    return conv_in(k, built->zq);
   }
 
   // ResnetBlock2D on x = cat(a, b) (b optional) -> out (raw + stats)
-  Act resnet(const std::string& n, const Act& a, const Act* b, int cout, bool out_pooled, const std::string& out_tag) {
-    const int cin = a.C + (b ? b->C : 0);
+  Act resnet(const Block& k, const Act& a, const Act* b) {
+    const std::string& n = k.name;
+    const int cin = a.C + (b ? b->C : 0), cout = k.cout;
     const int H = a.H, W = a.W;
     const float2* ss1 = gn_finalize(a, b, n + ".norm1");
     Act h1 = pooled("h1", cout, H, W, true);
@@ -459,80 +564,76 @@ struct Builder {
       ConvParams& p = op.conv;
       conv_common(p, h1);
       p.nseg = 1;
-      set_seg(p.seg[0], a.p, a.C, H, W, WP(n + ".conv1#0"), taps_3x3());
+      seg(p.seg[0], a, k.conv1[0], taps_conv(3));
       seg_norm(p.seg[0], ss1, cin, true);
       if (b) {
-        set_seg(p.seg[1], b->p, b->C, H, W, WP(n + ".conv1#1"), taps_3x3());
+        seg(p.seg[1], *b, k.conv1[1], taps_conv(3));
         seg_norm(p.seg[1], ss1 + a.C, cin, true);
         p.nseg = 2;
       }
       p.bias = P(n + ".conv1.bias");
-      if (h->temb_rows) {
-        p.temb = h->temb_proj + h->temb_row_off.at(n);
+      if (k.temb_row >= 0) {
+        p.temb = built->temb_proj + k.temb_row;
         p.temb_stride = h->temb_rows;
-      } else {
-        p.temb = nullptr;
-        p.temb_stride = 0;
       }
-      plan->push_back(op);
+      ops->push_back(op);
     }
     const float2* ss2 = gn_finalize(h1, nullptr, n + ".norm2");
-    Act out = out_pooled ? pooled(out_tag, cout, H, W, true) : alloc(cout, H, W, true);
+    Act out = output(k, cout, H, W);
     {
       Op op{};
       op.kind = OP_CONV;
       ConvParams& p = op.conv;
       conv_common(p, out);
       p.nseg = 1;
-      set_seg(p.seg[0], h1.p, cout, H, W, WP(n + ".conv2#0"), taps_3x3());
+      seg(p.seg[0], h1, k.conv2, taps_conv(3));
       seg_norm(p.seg[0], ss2, cout, true);
-      p.temb = nullptr;
-      p.temb_stride = 0;
       if (cin != cout) {  // 1x1 conv_shortcut over the raw input(s): extra K-segments into the same accumulators
-        set_seg(p.seg[1], a.p, a.C, H, W, WP(n + ".conv2#1"), taps_1x1());
+        seg(p.seg[1], a, k.shortcut[0], taps_conv(1));
         p.nseg = 2;
         if (b) {
-          set_seg(p.seg[2], b->p, b->C, H, W, WP(n + ".conv2#2"), taps_1x1());
+          seg(p.seg[2], *b, k.shortcut[1], taps_conv(1));
           p.nseg = 3;
         }
-        p.bias = MISC(n + ".bias2");
+        p.bias = PK<float>(k.bias);
       } else {            // identity shortcut: residual add as a 1-tap identity-weight segment over the raw input
-        set_seg(p.seg[1], a.p, a.C, H, W, IDENT(cout), taps_1x1());
+        seg(p.seg[1], a, k.ident, taps_conv(1));
         p.nseg = 2;
         p.bias = P(n + ".conv2.bias");
       }
-      plan->push_back(op);
+      ops->push_back(op);
     }
-    h->taps[n + ".h1"] = h1;
-    h->taps[n] = out;
+    built->taps[n + ".h1"] = h1;
+    built->taps[n] = out;
     return out;
   }
 
   // plain 1-tap conv (a linear layer over the pixel tokens) with optional fused GroupNorm of the source, identity residual
   // and per-sample additive vector
-  void linear(const Act& out, const Act& src, const std::string& wkey, const float* bias, const float2* ss = nullptr,
-              const Act* residual = nullptr, const float* vec = nullptr, int vec_stride = 0) {
+  void linear(const Act& out, const Act& src, size_t woff, const float* bias, const float2* ss = nullptr,
+              const Act* residual = nullptr, size_t ident = 0, const float* vec = nullptr, int vec_stride = 0) {
     Op op{};
     op.kind = OP_CONV;
     ConvParams& p = op.conv;
     conv_common(p, out);
     p.nseg = 1;
-    set_seg(p.seg[0], src.p, src.C, src.H, src.W, WP(wkey), taps_1x1());
+    seg(p.seg[0], src, woff, taps_conv(1));
     if (ss) seg_norm(p.seg[0], ss, src.C, false);
     if (residual) {
-      set_seg(p.seg[1], residual->p, residual->C, residual->H, residual->W, IDENT(residual->C), taps_1x1());
+      seg(p.seg[1], *residual, ident, taps_conv(1));
       p.nseg = 2;
     }
     p.bias = bias;
     p.temb = vec; p.temb_stride = vec_stride;
-    plan->push_back(op);
+    ops->push_back(op);
   }
 
   // Transformer2DModel with one BasicTransformerBlock (conditional U-Net), encoder sequence length 1:
   //   h0 = proj_in(GroupNorm(x));  h2 = h0 + attn1(LN1(h0)) + attn2(enc);  h3 = h2 + ff(LN3(h2));  out = proj_out(h3) + x
   // attn2 with ONE key is the per-sample vector to_out(to_v(enc)) (softmax over a single key is 1): it rides on the
   // per-sample additive term of the attn1 output projection.
-  Act transformer(const std::string& n, const Act& x, int heads, int X, bool out_pooled, const std::string& out_tag) {
+  Act transformer(const Block& k, const Act& x) {
+    const std::string& n = k.name;
     const int C = x.C, H = x.H, W = x.W;
     const std::string t = n + ".transformer_blocks.0";
     const float2* ssx = gn_finalize(x, nullptr, n + ".norm", 1e-6f);
@@ -540,66 +641,66 @@ struct Builder {
     {
       Op op{};
       op.kind = OP_XVEC;
-      op.C = C; op.cin = X;
+      op.C = C; op.cin = k.cross;
       op.fw = P(t + ".attn2.to_v.weight"); op.fb = P(t + ".attn2.to_out.0.weight"); op.fc = P(t + ".attn2.to_out.0.bias");
       op.f1 = vec;
-      plan->push_back(op);
+      ops->push_back(op);
     }
     Act h0 = pooled("tf_h0", C, H, W, false);
-    linear(h0, x, n + ".proj_in#0", P(n + ".proj_in.bias"), ssx);
+    linear(h0, x, k.proj_in, P(n + ".proj_in.bias"), ssx);
     Act n1 = pooled("tf_ln", C, H, W, false);
     auto layer_norm = [&](const Act& src, const Act& dst, const std::string& nm) {
       Op op{};
       op.kind = OP_LN;
       op.src = src.p; op.dst = dst.p; op.C = C; op.H = H; op.W = W;
       op.fw = P(nm + ".weight"); op.fb = P(nm + ".bias"); op.eps = 1e-5f;
-      plan->push_back(op);
+      ops->push_back(op);
     };
     layer_norm(h0, n1, t + ".norm1");
     Act qkv = pooled("tf_qkv", 3 * C, H, W, false);
-    linear(qkv, n1, t + ".qkv#q", nullptr);
+    linear(qkv, n1, k.qkv, nullptr);
     Act ao = pooled("tf_ao", C, H, W, false);
     {
       Op op{};
       op.kind = OP_MHA;
       op.src = qkv.p; op.dst = ao.p; op.C = C; op.H = H; op.W = W; op.cin = heads;
-      plan->push_back(op);
+      ops->push_back(op);
     }
     Act h2 = pooled("tf_h2", C, H, W, false);
-    linear(h2, ao, t + ".attn1.out#0", P(t + ".attn1.to_out.0.bias"), nullptr, &h0, vec, C);
+    linear(h2, ao, k.out, P(t + ".attn1.to_out.0.bias"), nullptr, &h0, k.ident, vec, C);
     layer_norm(h2, n1, t + ".norm3");
     Act ff1 = pooled("tf_ff1", 8 * C, H, W, false);
-    linear(ff1, n1, t + ".ff1#0", P(t + ".ff.net.0.proj.bias"));
+    linear(ff1, n1, k.ff1, P(t + ".ff.net.0.proj.bias"));
     Act gg = pooled("tf_gg", 4 * C, H, W, false);
     {
       Op op{};
       op.kind = OP_GEGLU;
       op.src = ff1.p; op.dst = gg.p; op.C = 4 * C; op.H = H; op.W = W;
-      plan->push_back(op);
+      ops->push_back(op);
     }
     Act h3 = pooled("tf_h0", C, H, W, false);     // h0 is dead after h2
-    linear(h3, gg, t + ".ff2#0", P(t + ".ff.net.2.bias"), nullptr, &h2);
-    Act out = out_pooled ? pooled(out_tag, C, H, W, true) : alloc(C, H, W, true);
-    linear(out, h3, n + ".proj_out#0", P(n + ".proj_out.bias"), nullptr, &x);
-    h->taps[n + ".attn2"] = h2;
-    h->taps[n] = out;
+    linear(h3, gg, k.ff2, P(t + ".ff.net.2.bias"), nullptr, &h2, k.ident);
+    Act out = output(k, C, H, W);
+    linear(out, h3, k.proj_out, P(n + ".proj_out.bias"), nullptr, &x, k.ident);
+    built->taps[n + ".attn2"] = h2;
+    built->taps[n] = out;
     return out;
   }
 
-  // Downsample2D(use_conv, padding 1): 3x3 stride-2 conv = four K-segments over the parity planes of the input
-  Act down2(const std::string& n, const Act& x) {
+  // Downsample2D: 3x3 stride-2 conv = four K-segments over the parity planes of the input
+  Act down2(const Block& k, const Act& x) {
     const int C = x.C, Ho = x.H / 2, Wo = x.W / 2;
     const Geom go = make_geom(N, Ho, Wo);
     const size_t tsz = (size_t)N * (C / 8) * go.PL * 8;  // elements per parity tensor
     Act par = pooled("parity", 4 * C, Ho, Wo, false);     // 4 tensors back to back (same bytes as 4C channels)
-    h->taps[n + ".parity"] = par;
+    built->taps[k.name + ".parity"] = par;
     {
       Op op{};
       op.kind = OP_PARITY;
       op.src = x.p; op.dst = par.p; op.C = C; op.H = x.H; op.W = x.W;
-      plan->push_back(op);
+      ops->push_back(op);
     }
-    Act y = alloc(C, Ho, Wo, true);
+    Act y = output(k, C, Ho, Wo);
     Op op{};
     op.kind = OP_CONV;
     ConvParams& p = op.conv;
@@ -607,21 +708,19 @@ struct Builder {
     p.nseg = 4;
     for (int a = 0; a < 2; ++a)
       for (int b = 0; b < 2; ++b)
-        set_seg(p.seg[a * 2 + b], par.p + (size_t)(a * 2 + b) * tsz, C, Ho, Wo, WP(n + S("#%d", a * 2 + b)), taps_parity(a, b), true);
-    p.bias = P(n + ".bias");
-    p.temb = nullptr; p.temb_stride = 0;
-    plan->push_back(op);
-    h->taps[n] = y;
+        seg(p.seg[a * 2 + b], par.p + (size_t)(a * 2 + b) * tsz, C, Ho, Wo, k.seg[a * 2 + b], down_taps(k, a, b));
+    p.bias = P(k.name + ".bias");
+    ops->push_back(op);
+    built->taps[k.name] = y;
     return y;
   }
 
   // Upsample2D(use_conv): nearest-2x + 3x3 conv folded into four 2x2 convs on the low-res tensor (one launch per parity)
-  Act up2(const std::string& nm, const Act& x) {
+  Act up2(const Block& k, const Act& x) {
     const int C = x.C, hh = x.H, ww = x.W;
-    Act y = pooled("up_conv", C, hh * 2, ww * 2, true);
+    Act y = output(k, C, hh * 2, ww * 2);
     for (int pa = 0; pa < 2; ++pa)
       for (int pb = 0; pb < 2; ++pb) {
-        const UpTaps ut = taps_up2(pa, pb);
         Op op{};
         op.kind = OP_CONV;
         ConvParams& p = op.conv;
@@ -630,25 +729,16 @@ struct Builder {
         conv_common(p, lo);
         p.up2 = 1; p.oy = pa; p.ox = pb;
         p.nseg = 1;
-        ConvSeg& sgm = p.seg[0];
-        set_seg(sgm, x.p, C, hh, ww, WP(nm + S("#p%d", pa * 2 + pb)), ut.pack);
-        sgm.ht = sgm.hb = sgm.hl = sgm.hr = 0;
-        for (int t = 0; t < 4; ++t) {
-          sgm.dh[t] = ut.dh[t]; sgm.dw[t] = ut.dw[t];
-          if (ut.dh[t] < 0) sgm.ht = 1;
-          if (ut.dh[t] > 0) sgm.hb = 1;
-          if (ut.dw[t] < 0) sgm.hl = 1;
-          if (ut.dw[t] > 0) sgm.hr = 1;
-        }
-        p.bias = P(nm + ".bias");
-        p.temb = nullptr; p.temb_stride = 0;
-        plan->push_back(op);
+        seg(p.seg[0], x, k.seg[pa * 2 + pb], taps_up2(pa, pb));
+        p.bias = P(k.name + ".bias");
+        ops->push_back(op);
       }
-    h->taps[nm] = y;
+    built->taps[k.name] = y;
     return y;
   }
 
-  Act attention(const std::string& n, const Act& x, bool out_pooled, const std::string& out_tag) {
+  Act attention(const Block& k, const Act& x) {
+    const std::string& n = k.name;
     const int C = x.C, H = x.H, W = x.W;
     // The q/k/v projection is a 1-tap conv with 3C/128 (= 12) cout tiles: fused, every one of those tiles would re-normalise
     // the same window in its transform warps, and a 1-tap k-step (192 MMA cycles) cannot hide that (measured 187 us per
@@ -663,46 +753,172 @@ struct Builder {
       g.gamma = P(n + ".group_norm.weight"); g.beta = P(n + ".group_norm.bias");
       g.dst = xn.p;
       g.N = N; g.H = H; g.W = W; g.groups = h->norm_groups; g.eps = h->norm_eps; g.silu = 0;
-      plan->push_back(op);
+      ops->push_back(op);
     }
     Act qkv = pooled("qkv", 3 * C, H, W, false);
-    {
-      Op op{};
-      op.kind = OP_CONV;
-      ConvParams& p = op.conv;
-      conv_common(p, qkv);
-      p.nseg = 1;
-      set_seg(p.seg[0], xn.p, C, H, W, WP(n + ".qkv#q"), taps_1x1());  // q|k|v blocks are contiguous
-      p.bias = MISC(n + ".bias_qkv");
-      p.temb = nullptr; p.temb_stride = 0; p.stats = nullptr;
-      plan->push_back(op);
-    }
+    linear(qkv, xn, k.qkv, PK<float>(k.bias));   // q|k|v blocks are contiguous
     Act ao = pooled("attn_o", C, H, W, false);
     {
       Op op{};
       op.kind = single_head ? OP_ATTN1 : OP_ATTN;
       op.src = qkv.p; op.dst = ao.p; op.C = C; op.H = H; op.W = W;
       if (single_head) op.f0 = (float*)ws.take((size_t)N * H * W * H * W * sizeof(float));
-      plan->push_back(op);
+      ops->push_back(op);
     }
-    Act out = out_pooled ? pooled(out_tag, C, H, W, true) : alloc(C, H, W, true);
+    Act out = output(k, C, H, W);
+    linear(out, ao, k.out, P(n + ".to_out.0.bias"), nullptr, &x, k.ident);   // + residual
+    built->taps[n + ".qkv"] = qkv;
+    built->taps[n + ".ao"] = ao;
+    built->taps[n] = out;
+    return out;
+  }
+
+  // conv_norm_out + SiLU + conv_out, fused with the scheduler update; the GroupNorm is finalised by the last conv's last
+  // CTA (null: in conv_out)
+  Act conv_out(const Block& k, const Act& x) {
+    const std::string& n = k.name;
+    Op op{};
+    op.kind = OP_CONV_OUT;
+    ConvOutParams& p = op.co;
+    p.src = x.p; p.stats = x.stats;
+    p.ss = gn_attach(x, nullptr, n + "conv_norm_out");
+    p.gamma = P(n + "conv_norm_out.weight"); p.beta = P(n + "conv_norm_out.bias");
+    p.w = P(n + "conv_out.weight"); p.b = P(n + "conv_out.bias");
+    p.N = N; p.C = x.C; p.H = x.H; p.W = x.W; p.cout = k.cout; p.groups = h->norm_groups; p.eps = h->norm_eps;
+    ops->push_back(op);
+    built->taps[n + "pre_out"] = x;
+    return x;
+  }
+
+  // conv_norm_out + SiLU + conv_out on the tensor cores (output padded to 128 channels), then quant_conv + sampling
+  Act latent_out(const Block& k, const Act& x) {
+    const std::string& n = k.name;
+    Act eo = pooled("enc_out", 128, x.H, x.W, false);
     {
+      const float2* ss = gn_finalize(x, nullptr, n + "conv_norm_out");
       Op op{};
       op.kind = OP_CONV;
       ConvParams& p = op.conv;
-      conv_common(p, out);
-      p.nseg = 2;
-      set_seg(p.seg[0], ao.p, C, H, W, WP(n + ".out#0"), taps_1x1());
-      set_seg(p.seg[1], x.p, C, H, W, IDENT(C), taps_1x1());          // + residual
-      p.bias = P(n + ".to_out.0.bias");
-      p.temb = nullptr; p.temb_stride = 0;
-      plan->push_back(op);
+      conv_common(p, eo);
+      p.nseg = 1;
+      seg(p.seg[0], x, k.seg[0], taps_conv(3));
+      seg_norm(p.seg[0], ss, x.C, true);
+      p.bias = PK<float>(k.bias);
+      ops->push_back(op);
     }
-    h->taps[n + ".qkv"] = qkv;
-    h->taps[n + ".ao"] = ao;
-    h->taps[n] = out;
-    return out;
+    built->taps[n + "conv_out"] = eo;
+    Op op{};
+    op.kind = OP_VAE_SAMPLE;
+    op.src = eo.p; op.C = 128; op.H = x.H; op.W = x.W; op.cin = k.cout / 2;
+    op.fw = P("quant_conv.weight"); op.fb = P("quant_conv.bias");
+    ops->push_back(op);
+    return eo;
+  }
+
+  // Appends the plan of a block list.
+  void run(const std::vector<Block>& blocks) {
+    std::vector<Act> outs(blocks.size());
+    for (size_t i = 0; i < blocks.size(); ++i) {
+      const Block& k = blocks[i];
+      const Act* x = k.in >= 0 ? &outs[k.in] : nullptr;
+      const Act* skip = k.skip >= 0 ? &outs[k.skip] : nullptr;
+      switch (k.kind) {
+        case BK_UNET_HEAD: outs[i] = unet_head(k); break;
+        case BK_CONV_IN: outs[i] = conv_in(k, nullptr); break;
+        case BK_LATENT_IN: outs[i] = latent_in(k); break;
+        case BK_RESNET: outs[i] = resnet(k, *x, skip); break;
+        case BK_ATTN: outs[i] = attention(k, *x); break;
+        case BK_TRANSFORMER: outs[i] = transformer(k, *x); break;
+        case BK_DOWN: case BK_DOWN_ASYM: outs[i] = down2(k, *x); break;
+        case BK_UP: outs[i] = up2(k, *x); break;
+        case BK_CONV_OUT: outs[i] = conv_out(k, *x); break;
+        case BK_LATENT_OUT: outs[i] = latent_out(k, *x); break;
+      }
+    }
   }
 };
+
+static bool debug_nopool() {
+  const char* e = getenv("B200AD_DEBUG_NOPOOL");
+  return e && e[0] == '1';
+}
+
+// ================================================================================= plan executor
+struct RunArgs {                        // the per-call inputs of a plan
+  const float* in = nullptr;            // U-Net: the sample x; autoencoder: the image (encode) or the latents (decode)
+  const float* t = nullptr;             // U-Net: timesteps [N]
+  const float* noise = nullptr;         // U-Net: the scheduler's noise z; autoencoder encode: the sampling noise
+  float* out = nullptr;                 // U-Net: eps (optional); autoencoder: z (encode) or the image (decode)
+  float* moments = nullptr;             // autoencoder encode (optional)
+  float* x_out = nullptr;               // U-Net: the scheduler update (optional), with coef or coef_dev
+  const b200ad_step_coef* coef = nullptr;
+  const b200ad_step_coef* coef_dev = nullptr;
+};
+
+static int run_ops(NetBase* h, const OpList& l, const RunArgs& a, cudaStream_t st) {
+  const Plan& pl = h->plan;
+  int launches = 0;
+  CK(cudaMemsetAsync(l.stats, 0, l.stats_bytes, st));
+  for (const Op& op : l.ops) {
+    switch (op.kind) {
+      case OP_TEMB:      // two launches: the MLP, then every resnet's projection
+        CK(launch_temb(a.t, h->N, op.C, h->pptr[h->pidx.at("time_embedding.linear_1.weight")],
+                       h->pptr[h->pidx.at("time_embedding.linear_1.bias")],
+                       h->pptr[h->pidx.at("time_embedding.linear_2.weight")],
+                       h->pptr[h->pidx.at("time_embedding.linear_2.bias")], pl.temb_act,
+                       (const float*)(h->packed + h->off_wcat), (const float*)(h->packed + h->off_bcat), h->temb_rows,
+                       pl.temb_proj, st, h->training ? pl.temb_emb : nullptr, h->training ? pl.temb_u1 : nullptr,
+                       h->training ? pl.temb_u2 : nullptr, h->training ? nullptr : pl.temb_lead));
+        launches += 1;
+        break;
+      case OP_CONV_IN:
+        CK(launch_conv_in(op.f0 ? op.f0 : a.in, op.fw, op.fb, h->N, op.cin, op.H, op.W, op.C, op.dst, op.conv.stats, st));
+        break;
+      case OP_GN: CK(launch_gn_finalize(op.gn, op.ss, st)); break;
+      case OP_GNAPPLY: CK(launch_gn_apply(op.gn, st)); break;
+      case OP_CONV: CK(launch_conv_tc(op.conv, h->num_sms, st)); break;
+      case OP_PARITY: CK(launch_parity_split(op.src, op.dst, h->N, op.C, op.H, op.W, st)); break;
+      case OP_ATTN: CK(launch_attention(op.src, op.dst, h->N, op.C, op.H, op.W, st)); break;
+      case OP_ATTN1:     // three launches: scores, softmax, output
+        CK(launch_attention_1head(op.src, op.dst, op.f0, h->N, op.C, op.H, op.W, st));
+        launches += 2;
+        break;
+      case OP_LN: CK(launch_layernorm_pf8(op.src, op.dst, op.fw, op.fb, h->N, op.C, op.H, op.W, op.eps, st)); break;
+      case OP_GEGLU: CK(launch_geglu_pf8(op.src, op.dst, h->N, op.C, op.H, op.W, st)); break;
+      case OP_MHA: CK(launch_mha_flash(op.src, op.dst, h->N, op.C, op.cin, op.H, op.W, st)); break;
+      case OP_XVEC:
+        if (!h->enc) return set_err("conditional U-Net: call b200ad_unet_set_encoding before forward");
+        if (h->enc_S != 1) return set_err("conditional U-Net: encoder sequence length %d (only 1 is implemented)", h->enc_S);
+        CK(launch_cross_attn_vec(h->enc, op.fw, op.fb, op.fc, op.f1, h->N, op.C, op.cin, st));
+        break;
+      case OP_VAE_SAMPLE:
+        CK(launch_vae_sample(op.src, op.fw, op.fb, a.noise, a.out, a.moments, h->N, op.C, op.cin, op.H, op.W, st));
+        break;
+      case OP_MIX1X1: CK(launch_mix1x1(a.in, op.fw, op.fb, op.f0, h->N, op.C, op.H * op.W, st)); break;
+      case OP_CONV_OUT: {
+        ConvOutParams p = op.co;
+        p.eps_out = a.out;
+        p.x = a.in; p.z = a.noise; p.x_out = a.x_out;
+        static_assert(sizeof(b200ad_step_coef) == sizeof(StepCoef), "step-coefficient layouts differ");
+        p.coef_dev = reinterpret_cast<const StepCoef*>(a.coef_dev);
+        if (a.coef) memcpy(&p.coef, a.coef, sizeof(StepCoef));
+        CK(launch_conv_out(p, st));
+        break;
+      }
+    }
+    ++launches;
+  }
+  h->last_launches = launches;
+  return 0;
+}
+
+static int debug_tensor(const NetBase* h, const char* name, float* dst, int* dims, cudaStream_t st) {
+  auto it = h->plan.taps.find(name);
+  if (it == h->plan.taps.end()) return set_err("unknown tap '%s'", name);
+  const Act& a = it->second;
+  if (dims) { dims[0] = a.C; dims[1] = a.H; dims[2] = a.W; }
+  if (dst) CK(launch_pf8_to_nchw(a.p, dst, h->N, a.C, a.H, a.W, st));
+  return a.C;
+}
 
 }  // namespace b200ad

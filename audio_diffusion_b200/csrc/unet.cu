@@ -21,107 +21,52 @@ using namespace b200ad;
 
 namespace b200ad {
 
-static void build_param_table(b200ad_unet* h) {
-  const b200ad_unet_config& c = h->cfg;
-  const int nb = c.num_blocks, temb = c.block_out_channels[0] * 4;
-  p_conv(h, "conv_in", c.in_channels, c.block_out_channels[0], 3);
-  p_lin(h, "time_embedding.linear_1", c.block_out_channels[0], temb);
-  p_lin(h, "time_embedding.linear_2", temb, temb);
-  int out_c = c.block_out_channels[0];
+// UNet2DModel.forward as a block list: conv_in, down blocks (each output a skip connection), mid block, up blocks (each
+// resnet consuming one skip, last first), conv_out.  The pool tags decide which outputs may share a buffer: a resnet
+// followed by attention writes the transient "res_tmp"; the up path alternates "up_a" / "up_b".
+static std::vector<Block> unet_blocks(const b200ad_unet_config& c) {
+  const int nb = c.num_blocks, D = c.block_out_channels[0] * 4, X = c.cross_attention_dim;
+  const int* boc = c.block_out_channels;
+  std::vector<Block> bl;
+  add_block(bl, BK_UNET_HEAD, "", c.in_channels, boc[0], "").temb = D;
+  std::vector<int> skips{0};
+  auto attn = [&](const std::string& n, bool self, bool cross, int ch, const char* pool) {
+    if (self || cross) add_block(bl, cross ? BK_TRANSFORMER : BK_ATTN, n, ch, ch, pool).cross = cross ? X : 0;
+  };
   for (int i = 0; i < nb; ++i) {
-    int in_c = out_c;
-    out_c = c.block_out_channels[i];
     for (int j = 0; j < c.layers_per_block; ++j) {
-      p_resnet(h, S("down_blocks.%d.resnets.%d", i, j), j == 0 ? in_c : out_c, out_c, temb);
-      if (c.down_attn[i]) p_attn(h, S("down_blocks.%d.attentions.%d", i, j), out_c);
-      if (c.down_cross[i]) p_transformer(h, S("down_blocks.%d.attentions.%d", i, j), out_c, c.cross_attention_dim);
-    }
-    if (i != nb - 1) p_conv(h, S("down_blocks.%d.downsamplers.0.conv", i), out_c, out_c, 3);
-  }
-  const int mid = c.block_out_channels[nb - 1];
-  p_resnet(h, "mid_block.resnets.0", mid, mid, temb);
-  if (c.cross_attention_dim) p_transformer(h, "mid_block.attentions.0", mid, c.cross_attention_dim);
-  else p_attn(h, "mid_block.attentions.0", mid);
-  p_resnet(h, "mid_block.resnets.1", mid, mid, temb);
-  out_c = c.block_out_channels[nb - 1];
-  for (int i = 0; i < nb; ++i) {
-    const int prev_c = out_c;
-    out_c = c.block_out_channels[nb - 1 - i];
-    const int in_c = c.block_out_channels[nb - 1 - (i + 1 < nb ? i + 1 : nb - 1)];
-    const int n = c.layers_per_block + 1;
-    for (int j = 0; j < n; ++j) {
-      const int skip_c = (j == n - 1) ? in_c : out_c;
-      const int res_in = (j == 0) ? prev_c : out_c;
-      p_resnet(h, S("up_blocks.%d.resnets.%d", i, j), res_in + skip_c, out_c, temb);
-      if (c.up_attn[i]) p_attn(h, S("up_blocks.%d.attentions.%d", i, j), out_c);
-      if (c.up_cross[i]) p_transformer(h, S("up_blocks.%d.attentions.%d", i, j), out_c, c.cross_attention_dim);
-    }
-    if (i != nb - 1) p_conv(h, S("up_blocks.%d.upsamplers.0.conv", i), out_c, out_c, 3);
-  }
-  p_gn(h, "conv_norm_out", c.block_out_channels[0]);
-  p_conv(h, "conv_out", c.block_out_channels[0], c.out_channels, 3);
-}
-
-
-static void build_packed_layout(b200ad_unet* h) {
-  const b200ad_unet_config& c = h->cfg;
-  const int nb = c.num_blocks;
-  Bump b;
-  b.base = nullptr;
-  h->jobs.clear();
-  h->temb_rows = 0;
-  int out_c = c.block_out_channels[0];
-  std::vector<int> skip_c{out_c};
-  h->ident_off.clear();
-  auto resnet = [&](const std::string& n, int ca, int cb, int co) { layout_resnet(h, b, n, ca, cb, co, true); };
-  auto attn = [&](const std::string& n, int ch) { layout_attn(h, b, n, ch); };
-  auto xattn = [&](const std::string& n, int ch) { layout_transformer(h, b, n, ch); };
-  for (int i = 0; i < nb; ++i) {
-    const int in_c = out_c;
-    out_c = c.block_out_channels[i];
-    for (int j = 0; j < c.layers_per_block; ++j) {
-      resnet(S("down_blocks.%d.resnets.%d", i, j), j == 0 ? in_c : out_c, 0, out_c);
-      if (c.down_attn[i]) attn(S("down_blocks.%d.attentions.%d", i, j), out_c);
-      if (c.down_cross[i]) xattn(S("down_blocks.%d.attentions.%d", i, j), out_c);
-      skip_c.push_back(out_c);
+      const bool att = c.down_attn[i] || c.down_cross[i];
+      add_block(bl, BK_RESNET, S("down_blocks.%d.resnets.%d", i, j), bl.back().cout, boc[i], att ? "res_tmp" : "").temb = D;
+      attn(S("down_blocks.%d.attentions.%d", i, j), c.down_attn[i], c.down_cross[i], boc[i], "");
+      skips.push_back((int)bl.size() - 1);
     }
     if (i != nb - 1) {
-      const std::string n = S("down_blocks.%d.downsamplers.0.conv", i);
-      for (int a = 0; a < 2; ++a)
-        for (int bb = 0; bb < 2; ++bb)
-          add_job(h, b, n + S("#%d", a * 2 + bb), n + ".weight", out_c, out_c, 3, 0, out_c, taps_parity(a, bb));
-      skip_c.push_back(out_c);
+      add_block(bl, BK_DOWN, S("down_blocks.%d.downsamplers.0.conv", i), boc[i], boc[i], "");
+      skips.push_back((int)bl.size() - 1);
     }
   }
-  const int mid = c.block_out_channels[nb - 1];
-  resnet("mid_block.resnets.0", mid, 0, mid);
-  if (c.cross_attention_dim) xattn("mid_block.attentions.0", mid);
-  else attn("mid_block.attentions.0", mid);
-  resnet("mid_block.resnets.1", mid, 0, mid);
-  out_c = mid;
+  const int mid = boc[nb - 1];
+  add_block(bl, BK_RESNET, "mid_block.resnets.0", mid, mid, "res_tmp").temb = D;
+  attn("mid_block.attentions.0", !X, X != 0, mid, "up_a");
+  add_block(bl, BK_RESNET, "mid_block.resnets.1", mid, mid, "up_b").temb = D;
+  int flip = 0;
   for (int i = 0; i < nb; ++i) {
-    const int prev_c = out_c;
-    out_c = c.block_out_channels[nb - 1 - i];
-    const int n = c.layers_per_block + 1;
-    for (int j = 0; j < n; ++j) {
-      const int sc = skip_c.back();
-      skip_c.pop_back();
-      const int res_in = (j == 0) ? prev_c : out_c;
-      resnet(S("up_blocks.%d.resnets.%d", i, j), res_in, sc, out_c);
-      if (c.up_attn[i]) attn(S("up_blocks.%d.attentions.%d", i, j), out_c);
-      if (c.up_cross[i]) xattn(S("up_blocks.%d.attentions.%d", i, j), out_c);
+    const int out_c = boc[nb - 1 - i];
+    for (int j = 0; j < c.layers_per_block + 1; ++j) {
+      const bool att = c.up_attn[i] || c.up_cross[i];
+      const int sk = skips.back();
+      skips.pop_back();
+      Block& r = add_block(bl, BK_RESNET, S("up_blocks.%d.resnets.%d", i, j), bl.back().cout, out_c,
+                           att ? "res_tmp" : (flip++ & 1) ? "up_b" : "up_a");
+      r.skip = sk;
+      r.cskip = bl[sk].cout;
+      r.temb = D;
+      if (att) attn(S("up_blocks.%d.attentions.%d", i, j), c.up_attn[i], c.up_cross[i], out_c, (flip++ & 1) ? "up_b" : "up_a");
     }
-    if (i != nb - 1) {
-      const std::string nm = S("up_blocks.%d.upsamplers.0.conv", i);
-      for (int pa = 0; pa < 2; ++pa)
-        for (int pb = 0; pb < 2; ++pb)
-          add_job(h, b, nm + S("#p%d", pa * 2 + pb), nm + ".weight", out_c, out_c, 3, 0, out_c, taps_up2(pa, pb).pack);
-    }
+    if (i != nb - 1) add_block(bl, BK_UP, S("up_blocks.%d.upsamplers.0.conv", i), out_c, out_c, "up_conv");
   }
-  const int D = c.block_out_channels[0] * 4;
-  h->off_wcat = take_off(b, (size_t)h->temb_rows * D * 4);
-  h->off_bcat = take_off(b, (size_t)h->temb_rows * 4);
-  h->packed_bytes = (b.off + 255) & ~(size_t)255;
+  add_block(bl, BK_CONV_OUT, "", boc[0], c.out_channels, "");
+  return bl;
 }
 
 }  // namespace b200ad
@@ -149,8 +94,14 @@ extern "C" int b200ad_unet_create(const b200ad_unet_config* cfg, b200ad_unet** o
   h->cfg = *cfg;
   h->norm_groups = cfg->norm_num_groups;
   h->norm_eps = cfg->norm_eps;
-  build_param_table(h);
-  build_packed_layout(h);
+  h->blocks = unet_blocks(*cfg);
+  for (const Block& k : h->blocks) p_block(h, k);
+  Bump b;
+  for (Block& k : h->blocks) layout_block(h, b, k);
+  const int D = cfg->block_out_channels[0] * 4;
+  h->off_wcat = take_off(b, (size_t)h->temb_rows * D * 4);
+  h->off_bcat = take_off(b, (size_t)h->temb_rows * 4);
+  h->packed_bytes = (b.off + 255) & ~(size_t)255;
   h->pptr.assign(h->params.size(), nullptr);
   *out = h;
   return 0;
@@ -178,13 +129,13 @@ extern "C" int b200ad_unet_set_params(b200ad_unet* h, const float* const* params
   if (pack_common(h, st)) return -1;
   // concatenated time_emb_proj weights / biases
   const int D = h->cfg.block_out_channels[0] * 4;
-  for (const auto& kv : h->temb_row_off) {
-    const int co = (int)h->params[h->pidx.at(kv.first + ".time_emb_proj.bias")].shape[0];
-    CK(cudaMemcpyAsync(h->packed + h->off_wcat + (size_t)kv.second * D * 4,
-                       h->pptr[h->pidx.at(kv.first + ".time_emb_proj.weight")], (size_t)co * D * 4,
+  for (const Block& k : h->blocks) {
+    if (k.temb_row < 0) continue;
+    CK(cudaMemcpyAsync(h->packed + h->off_wcat + (size_t)k.temb_row * D * 4,
+                       h->pptr[h->pidx.at(k.name + ".time_emb_proj.weight")], (size_t)k.cout * D * 4,
                        cudaMemcpyDeviceToDevice, st));
-    CK(cudaMemcpyAsync(h->packed + h->off_bcat + (size_t)kv.second * 4,
-                       h->pptr[h->pidx.at(kv.first + ".time_emb_proj.bias")], (size_t)co * 4, cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(h->packed + h->off_bcat + (size_t)k.temb_row * 4,
+                       h->pptr[h->pidx.at(k.name + ".time_emb_proj.bias")], (size_t)k.cout * 4, cudaMemcpyDeviceToDevice, st));
   }
   return 0;
 }
@@ -192,150 +143,46 @@ extern "C" int b200ad_unet_set_params(b200ad_unet* h, const float* const* params
 // ================================================================================= plan builder
 namespace b200ad {
 
-static int build_plan(b200ad_unet* h, uint8_t* ws_base, int N, int H, int W, size_t* ws_bytes_out) {
-  const b200ad_unet_config& c = h->cfg;
-  const int nb = c.num_blocks;
-  std::vector<Op> plan;
+// Two passes: the stats arena lives at the start of the workspace; its size is found by a dry run.
+static Plan build_plan(const b200ad_unet* h, uint8_t* ws_base, int N, int H, int W) {
+  Plan pl;
+  pl.lists.resize(1);
+  OpList& l = pl.lists[0];
   Builder B;
-  B.h = h; B.N = N; B.plan = &plan;
-  {
-    const char* e = getenv("B200AD_DEBUG_NOPOOL");
-    B.nopool = (e && e[0] == '1') || h->training;
-  }
+  B.h = h; B.built = &pl; B.ops = &l.ops;
+  B.N = N; B.H = H; B.W = W;
+  B.heads = h->cfg.attention_head_dim;
+  B.nopool = debug_nopool() || h->training;
   B.ws.base = ws_base;
-  // two-pass: the stats arena lives at the start of the workspace; its size is found by a dry run
-  size_t stats_bytes = 0;
   for (int pass = 0; pass < 2; ++pass) {
-    plan.clear();
+    l.ops.clear();
     B.pool.clear();
-    h->taps.clear();
-    B.ws.off = 0;
+    pl.taps.clear();
+    B.st.base = pass == 0 ? nullptr : ws_base;
     B.st.off = 0;
-    B.st.base = ws_base;  // stats arena first
-    B.ws.off = (pass == 0) ? 0 : ((stats_bytes + 255) & ~(size_t)255);
-    if (pass == 0) B.st.base = nullptr;
-    const int D = c.block_out_channels[0] * 4;
-    h->temb_act = (float*)B.ws.take((size_t)N * D * 4);
-    h->temb_proj = (float*)B.ws.take((size_t)N * h->temb_rows * 4);
-    h->temb_lead = (int*)B.ws.take((size_t)N * 4);
-    if (h->training) {
-      h->temb_emb = (float*)B.ws.take((size_t)N * c.block_out_channels[0] * 4);
-      h->temb_u1 = (float*)B.ws.take((size_t)N * D * 4);
-      h->temb_u2 = (float*)B.ws.take((size_t)N * D * 4);
-    }
-    {
-      Op op{};
-      op.kind = OP_TEMB;
-      plan.push_back(op);
-    }
-    int out_c = c.block_out_channels[0];
-    int hh = H, ww = W;
-    Act x = B.alloc(out_c, hh, ww, true);
-    {
-      Op op{};
-      op.kind = OP_CONV_IN;
-      op.dst = x.p; op.C = out_c; op.H = hh; op.W = ww;
-      op.conv.stats = x.stats;
-      plan.push_back(op);
-    }
-    h->taps["conv_in"] = x;
-    std::vector<Act> skips{x};
-    const int heads = c.attention_head_dim, X = c.cross_attention_dim;
-    for (int i = 0; i < nb; ++i) {
-      out_c = c.block_out_channels[i];
-      for (int j = 0; j < c.layers_per_block; ++j) {
-        const std::string rn = S("down_blocks.%d.resnets.%d", i, j);
-        const std::string an = S("down_blocks.%d.attentions.%d", i, j);
-        if (c.down_attn[i] || c.down_cross[i]) {
-          Act r = B.resnet(rn, x, nullptr, out_c, true, "res_tmp");
-          x = c.down_cross[i] ? B.transformer(an, r, heads, X, false, "") : B.attention(an, r, false, "");
-        } else {
-          x = B.resnet(rn, x, nullptr, out_c, false, "");
-        }
-        skips.push_back(x);
-      }
-      if (i != nb - 1) {
-        x = B.down2(S("down_blocks.%d.downsamplers.0.conv", i), x);
-        hh /= 2; ww /= 2;
-        skips.push_back(x);
-      }
-    }
-    x = B.resnet("mid_block.resnets.0", x, nullptr, out_c, true, "res_tmp");
-    x = X ? B.transformer("mid_block.attentions.0", x, heads, X, true, "up_a") : B.attention("mid_block.attentions.0", x, true, "up_a");
-    x = B.resnet("mid_block.resnets.1", x, nullptr, out_c, true, "up_b");
-    int flip = 0;
-    for (int i = 0; i < nb; ++i) {
-      out_c = c.block_out_channels[nb - 1 - i];
-      const int n = c.layers_per_block + 1;
-      for (int j = 0; j < n; ++j) {
-        Act sk = skips.back();
-        skips.pop_back();
-        const std::string rn = S("up_blocks.%d.resnets.%d", i, j);
-        const std::string an = S("up_blocks.%d.attentions.%d", i, j);
-        if (c.up_attn[i] || c.up_cross[i]) {
-          Act r = B.resnet(rn, x, &sk, out_c, true, "res_tmp");
-          const char* tag = (flip++ & 1) ? "up_b" : "up_a";
-          x = c.up_cross[i] ? B.transformer(an, r, heads, X, true, tag) : B.attention(an, r, true, tag);
-        } else {
-          x = B.resnet(rn, x, &sk, out_c, true, (flip++ & 1) ? "up_b" : "up_a");
-        }
-      }
-      if (i != nb - 1) {
-        x = B.up2(S("up_blocks.%d.upsamplers.0.conv", i), x);
-        hh *= 2; ww *= 2;
-      }
-    }
-    {
-      Op op{};
-      op.kind = OP_CONV_OUT;
-      ConvOutParams& p = op.co;
-      p.src = x.p; p.stats = x.stats;
-      p.ss = B.gn_attach(x, "conv_norm_out");     // finalised by the last up-block conv's last CTA (null: in conv_out)
-      p.gamma = B.P("conv_norm_out.weight"); p.beta = B.P("conv_norm_out.bias");
-      p.w = B.P("conv_out.weight"); p.b = B.P("conv_out.bias");
-      p.N = N; p.C = x.C; p.H = hh; p.W = ww; p.cout = c.out_channels; p.groups = c.norm_num_groups; p.eps = c.norm_eps;
-      plan.push_back(op);
-    }
-    h->taps["pre_out"] = x;
-    if (pass == 0) stats_bytes = B.st.off;
+    B.ws.off = pass == 0 ? 0 : ((l.stats_bytes + 255) & ~(size_t)255);
+    B.run(h->blocks);
+    if (pass == 0) l.stats_bytes = B.st.off;
   }
-  if (ws_bytes_out) *ws_bytes_out = (B.ws.off + 255) & ~(size_t)255;
-  if (ws_base) {
-    h->plan = plan;
-    h->stats_arena = (stat_t*)ws_base;
-    h->stats_bytes = stats_bytes;
-  }
-  return 0;
+  l.stats = (stat_t*)ws_base;
+  pl.ws_bytes = (B.ws.off + 255) & ~(size_t)255;
+  return pl;
 }
 
 }  // namespace b200ad
 
-extern "C" size_t b200ad_unet_workspace_bytes(const b200ad_unet* hc, int N, int H, int W) {
-  b200ad_unet* h = const_cast<b200ad_unet*>(hc);
-  // dry run on a scratch copy of the mutable plan state
-  auto saved_plan = h->plan;
-  auto saved_taps = h->taps;
-  stat_t* sa = h->stats_arena; size_t sb = h->stats_bytes; float* ta = h->temb_act; float* tp = h->temb_proj; int* tl = h->temb_lead;
-  float* te = h->temb_emb; float* tu1 = h->temb_u1; float* tu2 = h->temb_u2;
-  uint8_t* saved_packed = h->packed;
-  std::vector<const float*> saved_pptr = h->pptr;
-  size_t bytes = 0;
-  build_plan(h, nullptr, N, H, W, &bytes);
-  h->plan = saved_plan; h->taps = saved_taps; h->stats_arena = sa; h->stats_bytes = sb; h->temb_act = ta; h->temb_proj = tp; h->temb_lead = tl;
-  h->packed = saved_packed; h->pptr = saved_pptr;
-  h->temb_emb = te; h->temb_u1 = tu1; h->temb_u2 = tu2;
-  return bytes;
+extern "C" size_t b200ad_unet_workspace_bytes(const b200ad_unet* h, int N, int H, int W) {
+  return build_plan(h, nullptr, N, H, W).ws_bytes;
 }
 
 extern "C" int b200ad_unet_bind_workspace(b200ad_unet* h, void* workspace, size_t bytes, int N, int H, int W, void* stream) {
   if (!h->packed) return set_err("set_params must be called before bind_workspace");
   const int down = 1 << (h->cfg.num_blocks - 1);
   if (H % down || W % down) return set_err("H and W must be multiples of %d", down);
-  size_t need = 0;
-  build_plan(h, nullptr, N, H, W, &need);
+  const size_t need = build_plan(h, nullptr, N, H, W).ws_bytes;
   if (bytes < need) return set_err("workspace too small: %zu < %zu", bytes, need);
   CK(cudaMemsetAsync(workspace, 0, need, (cudaStream_t)stream));
-  build_plan(h, (uint8_t*)workspace, N, H, W, &need);
+  h->plan = build_plan(h, (uint8_t*)workspace, N, H, W);
   h->N = N; h->H = H; h->W = W;
   h->ws = (uint8_t*)workspace; h->ws_bytes = need;
   int dev = 0;
@@ -344,118 +191,34 @@ extern "C" int b200ad_unet_bind_workspace(b200ad_unet* h, void* workspace, size_
   return 0;
 }
 
-static int run_plan(b200ad_unet* h, const float* x, const float* t, const float* z, const b200ad_step_coef* coef,
-                    float* x_out, float* eps_out, cudaStream_t st, const b200ad_step_coef* coef_dev = nullptr) {
-  if (h->plan.empty()) return set_err("bind_workspace must be called before forward");
-  const b200ad_unet_config& c = h->cfg;
-  int launches = 0;
-  CK(cudaMemsetAsync(h->stats_arena, 0, h->stats_bytes, st));
-  for (Op& op : h->plan) {
-    switch (op.kind) {
-      case OP_TEMB: {
-        const int d0 = c.block_out_channels[0];
-        CK(launch_temb(t, h->N, d0, h->pptr[h->pidx.at("time_embedding.linear_1.weight")],
-                       h->pptr[h->pidx.at("time_embedding.linear_1.bias")],
-                       h->pptr[h->pidx.at("time_embedding.linear_2.weight")],
-                       h->pptr[h->pidx.at("time_embedding.linear_2.bias")], h->temb_act,
-                       (const float*)(h->packed + h->off_wcat), (const float*)(h->packed + h->off_bcat), h->temb_rows,
-                       h->temb_proj, st, h->training ? h->temb_emb : nullptr, h->training ? h->temb_u1 : nullptr,
-                       h->training ? h->temb_u2 : nullptr, h->training ? nullptr : h->temb_lead));
-        launches += 2;
-        break;
-      }
-      case OP_CONV_IN:
-        CK(launch_conv_in(x, h->pptr[h->pidx.at("conv_in.weight")], h->pptr[h->pidx.at("conv_in.bias")], h->N,
-                          c.in_channels, op.H, op.W, op.C, op.dst, op.conv.stats, st));
-        ++launches;
-        break;
-      case OP_GN:
-        CK(launch_gn_finalize(op.gn, op.ss, st));
-        ++launches;
-        break;
-      case OP_GNAPPLY:
-        CK(launch_gn_apply(op.gn, st));
-        ++launches;
-        break;
-      case OP_CONV:
-        CK(launch_conv_tc(op.conv, h->num_sms, st));
-        ++launches;
-        break;
-      case OP_UPSAMPLE:
-        CK(launch_upsample2x(op.src, op.dst, h->N, op.C, op.H, op.W, st));
-        ++launches;
-        break;
-      case OP_PARITY:
-        CK(launch_parity_split(op.src, op.dst, h->N, op.C, op.H, op.W, st));
-        ++launches;
-        break;
-      case OP_ATTN:
-        CK(launch_attention(op.src, op.dst, h->N, op.C, op.H, op.W, st));
-        ++launches;
-        break;
-      case OP_LN:
-        CK(launch_layernorm_pf8(op.src, op.dst, op.fw, op.fb, h->N, op.C, op.H, op.W, op.eps, st));
-        ++launches;
-        break;
-      case OP_GEGLU:
-        CK(launch_geglu_pf8(op.src, op.dst, h->N, op.C, op.H, op.W, st));
-        ++launches;
-        break;
-      case OP_MHA:
-        CK(launch_mha_flash(op.src, op.dst, h->N, op.C, op.cin, op.H, op.W, st));
-        ++launches;
-        break;
-      case OP_XVEC:
-        if (!h->enc) return set_err("conditional U-Net: call b200ad_unet_set_encoding before forward");
-        if (h->enc_S != 1) return set_err("conditional U-Net: encoder sequence length %d (only 1 is implemented)", h->enc_S);
-        CK(launch_cross_attn_vec(h->enc, op.fw, op.fb, op.fc, op.f1, h->N, op.C, op.cin, st));
-        ++launches;
-        break;
-      case OP_CONV_OUT: {
-        ConvOutParams p = op.co;
-        p.eps_out = eps_out;
-        p.x = x; p.z = z; p.x_out = x_out;
-        static_assert(sizeof(b200ad_step_coef) == sizeof(StepCoef), "step-coefficient layouts differ");
-        p.coef_dev = reinterpret_cast<const StepCoef*>(coef_dev);
-        if (coef) {
-          p.coef.sqrt_1m_at = coef->sqrt_1m_at; p.coef.inv_sqrt_at = coef->inv_sqrt_at; p.coef.clip = coef->clip;
-          p.coef.c_x0 = coef->c_x0; p.coef.c_xt = coef->c_xt; p.coef.c_eps = coef->c_eps; p.coef.c_z = coef->c_z;
-          p.coef.do_clip = coef->do_clip;
-        }
-        CK(launch_conv_out(p, st));
-        ++launches;
-        break;
-      }
-    }
-  }
-  h->last_launches = launches;
-  return 0;
+static int run_plan(b200ad_unet* h, const RunArgs& a, cudaStream_t st) {
+  if (h->plan.lists.empty()) return set_err("bind_workspace must be called before forward");
+  return run_ops(h, h->plan.lists[0], a, st);
 }
 
 // One step with a CUDA event pair around every launch of the plan (device time per op, on `stream`).
 extern "C" int b200ad_unet_profile_step(b200ad_unet* h, const float* x, const float* t, const float* z,
                                         const b200ad_step_coef* coef, float* x_out, float* op_ms, int* op_kind,
                                         double* op_flops, int max_ops, void* stream) {
-  if (h->plan.empty()) return set_err("bind_workspace must be called before profile_step");
+  if (h->plan.lists.empty()) return set_err("bind_workspace must be called before profile_step");
   cudaStream_t st = (cudaStream_t)stream;
-  const int nops = (int)h->plan.size();
+  const OpList& l = h->plan.lists[0];
+  const std::vector<Op>& saved = l.ops;
+  const int nops = (int)saved.size();
   if (nops > max_ops) return set_err("profile_step: %d ops > max_ops %d", nops, max_ops);
   std::vector<cudaEvent_t> ev(nops + 1);
   for (auto& e : ev) CK(cudaEventCreate(&e));
-  std::vector<Op> saved = h->plan;
-  CK(cudaMemsetAsync(h->stats_arena, 0, h->stats_bytes, st));
+  CK(cudaMemsetAsync(l.stats, 0, l.stats_bytes, st));
+  RunArgs a;
+  a.in = x; a.t = t; a.noise = z; a.coef = coef; a.x_out = x_out;
+  OpList one;                  // a one-op plan between two events (no stats to clear: stats_bytes 0)
+  one.stats = l.stats;
   for (int i = 0; i < nops; ++i) {
-    // run a one-op plan between two events (the stats memset of run_plan is skipped by clearing stats_bytes)
     CK(cudaEventRecord(ev[i], st));
-    h->plan.assign(1, saved[i]);
-    const size_t sb = h->stats_bytes;
-    h->stats_bytes = 0;
-    const int rc = run_plan(h, x, t, z, coef, x_out, nullptr, st);
-    h->stats_bytes = sb;
-    if (rc) { h->plan = saved; return rc; }
+    one.ops.assign(1, saved[i]);
+    if (const int rc = run_ops(h, one, a, st)) return rc;
   }
   CK(cudaEventRecord(ev[nops], st));
-  h->plan = saved;
   CK(cudaStreamSynchronize(st));
   for (int i = 0; i < nops; ++i) {
     CK(cudaEventElapsedTime(&op_ms[i], ev[i], ev[i + 1]));
@@ -489,12 +252,16 @@ extern "C" int b200ad_unet_set_encoding(b200ad_unet* h, const float* enc, int S)
 }
 
 extern "C" int b200ad_unet_forward(b200ad_unet* h, const float* x, const float* t, float* eps_out, void* stream) {
-  return run_plan(h, x, t, nullptr, nullptr, nullptr, eps_out, (cudaStream_t)stream);
+  RunArgs a;
+  a.in = x; a.t = t; a.out = eps_out;
+  return run_plan(h, a, (cudaStream_t)stream);
 }
 extern "C" int b200ad_unet_forward_step(b200ad_unet* h, const float* x, const float* t, const float* z,
                                         const b200ad_step_coef* coef, float* x_out, float* eps_out, void* stream) {
   if (!coef || !x_out) return set_err("coef and x_out are required");
-  return run_plan(h, x, t, z, coef, x_out, eps_out, (cudaStream_t)stream);
+  RunArgs a;
+  a.in = x; a.t = t; a.noise = z; a.coef = coef; a.x_out = x_out; a.out = eps_out;
+  return run_plan(h, a, (cudaStream_t)stream);
 }
 // per-step scalars -> device (kernel ARGUMENTS are copied at launch time, so the host may run any number of steps ahead)
 __global__ void step_scalars_kernel(b200ad_step_coef coef, float t, b200ad_step_coef* coef_dev, float* t_dev, int n) {
@@ -512,15 +279,12 @@ extern "C" int b200ad_step_scalars_upload(const b200ad_step_coef* coef, float t,
 extern "C" int b200ad_unet_forward_step_dev(b200ad_unet* h, const float* x, const float* t, const float* z,
                                             const b200ad_step_coef* coef_dev, float* x_out, void* stream) {
   if (!coef_dev || !x_out) return set_err("coef_dev and x_out are required");
-  return run_plan(h, x, t, z, nullptr, x_out, nullptr, (cudaStream_t)stream, coef_dev);
+  RunArgs a;
+  a.in = x; a.t = t; a.noise = z; a.coef_dev = coef_dev; a.x_out = x_out;
+  return run_plan(h, a, (cudaStream_t)stream);
 }
 extern "C" int b200ad_unet_last_launch_count(const b200ad_unet* h) { return h->last_launches; }
 
 extern "C" int b200ad_unet_debug_tensor(b200ad_unet* h, const char* name, float* dst, int* dims, void* stream) {
-  auto it = h->taps.find(name);
-  if (it == h->taps.end()) return set_err("unknown tap '%s'", name);
-  const Act& a = it->second;
-  if (dims) { dims[0] = a.C; dims[1] = a.H; dims[2] = a.W; }
-  if (dst) CK(launch_pf8_to_nchw(a.p, dst, h->N, a.C, a.H, a.W, (cudaStream_t)stream));
-  return a.C;
+  return debug_tensor(h, name, dst, dims, (cudaStream_t)stream);
 }

@@ -4,6 +4,7 @@
 
 struct b200ad_unet : b200ad::NetBase {
   b200ad_unet_config cfg;
+  std::vector<b200ad::Block> blocks;
   struct Backward* bwd = nullptr;   // built lazily by b200ad_unet_backward (unet_bwd.cu)
 };
 

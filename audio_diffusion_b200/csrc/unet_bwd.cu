@@ -75,7 +75,6 @@ struct BwdBuilder {
   std::map<std::string, Act> grad;            // gradient w.r.t. a forward tensor (by tap name)
   std::map<std::string, Act> skipgrad;        // contribution of the skip connection to that gradient
   std::map<std::string, Act> pool;
-  std::map<std::string, size_t> toff;         // transposed packed weights
   int N;
   float* cs = nullptr;                        // [N][maxC] channel sums scratch
   float* gsums = nullptr;                     // GroupNorm backward scratch [N][maxC][2]
@@ -100,7 +99,7 @@ struct BwdBuilder {
     if (it == pool.end()) it = pool.emplace(key, act_alloc(C, H, W)).first;
     return it->second;
   }
-  const Act& fwd(const std::string& name) const { return h->taps.at(name); }
+  const Act& fwd(const std::string& name) const { return h->plan.taps.at(name); }
   Act G(const std::string& name) {            // gradient tensor of a forward activation
     auto it = grad.find(name);
     if (it == grad.end()) {
@@ -113,9 +112,6 @@ struct BwdBuilder {
     return bw->grads ? bw->grads + bw->goff[h->pidx.at(pname)] : nullptr;
   }
   const float* P(const std::string& name) const { return h->pptr[h->pidx.at(name)]; }
-  const __nv_bfloat16* WT(const std::string& key) const {
-    return bw->arena ? (const __nv_bfloat16*)(bw->arena + toff.at(key)) : nullptr;
-  }
   static View view(const Act& a, int c0, int C) {
     View v;
     const Geom g = make_geom(1, a.H, a.W);
@@ -127,22 +123,16 @@ struct BwdBuilder {
 
   // ---- transposed weight packing jobs ----------------------------------------------------------------------------
   // GEMM out channels = the layer's input channels [i0, i0 + I) ... the kernel reads W[o][i][kh][kw] with i = co.
-  void tjob(const std::string& key, const std::string& wname, int O, int I, int K, const PackTaps& taps_in) {
+  // Returns the packed weights (null in the size pass).
+  const __nv_bfloat16* tjob(const std::string& wname, int O, int I, int K, const TapSet& t) {
     PackJob j;
     j.w_param = h->pidx.at(wname);
     j.cout = I; j.cin_total = O; j.KH = K; j.KW = K; j.cin_off = 0; j.ksteps = O / 16;
-    j.taps = taps_in;
-    j.taps.transpose = 1;
+    j.taps = t.pack;
     j.cout_real = I;
-    j.off = take_off(mem, (size_t)(I / 128) * j.ksteps * taps_in.ntaps * CONV_B_TAP);
-    toff[key] = j.off;
+    j.off = take_off(mem, (size_t)(I / 128) * j.ksteps * t.pack.ntaps * CONV_B_TAP);
     bw->jobs.push_back(j);
-  }
-  static PackTaps mirrored(int K) {
-    PackTaps t{};
-    t.ntaps = K * K;
-    for (int k = 0; k < K * K; ++k) { t.kh[k] = K - 1 - k / K; t.kw[k] = K - 1 - k % K; }
-    return t;
+    return bw->arena ? (const __nv_bfloat16*)(bw->arena + j.off) : nullptr;
   }
 
   // ---- op emitters ------------------------------------------------------------------------------------------------
@@ -152,51 +142,32 @@ struct BwdBuilder {
     p.N = N; p.H = out.H; p.W = out.W; p.Wp = g.Wp; p.lead = g.lead; p.PL = g.PL;
     p.cout = out.C; p.out = out.p;
   }
-  static void seg(ConvSeg& s, const View& src, const __nv_bfloat16* wpack, int ntaps, const signed char* dh,
-                  const signed char* dw) {
-    const Geom g = make_geom(1, src.H, src.W);
-    s.src = src.p; s.wpack = wpack;
-    s.img_stride = (long long)src.img_planes * g.PL * 8;
-    s.ksteps = src.C / 16;
-    s.ntaps = ntaps;
-    s.ht = s.hb = s.hl = s.hr = 0;
-    for (int t = 0; t < ntaps; ++t) {
-      s.dh[t] = dh[t]; s.dw[t] = dw[t];
-      if (dh[t] < 0) s.ht = 1;
-      if (dh[t] > 0) s.hb = 1;
-      if (dw[t] < 0) s.hl = 1;
-      if (dw[t] > 0) s.hr = 1;
-    }
-    s.ss = nullptr; s.ss_stride = 0; s.silu = 0;
+  static void seg(ConvSeg& s, const View& src, const __nv_bfloat16* wpack, const TapSet& t) {
+    set_seg(s, src.p, src.img_planes, src.C, src.H, src.W, wpack, t);
   }
   // data gradient of a stride-1 KxK conv: out (I channels) = conv^T(gy (O channels))
-  void dgrad(const std::string& key, const std::string& wname, const View& gy, const Act& out, int K) {
-    tjob(key, wname, gy.C, out.C, K, mirrored(K));
+  void dgrad(const std::string& wname, const View& gy, const Act& out, int K) {
+    const TapSet t = taps_mirrored(K);
     BOp op{};
     op.kind = BOp::CONV;
     conv_base(op.conv, out);
-    signed char dh[9], dw[9];
-    for (int k = 0; k < K * K; ++k) { dh[k] = (signed char)(k / K - K / 2); dw[k] = (signed char)(k % K - K / 2); }
-    seg(op.conv.seg[0], gy, WT(key), K * K, dh, dw);
+    seg(op.conv.seg[0], gy, tjob(wname, gy.C, out.C, K, t), t);
     op.conv.nseg = 1;
     bw->ops.push_back(op);
   }
-  void wgrad(const View& gy, const View& act, float* dw, int cin_total, int ci_off, int ntaps_total, int ntaps,
-             const signed char* dh, const signed char* dwv, const int* tapidx) {
+  // weight gradient of the forward K-segment with tap set t (of ntaps_total taps of the weight) that read `act`
+  void wgrad(const View& gy, const View& act, float* dw, int cin_total, int ci_off, int ntaps_total, const TapSet& t) {
     BOp op{};
     op.kind = BOp::WGRAD;
     WgradDesc& d = op.wg;
     d.gy = gy.p; d.act = act.p; d.dw = dw; d.N = N; d.H = gy.H; d.W = gy.W; d.cout = gy.C; d.cin = act.C;
     d.gy_img_planes = gy.img_planes; d.act_img_planes = act.img_planes;
-    d.cin_total = cin_total; d.ci_off = ci_off; d.ntaps_total = ntaps_total; d.ntaps = ntaps;
-    for (int t = 0; t < ntaps; ++t) { d.dh[t] = dh[t]; d.dw_[t] = dwv[t]; d.tapidx[t] = tapidx[t]; }
+    d.cin_total = cin_total; d.ci_off = ci_off; d.ntaps_total = ntaps_total; d.ntaps = t.pack.ntaps;
+    for (int k = 0; k < t.pack.ntaps; ++k) { d.dh[k] = t.dh[k]; d.dw_[k] = t.dw[k]; d.tapidx[k] = t.wtap[k]; }
     bw->ops.push_back(op);
   }
   void wgrad_conv(const View& gy, const View& act, const std::string& wname, int K) {   // plain stride-1 conv
-    signed char dh[9], dw[9];
-    int ti[9];
-    for (int k = 0; k < K * K; ++k) { dh[k] = (signed char)(k / K - K / 2); dw[k] = (signed char)(k % K - K / 2); ti[k] = k; }
-    wgrad(gy, act, PG(wname), act.C, 0, K * K, K * K, dh, dw, ti);
+    wgrad(gy, act, PG(wname), act.C, 0, K * K, taps_conv(K));
   }
   // per-channel sums of a gradient -> bias gradient(s); returns the [N][C] scratch (valid until the next chan_sum)
   void bias_grad(const View& g, const std::string& bname, const std::string& bname2 = "") {
@@ -243,15 +214,12 @@ struct BwdBuilder {
     p.dgamma = PG(norm + ".weight"); p.dbeta = PG(norm + ".bias");
     p.sums = gsums;
     p.csum0 = nullptr;
-    {
-      static const bool off = [] { const char* e = getenv("B200AD_NO_CSUM_FUSE"); return e && e[0] == '1'; }();   // A/B switch
-      const size_t need = (size_t)N * a.C;
-      if (!off && csum_used + need <= csum_floats) {
-        p.csum0 = csum_arena ? csum_arena + csum_used : nullptr;
-        csum_of[d0.p] = p.csum0;
-        csum_used += need;
-        if (!csum_arena) csum_of[d0.p] = (float*)1;           // size pass: the plan must have the same shape as the real one
-      }
+    const size_t need = (size_t)N * a.C;
+    if (csum_used + need <= csum_floats) {
+      p.csum0 = csum_arena ? csum_arena + csum_used : nullptr;
+      csum_of[d0.p] = p.csum0;
+      csum_used += need;
+      if (!csum_arena) csum_of[d0.p] = (float*)1;             // size pass: the plan must have the same shape as the real one
     }
     p.N = N; p.H = a.H; p.W = a.W; p.groups = h->norm_groups; p.eps = h->norm_eps; p.silu = silu ? 1 : 0;
     bw->ops.push_back(op);
@@ -263,7 +231,8 @@ struct BwdBuilder {
 
   // ---- blocks -----------------------------------------------------------------------------------------------------
   // ResnetBlock2D n over cat(a, b): consumes G(n), produces G(a) and (if b) the skip contribution of b.
-  void resnet_bwd(const std::string& n, const std::string& an, const std::string& bn) {
+  void resnet_bwd(const Block& k, const std::string& an, const std::string& bn) {
+    const std::string& n = k.name;
     const Act a = fwd(an);
     const bool has_b = !bn.empty();
     Act bsrc;
@@ -273,7 +242,7 @@ struct BwdBuilder {
     const Act Gout = G(n);
     // conv2
     Act T1 = tmp("T1", co, H, W);
-    dgrad(n + ".conv2.T", n + ".conv2.weight", whole(Gout), T1, 3);
+    dgrad(n + ".conv2.weight", whole(Gout), T1, 3);
     Act A = gn_apply("A", h1, nullptr, n + ".norm2", true);
     wgrad_conv(whole(Gout), whole(A), n + ".conv2.weight", 3);
     const bool sc = Ct != co;
@@ -286,23 +255,21 @@ struct BwdBuilder {
     {
       BOp op{};
       op.kind = BOp::SCATTER;
-      op.f0 = last_cs; op.o0 = gproj; op.C = co; op.a = h->temb_rows; op.b = h->temb_row_off.at(n);
+      op.f0 = last_cs; op.o0 = gproj; op.C = co; op.a = h->temb_rows; op.b = k.temb_row;
       bw->ops.push_back(op);
     }
     // conv1
     Act T2 = tmp("T2", Ct, H, W);
-    dgrad(n + ".conv1.T", n + ".conv1.weight", whole(Gh1), T2, 3);
+    dgrad(n + ".conv1.weight", whole(Gh1), T2, 3);
     Act A2 = gn_apply("A2", a, has_b ? &bsrc : nullptr, n + ".norm1", true);
     wgrad_conv(whole(Gh1), whole(A2), n + ".conv1.weight", 3);
     // shortcut
     const __nv_bfloat16* addS;
     if (sc) {
       Act T3 = tmp("T3", Ct, H, W);
-      dgrad(n + ".conv_shortcut.T", n + ".conv_shortcut.weight", whole(Gout), T3, 1);
-      const signed char z = 0;
-      const int zi = 0;
-      wgrad(whole(Gout), whole(a), PG(n + ".conv_shortcut.weight"), Ct, 0, 1, 1, &z, &z, &zi);
-      if (has_b) wgrad(whole(Gout), whole(bsrc), PG(n + ".conv_shortcut.weight"), Ct, a.C, 1, 1, &z, &z, &zi);
+      dgrad(n + ".conv_shortcut.weight", whole(Gout), T3, 1);
+      wgrad(whole(Gout), whole(a), PG(n + ".conv_shortcut.weight"), Ct, 0, 1, taps_conv(1));
+      if (has_b) wgrad(whole(Gout), whole(bsrc), PG(n + ".conv_shortcut.weight"), Ct, a.C, 1, taps_conv(1));
       addS = T3.p;
     } else {
       addS = Gout.p;
@@ -322,7 +289,7 @@ struct BwdBuilder {
     const int C = x.C, H = x.H, W = x.W;
     const Act Gout = G(n);
     Act T1 = tmp("T1", C, H, W);
-    dgrad(n + ".to_out.T", n + ".to_out.0.weight", whole(Gout), T1, 1);
+    dgrad(n + ".to_out.0.weight", whole(Gout), T1, 1);
     wgrad_conv(whole(Gout), whole(ao), n + ".to_out.0.weight", 1);
     bias_grad(whole(Gout), n + ".to_out.0.bias");
     Act Gqkv = tmp("Gqkv", 3 * C, H, W);
@@ -345,12 +312,9 @@ struct BwdBuilder {
       BOp op{};
       op.kind = BOp::CONV;
       conv_base(op.conv, T2);
-      const signed char z = 0;
-      for (int k = 0; k < 3; ++k) {
-        const std::string key = n + "." + names[k] + ".T";
-        tjob(key, n + "." + names[k] + ".weight", C, C, 1, mirrored(1));
-        seg(op.conv.seg[k], view(Gqkv, k * C, C), WT(key), 1, &z, &z);
-      }
+      const TapSet t = taps_mirrored(1);
+      for (int k = 0; k < 3; ++k)
+        seg(op.conv.seg[k], view(Gqkv, k * C, C), tjob(n + "." + names[k] + ".weight", C, C, 1, t), t);
       op.conv.nseg = 3;
       bw->ops.push_back(op);
     }
@@ -368,41 +332,23 @@ struct BwdBuilder {
     // weight gradient: per parity plane (a, b) of x the taps that read it (forward: taps_parity)
     for (int a = 0; a < 2; ++a)
       for (int b = 0; b < 2; ++b) {
-        const PackTaps pt = taps_parity(a, b);
-        signed char dh[9], dw[9];
-        int ti[9];
-        for (int t = 0; t < pt.ntaps; ++t) {
-          dh[t] = (pt.kh[t] == 0) ? -1 : 0; dw[t] = (pt.kw[t] == 0) ? -1 : 0; ti[t] = pt.kh[t] * 3 + pt.kw[t];
-        }
         Act plane = par;
         plane.C = C; plane.H = Ho; plane.W = Wo;
         plane.p = par.p ? par.p + (size_t)(a * 2 + b) * tsz : nullptr;
-        wgrad(whole(Gy), whole(plane), PG(n + ".weight"), C, 0, 9, pt.ntaps, dh, dw, ti);
+        wgrad(whole(Gy), whole(plane), PG(n + ".weight"), C, 0, 9, taps_parity(a, b));
       }
     // data gradient: input parity (a, b) <- taps with matching parity, scattered into the 2x tensor
     Act Gx = G(xn);
     for (int a = 0; a < 2; ++a)
       for (int b = 0; b < 2; ++b) {
-        PackTaps pt{};
-        signed char dh[9], dw[9];
-        const int khs[2][2] = {{1, -1}, {0, 2}};      // a = 0: kh 1;  a = 1: kh 0 (dh +1), kh 2 (dh 0)
-        for (int i = 0; i < 2; ++i)
-          for (int j = 0; j < 2; ++j) {
-            const int kh = khs[a][i], kw = khs[b][j];
-            if (kh < 0 || kw < 0) continue;
-            pt.kh[pt.ntaps] = kh; pt.kw[pt.ntaps] = kw;
-            dh[pt.ntaps] = (kh == 0) ? 1 : 0; dw[pt.ntaps] = (kw == 0) ? 1 : 0;
-            ++pt.ntaps;
-          }
-        const std::string key = n + S(".T%d", a * 2 + b);
-        tjob(key, n + ".weight", C, C, 3, pt);
+        const TapSet t = taps_scatter2(a, b);
         BOp op{};
         op.kind = BOp::CONV;
         Act lo = Gx;
         lo.H = Ho; lo.W = Wo;
         conv_base(op.conv, lo);
         op.conv.up2 = 1; op.conv.oy = a; op.conv.ox = b;
-        seg(op.conv.seg[0], whole(Gy), WT(key), pt.ntaps, dh, dw);
+        seg(op.conv.seg[0], whole(Gy), tjob(n + ".weight", C, C, 3, t), t);
         op.conv.nseg = 1;
         bw->ops.push_back(op);
       }
@@ -444,18 +390,13 @@ struct BwdBuilder {
     for (int oy = 0; oy < 2; ++oy)
       for (int ox = 0; ox < 2; ++ox) {
         const int pidx = oy * 2 + ox;
-        const UpTaps ut = taps_up2(oy, ox);
+        const TapSet fwd_taps = taps_up2(oy, ox), bwd_taps = taps_up2_neg(oy, ox);
         Act plane;
         plane.C = C; plane.H = H; plane.W = W;
         plane.p = gpar.p ? gpar.p + (size_t)pidx * tsz : nullptr;
-        int ti[4] = {0, 1, 2, 3};
-        wgrad(whole(plane), whole(x), dwf ? dwf + (size_t)pidx * C * C * 4 : nullptr, C, 0, 4, 4, ut.dh, ut.dw, ti);
-        for (int t = 0; t < 4; ++t) um.mask[pidx][t] = ut.pack.fold_mask[t];
-        const std::string key = n + S(".T%d", pidx);
-        tjob(key, n + ".weight", C, C, 3, ut.pack);
-        signed char ndh[4], ndw[4];
-        for (int t = 0; t < 4; ++t) { ndh[t] = (signed char)-ut.dh[t]; ndw[t] = (signed char)-ut.dw[t]; }
-        seg(dg.conv.seg[pidx], whole(plane), WT(key), 4, ndh, ndw);
+        wgrad(whole(plane), whole(x), dwf ? dwf + (size_t)pidx * C * C * 4 : nullptr, C, 0, 4, fwd_taps);
+        for (int t = 0; t < 4; ++t) um.mask[pidx][t] = fwd_taps.pack.fold_mask[t];
+        seg(dg.conv.seg[pidx], whole(plane), tjob(n + ".weight", C, C, 3, bwd_taps), bwd_taps);
       }
     dg.conv.nseg = 4;
     {
@@ -468,15 +409,9 @@ struct BwdBuilder {
   }
 };
 
-struct Rec {
-  int kind;  // 0 resnet, 1 attention, 2 down, 3 up
-  std::string n, a, b;
-};
-
 static int build_backward(b200ad_unet* h, Backward* bw, uint8_t* arena, float* grads, size_t* bytes_out) {
   const b200ad_unet_config& c = h->cfg;
-  const int nb = c.num_blocks;
-  if (!h->training || h->plan.empty()) return set_err("backward needs set_training(1) before bind_workspace");
+  if (!h->training || h->plan.lists.empty()) return set_err("backward needs set_training(1) before bind_workspace");
   bw->ops.clear();
   bw->jobs.clear();
   bw->arena = arena;
@@ -484,54 +419,8 @@ static int build_backward(b200ad_unet* h, Backward* bw, uint8_t* arena, float* g
   BwdBuilder B;
   B.h = h; B.bw = bw; B.N = h->N;
   B.mem.base = arena;
-  // forward structure, by tensor name (mirrors build_plan in unet.cu)
-  std::vector<Rec> recs;
-  std::string cur = "conv_in";
-  std::vector<std::string> skips{cur};
   int maxC = c.block_out_channels[0];
-  for (int i = 0; i < nb; ++i) {
-    for (int j = 0; j < c.layers_per_block; ++j) {
-      const std::string rn = S("down_blocks.%d.resnets.%d", i, j);
-      recs.push_back({0, rn, cur, ""});
-      cur = rn;
-      if (c.down_attn[i]) {
-        const std::string an = S("down_blocks.%d.attentions.%d", i, j);
-        recs.push_back({1, an, cur, ""});
-        cur = an;
-      }
-      skips.push_back(cur);
-    }
-    if (i != nb - 1) {
-      const std::string dn = S("down_blocks.%d.downsamplers.0.conv", i);
-      recs.push_back({2, dn, cur, ""});
-      cur = dn;
-      skips.push_back(cur);
-    }
-  }
-  recs.push_back({0, "mid_block.resnets.0", cur, ""});
-  recs.push_back({1, "mid_block.attentions.0", "mid_block.resnets.0", ""});
-  recs.push_back({0, "mid_block.resnets.1", "mid_block.attentions.0", ""});
-  cur = "mid_block.resnets.1";
-  for (int i = 0; i < nb; ++i) {
-    for (int j = 0; j < c.layers_per_block + 1; ++j) {
-      const std::string sk = skips.back();
-      skips.pop_back();
-      const std::string rn = S("up_blocks.%d.resnets.%d", i, j);
-      recs.push_back({0, rn, cur, sk});
-      cur = rn;
-      if (c.up_attn[i]) {
-        const std::string an = S("up_blocks.%d.attentions.%d", i, j);
-        recs.push_back({1, an, cur, ""});
-        cur = an;
-      }
-    }
-    if (i != nb - 1) {
-      const std::string un = S("up_blocks.%d.upsamplers.0.conv", i);
-      recs.push_back({3, un, cur, ""});
-      cur = un;
-    }
-  }
-  for (const auto& kv : h->taps) maxC = kv.second.C > maxC ? kv.second.C : maxC;
+  for (const auto& kv : h->plan.taps) maxC = kv.second.C > maxC ? kv.second.C : maxC;
   const int D = c.block_out_channels[0] * 4;
   B.cs = (float*)B.mem.take((size_t)h->N * 3 * maxC * sizeof(float));
   B.gsums = (float*)B.mem.take((size_t)h->N * 3 * maxC * 2 * sizeof(float));
@@ -550,100 +439,102 @@ static int build_backward(b200ad_unet* h, Backward* bw, uint8_t* arena, float* g
   float* wflip = (float*)B.mem.take((size_t)c.block_out_channels[0] * 9 * sizeof(float));
   const float* zbias = (const float*)B.mem.take((size_t)c.block_out_channels[0] * sizeof(float));   // never written: zeros
 
-  // ---- conv_out: g_eps -> gradient of the last activation ---------------------------------------------------------
-  {
-    const Act x = h->taps.at("pre_out");
-    const int C = x.C;
-    if (c.out_channels != 1) return set_err("backward: out_channels != 1 is not implemented");
-    Act A = B.gn_apply("A", x, nullptr, "conv_norm_out", true);
-    BOp w{};
-    w.kind = BOp::SCALAR_WGRAD;
-    w.src = A.p; w.x_is_geps = true; w.o0 = B.PG("conv_out.weight"); w.C = C; w.H = x.H; w.W = x.W; w.a = 1;
-    bw->ops.push_back(w);
-    BOp sb{};
-    sb.kind = BOp::SUMADD;
-    sb.x_is_geps = true; sb.n = (long long)h->N * x.H * x.W; sb.o0 = B.PG("conv_out.bias");
-    bw->ops.push_back(sb);
-    BOp f{};
-    f.kind = BOp::FLIP;
-    f.f0 = B.P("conv_out.weight"); f.o0 = wflip; f.C = C;
-    bw->ops.push_back(f);
-    Act T1 = B.tmp("T1", C, x.H, x.W);
-    BOp ci{};
-    ci.kind = BOp::CONVIN;        // conv_in kernel: g_a[c] = sum_t g_eps[p + s_t] * wflip[c][t]
-    ci.x_is_geps = true; ci.f0 = wflip; ci.f1 = zbias; ci.dst = T1.p; ci.C = C; ci.H = x.H; ci.W = x.W;
-    bw->ops.push_back(ci);
-    B.gn_bwd(T1, x, nullptr, "conv_norm_out", true, B.G(cur), nullptr, nullptr, nullptr);
-  }
-  // ---- blocks in reverse ------------------------------------------------------------------------------------------
-  {
-    BOp z{};
-    z.kind = BOp::MEMSET;
-    z.o0 = B.gproj; z.n = (long long)h->N * h->temb_rows * sizeof(float);
-    bw->ops.push_back(z);
-  }
-  for (int r = (int)recs.size() - 1; r >= 0; --r) {
-    const Rec& rc = recs[r];
-    if (rc.kind == 0) B.resnet_bwd(rc.n, rc.a, rc.b);
-    else if (rc.kind == 1) B.attention_bwd(rc.n, rc.a);
-    else if (rc.kind == 2) B.downsample_bwd(rc.n, rc.a);
-    else B.upsample_bwd(rc.n, rc.a);
-  }
-  // ---- conv_in ----------------------------------------------------------------------------------------------------
-  {
-    if (c.in_channels != 1) return set_err("backward: in_channels != 1 is not implemented");
-    const Act x = h->taps.at("conv_in");
-    const Act Gx = B.G("conv_in");
-    if (!B.skipgrad.count("conv_in")) return set_err("backward: conv_in skip gradient missing");
-    // (the first resnet's GroupNorm backward already added the skip contribution)
-    BOp w{};
-    w.kind = BOp::SCALAR_WGRAD;
-    w.src = Gx.p; w.x_is_input = true; w.o0 = B.PG("conv_in.weight"); w.C = x.C; w.H = x.H; w.W = x.W; w.a = 0;
-    bw->ops.push_back(w);
-    B.bias_grad(BwdBuilder::whole(Gx), "conv_in.bias");
-  }
-  // ---- timestep embedding MLP and the per-resnet projections ------------------------------------------------------
-  {
-    const int d0 = c.block_out_channels[0];
-    for (const auto& kv : h->temb_row_off) {     // time_emb_proj of every resnet: dW = g_proj_rows^T temb_act
-      const int co = (int)h->params[h->pidx.at(kv.first + ".time_emb_proj.bias")].shape[0];
-      BOp op{};
-      op.kind = BOp::LIN_W;
-      op.f0 = B.gproj + kv.second; op.a = h->temb_rows; op.f1 = h->temb_act; op.b = co; op.c = D;
-      op.o0 = B.PG(kv.first + ".time_emb_proj.weight"); op.o1 = B.PG(kv.first + ".time_emb_proj.bias");
-      bw->ops.push_back(op);
+  // the forward's blocks in reverse; a block's output is the forward tap of its name (the head's: conv_in)
+  const std::vector<Block>& bl = h->blocks;
+  auto tap = [&](int i) { return i < 0 ? std::string() : bl[i].kind == BK_UNET_HEAD ? bl[i].name + "conv_in" : bl[i].name; };
+  for (int i = (int)bl.size() - 1; i >= 0; --i) {
+    const Block& k = bl[i];
+    const std::string in = tap(k.in);
+    switch (k.kind) {
+      case BK_CONV_OUT: {    // g_eps -> gradient of the last activation
+        const Act x = B.fwd(in);
+        const int C = x.C;
+        if (c.out_channels != 1) return set_err("backward: out_channels != 1 is not implemented");
+        Act A = B.gn_apply("A", x, nullptr, k.name + "conv_norm_out", true);
+        BOp w{};
+        w.kind = BOp::SCALAR_WGRAD;
+        w.src = A.p; w.x_is_geps = true; w.o0 = B.PG(k.name + "conv_out.weight"); w.C = C; w.H = x.H; w.W = x.W; w.a = 1;
+        bw->ops.push_back(w);
+        BOp sb{};
+        sb.kind = BOp::SUMADD;
+        sb.x_is_geps = true; sb.n = (long long)h->N * x.H * x.W; sb.o0 = B.PG(k.name + "conv_out.bias");
+        bw->ops.push_back(sb);
+        BOp f{};
+        f.kind = BOp::FLIP;
+        f.f0 = B.P(k.name + "conv_out.weight"); f.o0 = wflip; f.C = C;
+        bw->ops.push_back(f);
+        Act T1 = B.tmp("T1", C, x.H, x.W);
+        BOp ci{};
+        ci.kind = BOp::CONVIN;        // conv_in kernel: g_a[c] = sum_t g_eps[p + s_t] * wflip[c][t]
+        ci.x_is_geps = true; ci.f0 = wflip; ci.f1 = zbias; ci.dst = T1.p; ci.C = C; ci.H = x.H; ci.W = x.W;
+        bw->ops.push_back(ci);
+        B.gn_bwd(T1, x, nullptr, k.name + "conv_norm_out", true, B.G(in), nullptr, nullptr, nullptr);
+        BOp z{};
+        z.kind = BOp::MEMSET;
+        z.o0 = B.gproj; z.n = (long long)h->N * h->temb_rows * sizeof(float);
+        bw->ops.push_back(z);
+        break;
+      }
+      case BK_RESNET: B.resnet_bwd(k, in, tap(k.skip)); break;
+      case BK_ATTN: B.attention_bwd(k.name, in); break;
+      case BK_DOWN: B.downsample_bwd(k.name, in); break;
+      case BK_UP: B.upsample_bwd(k.name, in); break;
+      case BK_UNET_HEAD: {   // conv_in, then the timestep embedding MLP and the per-resnet projections
+        if (c.in_channels != 1) return set_err("backward: in_channels != 1 is not implemented");
+        const std::string n = tap(i);
+        const Act x = B.fwd(n);
+        const Act Gx = B.G(n);
+        if (!B.skipgrad.count(n)) return set_err("backward: conv_in skip gradient missing");
+        // (the first resnet's GroupNorm backward already added the skip contribution)
+        BOp w{};
+        w.kind = BOp::SCALAR_WGRAD;
+        w.src = Gx.p; w.x_is_input = true; w.o0 = B.PG(n + ".weight"); w.C = x.C; w.H = x.H; w.W = x.W; w.a = 0;
+        bw->ops.push_back(w);
+        B.bias_grad(BwdBuilder::whole(Gx), n + ".bias");
+        const Plan& pl = h->plan;
+        for (const Block& r : bl) {     // time_emb_proj of every resnet: dW = g_proj_rows^T temb_act
+          if (r.temb_row < 0) continue;
+          BOp op{};
+          op.kind = BOp::LIN_W;
+          op.f0 = B.gproj + r.temb_row; op.a = h->temb_rows; op.f1 = pl.temb_act; op.b = r.cout; op.c = D;
+          op.o0 = B.PG(r.name + ".time_emb_proj.weight"); op.o1 = B.PG(r.name + ".time_emb_proj.bias");
+          bw->ops.push_back(op);
+        }
+        BOp gi{};
+        gi.kind = BOp::LIN_IN;   // g(temb_act) = g_proj Wcat
+        gi.f0 = B.gproj; gi.a = h->temb_rows; gi.f1 = h->packed ? (const float*)(h->packed + h->off_wcat) : nullptr;
+        gi.b = h->temb_rows; gi.c = D; gi.o0 = g_act;
+        bw->ops.push_back(gi);
+        BOp s2{};
+        s2.kind = BOp::SILU_BWD;
+        s2.o0 = g_act; s2.f0 = pl.temb_u2; s2.n = (long long)h->N * D;
+        bw->ops.push_back(s2);
+        BOp hf{};
+        hf.kind = BOp::SILU_FWD;
+        hf.f0 = pl.temb_u1; hf.o0 = h1v; hf.n = (long long)h->N * D;
+        bw->ops.push_back(hf);
+        BOp w2{};
+        w2.kind = BOp::LIN_W;
+        w2.f0 = g_act; w2.a = D; w2.f1 = h1v; w2.b = D; w2.c = D;
+        w2.o0 = B.PG("time_embedding.linear_2.weight"); w2.o1 = B.PG("time_embedding.linear_2.bias");
+        bw->ops.push_back(w2);
+        BOp g1{};
+        g1.kind = BOp::LIN_IN;
+        g1.f0 = g_act; g1.a = D; g1.f1 = B.P("time_embedding.linear_2.weight"); g1.b = D; g1.c = D; g1.o0 = g_h1;
+        bw->ops.push_back(g1);
+        BOp s1{};
+        s1.kind = BOp::SILU_BWD;
+        s1.o0 = g_h1; s1.f0 = pl.temb_u1; s1.n = (long long)h->N * D;
+        bw->ops.push_back(s1);
+        BOp w1{};
+        w1.kind = BOp::LIN_W;
+        w1.f0 = g_h1; w1.a = D; w1.f1 = pl.temb_emb; w1.b = D; w1.c = k.cout;
+        w1.o0 = B.PG("time_embedding.linear_1.weight"); w1.o1 = B.PG("time_embedding.linear_1.bias");
+        bw->ops.push_back(w1);
+        break;
+      }
+      default: return set_err("backward: block %s has no backward (only the unconditional U-Net trains)", k.name.c_str());
     }
-    BOp gi{};
-    gi.kind = BOp::LIN_IN;   // g(temb_act) = g_proj Wcat
-    gi.f0 = B.gproj; gi.a = h->temb_rows; gi.f1 = h->packed ? (const float*)(h->packed + h->off_wcat) : nullptr;
-    gi.b = h->temb_rows; gi.c = D; gi.o0 = g_act;
-    bw->ops.push_back(gi);
-    BOp s2{};
-    s2.kind = BOp::SILU_BWD;
-    s2.o0 = g_act; s2.f0 = h->temb_u2; s2.n = (long long)h->N * D;
-    bw->ops.push_back(s2);
-    BOp hf{};
-    hf.kind = BOp::SILU_FWD;
-    hf.f0 = h->temb_u1; hf.o0 = h1v; hf.n = (long long)h->N * D;
-    bw->ops.push_back(hf);
-    BOp w2{};
-    w2.kind = BOp::LIN_W;
-    w2.f0 = g_act; w2.a = D; w2.f1 = h1v; w2.b = D; w2.c = D;
-    w2.o0 = B.PG("time_embedding.linear_2.weight"); w2.o1 = B.PG("time_embedding.linear_2.bias");
-    bw->ops.push_back(w2);
-    BOp g1{};
-    g1.kind = BOp::LIN_IN;
-    g1.f0 = g_act; g1.a = D; g1.f1 = B.P("time_embedding.linear_2.weight"); g1.b = D; g1.c = D; g1.o0 = g_h1;
-    bw->ops.push_back(g1);
-    BOp s1{};
-    s1.kind = BOp::SILU_BWD;
-    s1.o0 = g_h1; s1.f0 = h->temb_u1; s1.n = (long long)h->N * D;
-    bw->ops.push_back(s1);
-    BOp w1{};
-    w1.kind = BOp::LIN_W;
-    w1.f0 = g_h1; w1.a = D; w1.f1 = h->temb_emb; w1.b = D; w1.c = d0;
-    w1.o0 = B.PG("time_embedding.linear_1.weight"); w1.o1 = B.PG("time_embedding.linear_1.bias");
-    bw->ops.push_back(w1);
   }
   if (bytes_out) *bytes_out = (B.mem.off + 255) & ~(size_t)255;
   return 0;
@@ -665,7 +556,7 @@ extern "C" int b200ad_unet_set_training(b200ad_unet* h, int on) {
   if (on && h->cfg.cross_attention_dim) return set_err("training of the conditional U-Net is not implemented (inference only)");
   if (h->training != (on != 0)) {
     h->training = on != 0;
-    h->plan.clear();          // the workspace layout changes: bind_workspace must be called again
+    h->plan.lists.clear();    // the workspace layout changes: bind_workspace must be called again
   }
   return 0;
 }
