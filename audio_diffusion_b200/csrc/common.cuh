@@ -57,15 +57,13 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
       : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
   return ok != 0;
 }
-// Bounded wait: a protocol bug must trap (reported as a launch failure) instead of hanging the GPU.
+// Bounded wait: a protocol bug must trap (reported as a launch failure) instead of hanging the GPU.  No printf here: it
+// is a function call, and a call anywhere in a wgmma loop makes ptxas serialise every wgmma of that loop (C7520).
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > 4000000000LL) {  // ~2 s at 2 GHz
-      printf("b200ad: mbarrier timeout (block %d thread %d bar %u parity %u)\n", blockIdx.x, threadIdx.x, bar, parity);
-      __trap();
-    }
+    if (clock64() - t0 > 4000000000LL) __trap();  // ~2 s at 2 GHz
   }
 }
 

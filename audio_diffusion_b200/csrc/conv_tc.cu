@@ -85,7 +85,9 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_c
   const int AS = p.as;      // activation stages of this launch (CONV_AS .. CONV_AS_MAX)
   const int BS = p.bs;      // weight-ring depth of this launch (whatever the activation stages leave, CONV_BS .. CONV_BS_MAX)
   extern __shared__ __align__(128) uint8_t smem[];
-  const int warp = threadIdx.x >> 5;
+  // Broadcast from lane 0 so that ptxas can prove the role branches warp-uniform; otherwise it treats the consumer's wgmma
+  // loop as a divergent path and waits for every wgmma to complete before issuing the next (C7520).
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
   const int a_bytes = p.a_stage;
 
