@@ -105,6 +105,8 @@ SYMBOLS = {
     "b200ad_conv2d_wgrad": (_I, [_VP, _VP, _VP] + [_I] * 6 + [_VP, _SZ, _VP]),
     "b200ad_gn_conv2d": (_I, [_VP, _VP, _VP, _I, C.c_float, _I, _VP, _VP, _VP] + [_I] * 6 + [_VP, _SZ, _VP]),
     "b200ad_group_norm": (_I, [_VP] * 4 + [_I] * 5 + [C.c_float, _I, _VP, _SZ, _VP]),
+    "b200ad_mha_scratch_bytes": (_SZ, [_I] * 5),
+    "b200ad_mha_forward_backward": (_I, [_VP] * 8 + [_I] * 5 + [_VP, _SZ, _VP]),
     "b200ad_mel_scratch_bytes": (_SZ, [C.POINTER(MelConfigC), _I]),
     "b200ad_mel_encode": (_I, [C.POINTER(MelConfigC), _VP, _VP, _VP, _I, _VP, _SZ, _VP]),
     "b200ad_mel_encode_ref": (_I, [C.POINTER(MelConfigC), _VP, _VP, _VP, _I, _VP, _VP, _VP, _SZ, _VP]),

@@ -242,6 +242,60 @@ extern "C" int b200ad_group_norm(const float* x, const float* gamma, const float
   return 0;
 }
 
+// Multi-head self-attention of the conditional U-Net's transformer blocks, forward and backward, on fp32 NCHW tensors:
+// the forward kernel (with its row log-sum-exp) and the three backward launches the training step runs.
+struct MhaScratch {
+  size_t qkv_f, qkv, o, go, gqkv, lse, dsum, total;
+};
+static MhaScratch mha_scratch_layout(int N, int C, int heads, int H, int W) {
+  MhaScratch s{};
+  const Geom g = make_geom(N, H, W);
+  const size_t pf = (size_t)N * (C / 8) * g.PL * 16, rows = (size_t)N * heads * H * W * sizeof(float);
+  size_t off = 0;
+  s.qkv_f = off; off = al(off + (size_t)N * 3 * C * H * W * sizeof(float));   // fp32 [N][3C][H][W] staging
+  s.qkv = off; off = al(off + 3 * pf);
+  s.o = off; off = al(off + pf);
+  s.go = off; off = al(off + pf);
+  s.gqkv = off; off = al(off + 3 * pf);
+  s.lse = off; off = al(off + rows);
+  s.dsum = off; off = al(off + rows);
+  s.total = off;
+  return s;
+}
+extern "C" size_t b200ad_mha_scratch_bytes(int N, int C, int heads, int H, int W) {
+  return mha_scratch_layout(N, C, heads, H, W).total;
+}
+extern "C" int b200ad_mha_forward_backward(const float* q, const float* k, const float* v, const float* dout, float* out,
+                                           float* dq, float* dk, float* dv, int N, int C, int heads, int H, int W,
+                                           void* scratch, size_t scratch_bytes, void* stream) {
+  if (heads < 1 || C % heads || (C / heads != 16 && C / heads != 32 && C / heads != 64))
+    return set_err("mha_forward_backward: head_dim C / heads must be 16, 32 or 64");
+  const MhaScratch L = mha_scratch_layout(N, C, heads, H, W);
+  if (scratch_bytes < L.total) return set_err("mha_forward_backward: scratch too small (%zu < %zu)", scratch_bytes, L.total);
+  cudaStream_t st = (cudaStream_t)stream;
+  uint8_t* sb = (uint8_t*)scratch;
+  CK(cudaMemsetAsync(sb, 0, L.total, st));
+  float* qkvf = (float*)(sb + L.qkv_f);
+  __nv_bfloat16* qkv = (__nv_bfloat16*)(sb + L.qkv);
+  __nv_bfloat16* o = (__nv_bfloat16*)(sb + L.o);
+  __nv_bfloat16* go = (__nv_bfloat16*)(sb + L.go);
+  __nv_bfloat16* gqkv = (__nv_bfloat16*)(sb + L.gqkv);
+  const size_t img = (size_t)C * H * W * sizeof(float);   // bytes of one image of one of q / k / v
+  const float* src[3] = {q, k, v};
+  for (int j = 0; j < 3; ++j)   // q | k | v concatenated along channels, as the model's fused projection writes them
+    CK(cudaMemcpy2DAsync((uint8_t*)qkvf + j * img, 3 * img, src[j], img, img, N, cudaMemcpyDeviceToDevice, st));
+  CK(launch_nchw_to_pf8(qkvf, qkv, N, 3 * C, H, W, st));
+  CK(launch_nchw_to_pf8(dout, go, N, C, H, W, st));
+  CK(launch_mha_flash(qkv, o, N, C, heads, H, W, st, (float*)(sb + L.lse)));
+  CK(launch_mha_bwd(qkv, o, go, (const float*)(sb + L.lse), (float*)(sb + L.dsum), gqkv, N, C, heads, H, W, st));
+  CK(launch_pf8_to_nchw(o, out, N, C, H, W, st));
+  CK(launch_pf8_to_nchw(gqkv, qkvf, N, 3 * C, H, W, st));
+  float* dst[3] = {dq, dk, dv};
+  for (int j = 0; j < 3; ++j)
+    CK(cudaMemcpy2DAsync(dst[j], img, (const uint8_t*)qkvf + j * img, 3 * img, img, N, cudaMemcpyDeviceToDevice, st));
+  return 0;
+}
+
 extern "C" int b200ad_sample_to_u8(const float* x, uint8_t* img, size_t n, void* stream) {
   CK(launch_sample_to_u8(x, img, n, (cudaStream_t)stream));
   return 0;

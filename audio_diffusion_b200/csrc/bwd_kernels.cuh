@@ -47,6 +47,23 @@ cudaError_t launch_lin_bwd_weight(const float* g, int gstride, const float* x, i
 cudaError_t launch_silu_bwd(float* g, const float* u, int n, cudaStream_t s);
 cudaError_t launch_silu_fwd(const float* u, float* y, int n, cudaStream_t s);
 
+// Transformer blocks of the conditional U-Net (cond_bwd.cu).
+// LayerNorm over channels: gx = LN-backward(gy; x) (+ add, optional, same shape); dgamma / dbeta [C] accumulated. C <= 512.
+cudaError_t launch_layernorm_bwd_pf8(const __nv_bfloat16* x, const __nv_bfloat16* gy, const __nv_bfloat16* add,
+                                     __nv_bfloat16* gx, const float* gamma, float* dgamma, float* dbeta, int N, int C, int H,
+                                     int W, float eps, cudaStream_t s);
+// GEGLU: src = the forward input (2*Ch channels: hidden | gate), gy: Ch channels -> dst: 2*Ch channels
+cudaError_t launch_geglu_bwd_pf8(const __nv_bfloat16* src, const __nv_bfloat16* gy, __nv_bfloat16* dst, int N, int Ch, int H,
+                                 int W, cudaStream_t s);
+// cross-attention against one encoder token: dvec [N][C] = gradient of the per-sample vector Wo (Wv enc) + bo ->
+// dWo [C][C], dWv [C][X] accumulated.  scratch: 2 * N * C floats.
+cudaError_t launch_cross_attn_vec_bwd(const float* enc, const float* dvec, const float* wv, const float* wo, float* dwo,
+                                      float* dwv, float* scratch, int N, int C, int X, cudaStream_t s);
+// multi-head self-attention (head_dim C / heads in {16, 32, 64}): qkv and o as the forward read / wrote them, go = dL/do
+// (PF8, C channels), lse from launch_mha_flash -> gqkv (PF8, 3C channels).  dsum: N * heads * H * W floats of scratch.
+cudaError_t launch_mha_bwd(const __nv_bfloat16* qkv, const __nv_bfloat16* o, const __nv_bfloat16* go, const float* lse,
+                           float* dsum, __nv_bfloat16* gqkv, int N, int C, int heads, int H, int W, cudaStream_t s);
+
 // Weight gradient on wgmma (wgrad_tc.cu):  dw[(co * cin_total + ci_off + ci) * ntaps_total + tapidx[t]] +=
 //   sum_{n, p} gy[n][co][p] * act[n][ci][p + shift[t]].   gy / act are channel views: `*_img_planes` planes per image in the
 // underlying tensors, the pointers already offset to the view's first plane.

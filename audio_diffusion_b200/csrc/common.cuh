@@ -259,6 +259,18 @@ __device__ __forceinline__ void stmatrix_x4_trans(uint32_t saddr, uint32_t r0, u
   asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};"
                ::"r"(saddr), "r"(r0), "r"(r1), "r"(r2), "r"(r3) : "memory");
 }
+
+// warp-level tensor-core MMA (attention kernels): C[16x8] += A[16x16] B[16x8], bf16 in, fp32 accumulate
+__device__ __forceinline__ void mma_bf16_16x8x16(float (&c)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0,
+                                                 uint32_t b1) {
+  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3]) : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+}
+
+// element offset of pixel p (row-major over H x W) inside one 8-channel plane
+__device__ __forceinline__ long long pf8_pixel(const Geom& g, int p, int W) {
+  return (long long)(g.lead + (p / W) * g.Wp + (p % W)) * 8;
+}
 #endif  // __CUDACC__
 
 }  // namespace b200ad

@@ -7,10 +7,6 @@
 
 namespace b200ad {
 
-__device__ __forceinline__ long long pf8_pixel(const Geom& g, int p, int W) {
-  return (long long)(g.lead + (p / W) * g.Wp + (p % W)) * 8;
-}
-
 // ------------------------------------------------------------------------------------ LayerNorm over channels (per token)
 // y[n][c][p] = (x - mean_p) * rstd_p * gamma[c] + beta[c];  one warp per pixel, lanes stride over the 8-channel planes.
 __global__ void __launch_bounds__(256) layernorm_pf8_kernel(const __nv_bfloat16* __restrict__ src, __nv_bfloat16* __restrict__ dst,
@@ -120,15 +116,11 @@ cudaError_t launch_cross_attn_vec(const float* enc, const float* wv, const float
 // qkv: PF8 with 3C channels (q | k | v), head h = channels [h D, (h+1) D) of each third.  One CTA = 64 queries of one
 // (sample, head): 4 warps x 16 query rows; K / V stream through shared memory in tiles of 64 keys; online softmax in
 // the exp2 domain; Q K^T and P V on mma.sync.m16n8k16 (bf16 in, fp32 accumulate), V fragments by transposing ldmatrix.
-__device__ __forceinline__ void mma_bf16_16x8x16(float (&c)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0,
-                                                 uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3]) : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-}
-
-template <int D>
+// lse (training, may be null): the row log-sum-exp of the scaled scores in the log2 domain, fp32 [N][heads][seq], which
+// the backward (cond_bwd.cu) recomputes P from.
+template <int D, bool LSE>
 __global__ void __launch_bounds__(128) mha_flash_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restrict__ out,
-                                                        int N, int C, int H, int W, float scale_log2) {
+                                                        int N, int C, int H, int W, float scale_log2, float* __restrict__ lse) {
   constexpr int DP = D / 8;    // planes per head
   constexpr int KS = D / 16;   // k-steps of Q K^T
   __shared__ __align__(16) uint4 ks[DP][64];   // [plane][key] 8 channels
@@ -232,15 +224,25 @@ __global__ void __launch_bounds__(128) mha_flash_kernel(const __nv_bfloat16* __r
     if (q_a < seq) *reinterpret_cast<uint32_t*>(ob + (long long)i * g.PL * 8 + o0 + 2 * tq) = pack_bf16x2(oacc[i][0] * i0, oacc[i][1] * i0);
     if (q_b < seq) *reinterpret_cast<uint32_t*>(ob + (long long)i * g.PL * 8 + o1 + 2 * tq) = pack_bf16x2(oacc[i][2] * i1, oacc[i][3] * i1);
   }
+  if (LSE && tq == 0) {
+    float* lr = lse + ((long long)n * gridDim.y + head) * seq;
+    if (q_a < seq) lr[q_a] = m0 + __log2f(l0);   // l >= 1 (the row maximum contributes 1)
+    if (q_b < seq) lr[q_b] = m1 + __log2f(l1);
+  }
 }
 
-cudaError_t launch_mha_flash(const __nv_bfloat16* qkv, __nv_bfloat16* out, int N, int C, int heads, int H, int W, cudaStream_t s) {
+cudaError_t launch_mha_flash(const __nv_bfloat16* qkv, __nv_bfloat16* out, int N, int C, int heads, int H, int W, cudaStream_t s,
+                             float* lse) {
   const int D = C / heads, seq = H * W;
   const float sl2 = 1.4426950408889634f / sqrtf((float)D);
   dim3 grid((seq + 63) / 64, heads, N);
-  if (D == 16) mha_flash_kernel<16><<<grid, 128, 0, s>>>(qkv, out, N, C, H, W, sl2);
-  else if (D == 32) mha_flash_kernel<32><<<grid, 128, 0, s>>>(qkv, out, N, C, H, W, sl2);
-  else if (D == 64) mha_flash_kernel<64><<<grid, 128, 0, s>>>(qkv, out, N, C, H, W, sl2);
+  // inference (lse null) runs an instantiation without the log-sum-exp store
+  if (D == 16) lse ? mha_flash_kernel<16, true><<<grid, 128, 0, s>>>(qkv, out, N, C, H, W, sl2, lse)
+                   : mha_flash_kernel<16, false><<<grid, 128, 0, s>>>(qkv, out, N, C, H, W, sl2, nullptr);
+  else if (D == 32) lse ? mha_flash_kernel<32, true><<<grid, 128, 0, s>>>(qkv, out, N, C, H, W, sl2, lse)
+                        : mha_flash_kernel<32, false><<<grid, 128, 0, s>>>(qkv, out, N, C, H, W, sl2, nullptr);
+  else if (D == 64) lse ? mha_flash_kernel<64, true><<<grid, 128, 0, s>>>(qkv, out, N, C, H, W, sl2, lse)
+                        : mha_flash_kernel<64, false><<<grid, 128, 0, s>>>(qkv, out, N, C, H, W, sl2, nullptr);
   else return cudaErrorInvalidValue;
   return cudaGetLastError();
 }

@@ -119,7 +119,9 @@ cudaError_t launch_layernorm_pf8(const __nv_bfloat16* src, __nv_bfloat16* dst, c
 cudaError_t launch_geglu_pf8(const __nv_bfloat16* src, __nv_bfloat16* dst, int N, int Ch, int H, int W, cudaStream_t s);
 cudaError_t launch_cross_attn_vec(const float* enc, const float* wv, const float* wo, const float* bo, float* vec, int N, int C,
                                   int X, cudaStream_t s);
-cudaError_t launch_mha_flash(const __nv_bfloat16* qkv, __nv_bfloat16* out, int N, int C, int heads, int H, int W, cudaStream_t s);
+// lse (optional, training): row log-sum-exp fp32 [N][heads][H*W] for the backward (log2 domain of the scaled scores)
+cudaError_t launch_mha_flash(const __nv_bfloat16* qkv, __nv_bfloat16* out, int N, int C, int heads, int H, int W, cudaStream_t s,
+                             float* lse = nullptr);
 
 // generic single-head attention over the fused qkv tensor (AutoencoderKL mid block); scores: N * seq * seq floats of scratch
 cudaError_t launch_attention_1head(const __nv_bfloat16* qkv, __nv_bfloat16* out, float* scores, int N, int C, int H, int W,

@@ -49,7 +49,8 @@ struct Op {
   int C = 0, H = 0, W = 0;
   ConvOutParams co;
   float2* ss = nullptr;  // OP_GN: output of gn_finalize
-  float* f0 = nullptr;   // OP_ATTN1: score scratch; OP_MIX1X1: fp32 destination; OP_CONV_IN: fp32 source (null: the caller's)
+  float* f0 = nullptr;   // OP_ATTN1: score scratch; OP_MIX1X1: fp32 destination; OP_CONV_IN: fp32 source (null: the caller's);
+                         // OP_MHA: row log-sum-exp for the backward (training; null: not kept)
   const float* fw = nullptr;  // OP_CONV_IN / OP_VAE_SAMPLE / OP_MIX1X1 / OP_LN: fp32 weight and bias
   const float* fb = nullptr;
   const float* fc = nullptr;  // OP_XVEC: to_out bias
@@ -147,6 +148,7 @@ struct Plan {    // everything a plan builder derives from the workspace and (N,
   float* temb_u1 = nullptr;          // training: [N][4 dim0] linear_1 output before SiLU
   float* temb_u2 = nullptr;          // training: [N][4 dim0] linear_2 output before SiLU
   float* zq = nullptr;               // autoencoder: post_quant_conv(z), [N][L][h][w]
+  std::map<std::string, float*> lse; // training, conditional U-Net: attn1's row log-sum-exp [N][heads][H*W] by block name
   size_t ws_bytes = 0;
 };
 
@@ -664,13 +666,15 @@ struct Builder {
       Op op{};
       op.kind = OP_MHA;
       op.src = qkv.p; op.dst = ao.p; op.C = C; op.H = H; op.W = W; op.cin = heads;
+      if (h->training) op.f0 = built->lse[n] = (float*)ws.take((size_t)N * heads * H * W * sizeof(float));
       ops->push_back(op);
     }
     Act h2 = pooled("tf_h2", C, H, W, false);
     linear(h2, ao, k.out, P(t + ".attn1.to_out.0.bias"), nullptr, &h0, k.ident, vec, C);
-    layer_norm(h2, n1, t + ".norm3");
+    Act n3 = pooled("tf_ln", C, H, W, false);     // the same buffer as n1 unless training
+    layer_norm(h2, n3, t + ".norm3");
     Act ff1 = pooled("tf_ff1", 8 * C, H, W, false);
-    linear(ff1, n1, k.ff1, P(t + ".ff.net.0.proj.bias"));
+    linear(ff1, n3, k.ff1, P(t + ".ff.net.0.proj.bias"));
     Act gg = pooled("tf_gg", 4 * C, H, W, false);
     {
       Op op{};
@@ -684,6 +688,16 @@ struct Builder {
     linear(out, h3, k.proj_out, P(n + ".proj_out.bias"), nullptr, &x, k.ident);
     built->taps[n + ".attn2"] = h2;
     built->taps[n] = out;
+    if (h->training) {   // no pooling: every intermediate has its own buffer, kept for BwdBuilder::transformer_bwd
+      built->taps[n + ".h0"] = h0;
+      built->taps[n + ".n1"] = n1;
+      built->taps[n + ".qkv"] = qkv;
+      built->taps[n + ".ao"] = ao;
+      built->taps[n + ".n3"] = n3;
+      built->taps[n + ".ff1"] = ff1;
+      built->taps[n + ".gg"] = gg;
+      built->taps[n + ".h3"] = h3;
+    }
     return out;
   }
 
@@ -885,7 +899,7 @@ static int run_ops(NetBase* h, const OpList& l, const RunArgs& a, cudaStream_t s
         break;
       case OP_LN: CK(launch_layernorm_pf8(op.src, op.dst, op.fw, op.fb, h->N, op.C, op.H, op.W, op.eps, st)); break;
       case OP_GEGLU: CK(launch_geglu_pf8(op.src, op.dst, h->N, op.C, op.H, op.W, st)); break;
-      case OP_MHA: CK(launch_mha_flash(op.src, op.dst, h->N, op.C, op.cin, op.H, op.W, st)); break;
+      case OP_MHA: CK(launch_mha_flash(op.src, op.dst, h->N, op.C, op.cin, op.H, op.W, st, op.f0)); break;
       case OP_XVEC:
         if (!h->enc) return set_err("conditional U-Net: call b200ad_unet_set_encoding before forward");
         if (h->enc_S != 1) return set_err("conditional U-Net: encoder sequence length %d (only 1 is implemented)", h->enc_S);

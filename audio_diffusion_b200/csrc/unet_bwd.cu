@@ -1,6 +1,7 @@
-// Backward pass of the U-Net (scripts/train_unet.py:259, `accelerator.backward(loss)`): walks UNet2DModel.forward in
-// reverse over the activations the training-mode forward kept (no buffer pooling), and fills one flat fp32 buffer with
-// the gradients of all parameters.
+// Backward pass of the U-Net (scripts/train_unet.py:259, `accelerator.backward(loss)`): walks UNet2DModel.forward (or
+// UNet2DConditionModel.forward) in reverse over the activations the training-mode forward kept (no buffer pooling), and
+// fills one flat fp32 buffer with the gradients of all parameters.  The transformer blocks of the conditional model run
+// their LayerNorm / GEGLU / cross-attention / multi-head attention backward kernels from cond_bwd.cu.
 //   * data gradients of every convolution run on conv_tc_kernel with transposed / mirrored weight packing (stride-2 convs
 //     as four scatter launches, the folded upsampling convs as one gather launch over the parity planes of the gradient);
 //   * weight gradients run on wgrad_tc_kernel (wgmma, pixels as the reduction dimension, MN-major operands);
@@ -20,7 +21,8 @@ struct View {            // channel range of a PF8 tensor
 
 struct BOp {
   enum Kind { CONV, WGRAD, GNBWD, GNAPPLY, CHANSUM, REDUCE_N, SCATTER, PF8ADD, ATTNBWD, PARITY, UNFOLD, SCALAR_WGRAD, CONVIN,
-              FLIP, SUMADD, LIN_IN, LIN_W, SILU_BWD, SILU_FWD, MEMSET } kind;
+              FLIP, SUMADD, LIN_IN, LIN_W, SILU_BWD, SILU_FWD, MEMSET,
+              LNBWD, GEGLUBWD, XVECBWD, MHABWD, NKINDS } kind;
   ConvParams conv;
   WgradDesc wg;
   GnBwdParams gb;
@@ -28,11 +30,14 @@ struct BOp {
   UnfoldMasks um;
   const __nv_bfloat16* src = nullptr;
   const __nv_bfloat16* src2 = nullptr;
+  const __nv_bfloat16* src3 = nullptr;
   __nv_bfloat16* dst = nullptr;
   const float* f0 = nullptr;
   const float* f1 = nullptr;
+  const float* f2 = nullptr;
   float* o0 = nullptr;
   float* o1 = nullptr;
+  float* o2 = nullptr;        // scratch (never a parameter gradient)
   int C = 0, H = 0, W = 0, a = 0, b = 0, c = 0, d = 0;
   long long n = 0;
   bool x_is_input = false;    // SCALAR_WGRAD: X = the forward input image passed to backward()
@@ -123,11 +128,12 @@ struct BwdBuilder {
 
   // ---- transposed weight packing jobs ----------------------------------------------------------------------------
   // GEMM out channels = the layer's input channels [i0, i0 + I) ... the kernel reads W[o][i][kh][kw] with i = co.
+  // Only the layer's output channels [o_off, o_off + o_cnt) are packed when o_cnt >= 0 (one K-segment of a split reduction).
   // Returns the packed weights (null in the size pass).
-  const __nv_bfloat16* tjob(const std::string& wname, int O, int I, int K, const TapSet& t) {
+  const __nv_bfloat16* tjob(const std::string& wname, int O, int I, int K, const TapSet& t, int o_off = 0, int o_cnt = -1) {
     PackJob j;
     j.w_param = h->pidx.at(wname);
-    j.cout = I; j.cin_total = O; j.KH = K; j.KW = K; j.cin_off = 0; j.ksteps = O / 16;
+    j.cout = I; j.cin_total = O; j.KH = K; j.KW = K; j.cin_off = o_off; j.ksteps = (o_cnt < 0 ? O : o_cnt) / 16;
     j.taps = t.pack;
     j.cout_real = I;
     j.off = take_off(mem, (size_t)(I / 128) * j.ksteps * t.pack.ntaps * CONV_B_TAP);
@@ -187,7 +193,7 @@ struct BwdBuilder {
     last_cs = cs;
     bw->ops.push_back(op);
   }
-  Act gn_apply(const std::string& tag, const Act& a, const Act* b, const std::string& norm, bool silu) {
+  Act gn_apply(const std::string& tag, const Act& a, const Act* b, const std::string& norm, bool silu, float eps = -1.f) {
     const int Ct = a.C + (b ? b->C : 0);
     Act out = tmp(tag, Ct, a.H, a.W);
     BOp op{};
@@ -196,12 +202,13 @@ struct BwdBuilder {
     p.src[0] = a.p; p.stats[0] = a.stats; p.C[0] = a.C;
     p.src[1] = b ? b->p : nullptr; p.stats[1] = b ? b->stats : nullptr; p.C[1] = b ? b->C : 0;
     p.gamma = P(norm + ".weight"); p.beta = P(norm + ".bias");
-    p.dst = out.p; p.N = N; p.H = a.H; p.W = a.W; p.groups = h->norm_groups; p.eps = h->norm_eps; p.silu = silu ? 1 : 0;
+    p.dst = out.p; p.N = N; p.H = a.H; p.W = a.W; p.groups = h->norm_groups; p.eps = eps < 0.f ? h->norm_eps : eps;
+    p.silu = silu ? 1 : 0;
     bw->ops.push_back(op);
     return out;
   }
   void gn_bwd(const Act& ga, const Act& a, const Act* b, const std::string& norm, bool silu, const Act& d0, const Act* d1,
-              const __nv_bfloat16* addS, const __nv_bfloat16* add0) {
+              const __nv_bfloat16* addS, const __nv_bfloat16* add0, float eps = -1.f) {
     BOp op{};
     op.kind = BOp::GNBWD;
     GnBwdParams& p = op.gb;
@@ -221,7 +228,7 @@ struct BwdBuilder {
       csum_used += need;
       if (!csum_arena) csum_of[d0.p] = (float*)1;             // size pass: the plan must have the same shape as the real one
     }
-    p.N = N; p.H = a.H; p.W = a.W; p.groups = h->norm_groups; p.eps = h->norm_eps; p.silu = silu ? 1 : 0;
+    p.N = N; p.H = a.H; p.W = a.W; p.groups = h->norm_groups; p.eps = eps < 0.f ? h->norm_eps : eps; p.silu = silu ? 1 : 0;
     bw->ops.push_back(op);
   }
   const __nv_bfloat16* skip_of(const std::string& name) const {
@@ -319,6 +326,113 @@ struct BwdBuilder {
       bw->ops.push_back(op);
     }
     gn_bwd(T2, x, nullptr, n + ".group_norm", false, G(xn), nullptr, Gout.p, skip_of(xn));
+  }
+
+  // LayerNorm over channels (eps 1e-5, as the forward): gx = LN-backward(gy; x) + add, gamma / beta gradients
+  void layer_norm_bwd(const Act& gy, const Act& x, const std::string& norm, const Act& gx, const Act& add) {
+    BOp op{};
+    op.kind = BOp::LNBWD;
+    op.src = x.p; op.src2 = gy.p; op.src3 = add.p; op.dst = gx.p;
+    op.f0 = P(norm + ".weight"); op.o0 = PG(norm + ".weight"); op.o1 = PG(norm + ".bias");
+    op.C = x.C; op.H = x.H; op.W = x.W;
+    bw->ops.push_back(op);
+  }
+
+  // Transformer2DModel with one BasicTransformerBlock (Builder::transformer) in reverse, from G(out) to G(x):
+  //   h0 = proj_in(GN(x));  h2 = h0 + attn1(LN1(h0)) + vec;  h3 = h2 + ff2(GEGLU(ff1(LN3(h2))));  out = proj_out(h3) + x
+  // attn2 over ONE key is the per-sample vector vec = Wo (Wv enc) + bo: its gradient is the per-sample channel sum of G(h2)
+  // (the sums the attn1.to_out bias gradient makes).  attn2.to_q, attn2.to_k and norm2 do not reach the output (softmax
+  // over one key is 1), so their gradients stay exactly zero: nothing is launched for them.
+  void transformer_bwd(const Block& k, const std::string& xn) {
+    const std::string& n = k.name;
+    const std::string t = n + ".transformer_blocks.0";
+    const Act x = fwd(xn), h0 = fwd(n + ".h0"), n1 = fwd(n + ".n1"), qkv = fwd(n + ".qkv"), ao = fwd(n + ".ao"),
+              h2 = fwd(n + ".attn2"), n3 = fwd(n + ".n3"), ff1 = fwd(n + ".ff1"), gg = fwd(n + ".gg"), h3 = fwd(n + ".h3");
+    const int C = x.C, H = x.H, W = x.W, heads = h->cfg.attention_head_dim;
+    const Act Gout = G(n);
+    // proj_out (its residual, G(x) += G(out), is added by the GroupNorm backward at the end)
+    Act Gh3 = tmp("tf_Gh3", C, H, W);
+    dgrad(n + ".proj_out.weight", whole(Gout), Gh3, 1);
+    wgrad_conv(whole(Gout), whole(h3), n + ".proj_out.weight", 1);
+    bias_grad(whole(Gout), n + ".proj_out.bias");
+    // ff.net.2 (+ residual h2)
+    Act Ggg = tmp("tf_Ggg", 4 * C, H, W);
+    dgrad(t + ".ff.net.2.weight", whole(Gh3), Ggg, 1);
+    wgrad_conv(whole(Gh3), whole(gg), t + ".ff.net.2.weight", 1);
+    bias_grad(whole(Gh3), t + ".ff.net.2.bias");
+    // GEGLU
+    Act Gff1 = tmp("tf_Gff1", 8 * C, H, W);
+    {
+      BOp op{};
+      op.kind = BOp::GEGLUBWD;
+      op.src = ff1.p; op.src2 = Ggg.p; op.dst = Gff1.p; op.C = 4 * C; op.H = H; op.W = W;
+      bw->ops.push_back(op);
+    }
+    // ff.net.0.proj: the 8C-channel reduction as two K-segments (a segment holds at most 255 k-steps of 16 channels)
+    Act Gn = tmp("tf_Gn", C, H, W);
+    {
+      BOp op{};
+      op.kind = BOp::CONV;
+      conv_base(op.conv, Gn);
+      const TapSet ts = taps_mirrored(1);
+      for (int j = 0; j < 2; ++j)
+        seg(op.conv.seg[j], view(Gff1, j * 4 * C, 4 * C), tjob(t + ".ff.net.0.proj.weight", 8 * C, C, 1, ts, j * 4 * C, 4 * C), ts);
+      op.conv.nseg = 2;
+      bw->ops.push_back(op);
+    }
+    wgrad_conv(whole(Gff1), whole(n3), t + ".ff.net.0.proj.weight", 1);
+    bias_grad(whole(Gff1), t + ".ff.net.0.proj.bias");
+    // norm3 (+ residual) -> G(h2)
+    Act Gh2 = tmp("tf_Gh2", C, H, W);
+    layer_norm_bwd(Gn, h2, t + ".norm3", Gh2, Gh3);
+    // attn1.to_out and attn2.to_out both add their bias to every pixel of h2: one channel sum gives both bias gradients
+    Act Gao = tmp("tf_Gao", C, H, W);
+    dgrad(t + ".attn1.to_out.0.weight", whole(Gh2), Gao, 1);
+    wgrad_conv(whole(Gh2), whole(ao), t + ".attn1.to_out.0.weight", 1);
+    bias_grad(whole(Gh2), t + ".attn1.to_out.0.bias", t + ".attn2.to_out.0.bias");
+    {
+      BOp op{};
+      op.kind = BOp::XVECBWD;   // dvec[n] = per-sample channel sums of G(h2) (last_cs, made just above)
+      op.f0 = last_cs; op.f1 = P(t + ".attn2.to_v.weight"); op.f2 = P(t + ".attn2.to_out.0.weight");
+      op.o0 = PG(t + ".attn2.to_out.0.weight"); op.o1 = PG(t + ".attn2.to_v.weight");
+      op.o2 = (float*)mem.take((size_t)2 * N * C * sizeof(float));
+      op.C = C; op.a = k.cross;
+      bw->ops.push_back(op);
+    }
+    // attention core (P recomputed from the forward's row log-sum-exp)
+    Act Gqkv = tmp("tf_Gqkv", 3 * C, H, W);
+    {
+      BOp op{};
+      op.kind = BOp::MHABWD;
+      op.src = qkv.p; op.src2 = Gao.p; op.src3 = ao.p; op.dst = Gqkv.p;
+      op.f0 = h->plan.lse.at(n);
+      op.o2 = (float*)mem.take((size_t)N * heads * H * W * sizeof(float));
+      op.C = C; op.H = H; op.W = W; op.a = heads;
+      bw->ops.push_back(op);
+    }
+    // q / k / v projections (no bias); g(n1) = sum over q, k, v of W^T g: one launch, three K-segments
+    const char* names[3] = {"to_q", "to_k", "to_v"};
+    for (int j = 0; j < 3; ++j) wgrad_conv(view(Gqkv, j * C, C), whole(n1), t + ".attn1." + names[j] + ".weight", 1);
+    {
+      BOp op{};
+      op.kind = BOp::CONV;
+      conv_base(op.conv, Gn);
+      const TapSet ts = taps_mirrored(1);
+      for (int j = 0; j < 3; ++j)
+        seg(op.conv.seg[j], view(Gqkv, j * C, C), tjob(t + ".attn1." + names[j] + ".weight", C, C, 1, ts), ts);
+      op.conv.nseg = 3;
+      bw->ops.push_back(op);
+    }
+    // norm1 (+ residual) -> G(h0)
+    Act Gh0 = tmp("tf_Gh0", C, H, W);
+    layer_norm_bwd(Gn, h0, t + ".norm1", Gh0, Gh2);
+    // proj_in over GroupNorm(x) (eps 1e-6, no SiLU), then the GroupNorm backward with the outer residual G(out)
+    Act T = tmp("tf_T", C, H, W);
+    dgrad(n + ".proj_in.weight", whole(Gh0), T, 1);
+    Act XN = gn_apply("A", x, nullptr, n + ".norm", false, 1e-6f);
+    wgrad_conv(whole(Gh0), whole(XN), n + ".proj_in.weight", 1);
+    bias_grad(whole(Gh0), n + ".proj_in.bias");
+    gn_bwd(T, x, nullptr, n + ".norm", false, G(xn), nullptr, Gout.p, skip_of(xn), 1e-6f);
   }
 
   // Downsample2D: stride-2 3x3 conv on the raw tensor xn -> y (tap n)
@@ -477,6 +591,7 @@ static int build_backward(b200ad_unet* h, Backward* bw, uint8_t* arena, float* g
       }
       case BK_RESNET: B.resnet_bwd(k, in, tap(k.skip)); break;
       case BK_ATTN: B.attention_bwd(k.name, in); break;
+      case BK_TRANSFORMER: B.transformer_bwd(k, in); break;
       case BK_DOWN: B.downsample_bwd(k.name, in); break;
       case BK_UP: B.upsample_bwd(k.name, in); break;
       case BK_UNET_HEAD: {   // conv_in, then the timestep embedding MLP and the per-resnet projections
@@ -533,7 +648,7 @@ static int build_backward(b200ad_unet* h, Backward* bw, uint8_t* arena, float* g
         bw->ops.push_back(w1);
         break;
       }
-      default: return set_err("backward: block %s has no backward (only the unconditional U-Net trains)", k.name.c_str());
+      default: return set_err("backward: block %s has no backward", k.name.c_str());
     }
   }
   if (bytes_out) *bytes_out = (B.mem.off + 255) & ~(size_t)255;
@@ -553,7 +668,6 @@ void release_backward(b200ad_unet* h) {
 // ================================================================================= C ABI
 extern "C" int b200ad_unet_set_training(b200ad_unet* h, int on) {
   if (!h) return set_err("null handle");
-  if (on && h->cfg.cross_attention_dim) return set_err("training of the conditional U-Net is not implemented (inference only)");
   if (h->training != (on != 0)) {
     h->training = on != 0;
     h->plan.lists.clear();    // the workspace layout changes: bind_workspace must be called again
@@ -658,6 +772,20 @@ extern "C" int b200ad_unet_backward(b200ad_unet* h, const float* x, const float*
       case BOp::SILU_BWD: CK(launch_silu_bwd(op.o0, op.f0, (int)op.n, st)); break;
       case BOp::SILU_FWD: CK(launch_silu_fwd(op.f0, op.o0, (int)op.n, st)); break;
       case BOp::MEMSET: CK(cudaMemsetAsync(op.o0, 0, (size_t)op.n, st)); break;
+      case BOp::LNBWD:
+        CK(launch_layernorm_bwd_pf8(op.src, op.src2, op.src3, op.dst, op.f0, op.o0, op.o1, N, op.C, op.H, op.W, 1e-5f, st));
+        break;
+      case BOp::GEGLUBWD: CK(launch_geglu_bwd_pf8(op.src, op.src2, op.dst, N, op.C, op.H, op.W, st)); break;
+      case BOp::XVECBWD:
+        if (!h->enc || h->enc_S != 1) return set_err("backward: the conditional U-Net needs the forward's encoding (S = 1) bound");
+        CK(launch_cross_attn_vec_bwd(h->enc, op.f0, op.f1, op.f2, op.o0, op.o1, op.o2, N, op.C, op.a, st));
+        launches += 1;
+        break;
+      case BOp::MHABWD:
+        CK(launch_mha_bwd(op.src, op.src3, op.src2, op.f0, op.o2, op.dst, N, op.C, op.a, op.H, op.W, st));
+        launches += 2;
+        break;
+      case BOp::NKINDS: break;
     }
     ++launches;
     if (prof) CK(cudaEventRecord(ev[2 + opi], st));
@@ -667,12 +795,13 @@ extern "C" int b200ad_unet_backward(b200ad_unet* h, const float* x, const float*
   }
   bw->launches = launches;
   if (prof) {
-    static const char* names[] = {"conv_tc(dgrad)", "wgrad_tc", "gn_bwd", "gn_apply", "chan_sum", "reduce_n", "scatter",
-                                  "pf8_add", "attention_bwd", "parity_split", "unfold_up2", "scalar_wgrad", "conv_in(dgrad)",
-                                  "flip", "sum_add", "lin_in", "lin_w", "silu_bwd", "silu_fwd", "memset"};
+    static const char* names[BOp::NKINDS] = {
+        "conv_tc(dgrad)", "wgrad_tc", "gn_bwd", "gn_apply", "chan_sum", "reduce_n", "scatter", "pf8_add", "attention_bwd",
+        "parity_split", "unfold_up2", "scalar_wgrad", "conv_in(dgrad)", "flip", "sum_add", "lin_in", "lin_w", "silu_bwd",
+        "silu_fwd", "memset", "layernorm_bwd", "geglu_bwd", "cross_attn_vec_bwd", "mha_bwd"};
     CK(cudaStreamSynchronize(st));
-    double tot[20] = {0};
-    int cnt[20] = {0};
+    double tot[BOp::NKINDS] = {0};
+    int cnt[BOp::NKINDS] = {0};
     float ms = 0.f;
     CK(cudaEventElapsedTime(&ms, ev[0], ev[1]));
     fprintf(stderr, "{\"backward_profile_ms\": {\"pack_transposed\": %.3f", ms);
@@ -681,7 +810,7 @@ extern "C" int b200ad_unet_backward(b200ad_unet* h, const float* x, const float*
       tot[bw->ops[i].kind] += ms;
       cnt[bw->ops[i].kind]++;
     }
-    for (int k = 0; k < 20; ++k)
+    for (int k = 0; k < BOp::NKINDS; ++k)
       if (cnt[k]) fprintf(stderr, ", \"%s x%d\": %.3f", names[k], cnt[k], tot[k]);
     fprintf(stderr, "}}\n");
     for (auto& e : ev) cudaEventDestroy(e);

@@ -204,10 +204,11 @@ class FusedAdamW(torch.optim.Optimizer):
 
 def train_step(model, optimizer: "FusedAdamW", noise_scheduler, clean_images: torch.Tensor, ema: Optional[EMAModel] = None,
                lr_scheduler=None, generator: Optional[torch.Generator] = None, noise: Optional[torch.Tensor] = None,
-               timesteps: Optional[torch.Tensor] = None):
+               timesteps: Optional[torch.Tensor] = None, encoder_hidden_states: Optional[torch.Tensor] = None):
     """One iteration of the training loop body, scripts/train_unet.py:238-267, on the engine: noise + per-sample timesteps,
     `add_noise`, U-Net forward, MSE, backward (CUDA), clip + AdamW + EMA (one fused kernel pass), LR scheduler step.
-    Returns the loss tensor (detached).  `noise` / `timesteps` may be given for reproducible tests."""
+    Returns the loss tensor (detached).  `noise` / `timesteps` may be given for reproducible tests.
+    `encoder_hidden_states`: the batch's audio encodings for a `UNet2DConditionModel` (train_unet.py --encodings, :255)."""
     x = clean_images
     if noise is None:
         noise = torch.randn(x.shape, generator=generator, device=x.device if generator is None else generator.device).to(x.device)
@@ -215,7 +216,10 @@ def train_step(model, optimizer: "FusedAdamW", noise_scheduler, clean_images: to
         timesteps = torch.randint(0, noise_scheduler.config.num_train_timesteps, (x.shape[0],), generator=generator,
                                   device=x.device if generator is None else generator.device).long().to(x.device)
     noisy = noise_scheduler.add_noise(x, noise, timesteps)
-    pred = model(noisy, timesteps)["sample"]
+    if encoder_hidden_states is None:
+        pred = model(noisy, timesteps)["sample"]
+    else:
+        pred = model(noisy, timesteps, encoder_hidden_states)["sample"]
     loss = torch.nn.functional.mse_loss(pred, noise)
     loss.backward()
     optimizer.step()

@@ -43,24 +43,26 @@ def _set_deep(root: nn.Module, dotted: str, p: nn.Parameter) -> None:
 
 class _UNetFunction(torch.autograd.Function):
     """Autograd node of the training forward: the backward pass is `b200ad_unet_backward` (all parameter gradients in one
-    call); the gradient w.r.t. the input sample is not produced (the reference never needs it)."""
+    call); the gradient w.r.t. the input sample is not produced (the reference never needs it).  `enc` is the conditional
+    model's encoding (None for UNet2DModel): the node keeps it alive and the backward binds it again, since the library
+    reads it for the cross-attention weight gradients; no gradient w.r.t. it is produced."""
 
     @staticmethod
-    def forward(ctx, model, x, t, *params):
-        out = model._forward_train(x, t)
+    def forward(ctx, model, x, t, enc, *params):
+        out = model._forward_train(x, t, enc)
         ctx.model = model
         ctx.gen = model._fwd_gen         # the activations live in the model's single workspace: backward must see THIS forward
-        ctx.save_for_backward(x)
+        ctx.save_for_backward(x, enc)
         return out
 
     @staticmethod
     def backward(ctx, g):
-        (x,) = ctx.saved_tensors
+        x, enc = ctx.saved_tensors
         if ctx.gen != ctx.model._fwd_gen:
             raise _lib.B200ADError("UNet2DModel(b200): another forward ran on this model before backward(); the saved "
                                    "activations of this graph were overwritten (one forward per backward)")
-        ctx.model._backward_train(x, g)          # fills p.grad (views of the flat gradient buffer)
-        return (None, None, None) + (None,) * len(ctx.model._pnames)
+        ctx.model._backward_train(x, g, enc)     # fills p.grad (views of the flat gradient buffer)
+        return (None, None, None, None) + (None,) * len(ctx.model._pnames)
 
 
 class UNet2DModel(nn.Module):
@@ -268,7 +270,7 @@ class UNet2DModel(nn.Module):
         if needs_grad:      # training step (scripts/train_unet.py:257-259): forward keeps every activation, backward in CUDA
             t = self._timesteps(timestep, n, x.device)
             named = self._named()
-            out = _UNetFunction.apply(self, x, t, *[named[k] for k in self._pnames])
+            out = _UNetFunction.apply(self, x, t, None, *[named[k] for k in self._pnames])
             return UNet2DOutput(out) if return_dict else (out,)
         with torch.cuda.device(x.device):
             self._fwd_gen += 1
@@ -290,7 +292,7 @@ class UNet2DModel(nn.Module):
             self._ws_key = None        # the workspace layout differs (no buffer pooling when training)
             self._bwd_key = None
 
-    def _forward_train(self, x: torch.Tensor, t: torch.Tensor) -> torch.Tensor:
+    def _forward_train(self, x: torch.Tensor, t: torch.Tensor, enc: Optional[torch.Tensor] = None) -> torch.Tensor:
         L = _lib.lib()
         n, _, hh, ww = x.shape
         with torch.cuda.device(x.device):
@@ -312,10 +314,12 @@ class UNet2DModel(nn.Module):
                 self._bwd_key = self._ws_key
                 self._bucket_key = None          # the library dropped its gradient buckets with the old plan
             out = torch.empty((n, self.out_channels, hh, ww), dtype=torch.float32, device=x.device)
+            if enc is not None:
+                _lib.check(L.b200ad_unet_set_encoding(self._h, enc.data_ptr(), enc.shape[1]))
             _lib.check(L.b200ad_unet_forward(self._h, x.data_ptr(), t.data_ptr(), out.data_ptr(), _lib.stream_ptr()))
         return out
 
-    def _backward_train(self, x: torch.Tensor, g: torch.Tensor):
+    def _backward_train(self, x: torch.Tensor, g: torch.Tensor, enc: Optional[torch.Tensor] = None):
         L = _lib.lib()
         g = g.to(torch.float32).contiguous()
         # torch semantics: gradients accumulate until they are zeroed. p.grad is None (zero_grad(set_to_none=True), the
@@ -327,6 +331,8 @@ class UNet2DModel(nn.Module):
         if any(have) and not accumulate:
             raise _lib.B200ADError("UNet2DModel(b200): either all parameter gradients are set (accumulate) or none")
         with torch.cuda.device(x.device):
+            if enc is not None:          # another call may have bound a different encoding since the forward
+                _lib.check(L.b200ad_unet_set_encoding(self._h, enc.data_ptr(), enc.shape[1]))
             _lib.check(L.b200ad_unet_backward(self._h, x.data_ptr(), g.data_ptr(), 1 if accumulate else 0, _lib.stream_ptr()))
         if not getattr(self, "_no_sync", False):
             self._allreduce_gradients()

@@ -4,10 +4,15 @@ audiodiffusion/pipeline_audio_diffusion.py:160-161; scripts/train_unet.py:255): 
 cross-attention reads the 100-d audio encodings of `audiodiffusion/audio_encoder.py:62-107`.
 
 Same constructor kwargs and diffusers state-dict keys (`down_blocks.i.attentions.j.transformer_blocks.0.attn1.to_q.weight`, ...).
-Inference runs in libb200ad.so: every projection / linear of the transformer blocks on the tcgen05 conv kernel, self-attention
-(8 heads, head_dim = channels / 8) on a flash-style tensor-core kernel, cross-attention against the ONE encoder token as a
-per-sample vector folded into the attn1 output projection.  Limits: encoder sequence length 1 (what the reference's
-AudioEncoder produces: (B, 1, 100)); no backward (training the conditional model is not built).
+Inference and training run in libb200ad.so: every projection / linear of the transformer blocks on the wgmma conv kernel
+(and, in the backward, its data- and weight-gradient forms), self-attention (8 heads, head_dim = channels / 8) on flash-style
+tensor-core kernels (the backward recomputes the attention matrix from the forward's row log-sum-exp), cross-attention
+against the ONE encoder token as a per-sample vector folded into the attn1 output projection.
+
+Training (`scripts/train_unet.py --encodings`: `model(noisy, t, enc)["sample"]`, MSE, `loss.backward()`) goes through the
+same autograd node as `UNet2DModel`: parameter gradients only, as `p.grad` views of one flat buffer.  Limits: encoder
+sequence length 1 (what the reference's AudioEncoder produces: (B, 1, 100)); no gradient w.r.t. the encoding (the
+reference's encodings are precomputed data), so an encoding with `requires_grad` is refused in training.
 """
 from __future__ import annotations
 
@@ -18,7 +23,7 @@ import torch
 
 from . import _lib
 from ._lib import MAX_BLOCKS, StepCoefC, UNetConfigC
-from .unet import UNet2DModel, UNet2DOutput, _Cfg
+from .unet import UNet2DModel, UNet2DOutput, _Cfg, _UNetFunction
 
 
 class UNet2DConditionModel(UNet2DModel):
@@ -107,12 +112,25 @@ class UNet2DConditionModel(UNet2DModel):
         return e.contiguous()
 
     def forward(self, sample: torch.Tensor, timestep, encoder_hidden_states: torch.Tensor = None, return_dict: bool = True):
-        """ε = unet(sample, timestep, encoding)["sample"] — pipeline_audio_diffusion.py:161."""
+        """ε = unet(sample, timestep, encoding)["sample"] — pipeline_audio_diffusion.py:161 (inference) and
+        scripts/train_unet.py:255 (training: in train mode with grad enabled, backward() fills the parameter gradients)."""
         if torch.is_grad_enabled() and self.training and any(p.requires_grad for p in self.parameters()):
-            raise NotImplementedError("UNet2DConditionModel(b200): inference only — call .eval() / torch.no_grad()")
+            if sample.requires_grad:
+                raise NotImplementedError("UNet2DConditionModel(b200): gradients w.r.t. the input sample are not computed")
+            if torch.is_tensor(encoder_hidden_states) and encoder_hidden_states.requires_grad:
+                raise NotImplementedError("UNet2DConditionModel(b200): gradients w.r.t. encoder_hidden_states are not computed "
+                                          "(pass precomputed encodings, e.g. .detach())")
+            x = self._check_input(sample)
+            n = x.shape[0]
+            t = self._timesteps(timestep, n, x.device)
+            e = self._encoding(encoder_hidden_states, n, x.device)
+            named = self._named()
+            out = _UNetFunction.apply(self, x, t, e, *[named[k] for k in self._pnames])
+            return UNet2DOutput(out) if return_dict else (out,)
         x = self._check_input(sample)
         n, _, hh, ww = x.shape
         with torch.cuda.device(x.device):
+            self._fwd_gen += 1
             self._set_training_mode(False)
             self._ensure_bound(n, hh, ww)
             t = self._timesteps(timestep, n, x.device)
@@ -130,6 +148,7 @@ class UNet2DConditionModel(UNet2DModel):
         x = self._check_input(sample)
         n, _, hh, ww = x.shape
         with torch.cuda.device(x.device):
+            self._fwd_gen += 1
             self._set_training_mode(False)
             self._ensure_bound(n, hh, ww)
             t = self._timesteps(timestep, n, x.device)

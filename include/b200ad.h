@@ -116,7 +116,10 @@ int b200ad_unet_last_launch_count(const b200ad_unet* h);
 /* ---- U-Net backward (scripts/train_unet.py:259 `accelerator.backward(loss)`) ----------------------------
  * Protocol: set_training(1) -> bind_workspace (every activation is kept) -> bind_backward -> per step: forward(x, t),
  * then backward(x, dL/d eps). Parameter gradients land in ONE flat fp32 buffer; parameter i of the
- * table lives at float offset b200ad_unet_grad_offset(h, i) — the Python mirror exposes them as `p.grad` views. */
+ * table lives at float offset b200ad_unet_grad_offset(h, i) — the Python mirror exposes them as `p.grad` views.
+ * Conditional model (scripts/train_unet.py --encodings): set_encoding before forward, and the same encoding must still be
+ * bound (and alive) at backward, which reads it for attn2.to_v's gradient.  No gradient w.r.t. the encoding is computed;
+ * attn2.to_q, attn2.to_k and norm2 get exactly zero gradients (softmax over one encoder token is constant). */
 int b200ad_unet_set_training(b200ad_unet* h, int on);
 size_t b200ad_unet_grad_floats(b200ad_unet* h);
 size_t b200ad_unet_grad_offset(b200ad_unet* h, int i);
@@ -218,6 +221,15 @@ int b200ad_conv2d_dgrad(const float* gy, const float* w, float* gx, int N, int c
 size_t b200ad_conv2d_wgrad_scratch_bytes(int N, int cin, int cout, int H, int W);
 int b200ad_conv2d_wgrad(const float* gy, const float* a, float* dw, int N, int cin, int cout, int H, int W, int K,
                         void* scratch, size_t scratch_bytes, void* stream);
+/* Multi-head self-attention of the conditional U-Net (8 heads of dim C / heads in {16, 32, 64}, seq = H * W, the
+ * transformer blocks' attn1) forward and backward in one call, for parity tests: q, k, v, dout fp32 [N, C, H, W] (channel
+ * c of head c / (C / heads)) -> out = softmax(q k^T / sqrt(D)) v and dq, dk, dv = the gradients of <out, dout>, all fp32
+ * [N, C, H, W]. Runs the training forward kernel (with its row log-sum-exp) and the backward kernels the model runs.
+ * scratch >= b200ad_mha_scratch_bytes. */
+size_t b200ad_mha_scratch_bytes(int N, int C, int heads, int H, int W);
+int b200ad_mha_forward_backward(const float* q, const float* k, const float* v, const float* dout, float* out, float* dq,
+                                float* dk, float* dv, int N, int C, int heads, int H, int W, void* scratch,
+                                size_t scratch_bytes, void* stream);
 /* GroupNorm(groups, eps) [+ SiLU] on fp32 NCHW through the stats + apply kernels. */
 int b200ad_group_norm(const float* x, const float* gamma, const float* beta, float* y, int N, int C, int H, int W,
                       int groups, float eps, int silu, void* scratch, size_t scratch_bytes, void* stream);
