@@ -31,8 +31,8 @@ constexpr int GB_PIX = 4096;     // pixels per CTA of the scalar-conv weight gra
 constexpr int GB_CHUNK = 8192;   // flat PF8 positions per CTA of the GroupNorm passes (32 vectors per thread, 4 in flight)
 
 // Both passes walk the FLAT position range [0, H * Wp) of one 8-channel plane (coalesced 16-byte vectors, no div / mod per
-// pixel).  The pad column of every row is zero in the raw tensors AND in the incoming gradient (conv_tc_kernel writes the
-// layout's guards as zeros), so it contributes nothing to the sums; the apply pass writes zeros there.
+// pixel).  The pad column of every row is zero in the raw tensors AND in the incoming gradient (buffers are zeroed at bind
+// time and every writer, conv_tc_kernel included, leaves the layout's guards zero), so it contributes nothing to the sums; the apply pass writes zeros there.
 // A CTA only needs the statistics of the (at most two) groups its plane touches: eight threads derive them.
 struct PlaneCoef {
   float mean[8], rstd[8], gam[8], bet[8];

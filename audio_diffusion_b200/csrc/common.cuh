@@ -1,5 +1,5 @@
-// Shared device helpers for the sm_90a kernels: mbarrier, 1-D bulk async copies (TMA engine,
-// SASS UBLKCP), wgmma (descriptors / mma / commit / wait) and the activation-layout arithmetic.
+// Shared device helpers for the sm_90a kernels: mbarrier, 1-D bulk async copies and tensor-map copies (TMA engine,
+// SASS UBLKCP / UTMALDG / UTMASTG), wgmma (descriptors / mma / commit / wait) and the activation-layout arithmetic.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -100,6 +100,19 @@ __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wa
 // named barrier among `nthreads` threads (ids 1..15; 0 is __syncthreads)
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+
+// 5-D tensor copies (TMA engine) through a tensor map; coordinates innermost first, signed: elements outside the tensor
+// read as zeros, and are not written by a store.  `tmap` is the generic address of a CUtensorMap in a __grid_constant__ param.
+__device__ __forceinline__ void tensor_g2s_5d(uint32_t dst_smem, const void* tmap, int c0, int c1, int c2, int c3, int c4,
+                                              uint32_t bar) {
+  asm volatile(
+      "cp.async.bulk.tensor.5d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5, %6}], [%7];"
+      ::"r"(dst_smem), "l"(tmap), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4), "r"(bar) : "memory");
+}
+__device__ __forceinline__ void tensor_s2g_5d(const void* tmap, int c0, int c1, int c2, int c3, int c4, uint32_t src_smem) {
+  asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.tile.bulk_group [%0, {%1, %2, %3, %4, %5}], [%6];"
+               ::"l"(tmap), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4), "r"(src_smem) : "memory");
 }
 
 __device__ __forceinline__ void bulk_prefetch_l2(const void* src, uint32_t bytes) {

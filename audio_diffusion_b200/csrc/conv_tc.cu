@@ -6,10 +6,17 @@
 //   pixels (activations are the B operand), K = 16 input channels per wgmma.m64nNk16.  The accumulators of an item
 //   (64 x 256 fp32 per warpgroup) live in registers, which caps an item at two 128-pixel tiles.
 // Pixel operand: the PF8 layout stores 8-channel vectors of consecutive pixels contiguously, which *is* the K-major
-//   no-swizzle core-matrix layout (8 rows x 16 B). A work item covers 2 x 128 consecutive flat pixels; per 16 input
-//   channels ONE contiguous window per 8-channel plane (the run plus a halo of Wp+1 pixels on both sides) is bulk-copied
-//   (TMA engine) into shared memory, and every tap is a descriptor whose start address is shifted by (dh*Wp + dw) * 16 B.
-//   (Few large copies: a bulk copy has a fixed cost however small it is.)
+//   no-swizzle core-matrix layout (8 rows x 16 B); along N the core matrices follow each other at a uniform stride (SBO).
+//   A work item covers 256 output pixels in one of two shapes, chosen per launch from the shape alone:
+//   - flat: 2 x 128 consecutive flat pixels.  Per 16 input channels ONE contiguous window per 8-channel plane (the run
+//     plus a halo of Wp+1 pixels on both sides) is bulk-copied (TMA engine) into shared memory; SBO = 128 B and every tap
+//     is a descriptor whose start address is shifted by (dh*Wp + dw) * 16 B.  (Few large copies: a bulk copy has a fixed
+//     cost however small it is.)
+//   - 2-D tile (ConvParams::tile2d): CONV_TW = 8 columns x CONV_TH = 32 rows.  Per 16 input channels one tensor-map copy
+//     lands the box [2 planes][32 + ht + hb rows][8 + hl + hr cols][8 ch]; each tile row is one core matrix, so SBO is the
+//     box row pitch (8 + hl + hr) * 16 B and a tap shifts the start address by (dh * pitch + dw) * 16 B.  At W = 256 the
+//     window is 10 x 34 pixels instead of 772, so each input pixel is loaded and normalised about once instead of three
+//     times.  Elements outside the image are zero-filled by the copy (the box is clipped at W, not at the pad column).
 // Fused GroupNorm(+SiLU): the windows hold the RAW producer output; the transform warps rewrite them in place
 //   (x * scale[n][c] + shift[n][c], SiLU via one tanh.approx, zero on pad/guard positions) between the TMA landing and
 //   the MMA reading them, so the normalised tensor never exists in HBM.
@@ -20,18 +27,40 @@
 //   a weight slot (and, after the last slot of a k-step, the activation stage) is released once its group has retired.
 // Epilogue (per consumer warpgroup, from registers): +bias/temb and GroupNorm partial sums -> cvt.rn.bf16x2 ->
 //   stmatrix.trans into a staging buffer ([plane][pixel][8 ch] = finished PF8 runs; the wgmma fragment puts the 8 channels
-//   of a plane in lanes 4 apart, which is exactly a transposed 8x8 matrix) -> one bulk store (TMA engine) per plane and
-//   tile, draining while the next item is multiplied.  Pad columns and the run-off behind the image are stored as the
-//   zeros the layout requires there.
+//   of a plane in lanes 4 apart, which is exactly a transposed 8x8 matrix) -> bulk stores (TMA engine) draining while the
+//   next item is multiplied.  Flat items: one bulk store per plane and tile; pad columns and the run-off behind the image
+//   are stored as the zeros the layout requires there.  2-D tiles: the staging pixels are tile-row-major, and one
+//   tensor-map store writes the warpgroup's 8 planes; every pixel is inside the image, so pads and guards are never
+//   written (they are zero from the workspace memset at bind time and no writer of a PF8 tensor puts anything else there).
 // Small images (H * Wp + bottom halo <= 128 pixels: 8x8 and below): an item's tiles are the first tiles of CONSECUTIVE
 //   IMAGES, so one weight fetch and one N = 256 MMA serve two samples (ConvParams::pack).
 // Warp roles (12 warps): 0 activation producer, 1 weight producer, 2-3 transform, 4-7 and 8-11 the two consumer
 //   warpgroups (MMA + epilogue).
+#include <cuda.h>
+#include <cudaTypedefs.h>
+
 #include <cstdlib>
 
 #include "conv_tc.cuh"
 
 namespace b200ad {
+
+// Tensor maps of a 2-D-tiled launch (encoded by launch_conv_tc; unused by flat launches).  5-D over a PF8 tensor:
+// {8 channels, W columns, H rows, 8-channel planes, images}, based at pixel (0, 0) of plane 0.
+struct alignas(64) ConvMaps {
+  CUtensorMap src[CONV_MAXSEG];   // box {8, 8 + hl + hr, 32 + ht + hb, 2, 1}: one k-step's window of segment s
+  CUtensorMap out;                // box {8, 8, 32, 8, 1}: one consumer warpgroup's staging buffer
+};
+
+// pixels per 8-channel plane of a segment's window (G: the item's 128-pixel tiles, flat items only)
+__host__ __device__ __forceinline__ int window_pixels(const ConvParams& p, const ConvSeg& sg, int G) {
+  return p.tile2d ? (CONV_TW + sg.hl + sg.hr) * (CONV_TH + sg.ht + sg.hb)
+                  : G * CONV_TM + (sg.ht + sg.hb) * p.Wp + sg.hl + sg.hr;
+}
+// pixels from one window row to the next
+__host__ __device__ __forceinline__ int window_pitch(const ConvParams& p, const ConvSeg& sg) {
+  return p.tile2d ? CONV_TW + sg.hl + sg.hr : p.Wp;
+}
 
 constexpr int CONV_THREADS = 384;     // 12 warps
 constexpr int CONV_XF_THREADS = 64;   // transform warps 2, 3
@@ -42,12 +71,23 @@ constexpr int CONV_STAGING = 2 * CONV_STG_WG;
 
 struct WorkItem {
   int n, ntile, m0, G;
+  int r0, c0;   // 2-D tiles: first row / column of the tile
 };
 
 __device__ __forceinline__ WorkItem decode_work(const ConvParams& p, int w) {
   WorkItem wi;
   wi.ntile = w % p.ntiles_n;
   const int gidx = w / p.ntiles_n;
+  if (p.tile2d) {   // tiles in column-major order: consecutive CTAs take vertically adjacent tiles, whose halos overlap in L2
+    wi.n = gidx / p.groups_per_img;
+    const int t = gidx - wi.n * p.groups_per_img, tx = t / p.tiles_y;
+    wi.r0 = (t - tx * p.tiles_y) * CONV_TH;
+    wi.c0 = tx * CONV_TW;
+    wi.m0 = 0;
+    wi.G = CONV_MAXG;
+    return wi;
+  }
+  wi.r0 = wi.c0 = 0;
   if (p.pack) {   // small images: the item's tiles are the first (only) tiles of p.pack (1, 2 or 4) CONSECUTIVE IMAGES n, n+1, ..
     wi.n = gidx * p.pack;
     wi.m0 = 0;
@@ -80,7 +120,8 @@ __device__ __forceinline__ uint4 xform_vec(uint4 v, const f32x2_t (&sc)[4], cons
   return make_uint4(u[0], u[1], u[2], u[3]);
 }
 
-__global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_constant__ ConvParams p) {
+__global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_constant__ ConvParams p,
+                                                                  const __grid_constant__ ConvMaps maps) {
   constexpr int ASM = CONV_AS_MAX, BSM = CONV_BS_MAX;
   const int AS = p.as;      // activation stages of this launch (CONV_AS .. CONV_AS_MAX)
   const int BS = p.bs;      // weight-ring depth of this launch (whatever the activation stages leave, CONV_BS .. CONV_BS_MAX)
@@ -130,6 +171,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_c
 
   if (warp == 0) {
     // ================================ activation producer: per k-step two windows (one per 8-channel plane), lanes 0 / 1
+    // (2-D tiles: one box holding both)
     int stage = 0;
     uint32_t phase = 0;
     if (p.dbg & 4) {   // experiment: start the CTAs out of phase so that their epilogue store bursts do not coincide
@@ -140,8 +182,9 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_c
       const WorkItem wi = decode_work(p, w);
       for (int it = 0; it < p.ktotal; ++it) {
         const int ks = p.sched[it] & 255;
-        const ConvSeg& sg = p.seg[p.sched[it] >> 8];
-        const int npix = wi.G * CONV_TM + (sg.ht + sg.hb) * p.Wp + sg.hl + sg.hr;
+        const int s = p.sched[it] >> 8;
+        const ConvSeg& sg = p.seg[s];
+        const int npix = window_pixels(p, sg, wi.G);
         const uint32_t row_bytes = (uint32_t)npix * 16u;
         const uint32_t full = bar_fullA + 8 * stage;
         if (lane == 0) {
@@ -150,7 +193,10 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_c
         }
         __syncwarp();
         const long long plane = (long long)(2 * ks + (lane & 1)) * p.PL;     // this lane's 8-channel plane of the k-step
-        if (!p.pack) {
+        if (p.tile2d) {   // both planes in one box
+          if (lane == 0)
+            tensor_g2s_5d(smem_base + stage * a_bytes, &maps.src[s], 0, wi.c0 - sg.hl, wi.r0 - sg.ht, 2 * ks, wi.n, full);
+        } else if (!p.pack) {
           const int pix0 = p.lead + wi.m0 - sg.ht * p.Wp - sg.hl;
           if (lane < 2)
             bulk_g2s(smem_base + stage * a_bytes + (uint32_t)lane * row_bytes,
@@ -229,8 +275,8 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_c
       };
       for (int kidx = 0; kidx < p.ktotal; ++kidx) {
         const ConvSeg& sg = p.seg[p.sched[kidx] >> 8];
-        const int npix = wi.G * CONV_TM + (sg.ht + sg.hb) * p.Wp + sg.hl + sg.hr;
-        const uint32_t xlbo = (uint32_t)npix * 16u;   // the second 8-channel plane of the window
+        const uint32_t xlbo = (uint32_t)window_pixels(p, sg, wi.G) * 16u;   // the second 8-channel plane of the window
+        const uint32_t xsbo = p.tile2d ? (uint32_t)window_pitch(p, sg) * 16u : 128u;   // the next 8 pixels along N
         const int ntaps = sg.ntaps;
         mbar_wait(bar_readyA + 8 * sa, pa);   // windows landed and (if asked) normalised in place
         const uint32_t abase = smem_base + sa * a_bytes;
@@ -241,7 +287,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_c
           wgmma_fence();
           for (int t = 0; t < nt; ++t) {
             const uint64_t wdesc = gmma_desc(bbase + (uint32_t)t * CONV_B_TAP, (CONV_NT / 8) * 128, 128);
-            const uint64_t xdesc = gmma_desc(abase + (uint32_t)sg.aoff[t0 + t] * 16u, xlbo, 128);
+            const uint64_t xdesc = gmma_desc(abase + (uint32_t)sg.aoff[t0 + t] * 16u, xlbo, xsbo);
             if (wi.G == 2) wgmma_m64n256k16<0, 0>(acc, wdesc, xdesc);
             else           wgmma_m64n128k16<0, 0>(acc, wdesc, xdesc);
           }
@@ -282,9 +328,9 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_c
 #pragma unroll
               for (int u = 0; u < 2; ++u) {
                 // pad columns and the run-off behind the image are written as ZEROS (they are zero guards of the layout)
-                // and do not count for the statistics
+                // and do not count for the statistics (a 2-D tile has none)
                 const int col1 = (col + 1 == p.Wp) ? 0 : col + 1;
-                const bool v0 = m < hw_end && col < p.W, v1 = m + 1 < hw_end && col1 < p.W;
+                const bool v0 = p.tile2d || (m < hw_end && col < p.W), v1 = p.tile2d || (m + 1 < hw_end && col1 < p.W);
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
                   const int j = g * (CONV_TM / 8) + 2 * k + u;
@@ -323,8 +369,15 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_c
           }
         }
       }
-      if (!p.up2) {
+      if (p.tile2d) {
         fence_proxy_async_smem();   // staging rows written through the generic proxy -> visible to the TMA engine
+        named_bar_sync(1 + cw, 128);
+        if (tid == 0 && !(p.dbg & 2)) {
+          tensor_s2g_5d(&maps.out, 0, wi.c0, wi.r0, wi.ntile * 16 + cw * 8, wi.n, stg_w);
+          bulk_commit();
+        }
+      } else if (!p.up2) {
+        fence_proxy_async_smem();
         named_bar_sync(1 + cw, 128);
         const int g = tid >> 3, pl = tid & 7;
         if (issuer && g < wi.G && !(p.dbg & 2)) {
@@ -362,7 +415,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_c
     uint32_t phase = 0;
     for (int w = blockIdx.x; w < p.total_work; w += gridDim.x) {
       const WorkItem wi = decode_work(p, w);
-      int last_s = -1, npix = 0, drow = 0, dcol = 0;
+      int last_s = -1, npix = 0, pitch = 0, cbase = 0, drow = 0, dcol = 0;
       const float2* ssn = nullptr;
       bool silu = false;
       int row0[2] = {0, 0}, col0[2] = {0, 0};
@@ -371,17 +424,27 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_c
         const ConvSeg& sg = p.seg[s];
         if (s != last_s) {     // per-segment state (the schedule may alternate between segments)
           last_s = s;
-          npix = wi.G * CONV_TM + (sg.ht + sg.hb) * p.Wp + sg.hl + sg.hr;
+          npix = window_pixels(p, sg, wi.G);
+          pitch = window_pitch(p, sg);
           ssn = sg.ss ? sg.ss + (long long)wi.n * sg.ss_stride : nullptr;
-          // flat position of this thread's first pixel(s); (row, col) advance incrementally (one sweep per iteration)
+          // Window pixel i is image pixel (row, cbase + col), col in [0, pitch): flat items start at flat position
+          // m0 - ht * Wp - hl (cbase 0), 2-D tiles at (r0 - ht, c0 - hl).  (row, col) of this thread's first pixel(s)
+          // advance incrementally (one sweep per iteration).
+          cbase = p.tile2d ? wi.c0 - sg.hl : 0;
 #pragma unroll
           for (int u = 0; u < 2; ++u) {
-            const int m_first = wi.m0 - sg.ht * p.Wp - sg.hl + (xg0 + u) * 32 + lane;
-            row0[u] = (m_first >= 0) ? m_first / p.Wp : -1 - ((-1 - m_first) / p.Wp);  // floor division
-            col0[u] = m_first - row0[u] * p.Wp;
+            const int i = (xg0 + u) * 32 + lane;
+            if (p.tile2d) {
+              row0[u] = wi.r0 - sg.ht + i / pitch;
+              col0[u] = i - (i / pitch) * pitch;
+            } else {
+              const int m_first = wi.m0 - sg.ht * p.Wp - sg.hl + i;
+              row0[u] = (m_first >= 0) ? m_first / p.Wp : -1 - ((-1 - m_first) / p.Wp);  // floor division
+              col0[u] = m_first - row0[u] * p.Wp;
+            }
           }
-          drow = XSWEEP / p.Wp;
-          dcol = XSWEEP - drow * p.Wp;
+          drow = XSWEEP / pitch;
+          dcol = XSWEEP - drow * pitch;
           silu = sg.silu != 0;
         }
         {
@@ -436,7 +499,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_c
                 if (u < xng) {
                   const int px = px0 + u * 32;
                   if (px < npix) {
-                    const bool valid = (row[u] >= 0) && (row[u] < p.H) && (col[u] < p.W);
+                    const bool valid = (row[u] >= 0) && (row[u] < p.H) && ((unsigned)(cbase + col[u]) < (unsigned)p.W);
                     uint4 a = make_uint4(0, 0, 0, 0), b = make_uint4(0, 0, 0, 0);
                     if (valid) {
                       a = base[px];
@@ -448,7 +511,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_c
                     base[npix + px] = b;
                   }
                   row[u] += drow; col[u] += dcol;
-                  if (col[u] >= p.Wp) { col[u] -= p.Wp; ++row[u]; }
+                  if (col[u] >= pitch) { col[u] -= pitch; ++row[u]; }
                 }
               }
             }
@@ -527,6 +590,29 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_c
       if (threadIdx.x == 0) *f.counter = 0u;
     }
   }
+}
+
+// Tensor map over `planes` 8-channel planes of a PF8 tensor of the launch's geometry, images `img_stride` elements apart;
+// box {8, bw, bh, bplanes, 1}.  The driver's encoder is reached through the runtime, so the library links only cudart.
+static cudaError_t encode_pf8_map(CUtensorMap* m, const __nv_bfloat16* base, const ConvParams& p, int planes,
+                                  long long img_stride, int bw, int bh, int bplanes) {
+  static PFN_cuTensorMapEncodeTiled_v12000 encode = nullptr;
+  if (!encode) {
+    void* fn = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    cudaError_t e = cudaGetDriverEntryPointByVersion("cuTensorMapEncodeTiled", &fn, 12000, cudaEnableDefault, &q);
+    if (e != cudaSuccess) return e;
+    if (q != cudaDriverEntryPointSuccess || !fn) return cudaErrorNotSupported;
+    encode = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(fn);
+  }
+  const cuuint64_t dim[5] = {8, (cuuint64_t)p.W, (cuuint64_t)p.H, (cuuint64_t)planes, (cuuint64_t)p.N};
+  const cuuint64_t stride[4] = {16, (cuuint64_t)p.Wp * 16, (cuuint64_t)p.PL * 16, (cuuint64_t)img_stride * 2};
+  const cuuint32_t box[5] = {8, (cuuint32_t)bw, (cuuint32_t)bh, (cuuint32_t)bplanes, 1};
+  const cuuint32_t estride[5] = {1, 1, 1, 1, 1};
+  const CUresult r = encode(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, (void*)(base + (long long)p.lead * 8), dim, stride, box,
+                            estride, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? cudaSuccess : cudaErrorInvalidValue;
 }
 
 cudaError_t launch_conv_tc(const ConvParams& p_in, int num_sms, cudaStream_t stream) {
@@ -621,18 +707,48 @@ cudaError_t launch_conv_tc(const ConvParams& p_in, int num_sms, cudaStream_t str
       p.total_work = ((p.N + best - 1) / best) * p.ntiles_n;
     }
   }
-  // the two windows of one k-step must fit an activation slot
-  int a_stage = 0;
   const int tiles_img = (p.H * p.Wp + CONV_TM - 1) / CONV_TM;
   const int max_g = p.pack ? p.pack : (tiles_img < CONV_MAXG ? tiles_img : CONV_MAXG);   // most tiles any item of this launch has
+  // 2-D tiles where their windows, summed over the segments, are smaller than the flat ones: W >= 64 for a 3x3 conv (the
+  // flat halo is two image rows, the tile's two rows of 8 + 2 pixels and two columns of 32 + 2).  The folded upsample
+  // scatters its output and packed small images are one tile each, so both stay flat.
+  p.tile2d = 0;
+  if (!p.pack && !p.up2 && !(dbg & 4096) && p.W % CONV_TW == 0 && p.H % CONV_TH == 0) {
+    ConvParams q = p;
+    q.tile2d = 1;
+    long long flat = 0, tiled = 0;
+    for (int s = 0; s < p.nseg; ++s) {
+      flat += window_pixels(p, p.seg[s], max_g);
+      tiled += window_pixels(q, p.seg[s], max_g);
+    }
+    if (tiled < flat) {
+      p.tile2d = 1;
+      p.tiles_y = p.H / CONV_TH;
+      p.groups_per_img = (p.W / CONV_TW) * p.tiles_y;
+      p.total_work = p.N * p.groups_per_img * p.ntiles_n;
+    }
+  }
+  // the two windows of one k-step must fit an activation slot
+  int a_stage = 0;
   for (int s = 0; s < p.nseg; ++s) {
     const ConvSeg& sg = p.seg[s];
-    const int npix = max_g * CONV_TM + (sg.ht + sg.hb) * p.Wp + sg.hl + sg.hr;
+    const int npix = window_pixels(p, sg, max_g), pitch = window_pitch(p, sg);
     a_stage = npix * 32 > a_stage ? npix * 32 : a_stage;
     if (sg.ntaps > CONV_MAXTAPS || sg.ntaps > CONV_BT * (CONV_BS - 1) || npix > 0x3FFF) return cudaErrorInvalidValue;
-    for (int t = 0; t < sg.ntaps; ++t) p.seg[s].aoff[t] = (sg.dh[t] + sg.ht) * p.Wp + sg.dw[t] + sg.hl;
+    for (int t = 0; t < sg.ntaps; ++t) p.seg[s].aoff[t] = (sg.dh[t] + sg.ht) * pitch + sg.dw[t] + sg.hl;
   }
   p.a_stage = (a_stage + 255) & ~255;
+  ConvMaps maps{};
+  if (p.tile2d) {
+    for (int s = 0; s < p.nseg; ++s) {
+      const ConvSeg& sg = p.seg[s];
+      cudaError_t e = encode_pf8_map(&maps.src[s], sg.src, p, 2 * sg.ksteps, sg.img_stride, CONV_TW + sg.hl + sg.hr,
+                                     CONV_TH + sg.ht + sg.hb, 2);
+      if (e != cudaSuccess) return e;
+    }
+    cudaError_t e = encode_pf8_map(&maps.out, p.out, p, p.cout / 8, (long long)(p.cout / 8) * p.PL * 8, CONV_TW, CONV_TH, 8);
+    if (e != cudaSuccess) return e;
+  }
   // Ring depths: W = 256 fills shared memory with 3 activation stages + 5 weight slots.  Launches with smaller windows (narrow
   // images, packed small images, 1-tap convs) have SHORT k-steps, and the TMA -> transform -> MMA chain of a stage (a few
   // thousand cycles of L2 latency) is then covered only by more stages in flight: first up to 6 activation stages, then the
@@ -660,7 +776,7 @@ cudaError_t launch_conv_tc(const ConvParams& p_in, int num_sms, cudaStream_t str
   }
   p.pdl = (dbg & 1024) ? 0 : 1;
   if (!p.pdl) {
-    conv_tc_kernel<<<grid, CONV_THREADS, smem, stream>>>(p);
+    conv_tc_kernel<<<grid, CONV_THREADS, smem, stream>>>(p, maps);
     return cudaGetLastError();
   }
   // launch with programmatic stream serialization: the grid may begin (prologue, weight prefetch) before its predecessor
@@ -675,7 +791,7 @@ cudaError_t launch_conv_tc(const ConvParams& p_in, int num_sms, cudaStream_t str
   at[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = at;
   cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, conv_tc_kernel, p);
+  return cudaLaunchKernelEx(&cfg, conv_tc_kernel, p, maps);
 }
 
 // ------------------------------------------------------------------------------------ identity weights

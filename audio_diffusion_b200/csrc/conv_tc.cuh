@@ -7,6 +7,8 @@ namespace b200ad {
 constexpr int CONV_NT = 128;        // output-channel tile = 2 x MMA M (one 64-row half per consumer warpgroup)
 constexpr int CONV_TM = 128;        // pixels per tile; an MMA covers up to two tiles (N = 256)
 constexpr int CONV_MAXG = 2;        // pixel tiles per work item: 64 x 256 fp32 accumulators = 128 registers per thread
+constexpr int CONV_TW = 8;          // 2-D item: CONV_TW columns (one core matrix of the MMA's N direction per tile row) ...
+constexpr int CONV_TH = CONV_MAXG * CONV_TM / CONV_TW;   // ... x 32 rows = 256 pixels
 constexpr int CONV_MAXSEG = 6;      // K-segments per launch (callers use up to 4; the launcher may split one, see below)
 constexpr int CONV_MAXTAPS = 9;
 constexpr int CONV_MAXSCHED = 256;  // k-steps of one item (all segments); a k-step index within its segment is 8 bits
@@ -36,7 +38,8 @@ struct ConvSeg {
   int ht, hb, hl, hr;          // halo rows above / below, pixels left / right, filled in by launch_conv_tc from dh / dw
   signed char dh[CONV_MAXTAPS];
   signed char dw[CONV_MAXTAPS];
-  int aoff[CONV_MAXTAPS];      // (dh + ht) * Wp + dw + hl, filled in by launch_conv_tc: window offset of each tap
+  int aoff[CONV_MAXTAPS];      // (dh + ht) * pitch + dw + hl, filled in by launch_conv_tc: window offset of each tap (pitch:
+                               // Wp for flat items, CONV_TW + hl + hr for 2-D tiles)
   // Fused GroupNorm(+SiLU) of this source, applied to the A strips in shared memory before the MMAs read them:
   // value = silu?(x * ss[n][c].x + ss[n][c].y), forced to 0 on pad / guard positions. nullptr: source is used as is.
   const float2* ss;            // [N][ss_stride] (pointer already offset to this source's first channel)
@@ -68,7 +71,10 @@ struct ConvParams {
   // window loads between many-tap k-steps.
   unsigned short sched[CONV_MAXSCHED];
   int a_stage;          // bytes reserved for the A strips of one stage (set by the launcher)
-  int groups_per_img;
+  // Item shape (set by the launcher): 0 = 256 consecutive flat pixels, 1 = a 2-D tile of CONV_TW columns x CONV_TH rows
+  int tile2d;
+  int tiles_y;          // 2-D tiles: H / CONV_TH (tiles per column of tiles)
+  int groups_per_img;   // items per image and cout tile
   int ntiles_n;         // cout / 128
   int total_work;       // N * groups_per_img * ntiles_n  (packed: ceil(N / 4) * ntiles_n)
   int pack;             // 0, or the images per item (1, 2, 4) for small images (image + bottom halo fit one 128-pixel tile):
@@ -85,7 +91,7 @@ struct ConvParams {
   // (2h + oy, 2w + ox) of the (2H, 2W) output tensor. One launch per output parity (oy, ox) with pre-summed 2x2 weights.
   int up2, oy, ox;
   ConvGnFin fin;
-  int dbg;                      // B200AD_CONV_DBG bit flags (timing experiments only): 2 no stores, 4 CTAs out of phase, 8 no epilogue work, 32 no weight loads, 64 no transform, 128 reorder 1-tap segments before the last main k-step, 256 no small-image packing, 512 rings fixed at CONV_AS stages / CONV_BS slots, 1024 no programmatic dependent launch, 2048 interleave 1-tap k-steps between many-tap ones
+  int dbg;                      // B200AD_CONV_DBG bit flags (timing experiments only): 2 no stores, 4 CTAs out of phase, 8 no epilogue work, 32 no weight loads, 64 no transform, 128 reorder 1-tap segments before the last main k-step, 256 no small-image packing, 512 rings fixed at CONV_AS stages / CONV_BS slots, 1024 no programmatic dependent launch, 2048 interleave 1-tap k-steps between many-tap ones, 4096 flat items only (no 2-D tiles)
 };
 
 cudaError_t launch_conv_tc(const ConvParams& p, int num_sms, cudaStream_t stream);
