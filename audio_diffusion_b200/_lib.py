@@ -74,8 +74,6 @@ SYMBOLS = {
     "b200ad_unet_set_training": (_I, [_VP, _I]),
     "b200ad_unet_grad_floats": (_SZ, [_VP]),
     "b200ad_unet_grad_offset": (_SZ, [_VP, _I]),
-    "b200ad_unet_set_grad_buckets": (_I, [_VP, _I, C.POINTER(C.c_size_t)]),
-    "b200ad_unet_grad_bucket_wait": (_I, [_VP, _I, _VP]),
     "b200ad_unet_backward_bytes": (_SZ, [_VP]),
     "b200ad_unet_bind_backward": (_I, [_VP, _VP, _SZ, _VP, _VP]),
     "b200ad_unet_backward": (_I, [_VP, _VP, _VP, _I, _VP]),

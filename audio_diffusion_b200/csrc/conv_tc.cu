@@ -164,56 +164,50 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_c
   // draining (its last wave, its last-CTA GroupNorm finalize).  Everything above, and the weight producer's prefetch below,
   // touches nothing that kernel writes (the packed weights are older); every other role waits for it here.  The next
   // launch is released at once - it parks at this same point.
-  if (p.pdl) {
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-    if (warp != 1) asm volatile("griddepcontrol.wait;" ::: "memory");
-  }
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  if (warp != 1) asm volatile("griddepcontrol.wait;" ::: "memory");
 
+  // Every role walks the k-steps of an item in the same order: segment by segment, k-step by k-step.
   if (warp == 0) {
     // ================================ activation producer: per k-step two windows (one per 8-channel plane), lanes 0 / 1
     // (2-D tiles: one box holding both)
     int stage = 0;
     uint32_t phase = 0;
-    if (p.dbg & 4) {   // experiment: start the CTAs out of phase so that their epilogue store bursts do not coincide
-      const long long t0 = clock64(), wait = (long long)(blockIdx.x & 7) * 2304;
-      while (clock64() - t0 < wait) {}
-    }
     for (int w = blockIdx.x; w < p.total_work; w += gridDim.x) {
       const WorkItem wi = decode_work(p, w);
-      for (int it = 0; it < p.ktotal; ++it) {
-        const int ks = p.sched[it] & 255;
-        const int s = p.sched[it] >> 8;
+      for (int s = 0; s < p.nseg; ++s) {
         const ConvSeg& sg = p.seg[s];
-        const int npix = window_pixels(p, sg, wi.G);
-        const uint32_t row_bytes = (uint32_t)npix * 16u;
-        const uint32_t full = bar_fullA + 8 * stage;
-        if (lane == 0) {
-          mbar_wait(bar_emptyA + 8 * stage, phase ^ 1);
-          mbar_arrive_expect_tx(full, 2u * row_bytes);
+        const uint32_t row_bytes = (uint32_t)window_pixels(p, sg, wi.G) * 16u;
+        for (int ks = 0; ks < sg.ksteps; ++ks) {
+          const uint32_t full = bar_fullA + 8 * stage;
+          if (lane == 0) {
+            mbar_wait(bar_emptyA + 8 * stage, phase ^ 1);
+            mbar_arrive_expect_tx(full, 2u * row_bytes);
+          }
+          __syncwarp();
+          const long long plane = (long long)(2 * ks + (lane & 1)) * p.PL;     // this lane's 8-channel plane of the k-step
+          if (p.tile2d) {   // both planes in one box
+            if (lane == 0)
+              tensor_g2s_5d(smem_base + stage * a_bytes, &maps.src[s], 0, wi.c0 - sg.hl, wi.r0 - sg.ht, 2 * ks, wi.n, full);
+          } else if (!p.pack) {
+            const int pix0 = p.lead + wi.m0 - sg.ht * p.Wp - sg.hl;
+            if (lane < 2)
+              bulk_g2s(smem_base + stage * a_bytes + (uint32_t)lane * row_bytes,
+                       sg.src + (long long)wi.n * sg.img_stride + (plane + pix0) * 8, row_bytes, full);
+          } else {
+            // packed small images: the window is [leading halo | tile 0 = image n | tile 1 = image n+1 | .. | trailing halo];
+            // lane 2g + plane copies tile g (tile 0 with the leading halo, the last tile with the trailing one) of its plane.
+            // Everything behind an image's H * Wp pixels is the zero guard of its own plane.
+            const int g = lane >> 1, lead_px = sg.ht * p.Wp + sg.hl, trail_px = sg.hb * p.Wp + sg.hr;
+            const int cnt = CONV_TM + (g == 0 ? lead_px : 0) + (g == wi.G - 1 ? trail_px : 0);
+            const int doff = (g == 0) ? 0 : lead_px + g * CONV_TM;                      // pixels into the plane's window
+            const int pix0 = p.lead - (g == 0 ? lead_px : 0);
+            if (g < wi.G && lane < 2 * CONV_MAXG)
+              bulk_g2s(smem_base + stage * a_bytes + (uint32_t)(lane & 1) * row_bytes + (uint32_t)doff * 16u,
+                       sg.src + (long long)(wi.n + g) * sg.img_stride + (plane + pix0) * 8, (uint32_t)cnt * 16u, full);
+          }
+          if (++stage == AS) { stage = 0; phase ^= 1; }
         }
-        __syncwarp();
-        const long long plane = (long long)(2 * ks + (lane & 1)) * p.PL;     // this lane's 8-channel plane of the k-step
-        if (p.tile2d) {   // both planes in one box
-          if (lane == 0)
-            tensor_g2s_5d(smem_base + stage * a_bytes, &maps.src[s], 0, wi.c0 - sg.hl, wi.r0 - sg.ht, 2 * ks, wi.n, full);
-        } else if (!p.pack) {
-          const int pix0 = p.lead + wi.m0 - sg.ht * p.Wp - sg.hl;
-          if (lane < 2)
-            bulk_g2s(smem_base + stage * a_bytes + (uint32_t)lane * row_bytes,
-                     sg.src + (long long)wi.n * sg.img_stride + (plane + pix0) * 8, row_bytes, full);
-        } else {
-          // packed small images: the window is [leading halo | tile 0 = image n | tile 1 = image n+1 | .. | trailing halo];
-          // lane 2g + plane copies tile g (tile 0 with the leading halo, the last tile with the trailing one) of its plane.
-          // Everything behind an image's H * Wp pixels is the zero guard of its own plane.
-          const int g = lane >> 1, lead_px = sg.ht * p.Wp + sg.hl, trail_px = sg.hb * p.Wp + sg.hr;
-          const int cnt = CONV_TM + (g == 0 ? lead_px : 0) + (g == wi.G - 1 ? trail_px : 0);
-          const int doff = (g == 0) ? 0 : lead_px + g * CONV_TM;                      // pixels into the plane's window
-          const int pix0 = p.lead - (g == 0 ? lead_px : 0);
-          if (g < wi.G && lane < 2 * CONV_MAXG)
-            bulk_g2s(smem_base + stage * a_bytes + (uint32_t)(lane & 1) * row_bytes + (uint32_t)doff * 16u,
-                     sg.src + (long long)(wi.n + g) * sg.img_stride + (plane + pix0) * 8, (uint32_t)cnt * 16u, full);
-        }
-        if (++stage == AS) { stage = 0; phase ^= 1; }
       }
     }
   } else if (warp == 1) {
@@ -223,22 +217,23 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_c
       uint32_t phase = 0;
       for (int w = blockIdx.x; w < p.total_work; w += gridDim.x) {
         const int ntile = w % p.ntiles_n;
-        for (int it = 0; it < p.ktotal; ++it) {
-          const int ks = p.sched[it] & 255;
-          const ConvSeg& sg = p.seg[p.sched[it] >> 8];
-          const char* src = reinterpret_cast<const char*>(sg.wpack + (long long)ntile * sg.wtile_stride +
-                                                          (long long)ks * sg.ntaps * (CONV_B_TAP / 2));
-          for (int t0 = 0; t0 < sg.ntaps; t0 += CONV_BT) {
-            const uint32_t bytes = (uint32_t)min(CONV_BT, sg.ntaps - t0) * CONV_B_TAP;
-            mbar_wait(bar_emptyB + 8 * stage, phase ^ 1);
-            if (p.dbg & 32) {      // experiment: no weight traffic at all (bounds what sharing weight fetches could buy)
-              mbar_arrive(bar_fullB + 8 * stage);
-            } else {
-              mbar_arrive_expect_tx(bar_fullB + 8 * stage, bytes);
-              bulk_g2s(bring_base + stage * CONV_B_SLOT, src, bytes, bar_fullB + 8 * stage);
+        for (int s = 0; s < p.nseg; ++s) {
+          const ConvSeg& sg = p.seg[s];
+          // a segment's weights of one cout tile are its k-steps' tap blocks, one after the other
+          const char* src = reinterpret_cast<const char*>(sg.wpack + (long long)ntile * sg.wtile_stride);
+          for (int ks = 0; ks < sg.ksteps; ++ks) {
+            for (int t0 = 0; t0 < sg.ntaps; t0 += CONV_BT) {
+              const uint32_t bytes = (uint32_t)min(CONV_BT, sg.ntaps - t0) * CONV_B_TAP;
+              mbar_wait(bar_emptyB + 8 * stage, phase ^ 1);
+              if (p.dbg & 32) {      // experiment: no weight traffic at all (bounds what sharing weight fetches could buy)
+                mbar_arrive(bar_fullB + 8 * stage);
+              } else {
+                mbar_arrive_expect_tx(bar_fullB + 8 * stage, bytes);
+                bulk_g2s(bring_base + stage * CONV_B_SLOT, src, bytes, bar_fullB + 8 * stage);
+              }
+              src += bytes;
+              if (++stage == BS) { stage = 0; phase ^= 1; }
             }
-            src += bytes;
-            if (++stage == BS) { stage = 0; phase ^= 1; }
           }
         }
       }
@@ -273,8 +268,9 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_c
           if (pend_a >= 0) mbar_arrive(bar_emptyA + 8 * pend_a);
         }
       };
-      for (int kidx = 0; kidx < p.ktotal; ++kidx) {
-        const ConvSeg& sg = p.seg[p.sched[kidx] >> 8];
+      // one loop with a (segment, k-step) cursor: nested loops cost this role two registers (162 instead of 160)
+      for (int s = 0, ks = 0; s < p.nseg;) {
+        const ConvSeg& sg = p.seg[s];
         const uint32_t xlbo = (uint32_t)window_pixels(p, sg, wi.G) * 16u;   // the second 8-channel plane of the window
         const uint32_t xsbo = p.tile2d ? (uint32_t)window_pitch(p, sg) * 16u : 128u;   // the next 8 pixels along N
         const int ntaps = sg.ntaps;
@@ -299,6 +295,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_c
           if (++sb == BS) { sb = 0; pb ^= 1; }
         }
         if (++sa == AS) { sa = 0; pa ^= 1; }
+        if (++ks == sg.ksteps) { ks = 0; ++s; }
       }
       wgmma_wait<0>();
       release();
@@ -408,46 +405,33 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_c
   } else {
     // ================================ transform warps (2, 3): GroupNorm(+SiLU) of the landed windows, in place.
     // Every 64-pixel sweep of a window is two groups of 32 pixels, one per transform warp.
-    const int xg0 = warp - 2;
-    constexpr int xng = 1;
-    constexpr int XSWEEP = CONV_XF_THREADS;
+    const int tidx = (warp - 2) * 32 + lane;   // this thread's first pixel of a window
     int stage = 0;
     uint32_t phase = 0;
     for (int w = blockIdx.x; w < p.total_work; w += gridDim.x) {
       const WorkItem wi = decode_work(p, w);
-      int last_s = -1, npix = 0, pitch = 0, cbase = 0, drow = 0, dcol = 0;
-      const float2* ssn = nullptr;
-      bool silu = false;
-      int row0[2] = {0, 0}, col0[2] = {0, 0};
-      for (int it = 0; it < p.ktotal; ++it) {
-        const int ks = p.sched[it] & 255, s = p.sched[it] >> 8;
+      for (int s = 0; s < p.nseg; ++s) {
         const ConvSeg& sg = p.seg[s];
-        if (s != last_s) {     // per-segment state (the schedule may alternate between segments)
-          last_s = s;
-          npix = window_pixels(p, sg, wi.G);
-          pitch = window_pitch(p, sg);
-          ssn = sg.ss ? sg.ss + (long long)wi.n * sg.ss_stride : nullptr;
-          // Window pixel i is image pixel (row, cbase + col), col in [0, pitch): flat items start at flat position
-          // m0 - ht * Wp - hl (cbase 0), 2-D tiles at (r0 - ht, c0 - hl).  (row, col) of this thread's first pixel(s)
-          // advance incrementally (one sweep per iteration).
-          cbase = p.tile2d ? wi.c0 - sg.hl : 0;
-#pragma unroll
-          for (int u = 0; u < 2; ++u) {
-            const int i = (xg0 + u) * 32 + lane;
-            if (p.tile2d) {
-              row0[u] = wi.r0 - sg.ht + i / pitch;
-              col0[u] = i - (i / pitch) * pitch;
-            } else {
-              const int m_first = wi.m0 - sg.ht * p.Wp - sg.hl + i;
-              row0[u] = (m_first >= 0) ? m_first / p.Wp : -1 - ((-1 - m_first) / p.Wp);  // floor division
-              col0[u] = m_first - row0[u] * p.Wp;
-            }
-          }
-          drow = XSWEEP / pitch;
-          dcol = XSWEEP - drow * pitch;
-          silu = sg.silu != 0;
+        const int npix = window_pixels(p, sg, wi.G);
+        const int pitch = window_pitch(p, sg);
+        const float2* ssn = sg.ss ? sg.ss + (long long)wi.n * sg.ss_stride : nullptr;
+        // Window pixel i is image pixel (row, cbase + col), col in [0, pitch): flat items start at flat position
+        // m0 - ht * Wp - hl (cbase 0), 2-D tiles at (r0 - ht, c0 - hl).  (row, col) of this thread's pixel advance
+        // incrementally (one sweep per iteration).
+        const int cbase = p.tile2d ? wi.c0 - sg.hl : 0;
+        int row0, col0;
+        if (p.tile2d) {
+          row0 = wi.r0 - sg.ht + tidx / pitch;
+          col0 = tidx - (tidx / pitch) * pitch;
+        } else {
+          const int m_first = wi.m0 - sg.ht * p.Wp - sg.hl + tidx;
+          row0 = (m_first >= 0) ? m_first / p.Wp : -1 - ((-1 - m_first) / p.Wp);  // floor division
+          col0 = m_first - row0 * p.Wp;
         }
-        {
+        const int drow = CONV_XF_THREADS / pitch;
+        const int dcol = CONV_XF_THREADS - drow * pitch;
+        const bool silu = sg.silu != 0;
+        for (int ks = 0; ks < sg.ksteps; ++ks) {
           f32x2_t sc0[4], sh0[4], sc1[4], sh1[4];
           if (ssn && !p.pack) {
             const float4* sp = reinterpret_cast<const float4*>(ssn + ks * 16);
@@ -465,7 +449,6 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_c
             // touched - everything else in the window is zero guard from global memory and stays zero
             uint4* base = reinterpret_cast<uint4*>(smem + stage * a_bytes);
             const int lead_px = sg.ht * p.Wp + sg.hl, hw = p.H * p.Wp;
-            const int tidx = (warp - 2) * 32 + lane;
             const float hs = silu ? 0.5f : 1.0f;
             for (int g = 0; g < wi.G; ++g) {
               const float4* sp = reinterpret_cast<const float4*>(ssn + (long long)g * sg.ss_stride + ks * 16);
@@ -492,28 +475,20 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_c
             fence_proxy_async_smem();
           } else if (ssn && !(p.dbg & 64)) {
             uint4* base = reinterpret_cast<uint4*>(smem + stage * a_bytes);
-            int row[2] = {row0[0], row0[1]}, col[2] = {col0[0], col0[1]};
-            for (int px0 = xg0 * 32 + lane; px0 < npix; px0 += XSWEEP) {
-#pragma unroll
-              for (int u = 0; u < 2; ++u) {
-                if (u < xng) {
-                  const int px = px0 + u * 32;
-                  if (px < npix) {
-                    const bool valid = (row[u] >= 0) && (row[u] < p.H) && ((unsigned)(cbase + col[u]) < (unsigned)p.W);
-                    uint4 a = make_uint4(0, 0, 0, 0), b = make_uint4(0, 0, 0, 0);
-                    if (valid) {
-                      a = base[px];
-                      b = base[npix + px];
-                      if (silu) { a = xform_vec<true>(a, sc0, sh0); b = xform_vec<true>(b, sc1, sh1); }
-                      else      { a = xform_vec<false>(a, sc0, sh0); b = xform_vec<false>(b, sc1, sh1); }
-                    }
-                    base[px] = a;
-                    base[npix + px] = b;
-                  }
-                  row[u] += drow; col[u] += dcol;
-                  if (col[u] >= pitch) { col[u] -= pitch; ++row[u]; }
-                }
+            int row = row0, col = col0;
+            for (int px = tidx; px < npix; px += CONV_XF_THREADS) {
+              const bool valid = (row >= 0) && (row < p.H) && ((unsigned)(cbase + col) < (unsigned)p.W);
+              uint4 a = make_uint4(0, 0, 0, 0), b = make_uint4(0, 0, 0, 0);
+              if (valid) {
+                a = base[px];
+                b = base[npix + px];
+                if (silu) { a = xform_vec<true>(a, sc0, sh0); b = xform_vec<true>(b, sc1, sh1); }
+                else      { a = xform_vec<false>(a, sc0, sh0); b = xform_vec<false>(b, sc1, sh1); }
               }
+              base[px] = a;
+              base[npix + px] = b;
+              row += drow; col += dcol;
+              if (col >= pitch) { col -= pitch; ++row; }
             }
             fence_proxy_async_smem();
           }
@@ -624,58 +599,12 @@ cudaError_t launch_conv_tc(const ConvParams& p_in, int num_sms, cudaStream_t str
   p.dbg = dbg;
   for (int s = 0; s < p.nseg; ++s) {
     ConvSeg& sg = p.seg[s];
-    if (sg.ntaps > CONV_MAXTAPS) return cudaErrorInvalidValue;
+    if (sg.ntaps > CONV_MAXTAPS || sg.ksteps < 1) return cudaErrorInvalidValue;
     if (sg.wtile_stride == 0) sg.wtile_stride = (long long)sg.ksteps * sg.ntaps * (CONV_B_TAP / 2);
     sg.ht = sg.hb = sg.hl = sg.hr = 0;
     for (int t = 0; t < sg.ntaps; ++t) {
       sg.ht |= sg.dh[t] < 0; sg.hb |= sg.dh[t] > 0;
       sg.hl |= sg.dw[t] < 0; sg.hr |= sg.dw[t] > 0;
-    }
-  }
-  // Experiment (B200AD_CONV_DBG & 128, off by default): move trailing 1-tap segments (shortcut / residual) in front of the
-  // main segment's last k-step so that a many-tap k-step closes the K loop.  The 1-tap k-steps are load-bound (a 16 KB
-  // window per k-step of MMAs) and would stall the ring in the middle of the item instead of next to the epilogue.
-  if ((dbg & 128) && p.nseg >= 2 && p.nseg < CONV_MAXSEG && p.seg[0].ksteps >= 2 && p.seg[p.nseg - 1].ntaps < p.seg[0].ntaps) {
-    ConvSeg tail = p.seg[0];
-    const int ka = tail.ksteps - 1;
-    p.seg[0].ksteps = ka;
-    tail.ksteps = 1;
-    tail.src += (long long)ka * 2 * p.PL * 8;
-    tail.wpack += (long long)ka * tail.ntaps * (CONV_B_TAP / 2);
-    if (tail.ss) tail.ss += ka * 16;
-    p.seg[p.nseg++] = tail;
-  }
-  p.ktotal = 0;
-  for (int s = 0; s < p.nseg; ++s) {
-    if (p.seg[s].ksteps > 255) return cudaErrorInvalidValue;
-    p.ktotal += p.seg[s].ksteps;
-  }
-  if (p.ktotal > CONV_MAXSCHED) return cudaErrorInvalidValue;
-  {
-    // heavy = many-tap k-steps in segment order, light = 1-tap k-steps in segment order; light ones are spread evenly over
-    // the gaps between heavy ones
-    int nh = 0, nl = 0;
-    for (int s = 0; s < p.nseg; ++s) (p.seg[s].ntaps > 1 ? nh : nl) += p.seg[s].ksteps;
-    int n = 0;
-    // (interleaving is an experiment switch, B200AD_CONV_DBG & 2048, not the default)
-    if (!(dbg & 2048) || nh < 2 || nl == 0) {
-      for (int s = 0; s < p.nseg; ++s)
-        for (int ks = 0; ks < p.seg[s].ksteps; ++ks) p.sched[n++] = (unsigned short)((s << 8) | ks);
-    } else {
-      int hs = 0, hk = 0, ls = 0, lk = 0;      // cursors (segment, k-step) into the heavy / light sequences
-      auto next = [&](bool heavy, int& cs, int& ck) {
-        while ((p.seg[cs].ntaps > 1) != heavy || ck >= p.seg[cs].ksteps) { ++cs; ck = 0; }
-        p.sched[n++] = (unsigned short)((cs << 8) | ck);
-        ++ck;
-      };
-      int emitted_light = 0;
-      for (int i = 0; i < nh; ++i) {
-        next(true, hs, hk);
-        if (i < nh - 1) {
-          const int want = (int)((long long)(i + 1) * nl / (nh - 1));     // light k-steps due after heavy k-step i
-          for (; emitted_light < want; ++emitted_light) next(false, ls, lk);
-        }
-      }
     }
   }
   p.groups_per_img = (p.H * p.Wp + CONV_MAXG * CONV_TM - 1) / (CONV_MAXG * CONV_TM);
@@ -687,25 +616,23 @@ cudaError_t launch_conv_tc(const ConvParams& p_in, int num_sms, cudaStream_t str
   // n + g's plane from its pixel 0 on, whose tail is that image's own zero guard, so every tap of a valid output pixel stays
   // inside its tile (needs H * Wp + the bottom halo <= 128) and the MMA issue is unchanged.
   p.pack = 0;
-  if (!(dbg & 256)) {
-    int fits = 1;
-    for (int s = 0; s < p.nseg; ++s) {
-      const ConvSeg& sg = p.seg[s];
-      if (p.H * p.Wp + sg.hb * p.Wp + sg.hr > CONV_TM || sg.ht * p.Wp + sg.hl > CONV_TM) fits = 0;
+  int fits = 1;
+  for (int s = 0; s < p.nseg; ++s) {
+    const ConvSeg& sg = p.seg[s];
+    if (p.H * p.Wp + sg.hb * p.Wp + sg.hr > CONV_TM || sg.ht * p.Wp + sg.hl > CONV_TM) fits = 0;
+  }
+  if (fits) {
+    // images per item: the MMA time of an item grows with its tiles (1 : 2 : 4), the number of waves shrinks with them;
+    // take the fewest (waves x tiles), the larger group on a tie (fewer weight fetches)
+    int best = 1;
+    long long best_cost = -1;
+    for (int g = 1; g <= CONV_MAXG; g *= 2) {
+      const long long items = (long long)((p.N + g - 1) / g) * p.ntiles_n;
+      const long long cost = ((items + num_sms - 1) / num_sms) * g;
+      if (best_cost < 0 || cost <= best_cost) { best_cost = cost; best = g; }
     }
-    if (fits) {
-      // images per item: the MMA time of an item grows with its tiles (1 : 2 : 4), the number of waves shrinks with them;
-      // take the fewest (waves x tiles), the larger group on a tie (fewer weight fetches)
-      int best = 1;
-      long long best_cost = -1;
-      for (int g = 1; g <= CONV_MAXG; g *= 2) {
-        const long long items = (long long)((p.N + g - 1) / g) * p.ntiles_n;
-        const long long cost = ((items + num_sms - 1) / num_sms) * g;
-        if (best_cost < 0 || cost <= best_cost) { best_cost = cost; best = g; }
-      }
-      p.pack = best;
-      p.total_work = ((p.N + best - 1) / best) * p.ntiles_n;
-    }
+    p.pack = best;
+    p.total_work = ((p.N + best - 1) / best) * p.ntiles_n;
   }
   const int tiles_img = (p.H * p.Wp + CONV_TM - 1) / CONV_TM;
   const int max_g = p.pack ? p.pack : (tiles_img < CONV_MAXG ? tiles_img : CONV_MAXG);   // most tiles any item of this launch has
@@ -755,15 +682,13 @@ cudaError_t launch_conv_tc(const ConvParams& p_in, int num_sms, cudaStream_t str
   // weight ring up to its maximum, then the remaining activation stages.
   p.as = CONV_AS;
   p.bs = CONV_BS;
-  if (!(dbg & 512)) {
-    auto fits = [&](int as, int bs) {
-      // 1 KB of head room: the kernel's static shared memory counts against the same 227 KB
-      return (size_t)as * p.a_stage + (size_t)bs * CONV_B_SLOT + CONV_STAGING + 2048 <= (size_t)CONV_SMEM_MAX;
-    };
-    while (p.as < 6 && fits(p.as + 1, p.bs)) ++p.as;
-    while (p.bs < CONV_BS_MAX && fits(p.as, p.bs + 1)) ++p.bs;
-    while (p.as < CONV_AS_MAX && fits(p.as + 1, p.bs)) ++p.as;
-  }
+  auto rings_fit = [&](int as, int bs) {
+    // 1 KB of head room: the kernel's static shared memory counts against the same 227 KB
+    return (size_t)as * p.a_stage + (size_t)bs * CONV_B_SLOT + CONV_STAGING + 2048 <= (size_t)CONV_SMEM_MAX;
+  };
+  while (p.as < 6 && rings_fit(p.as + 1, p.bs)) ++p.as;
+  while (p.bs < CONV_BS_MAX && rings_fit(p.as, p.bs + 1)) ++p.bs;
+  while (p.as < CONV_AS_MAX && rings_fit(p.as + 1, p.bs)) ++p.as;
   const size_t smem = (size_t)p.as * p.a_stage + (size_t)p.bs * CONV_B_SLOT + CONV_STAGING + 1024;
   if (smem > (size_t)CONV_SMEM_MAX) return cudaErrorInvalidValue;  // image too wide for this tiling
   const int grid = p.total_work < num_sms ? p.total_work : num_sms;
@@ -773,11 +698,6 @@ cudaError_t launch_conv_tc(const ConvParams& p_in, int num_sms, cudaStream_t str
     cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     attr = smem;
-  }
-  p.pdl = (dbg & 1024) ? 0 : 1;
-  if (!p.pdl) {
-    conv_tc_kernel<<<grid, CONV_THREADS, smem, stream>>>(p, maps);
-    return cudaGetLastError();
   }
   // launch with programmatic stream serialization: the grid may begin (prologue, weight prefetch) before its predecessor
   // has completed; it synchronises on the predecessor itself (griddepcontrol.wait) before touching anything it depends on

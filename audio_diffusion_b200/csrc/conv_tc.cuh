@@ -9,9 +9,8 @@ constexpr int CONV_TM = 128;        // pixels per tile; an MMA covers up to two 
 constexpr int CONV_MAXG = 2;        // pixel tiles per work item: 64 x 256 fp32 accumulators = 128 registers per thread
 constexpr int CONV_TW = 8;          // 2-D item: CONV_TW columns (one core matrix of the MMA's N direction per tile row) ...
 constexpr int CONV_TH = CONV_MAXG * CONV_TM / CONV_TW;   // ... x 32 rows = 256 pixels
-constexpr int CONV_MAXSEG = 6;      // K-segments per launch (callers use up to 4; the launcher may split one, see below)
+constexpr int CONV_MAXSEG = 4;      // K-segments per launch
 constexpr int CONV_MAXTAPS = 9;
-constexpr int CONV_MAXSCHED = 256;  // k-steps of one item (all segments); a k-step index within its segment is 8 bits
 constexpr int CONV_B_TAP = 16 * CONV_NT * 2;     // one tap, 16 input channels: 4096 B
 constexpr int CONV_SMEM_MAX = 227 * 1024;
 
@@ -65,11 +64,6 @@ struct ConvParams {
   ConvSeg seg[CONV_MAXSEG];
   int nseg;
   int N, H, W, Wp, lead, PL;
-  int ktotal;           // sum of the segments' k-steps (set by the launcher)
-  // Order of the k-steps of an item, (segment << 8) | k-step (set by the launcher): segment by segment.  Experiment
-  // (B200AD_CONV_DBG & 2048): many-tap and 1-tap k-steps (shortcut, residual) interleaved, to spread the 1-tap k-steps'
-  // window loads between many-tap k-steps.
-  unsigned short sched[CONV_MAXSCHED];
   int a_stage;          // bytes reserved for the A strips of one stage (set by the launcher)
   // Item shape (set by the launcher): 0 = 256 consecutive flat pixels, 1 = a 2-D tile of CONV_TW columns x CONV_TH rows
   int tile2d;
@@ -80,7 +74,6 @@ struct ConvParams {
   int pack;             // 0, or the images per item (1, 2, 4) for small images (image + bottom halo fit one 128-pixel tile):
                         // an item's tiles are consecutive images, so a weight fetch and an N = 256 MMA serve several samples
   int as, bs;           // activation stages / weight-ring slots of this launch (set by the launcher)
-  int pdl;              // launched with programmatic stream serialization (set by the launcher)
   int cout;
   __nv_bfloat16* out;           // PF8, cout channels
   const float* bias;            // [cout]
@@ -91,7 +84,7 @@ struct ConvParams {
   // (2h + oy, 2w + ox) of the (2H, 2W) output tensor. One launch per output parity (oy, ox) with pre-summed 2x2 weights.
   int up2, oy, ox;
   ConvGnFin fin;
-  int dbg;                      // B200AD_CONV_DBG bit flags (timing experiments only): 2 no stores, 4 CTAs out of phase, 8 no epilogue work, 32 no weight loads, 64 no transform, 128 reorder 1-tap segments before the last main k-step, 256 no small-image packing, 512 rings fixed at CONV_AS stages / CONV_BS slots, 1024 no programmatic dependent launch, 2048 interleave 1-tap k-steps between many-tap ones, 4096 flat items only (no 2-D tiles)
+  int dbg;                      // B200AD_CONV_DBG bit flags: 2 no stores, 8 no epilogue work, 32 no weight loads, 64 no transform (each removes a piece of work to measure its cost); 4096 flat items only (no 2-D tiles: the reference of the tiled path)
 };
 
 cudaError_t launch_conv_tc(const ConvParams& p, int num_sms, cudaStream_t stream);

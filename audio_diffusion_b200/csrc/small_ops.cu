@@ -2,8 +2,6 @@
 // Reference semantics: diffusers get_timestep_embedding(flip_sin_to_cos=True, freq_shift=0), TimestepEmbedding,
 // ResnetBlock2D.time_emb_proj(silu(emb)) and Attention/AttnProcessor2_0 (oracle/unet_oracle.py restates them;
 // reached from audiodiffusion/pipeline_audio_diffusion.py:163).
-#include <cstdlib>
-
 #include "kernels.cuh"
 
 namespace b200ad {
@@ -252,8 +250,7 @@ __global__ void __launch_bounds__(128) attention_mma_kernel(const __nv_bfloat16*
 cudaError_t launch_attention(const __nv_bfloat16* qkv, __nv_bfloat16* out, int N, int C, int H, int W, cudaStream_t s) {
   const int seq = H * W;
   dim3 grid(C >> 3, N);
-  static const bool force_simt = [] { const char* e = getenv("B200AD_ATTN_SIMT"); return e && e[0] == '1'; }();
-  if ((seq % 16) == 0 && (size_t)seq * 32 <= 48 * 1024 && !force_simt) {
+  if ((seq % 16) == 0 && (size_t)seq * 32 <= 48 * 1024) {
     attention_mma_kernel<<<grid, 128, (size_t)seq * 32, s>>>(qkv, out, N, C, H, W);
     return cudaGetLastError();
   }

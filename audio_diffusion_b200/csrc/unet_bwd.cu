@@ -56,20 +56,7 @@ struct Backward {
   float* grads = nullptr;
   int launches = 0;
   PackBatch pack_batch;              // one launch for all transposed packs
-  // gradient buckets (data-parallel all-reduce overlapped with the rest of the backward pass): bucket k = floats
-  // [bucket_lo[k], bucket_lo[k+1]); its event is recorded right after the last launch that adds into it
-  std::vector<size_t> bucket_lo;
-  std::vector<cudaEvent_t> bucket_ev;
-  std::vector<int> bucket_last_op;   // index into ops (-1: nothing writes it -> recorded before the first op)
 };
-
-static void free_bucket_events(Backward* bw) {
-  for (cudaEvent_t e : bw->bucket_ev) cudaEventDestroy(e);
-  bw->bucket_ev.clear();
-  bw->bucket_lo.clear();
-  bw->bucket_last_op.clear();
-}
-
 
 namespace b200ad {
 
@@ -128,12 +115,11 @@ struct BwdBuilder {
 
   // ---- transposed weight packing jobs ----------------------------------------------------------------------------
   // GEMM out channels = the layer's input channels [i0, i0 + I) ... the kernel reads W[o][i][kh][kw] with i = co.
-  // Only the layer's output channels [o_off, o_off + o_cnt) are packed when o_cnt >= 0 (one K-segment of a split reduction).
   // Returns the packed weights (null in the size pass).
-  const __nv_bfloat16* tjob(const std::string& wname, int O, int I, int K, const TapSet& t, int o_off = 0, int o_cnt = -1) {
+  const __nv_bfloat16* tjob(const std::string& wname, int O, int I, int K, const TapSet& t) {
     PackJob j;
     j.w_param = h->pidx.at(wname);
-    j.cout = I; j.cin_total = O; j.KH = K; j.KW = K; j.cin_off = o_off; j.ksteps = (o_cnt < 0 ? O : o_cnt) / 16;
+    j.cout = I; j.cin_total = O; j.KH = K; j.KW = K; j.cin_off = 0; j.ksteps = O / 16;
     j.taps = t.pack;
     j.cout_real = I;
     j.off = take_off(mem, (size_t)(I / 128) * j.ksteps * t.pack.ntaps * CONV_B_TAP);
@@ -368,18 +354,9 @@ struct BwdBuilder {
       op.src = ff1.p; op.src2 = Ggg.p; op.dst = Gff1.p; op.C = 4 * C; op.H = H; op.W = W;
       bw->ops.push_back(op);
     }
-    // ff.net.0.proj: the 8C-channel reduction as two K-segments (a segment holds at most 255 k-steps of 16 channels)
+    // ff.net.0.proj
     Act Gn = tmp("tf_Gn", C, H, W);
-    {
-      BOp op{};
-      op.kind = BOp::CONV;
-      conv_base(op.conv, Gn);
-      const TapSet ts = taps_mirrored(1);
-      for (int j = 0; j < 2; ++j)
-        seg(op.conv.seg[j], view(Gff1, j * 4 * C, 4 * C), tjob(t + ".ff.net.0.proj.weight", 8 * C, C, 1, ts, j * 4 * C, 4 * C), ts);
-      op.conv.nseg = 2;
-      bw->ops.push_back(op);
-    }
+    dgrad(t + ".ff.net.0.proj.weight", whole(Gff1), Gn, 1);
     wgrad_conv(whole(Gff1), whole(n3), t + ".ff.net.0.proj.weight", 1);
     bias_grad(whole(Gff1), t + ".ff.net.0.proj.bias");
     // norm3 (+ residual) -> G(h2)
@@ -659,7 +636,6 @@ static int build_backward(b200ad_unet* h, Backward* bw, uint8_t* arena, float* g
 
 namespace b200ad {
 void release_backward(b200ad_unet* h) {
-  if (h->bwd) free_bucket_events(h->bwd);
   delete h->bwd;
   h->bwd = nullptr;
 }
@@ -711,7 +687,6 @@ extern "C" int b200ad_unet_bind_backward(b200ad_unet* h, void* arena, size_t byt
   }
   if (bytes < need) return set_err("backward arena too small: %zu < %zu", bytes, need);
   CK(cudaMemsetAsync(arena, 0, need, (cudaStream_t)stream));
-  free_bucket_events(h->bwd);          // the op list is rebuilt: buckets must be set again
   if (build_backward(h, h->bwd, (uint8_t*)arena, grads, &need)) return -1;
   h->bwd->arena_bytes = need;
   return 0;
@@ -742,8 +717,6 @@ extern "C" int b200ad_unet_backward(b200ad_unet* h, const float* x, const float*
   launches += 1;
   if (prof) CK(cudaEventRecord(ev[1], st));
   size_t opi = 0;
-  for (size_t k = 0; k < bw->bucket_ev.size(); ++k)
-    if (bw->bucket_last_op[k] < 0) CK(cudaEventRecord(bw->bucket_ev[k], st));
   for (BOp& op : bw->ops) {
     switch (op.kind) {
       case BOp::CONV: CK(launch_conv_tc(op.conv, h->num_sms, st)); break;
@@ -789,8 +762,6 @@ extern "C" int b200ad_unet_backward(b200ad_unet* h, const float* x, const float*
     }
     ++launches;
     if (prof) CK(cudaEventRecord(ev[2 + opi], st));
-    for (size_t k = 0; k < bw->bucket_ev.size(); ++k)
-      if (bw->bucket_last_op[k] == (int)opi) CK(cudaEventRecord(bw->bucket_ev[k], st));
     ++opi;
   }
   bw->launches = launches;
@@ -819,35 +790,3 @@ extern "C" int b200ad_unet_backward(b200ad_unet* h, const float* x, const float*
 }
 
 extern "C" int b200ad_unet_backward_launch_count(const b200ad_unet* h) { return h && h->bwd ? h->bwd->launches : 0; }
-
-extern "C" int b200ad_unet_set_grad_buckets(b200ad_unet* h, int n, const size_t* lo) {
-  if (!h || !h->bwd || !h->bwd->grads) return set_err("set_grad_buckets: bind_backward first");
-  Backward* bw = h->bwd;
-  free_bucket_events(bw);
-  if (n <= 0) return 0;
-  if (n > 64 || !lo || lo[0] != 0 || lo[n] != bw->grad_floats) return set_err("set_grad_buckets: bad bucket table");
-  for (int k = 0; k < n; ++k)
-    if (lo[k + 1] <= lo[k]) return set_err("set_grad_buckets: boundaries must ascend");
-  bw->bucket_lo.assign(lo, lo + n + 1);
-  bw->bucket_last_op.assign(n, -1);
-  // every float* an op may ADD parameter gradients through (an over-approximation only delays an event)
-  for (size_t i = 0; i < bw->ops.size(); ++i) {
-    const BOp& op = bw->ops[i];
-    const float* outs[6] = {op.wg.dw, op.gb.dgamma, op.gb.dbeta, op.o0, op.o1, op.f1};
-    for (const float* q : outs) {
-      if (!q || q < bw->grads || q >= bw->grads + bw->grad_floats) continue;
-      const size_t off = (size_t)(q - bw->grads);
-      for (int k = 0; k < n; ++k)
-        if (off >= lo[k] && off < lo[k + 1]) bw->bucket_last_op[k] = (int)i;
-    }
-  }
-  bw->bucket_ev.resize(n);
-  for (int k = 0; k < n; ++k) CK(cudaEventCreateWithFlags(&bw->bucket_ev[k], cudaEventDisableTiming));
-  return 0;
-}
-
-extern "C" int b200ad_unet_grad_bucket_wait(b200ad_unet* h, int k, void* stream) {
-  if (!h || !h->bwd || k < 0 || k >= (int)h->bwd->bucket_ev.size()) return set_err("grad_bucket_wait: no such bucket");
-  CK(cudaStreamWaitEvent((cudaStream_t)stream, h->bwd->bucket_ev[k], 0));
-  return 0;
-}

@@ -45,35 +45,3 @@ def allreduce_mean_(flat: torch.Tensor) -> torch.Tensor:
     dist.all_reduce(flat, op=dist.ReduceOp.SUM)
     flat.div_(dist.get_world_size())
     return flat
-
-
-def grad_bucket_bounds(offsets: Sequence[int], total: int, nbuckets: int = 4) -> list:
-    """Bucket boundaries (float offsets into the flat gradient buffer, on parameter boundaries) of roughly equal size:
-    [0, b1, ..., total].  `offsets` are the parameters' start offsets."""
-    starts = sorted(set(int(o) for o in offsets) | {0})
-    bounds = [0]
-    for k in range(1, nbuckets):
-        target = total * k // nbuckets
-        best = min(starts, key=lambda o: abs(o - target))
-        if best > bounds[-1] and best < total:
-            bounds.append(best)
-    bounds.append(int(total))
-    return bounds
-
-
-def allreduce_mean_bucketed_(flat: torch.Tensor, bounds: Sequence[int], wait_bucket, comm_stream: "torch.cuda.Stream") -> torch.Tensor:
-    """The same mean as `allreduce_mean_`, issued bucket by bucket while the backward kernels that fill the LOWER buckets are
-    still running: `wait_bucket(k, stream_ptr)` makes `comm_stream` wait for the event the engine records once bucket k of
-    the flat buffer is complete (b200ad_unet_grad_bucket_wait); the collective of a bucket is enqueued behind that event.
-    The backward pass walks the network in reverse, so the HIGH buckets (up blocks) complete first."""
-    import torch.distributed as dist
-    world = dist.get_world_size()
-    works = []
-    for k in reversed(range(len(bounds) - 1)):
-        wait_bucket(k, comm_stream.cuda_stream)
-        with torch.cuda.stream(comm_stream):
-            works.append(dist.all_reduce(flat[bounds[k]:bounds[k + 1]], op=dist.ReduceOp.SUM, async_op=True))
-    for w in works:
-        w.wait()            # the CURRENT stream (the one the optimizer runs on) waits for the collectives
-    flat.div_(world)
-    return flat

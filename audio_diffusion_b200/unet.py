@@ -312,7 +312,6 @@ class UNet2DModel(nn.Module):
                 _lib.check(L.b200ad_unet_bind_backward(self._h, self._bwd_arena.data_ptr(), self._bwd_arena.numel(),
                                                        self._grad_flat.data_ptr(), _lib.stream_ptr()))
                 self._bwd_key = self._ws_key
-                self._bucket_key = None          # the library dropped its gradient buckets with the old plan
             out = torch.empty((n, self.out_channels, hh, ww), dtype=torch.float32, device=x.device)
             if enc is not None:
                 _lib.check(L.b200ad_unet_set_encoding(self._h, enc.data_ptr(), enc.shape[1]))
@@ -352,33 +351,12 @@ class UNet2DModel(nn.Module):
 
     def _allreduce_gradients(self) -> None:
         """Data parallel (accelerate's DDP, scripts/train_unet.py:181): mean of the flat gradient buffer over the ranks, ONE
-        collective after the backward pass.  B200AD_AR_OVERLAP=1 (NCCL only) reduces it in four buckets whose collectives
-        start as soon as the backward pass has finished writing them (the engine records an event per bucket).  Measured
-        at 2 GPUs (tools/run_n2_train.sh): 53.1 ms per iteration either way - the backward kernels are persistent CTAs
-        that fill every SM (512 threads x 122 registers, 227 KB of shared memory), so NCCL's CTAs only get SMs at kernel
-        boundaries and the time they hold them is taken from the next kernel: the collective is not free to hide."""
-        import os
-        import torch.distributed as dist
-        from .parallel import allreduce_mean_, allreduce_mean_bucketed_, grad_bucket_bounds
-        if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size() == 1:
-            return
-        flat = self._grad_flat
-        if dist.get_backend() != "nccl" or not flat.is_cuda or os.environ.get("B200AD_AR_OVERLAP", "0") != "1":
-            allreduce_mean_(flat)
-            return
-        L = _lib.lib()
-        key = (flat.data_ptr(), self._bwd_key)
-        if getattr(self, "_bucket_key", None) != key:
-            offs = [L.b200ad_unet_grad_offset(self._h, i) for i in range(len(self._pnames))]
-            self._bucket_bounds = grad_bucket_bounds(offs, flat.numel(), nbuckets=4)
-            arr = (C.c_size_t * len(self._bucket_bounds))(*self._bucket_bounds)
-            _lib.check(L.b200ad_unet_set_grad_buckets(self._h, len(self._bucket_bounds) - 1, arr))
-            self._comm_stream = torch.cuda.Stream(device=flat.device)
-            self._bucket_key = key
-            allreduce_mean_(flat)          # the events of THIS backward were not recorded yet: plain collective once
-            return
-        allreduce_mean_bucketed_(flat, self._bucket_bounds,
-                                 lambda k, sp: _lib.check(L.b200ad_unet_grad_bucket_wait(self._h, k, sp)), self._comm_stream)
+        collective after the backward pass.  It is not overlapped with the backward pass: an all-reduce in four buckets,
+        each started as soon as the backward pass had written it, measured 53.1 ms per iteration at 2 GPUs (B200, before
+        the port to H100) with or without the overlap - the backward kernels are persistent CTAs that fill every SM, so
+        NCCL's CTAs only get SMs at kernel boundaries and the time they hold them is taken from the next kernel."""
+        from .parallel import allreduce_mean_
+        allreduce_mean_(self._grad_flat)
 
     def no_sync(self):
         """Like `DistributedDataParallel.no_sync()`: backward passes inside the context skip the gradient all-reduce, so

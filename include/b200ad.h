@@ -123,13 +123,6 @@ int b200ad_unet_last_launch_count(const b200ad_unet* h);
 int b200ad_unet_set_training(b200ad_unet* h, int on);
 size_t b200ad_unet_grad_floats(b200ad_unet* h);
 size_t b200ad_unet_grad_offset(b200ad_unet* h, int i);
-/* Data-parallel training: overlap the gradient all-reduce with the rest of the backward pass (accelerate's DDP buckets,
- * scripts/train_unet.py:181).  Bucket k = floats [lo[k], lo[k+1]) of the flat gradient buffer (lo[0] = 0, lo[n] =
- * b200ad_unet_grad_floats, ascending, on parameter boundaries).  b200ad_unet_backward records bucket k's event on its stream
- * right after the last launch that adds into the bucket; b200ad_unet_grad_bucket_wait makes another stream (the one the
- * collective is issued on) wait for it.  Call after b200ad_unet_bind_backward; n = 0 removes the buckets. */
-int b200ad_unet_set_grad_buckets(b200ad_unet* h, int n, const size_t* lo);
-int b200ad_unet_grad_bucket_wait(b200ad_unet* h, int k, void* stream);
 size_t b200ad_unet_backward_bytes(b200ad_unet* h);       /* arena for activation gradients, temporaries, transposed weights */
 int b200ad_unet_bind_backward(b200ad_unet* h, void* arena, size_t bytes, float* grads, void* stream);
 /* x: the forward input [N, 1, H, W]; g_eps: gradient of the loss w.r.t. the forward output, fp32 [N, 1, H, W].

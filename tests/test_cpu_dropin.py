@@ -329,21 +329,6 @@ print('ok')
     assert r.returncode == 0 and "ok" in r.stdout, r.stderr[-2000:]
 
 
-def test_grad_bucket_bounds_are_parameter_boundaries():
-    """Buckets of the (opt-in) overlapped gradient all-reduce: ascending, start at 0, end at the buffer size, every inner
-    boundary on a parameter's start offset (b200ad_unet_set_grad_buckets requires it)."""
-    from audio_diffusion_b200.parallel import grad_bucket_bounds
-    sizes = [1152, 128, 147456, 128, 65536, 512, 589824, 256, 36864, 128]
-    offs, tot = [], 0
-    for n in sizes:
-        offs.append(tot)
-        tot += n
-    b = grad_bucket_bounds(offs, tot, nbuckets=4)
-    assert b[0] == 0 and b[-1] == tot and all(x < y for x, y in zip(b, b[1:]))
-    assert all(x in offs for x in b[1:-1])
-    assert grad_bucket_bounds([0], 100, nbuckets=4) == [0, 100]          # a single tensor: one bucket
-
-
 def test_bench_extras_formatting():
     """bench.py's `configs` object (C3 / C4 / B1 / C5 / Mel) is assembled on the host from a flat {name: seconds} dict that
     travelled through a max-over-ranks all-reduce: every sub-object and the rates derived from it."""

@@ -156,19 +156,25 @@ def _rel(a, b):
     return (err.abs().max() / b.abs().max()).item(), (err.pow(2).mean().sqrt() / b.pow(2).mean().sqrt()).item()
 
 
-def _check_against_order_noise(run):
-    """Tiles against flat items, with the bar set by the flat path itself: B200AD_CONV_DBG=2048 only reorders the k-steps of
-    convs with 1-tap segments, a last-bit change of the same kind as regrouped GroupNorm partial sums.  Through a deep net of
-    bf16 activations either grows to the same spread (about 0.75 % rms for the published U-Net at 256 x 256), so the tiles
-    must not move the result further than that.  A non-zero pad or guard would add errors along the image borders."""
+# Bars (rms-rel, max-rel) of tiles against flat items, set by the flat path's own order noise: the flat items with the
+# 1-tap k-steps of each conv interleaved between its 3x3 k-steps (a last-bit change of the same kind as regrouped GroupNorm
+# partial sums) moved each output by (rms0, mx0) against the flat items; the bar is (max(1.5 rms0, 2e-3), max(2 mx0, 2e-2)).
+# Measured on an NVIDIA H100 80GB HBM3 (700 W power limit) with the inputs of the tests below.
+BARS_UNET_EPS = (0.01159, 0.02)          # rms0 0.00772, mx0 0.00919
+BARS_VAE_MEAN = (0.009258, 0.02122)      # rms0 0.00617, mx0 0.01061
+BARS_VAE_DECODE = (0.03208, 0.04575)     # rms0 0.02138, mx0 0.02287
+
+
+def _check_against_order_noise(run, bars):
+    """Tiles against flat items, within the spread that reordering the flat path's accumulation alone produces: through a
+    deep net of bf16 activations a last-bit change grows to about 0.75 % rms for the published U-Net at 256 x 256, so the
+    tiles must not move the result further than that.  A non-zero pad or guard would add errors along the image borders."""
     tiled = run(None)
     flat = run(FLAT)
-    reordered = run(str(int(FLAT) | 2048))
-    for t, f, r in zip(tiled, flat, reordered):
+    for t, f, (rms_bar, mx_bar) in zip(tiled, flat, bars):
         mx, rms = _rel(t, f)
-        mx0, rms0 = _rel(r, f)
-        assert rms <= max(1.5 * rms0, 2e-3) and mx <= max(2 * mx0, 2e-2), \
-            f"tiles vs flat max-rel {mx:.5f} rms-rel {rms:.5f}; reordered flat {mx0:.5f} / {rms0:.5f}"
+        assert rms <= rms_bar and mx <= mx_bar, \
+            f"tiles vs flat max-rel {mx:.5f} rms-rel {rms:.5f}; bars {mx_bar:.5f} / {rms_bar:.5f}"
         d = (t - f).pow(2).mean(dim=(0, 1)).sqrt()
         H, W = d.shape
         border = torch.zeros(H, W, dtype=torch.bool)
@@ -189,7 +195,7 @@ def test_denoising_step_tiles_vs_flat(cuda):
     def run(mode):
         with torch.no_grad(), _dbg(mode):
             return (model(x, 500)["sample"].float().cpu(),)
-    _check_against_order_noise(run)
+    _check_against_order_noise(run, [BARS_UNET_EPS])
 
 
 def test_vae_encode_decode_tiles_vs_flat(cuda):
@@ -206,4 +212,4 @@ def test_vae_encode_decode_tiles_vs_flat(cuda):
     def run(mode):
         with torch.no_grad(), _dbg(mode):
             return model.encode(x).latent_dist.mean.float().cpu(), model.decode(z)["sample"].float().cpu()
-    _check_against_order_noise(run)
+    _check_against_order_noise(run, [BARS_VAE_MEAN, BARS_VAE_DECODE])

@@ -2,7 +2,7 @@
 B200AD_CONV_DBG given on the command line are applied round-robin, `--steps` fused denoise steps each, `--reps` times;
 prints mean / min / max ms per step per setting.
 
-    python tools/ab_conv.py 0 16 128 144 [--steps 5] [--reps 6] [--batch 64] [--res 256]
+    python tools/ab_conv.py 0 8 64 4096 [--steps 5] [--reps 6] [--batch 64] [--res 256]
 """
 import argparse
 import os

@@ -1,6 +1,6 @@
 #!/bin/bash
 # usage: tools/conv_decomp.sh <tag> "<dbg masks>" [lib ...] — bench.py per lib (default: the product lib) with parts of the conv
-# kernel switched off (B200AD_CONV_DBG: 2 = no global stores, 4 = CTAs started out of phase, 8 = no epilogue work,
+# kernel switched off (B200AD_CONV_DBG: 2 = no global stores, 8 = no epilogue work, 32 = no weight loads,
 # 64 = no transform); prints conv_tc ms per step.
 tag=$1; masks=$2; shift 2
 libs=${@:-audio_diffusion_b200/libb200ad.so}

@@ -23,23 +23,11 @@ x = torch.randn(2 * world, 1, 32, 32, generator=g)
 tgt = torch.randn(2 * world, 1, 32, 32, generator=g)
 t = torch.randint(0, 1000, (2 * world,), generator=g)
 sl = slice(2 * rank, 2 * rank + 2)
-for it in range(3):     # the first backward sets the gradient buckets up (plain all-reduce); the later ones overlap bucket by bucket
-    for p in model.parameters():
-        p.grad = None
-    pred = model(x[sl].to(dev), t[sl].to(dev))["sample"]
-    torch.nn.functional.mse_loss(pred, tgt[sl].to(dev)).backward()               # all-reduce happens inside backward
-    torch.cuda.synchronize()
-    if it == 0:
-        flat_first = model._grad_flat.clone()
+pred = model(x[sl].to(dev), t[sl].to(dev))["sample"]
+torch.nn.functional.mse_loss(pred, tgt[sl].to(dev)).backward()                   # all-reduce happens inside backward
+torch.cuda.synchronize()
 flat_dp = model._grad_flat.clone()
-bucketed = getattr(model, "_bucket_bounds", None)
-rel_b = ((flat_first - flat_dp).norm() / flat_first.norm()).item()      # fp32 atomics in the weight gradients: not bit-stable
-assert rel_b < 1e-5, f"bucketed all-reduce differs from the single collective: {rel_b}"
 
-ok = True
-msg = {}
-if rank == 0:
-    dist_was = True
 gathered = [torch.empty_like(flat_dp) for _ in range(world)]
 dist.all_gather(gathered, flat_dp)
 same = all(torch.equal(gathered[0], gg) for gg in gathered)
@@ -53,5 +41,5 @@ if rank == 0:
     ref = model._grad_flat
     rel = ((flat_dp - ref).norm() / ref.norm()).item()
     print(json.dumps({"world": world, "ranks_identical": bool(same), "rel_l2_vs_single_process": rel,
-                      "grad_floats": ref.numel(), "bucket_bounds": bucketed}))
+                      "grad_floats": ref.numel()}))
     assert same and rel < 5e-3, (same, rel)
