@@ -492,15 +492,16 @@ cudaError_t launch_scalar_conv_wgrad(const __nv_bfloat16* G, const float* X, flo
   return cudaGetLastError();
 }
 
-// conv_out's data gradient is a cin = 1 convolution of g_eps with the mirrored weights: w'[c][t] = w[c][8 - t]
-__global__ void flip_taps_kernel(const float* __restrict__ w, float* __restrict__ wf, int C) {
+// conv_out's data gradient is a cin = O convolution of its output gradient with the transposed, mirrored weights:
+// w'[c][o][t] = w[o][c][8 - t]
+__global__ void flip_taps_kernel(const float* __restrict__ w, float* __restrict__ wf, int C, int O) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= C * 9) return;
-  const int c = i / 9, t = i - c * 9;
-  wf[i] = w[c * 9 + 8 - t];
+  if (i >= C * O * 9) return;
+  const int co = i / 9, t = i - co * 9, c = co / O, o = co - c * O;
+  wf[i] = w[((long long)o * C + c) * 9 + 8 - t];
 }
-cudaError_t launch_flip_taps(const float* w, float* wf, int C, cudaStream_t s) {
-  flip_taps_kernel<<<(C * 9 + 255) / 256, 256, 0, s>>>(w, wf, C);
+cudaError_t launch_flip_taps(const float* w, float* wf, int C, cudaStream_t s, int O) {
+  flip_taps_kernel<<<(C * O * 9 + 255) / 256, 256, 0, s>>>(w, wf, C, O);
   return cudaGetLastError();
 }
 

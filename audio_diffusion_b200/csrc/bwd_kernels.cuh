@@ -36,7 +36,7 @@ cudaError_t launch_attention_bwd(const __nv_bfloat16* qkv, const __nv_bfloat16* 
                                  int W, cudaStream_t s);
 cudaError_t launch_scalar_conv_wgrad(const __nv_bfloat16* G, const float* X, float* dW, int N, int C, int H, int W, int flip,
                                      cudaStream_t s);
-cudaError_t launch_flip_taps(const float* w, float* wf, int C, cudaStream_t s);
+cudaError_t launch_flip_taps(const float* w, float* wf, int C, cudaStream_t s, int O = 1);
 cudaError_t launch_sum_add(const float* x, long long n, float* dst, cudaStream_t s);
 struct UnfoldMasks { unsigned mask[4][4]; };
 cudaError_t launch_unfold_up2(const float* dwf, float* dw3, long long nco_ci, const UnfoldMasks& m, cudaStream_t s);
@@ -63,6 +63,22 @@ cudaError_t launch_cross_attn_vec_bwd(const float* enc, const float* dvec, const
 // (PF8, C channels), lse from launch_mha_flash -> gqkv (PF8, 3C channels).  dsum: N * heads * H * W floats of scratch.
 cudaError_t launch_mha_bwd(const __nv_bfloat16* qkv, const __nv_bfloat16* o, const __nv_bfloat16* go, const float* lse,
                            float* dsum, __nv_bfloat16* gqkv, int N, int C, int heads, int H, int W, cudaStream_t s);
+
+// Autoencoder layers (vae_bwd_kernels.cu).
+// single-head attention (one head of dim C, S = H * W tokens, S % 64 == 0, C % 64 == 0): qkv and o as the forward read /
+// wrote them, go = dL/do (PF8, C channels), P the forward's softmax (fp32 [N][S][S]) -> gqkv (PF8, 3C channels).
+// Scratch: D (N * S floats), dS (N * S * S bf16).
+cudaError_t launch_attention_1head_bwd(const __nv_bfloat16* qkv, const __nv_bfloat16* o, const __nv_bfloat16* go,
+                                       const float* P, float* D, __nv_bfloat16* dS, __nv_bfloat16* gqkv, int N, int C, int H,
+                                       int W, cudaStream_t s);
+// quant_conv (1x1, L2 -> L2) on the first L2 channels of h (PF8, 128 channels), from gm (fp32 [N][L2][H][W]) -> g_h as
+// fp32 [N][L2][H][W] (gh_nc) and [L2][N][H][W] (gh_cn); dwq / dbq accumulated.  L2 <= 8.
+cudaError_t launch_quant_conv_bwd(const float* gm, const __nv_bfloat16* h, const float* wq, float* gh_nc, float* gh_cn,
+                                  float* dwq, float* dbq, int N, int L2, int H, int W, cudaStream_t s);
+// conv_in (3x3, L -> C) on post_quant_conv(z) (1x1, L -> L): gy (PF8, C channels) -> gz (fp32 [N][L][H][W]);
+// dwpq / dbpq accumulated (z: the forward's input latents).  L <= 4.
+cudaError_t launch_latent_in_bwd(const __nv_bfloat16* gy, const float* win, const float* wpq, const float* z, float* gz,
+                                 float* dwpq, float* dbpq, int N, int C, int L, int H, int W, cudaStream_t s);
 
 // Weight gradient on wgmma (wgrad_tc.cu):  dw[(co * cin_total + ci_off + ci) * ntaps_total + tapidx[t]] +=
 //   sum_{n, p} gy[n][co][p] * act[n][ci][p + shift[t]].   gy / act are channel views: `*_img_planes` planes per image in the

@@ -54,7 +54,7 @@ struct Op {
   const float* fw = nullptr;  // OP_CONV_IN / OP_VAE_SAMPLE / OP_MIX1X1 / OP_LN: fp32 weight and bias
   const float* fb = nullptr;
   const float* fc = nullptr;  // OP_XVEC: to_out bias
-  float* f1 = nullptr;        // OP_XVEC: destination [N][C]
+  float* f1 = nullptr;        // OP_XVEC: destination [N][C]; OP_MIX1X1: copy of the input (training)
   int cin = 0;                // OP_CONV_IN / OP_XVEC: input channels; OP_MHA: heads; OP_VAE_SAMPLE: latent channels
   float eps = 0.f;            // OP_LN
 };
@@ -149,6 +149,8 @@ struct Plan {    // everything a plan builder derives from the workspace and (N,
   float* temb_u2 = nullptr;          // training: [N][4 dim0] linear_2 output before SiLU
   float* zq = nullptr;               // autoencoder: post_quant_conv(z), [N][L][h][w]
   std::map<std::string, float*> lse; // training, conditional U-Net: attn1's row log-sum-exp [N][heads][H*W] by block name
+  std::map<std::string, float*> probs; // training, autoencoder: the single-head attention's softmax P [N][HW][HW] by block name
+  float* z_in = nullptr;             // training, autoencoder: the decoder's input latents [N][L][h][w] (post_quant_conv wgrad)
   size_t ws_bytes = 0;
 };
 
@@ -549,6 +551,7 @@ struct Builder {
     op.kind = OP_MIX1X1;
     op.f0 = built->zq; op.C = k.cin; op.H = H; op.W = W;
     op.fw = P("post_quant_conv.weight"); op.fb = P("post_quant_conv.bias");
+    if (h->training) op.f1 = built->z_in = (float*)ws.take((size_t)N * k.cin * H * W * 4);
     ops->push_back(op);
     return conv_in(k, built->zq);
   }
@@ -777,6 +780,7 @@ struct Builder {
       op.kind = single_head ? OP_ATTN1 : OP_ATTN;
       op.src = qkv.p; op.dst = ao.p; op.C = C; op.H = H; op.W = W;
       if (single_head) op.f0 = (float*)ws.take((size_t)N * H * W * H * W * sizeof(float));
+      if (single_head && h->training) built->probs[n] = op.f0;
       ops->push_back(op);
     }
     Act out = output(k, C, H, W);
@@ -908,7 +912,10 @@ static int run_ops(NetBase* h, const OpList& l, const RunArgs& a, cudaStream_t s
       case OP_VAE_SAMPLE:
         CK(launch_vae_sample(op.src, op.fw, op.fb, a.noise, a.out, a.moments, h->N, op.C, op.cin, op.H, op.W, st));
         break;
-      case OP_MIX1X1: CK(launch_mix1x1(a.in, op.fw, op.fb, op.f0, h->N, op.C, op.H * op.W, st)); break;
+      case OP_MIX1X1:    // training: the input is kept for the weight gradient
+        if (op.f1) CK(cudaMemcpyAsync(op.f1, a.in, (size_t)h->N * op.C * op.H * op.W * 4, cudaMemcpyDeviceToDevice, st));
+        CK(launch_mix1x1(a.in, op.fw, op.fb, op.f0, h->N, op.C, op.H * op.W, st));
+        break;
       case OP_CONV_OUT: {
         ConvOutParams p = op.co;
         p.eps_out = a.out;

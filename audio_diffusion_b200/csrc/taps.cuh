@@ -102,6 +102,22 @@ inline TapSet taps_scatter2(int a, int b) {
     }
   return t;
 }
+// Downsample2D(padding (0, 1, 0, 1)) of the autoencoder: input parity (a, b) <- the taps of matching parity
+// (a = 0: kh 0 at dh 0, kh 2 at dh -1;  a = 1: kh 1 at dh 0).  The padded row and column receive no gradient.
+inline TapSet taps_scatter2_asym(int a, int b) {
+  TapSet t{};
+  t.pack.transpose = 1;
+  const int khs[2][2] = {{0, 2}, {1, -1}};
+  for (int i = 0; i < 2; ++i)
+    for (int j = 0; j < 2; ++j) {
+      const int kh = khs[a][i], kw = khs[b][j];
+      if (kh < 0 || kw < 0) continue;
+      const int n = t.pack.ntaps++;
+      t.pack.kh[n] = kh; t.pack.kw[n] = kw;
+      t.dh[n] = kh == 2 ? -1 : 0; t.dw[n] = kw == 2 ? -1 : 0;
+    }
+  return t;
+}
 // folded Upsample2D, output parity (a, b): the folded taps with negated offsets, gathered from the gradient's parity plane
 inline TapSet taps_up2_neg(int a, int b) {
   TapSet t = taps_up2(a, b);

@@ -2,6 +2,8 @@
 // UNet2DConditionModel.forward) in reverse over the activations the training-mode forward kept (no buffer pooling), and
 // fills one flat fp32 buffer with the gradients of all parameters.  The transformer blocks of the conditional model run
 // their LayerNorm / GEGLU / cross-attention / multi-head attention backward kernels from cond_bwd.cu.
+// The autoencoder (scripts/train_vae.py) walks its decoder and encoder block lists the same way, one backward plan per
+// part; its single-head attention, encoder tail and decoder head run the kernels of vae_bwd_kernels.cu.
 //   * data gradients of every convolution run on conv_tc_kernel with transposed / mirrored weight packing (stride-2 convs
 //     as four scatter launches, the folded upsampling convs as one gather launch over the parity planes of the gradient);
 //   * weight gradients run on wgrad_tc_kernel (wgmma, pixels as the reduction dimension, MN-major operands);
@@ -9,6 +11,7 @@
 // This first version materialises the normalised activations for the weight gradients (no fusion yet) — DESIGN.md §6.
 #include "bwd_kernels.cuh"
 #include "unet.cuh"
+#include "vae.cuh"
 
 using namespace b200ad;
 
@@ -22,7 +25,7 @@ struct View {            // channel range of a PF8 tensor
 struct BOp {
   enum Kind { CONV, WGRAD, GNBWD, GNAPPLY, CHANSUM, REDUCE_N, SCATTER, PF8ADD, ATTNBWD, PARITY, UNFOLD, SCALAR_WGRAD, CONVIN,
               FLIP, SUMADD, LIN_IN, LIN_W, SILU_BWD, SILU_FWD, MEMSET,
-              LNBWD, GEGLUBWD, XVECBWD, MHABWD, NKINDS } kind;
+              LNBWD, GEGLUBWD, XVECBWD, MHABWD, ATTN1BWD, QUANTBWD, LATENTINBWD, NKINDS } kind;
   ConvParams conv;
   WgradDesc wg;
   GnBwdParams gb;
@@ -32,6 +35,7 @@ struct BOp {
   const __nv_bfloat16* src2 = nullptr;
   const __nv_bfloat16* src3 = nullptr;
   __nv_bfloat16* dst = nullptr;
+  __nv_bfloat16* dst2 = nullptr;  // bf16 scratch
   const float* f0 = nullptr;
   const float* f1 = nullptr;
   const float* f2 = nullptr;
@@ -44,6 +48,13 @@ struct BOp {
   bool x_is_geps = false;     // X / source = the output gradient passed to backward()
 };
 
+struct BwdArgs {              // the per-call inputs of a backward plan
+  const float* x = nullptr;   // the forward's input image (SCALAR_WGRAD x_is_input)
+  const float* g_eps = nullptr;   // the gradient of the model output (U-Net: eps; autoencoder decoder: the image)
+  const float* g_mom = nullptr;   // autoencoder encoder: the gradient of the moments
+  float* g_z = nullptr;           // autoencoder decoder: the gradient w.r.t. the latents (written)
+};
+
 }  // namespace b200ad
 
 struct Backward {
@@ -51,6 +62,7 @@ struct Backward {
   std::vector<PackJob> jobs;         // transposed weight packs, redone at every backward (the weights move every step)
   std::vector<size_t> goff;          // float offset of every parameter's gradient in the flat buffer
   size_t grad_floats = 0;
+  size_t zero_off = 0, zero_floats = 0;   // the slots of the flat buffer this plan writes (zeroed unless accumulating)
   uint8_t* arena = nullptr;
   size_t arena_bytes = 0;
   float* grads = nullptr;
@@ -61,7 +73,7 @@ struct Backward {
 namespace b200ad {
 
 struct BwdBuilder {
-  b200ad_unet* h;
+  NetBase* h;
   Backward* bw;
   Bump mem;                                   // arena allocator (base == nullptr: size pass)
   std::map<std::string, Act> grad;            // gradient w.r.t. a forward tensor (by tap name)
@@ -70,7 +82,9 @@ struct BwdBuilder {
   int N;
   float* cs = nullptr;                        // [N][maxC] channel sums scratch
   float* gsums = nullptr;                     // GroupNorm backward scratch [N][maxC][2]
-  float* gproj = nullptr;                     // [N][temb_rows]
+  float* gproj = nullptr;                     // U-Net: [N][temb_rows]
+  int heads = 8;                              // conditional U-Net: attention heads of the transformer blocks
+  bool single_head = false;                   // attention with one head of dim C (the autoencoder) instead of head_dim 8
   // per-sample channel sums produced by the GroupNorm-backward apply pass for the gradient tensor it writes (keyed by that
   // tensor): the producer's bias gradient then is a reduction over N of a [N][C] array instead of a pass over the tensor
   float* csum_arena = nullptr;
@@ -245,7 +259,7 @@ struct BwdBuilder {
     gn_bwd(T1, h1, nullptr, n + ".norm2", true, Gh1, nullptr, nullptr, nullptr);
     // conv1 bias + time embedding projection rows of this block
     bias_grad(whole(Gh1), n + ".conv1.bias");
-    {
+    if (k.temb_row >= 0) {
       BOp op{};
       op.kind = BOp::SCATTER;
       op.f0 = last_cs; op.o0 = gproj; op.C = co; op.a = h->temb_rows; op.b = k.temb_row;
@@ -286,7 +300,16 @@ struct BwdBuilder {
     wgrad_conv(whole(Gout), whole(ao), n + ".to_out.0.weight", 1);
     bias_grad(whole(Gout), n + ".to_out.0.bias");
     Act Gqkv = tmp("Gqkv", 3 * C, H, W);
-    {
+    if (single_head) {   // the forward's softmax P is kept: four GEMMs on the tensor cores
+      const long long S = (long long)H * W;
+      BOp op{};
+      op.kind = BOp::ATTN1BWD;
+      op.src = qkv.p; op.src2 = T1.p; op.src3 = ao.p; op.dst = Gqkv.p; op.f0 = h->plan.probs.at(n);
+      op.o2 = (float*)mem.take((size_t)N * S * sizeof(float));
+      op.dst2 = (__nv_bfloat16*)mem.take((size_t)N * S * S * sizeof(__nv_bfloat16));
+      op.C = C; op.H = H; op.W = W;
+      bw->ops.push_back(op);
+    } else {
       BOp op{};
       op.kind = BOp::ATTNBWD;
       op.src = qkv.p; op.src2 = T1.p; op.dst = Gqkv.p; op.C = C; op.H = H; op.W = W;
@@ -334,7 +357,7 @@ struct BwdBuilder {
     const std::string t = n + ".transformer_blocks.0";
     const Act x = fwd(xn), h0 = fwd(n + ".h0"), n1 = fwd(n + ".n1"), qkv = fwd(n + ".qkv"), ao = fwd(n + ".ao"),
               h2 = fwd(n + ".attn2"), n3 = fwd(n + ".n3"), ff1 = fwd(n + ".ff1"), gg = fwd(n + ".gg"), h3 = fwd(n + ".h3");
-    const int C = x.C, H = x.H, W = x.W, heads = h->cfg.attention_head_dim;
+    const int C = x.C, H = x.H, W = x.W;
     const Act Gout = G(n);
     // proj_out (its residual, G(x) += G(out), is added by the GroupNorm backward at the end)
     Act Gh3 = tmp("tf_Gh3", C, H, W);
@@ -412,27 +435,28 @@ struct BwdBuilder {
     gn_bwd(T, x, nullptr, n + ".norm", false, G(xn), nullptr, Gout.p, skip_of(xn), 1e-6f);
   }
 
-  // Downsample2D: stride-2 3x3 conv on the raw tensor xn -> y (tap n)
-  void downsample_bwd(const std::string& n, const std::string& xn) {
+  // Downsample2D (BK_DOWN: padding 1; BK_DOWN_ASYM: padding (0, 1, 0, 1)): stride-2 3x3 conv on the raw tensor xn -> y
+  void downsample_bwd(const Block& k, const std::string& xn) {
+    const std::string& n = k.name;
     const Act x = fwd(xn), y = fwd(n), par = fwd(n + ".parity");
     const int C = x.C, Ho = y.H, Wo = y.W;
     const Act Gy = G(n);
     const Geom go = make_geom(N, Ho, Wo);
     const size_t tsz = (size_t)N * (C / 8) * go.PL * 8;
     bias_grad(whole(Gy), n + ".bias");
-    // weight gradient: per parity plane (a, b) of x the taps that read it (forward: taps_parity)
+    // weight gradient: per parity plane (a, b) of x the taps that read it (forward: down_taps)
     for (int a = 0; a < 2; ++a)
       for (int b = 0; b < 2; ++b) {
         Act plane = par;
         plane.C = C; plane.H = Ho; plane.W = Wo;
         plane.p = par.p ? par.p + (size_t)(a * 2 + b) * tsz : nullptr;
-        wgrad(whole(Gy), whole(plane), PG(n + ".weight"), C, 0, 9, taps_parity(a, b));
+        wgrad(whole(Gy), whole(plane), PG(n + ".weight"), C, 0, 9, down_taps(k, a, b));
       }
     // data gradient: input parity (a, b) <- taps with matching parity, scattered into the 2x tensor
     Act Gx = G(xn);
     for (int a = 0; a < 2; ++a)
       for (int b = 0; b < 2; ++b) {
-        const TapSet t = taps_scatter2(a, b);
+        const TapSet t = k.kind == BK_DOWN ? taps_scatter2(a, b) : taps_scatter2_asym(a, b);
         BOp op{};
         op.kind = BOp::CONV;
         Act lo = Gx;
@@ -498,6 +522,31 @@ struct BwdBuilder {
     }
     bw->ops.push_back(dg);
   }
+
+  // conv_norm_out + SiLU + conv_out (C -> 1) on the last activation `in`, from the output gradient passed to backward()
+  void conv_out_bwd(const Block& k, const std::string& in, float* wflip, const float* zbias) {
+    const Act x = fwd(in);
+    const int C = x.C;
+    Act A = gn_apply("A", x, nullptr, k.name + "conv_norm_out", true);
+    BOp w{};
+    w.kind = BOp::SCALAR_WGRAD;
+    w.src = A.p; w.x_is_geps = true; w.o0 = PG(k.name + "conv_out.weight"); w.C = C; w.H = x.H; w.W = x.W; w.a = 1;
+    bw->ops.push_back(w);
+    BOp sb{};
+    sb.kind = BOp::SUMADD;
+    sb.x_is_geps = true; sb.n = (long long)N * x.H * x.W; sb.o0 = PG(k.name + "conv_out.bias");
+    bw->ops.push_back(sb);
+    BOp f{};
+    f.kind = BOp::FLIP;
+    f.f0 = P(k.name + "conv_out.weight"); f.o0 = wflip; f.C = C;
+    bw->ops.push_back(f);
+    Act T1 = tmp("T1", C, x.H, x.W);
+    BOp ci{};
+    ci.kind = BOp::CONVIN;        // conv_in kernel: g_a[c] = sum_t g_eps[p + s_t] * wflip[c][t]
+    ci.x_is_geps = true; ci.f0 = wflip; ci.f1 = zbias; ci.dst = T1.p; ci.C = C; ci.H = x.H; ci.W = x.W;
+    bw->ops.push_back(ci);
+    gn_bwd(T1, x, nullptr, k.name + "conv_norm_out", true, G(in), nullptr, nullptr, nullptr);
+  }
 };
 
 static int build_backward(b200ad_unet* h, Backward* bw, uint8_t* arena, float* grads, size_t* bytes_out) {
@@ -509,6 +558,7 @@ static int build_backward(b200ad_unet* h, Backward* bw, uint8_t* arena, float* g
   bw->grads = grads;
   BwdBuilder B;
   B.h = h; B.bw = bw; B.N = h->N;
+  B.heads = c.attention_head_dim;
   B.mem.base = arena;
   int maxC = c.block_out_channels[0];
   for (const auto& kv : h->plan.taps) maxC = kv.second.C > maxC ? kv.second.C : maxC;
@@ -538,28 +588,8 @@ static int build_backward(b200ad_unet* h, Backward* bw, uint8_t* arena, float* g
     const std::string in = tap(k.in);
     switch (k.kind) {
       case BK_CONV_OUT: {    // g_eps -> gradient of the last activation
-        const Act x = B.fwd(in);
-        const int C = x.C;
         if (c.out_channels != 1) return set_err("backward: out_channels != 1 is not implemented");
-        Act A = B.gn_apply("A", x, nullptr, k.name + "conv_norm_out", true);
-        BOp w{};
-        w.kind = BOp::SCALAR_WGRAD;
-        w.src = A.p; w.x_is_geps = true; w.o0 = B.PG(k.name + "conv_out.weight"); w.C = C; w.H = x.H; w.W = x.W; w.a = 1;
-        bw->ops.push_back(w);
-        BOp sb{};
-        sb.kind = BOp::SUMADD;
-        sb.x_is_geps = true; sb.n = (long long)h->N * x.H * x.W; sb.o0 = B.PG(k.name + "conv_out.bias");
-        bw->ops.push_back(sb);
-        BOp f{};
-        f.kind = BOp::FLIP;
-        f.f0 = B.P(k.name + "conv_out.weight"); f.o0 = wflip; f.C = C;
-        bw->ops.push_back(f);
-        Act T1 = B.tmp("T1", C, x.H, x.W);
-        BOp ci{};
-        ci.kind = BOp::CONVIN;        // conv_in kernel: g_a[c] = sum_t g_eps[p + s_t] * wflip[c][t]
-        ci.x_is_geps = true; ci.f0 = wflip; ci.f1 = zbias; ci.dst = T1.p; ci.C = C; ci.H = x.H; ci.W = x.W;
-        bw->ops.push_back(ci);
-        B.gn_bwd(T1, x, nullptr, k.name + "conv_norm_out", true, B.G(in), nullptr, nullptr, nullptr);
+        B.conv_out_bwd(k, in, wflip, zbias);
         BOp z{};
         z.kind = BOp::MEMSET;
         z.o0 = B.gproj; z.n = (long long)h->N * h->temb_rows * sizeof(float);
@@ -569,7 +599,7 @@ static int build_backward(b200ad_unet* h, Backward* bw, uint8_t* arena, float* g
       case BK_RESNET: B.resnet_bwd(k, in, tap(k.skip)); break;
       case BK_ATTN: B.attention_bwd(k.name, in); break;
       case BK_TRANSFORMER: B.transformer_bwd(k, in); break;
-      case BK_DOWN: B.downsample_bwd(k.name, in); break;
+      case BK_DOWN: B.downsample_bwd(k, in); break;
       case BK_UP: B.upsample_bwd(k.name, in); break;
       case BK_UNET_HEAD: {   // conv_in, then the timestep embedding MLP and the per-resnet projections
         if (c.in_channels != 1) return set_err("backward: in_channels != 1 is not implemented");
@@ -662,6 +692,7 @@ static void ensure_bwd(b200ad_unet* h) {
     off += (n + 63) & ~(size_t)63;
   }
   bw->grad_floats = off;
+  bw->zero_floats = off;
   h->bwd = bw;
 }
 
@@ -692,12 +723,11 @@ extern "C" int b200ad_unet_bind_backward(b200ad_unet* h, void* arena, size_t byt
   return 0;
 }
 
-extern "C" int b200ad_unet_backward(b200ad_unet* h, const float* x, const float* g_eps, int accumulate, void* stream) {
-  if (!h || !h->bwd || h->bwd->ops.empty()) return set_err("bind_backward must be called before backward");
-  if (!x || !g_eps) return set_err("backward: x and g_eps are required");
-  Backward* bw = h->bwd;
-  cudaStream_t st = (cudaStream_t)stream;
+// Runs a bound backward plan.
+static int run_backward(NetBase* h, Backward* bw, const BwdArgs& a, int accumulate, cudaStream_t st) {
   const int N = h->N;
+  const float* x = a.x;
+  const float* g_eps = a.g_eps;
   int launches = 0;
   // B200AD_BWD_PROFILE=1: CUDA events around every op, per-kind totals printed to stderr (tools/train_bench.py)
   static const bool prof = [] { const char* e = getenv("B200AD_BWD_PROFILE"); return e && e[0] == '1'; }();
@@ -707,7 +737,7 @@ extern "C" int b200ad_unet_backward(b200ad_unet* h, const float* x, const float*
     for (auto& e : ev) CK(cudaEventCreate(&e));
     CK(cudaEventRecord(ev[0], st));
   }
-  if (!accumulate) CK(cudaMemsetAsync(bw->grads, 0, bw->grad_floats * sizeof(float), st));   // every kernel below ADDS
+  if (!accumulate) CK(cudaMemsetAsync(bw->grads + bw->zero_off, 0, bw->zero_floats * sizeof(float), st));   // every kernel below ADDS
   {
     std::vector<PackItem> items;
     items.reserve(bw->jobs.size());
@@ -732,14 +762,14 @@ extern "C" int b200ad_unet_backward(b200ad_unet* h, const float* x, const float*
       case BOp::ATTNBWD: CK(launch_attention_bwd(op.src, op.src2, op.dst, N, op.C, op.H, op.W, st)); break;
       case BOp::PARITY: CK(launch_parity_split(op.src, op.dst, N, op.C, op.H, op.W, st)); break;
       case BOp::UNFOLD: CK(launch_unfold_up2(op.f0, op.o0, op.n, op.um, st)); break;
-      case BOp::SCALAR_WGRAD:
-        CK(launch_scalar_conv_wgrad(op.src, op.x_is_geps ? g_eps : x, op.o0, N, op.C, op.H, op.W, op.a, st));
+      case BOp::SCALAR_WGRAD:     // X: f0, or an input of the call
+        CK(launch_scalar_conv_wgrad(op.src, op.f0 ? op.f0 : op.x_is_geps ? g_eps : x, op.o0, N, op.C, op.H, op.W, op.a, st));
         break;
-      case BOp::CONVIN:
-        CK(launch_conv_in(g_eps, op.f0, op.f1, N, 1, op.H, op.W, op.C, op.dst, nullptr, st));
+      case BOp::CONVIN:           // source: f2 (c channels), or the output gradient (1 channel)
+        CK(launch_conv_in(op.f2 ? op.f2 : g_eps, op.f0, op.f1, N, op.c ? op.c : 1, op.H, op.W, op.C, op.dst, nullptr, st));
         break;
-      case BOp::FLIP: CK(launch_flip_taps(op.f0, op.o0, op.C, st)); break;
-      case BOp::SUMADD: CK(launch_sum_add(g_eps, op.n, op.o0, st)); break;
+      case BOp::FLIP: CK(launch_flip_taps(op.f0, op.o0, op.C, st, op.a ? op.a : 1)); break;
+      case BOp::SUMADD: CK(launch_sum_add(op.f0 ? op.f0 : g_eps, op.n, op.o0, st)); break;
       case BOp::LIN_IN: CK(launch_lin_bwd_input(op.f0, op.a, op.f1, op.b, op.c, op.o0, N, 0, st)); break;
       case BOp::LIN_W: CK(launch_lin_bwd_weight(op.f0, op.a, op.f1, op.b, op.c, op.o0, op.o1, N, st)); break;
       case BOp::SILU_BWD: CK(launch_silu_bwd(op.o0, op.f0, (int)op.n, st)); break;
@@ -758,6 +788,17 @@ extern "C" int b200ad_unet_backward(b200ad_unet* h, const float* x, const float*
         CK(launch_mha_bwd(op.src, op.src3, op.src2, op.f0, op.o2, op.dst, N, op.C, op.a, op.H, op.W, st));
         launches += 2;
         break;
+      case BOp::ATTN1BWD:   // row dot products, then the dS, dV, dQ, dK GEMMs
+        CK(launch_attention_1head_bwd(op.src, op.src3, op.src2, op.f0, op.o2, op.dst2, op.dst, N, op.C, op.H, op.W, st));
+        launches += 4;
+        break;
+      case BOp::QUANTBWD:
+        CK(launch_quant_conv_bwd(a.g_mom, op.src, op.f0, op.o2, op.o2 + (size_t)N * op.c * op.H * op.W, op.o0, op.o1, N,
+                                 op.c, op.H, op.W, st));
+        break;
+      case BOp::LATENTINBWD:
+        CK(launch_latent_in_bwd(op.src, op.f0, op.f1, op.f2, a.g_z, op.o0, op.o1, N, op.C, op.c, op.H, op.W, st));
+        break;
       case BOp::NKINDS: break;
     }
     ++launches;
@@ -769,7 +810,8 @@ extern "C" int b200ad_unet_backward(b200ad_unet* h, const float* x, const float*
     static const char* names[BOp::NKINDS] = {
         "conv_tc(dgrad)", "wgrad_tc", "gn_bwd", "gn_apply", "chan_sum", "reduce_n", "scatter", "pf8_add", "attention_bwd",
         "parity_split", "unfold_up2", "scalar_wgrad", "conv_in(dgrad)", "flip", "sum_add", "lin_in", "lin_w", "silu_bwd",
-        "silu_fwd", "memset", "layernorm_bwd", "geglu_bwd", "cross_attn_vec_bwd", "mha_bwd"};
+        "silu_fwd", "memset", "layernorm_bwd", "geglu_bwd", "cross_attn_vec_bwd", "mha_bwd", "attention_1head_bwd",
+        "quant_conv_bwd", "latent_in_bwd"};
     CK(cudaStreamSynchronize(st));
     double tot[BOp::NKINDS] = {0};
     int cnt[BOp::NKINDS] = {0};
@@ -789,4 +831,222 @@ extern "C" int b200ad_unet_backward(b200ad_unet* h, const float* x, const float*
   return 0;
 }
 
+extern "C" int b200ad_unet_backward(b200ad_unet* h, const float* x, const float* g_eps, int accumulate, void* stream) {
+  if (!h || !h->bwd || h->bwd->ops.empty()) return set_err("bind_backward must be called before backward");
+  if (!x || !g_eps) return set_err("backward: x and g_eps are required");
+  BwdArgs a;
+  a.x = x; a.g_eps = g_eps;
+  return run_backward(h, h->bwd, a, accumulate, (cudaStream_t)stream);
+}
+
 extern "C" int b200ad_unet_backward_launch_count(const b200ad_unet* h) { return h && h->bwd ? h->bwd->launches : 0; }
+
+// ================================================================================= autoencoder backward
+namespace b200ad {
+
+// Both parts' plans over one arena: the decoder first, then the encoder (the order of a training step's backward).
+static int build_vae_backward(b200ad_vae* h, Backward* const* bws, uint8_t* arena, float* grads, size_t* bytes_out) {
+  const b200ad_vae_config& c = h->cfg;
+  if (!h->training || h->plan.lists.empty()) return set_err("backward needs set_training(1) before bind_workspace");
+  if (c.in_channels != 1 || c.out_channels != 1 || c.latent_channels != 1)
+    return set_err("autoencoder backward: only in_channels = out_channels = latent_channels = 1 is implemented");
+  const int f = 1 << (c.num_blocks - 1), hl = h->H / f, wl = h->W / f, L2 = 2 * c.latent_channels;
+  const int Cmax = c.block_out_channels[c.num_blocks - 1] > c.block_out_channels[0] ? c.block_out_channels[c.num_blocks - 1]
+                                                                                    : c.block_out_channels[0];
+  if ((hl * wl) % 64) return set_err("autoencoder backward: the latent must have a multiple of 64 pixels");
+  BwdBuilder B;
+  B.h = h; B.N = h->N;
+  B.single_head = true;
+  B.mem.base = arena;
+  int maxC = Cmax;
+  for (const auto& kv : h->plan.taps) maxC = kv.second.C > maxC ? kv.second.C : maxC;
+  B.cs = (float*)B.mem.take((size_t)h->N * 3 * maxC * sizeof(float));
+  B.gsums = (float*)B.mem.take((size_t)h->N * 3 * maxC * 2 * sizeof(float));
+  B.csum_floats = (size_t)h->N * 65536;
+  B.csum_arena = (float*)B.mem.take(B.csum_floats * sizeof(float));
+  float* wflip = (float*)B.mem.take((size_t)Cmax * L2 * 9 * sizeof(float));
+  const float* zbias = (const float*)B.mem.take((size_t)Cmax * sizeof(float));   // never written: zeros
+  float* gh = (float*)B.mem.take((size_t)2 * h->N * L2 * hl * wl * sizeof(float));  // encoder tail: [N][2L] | [2L][N]
+  const Plan& pl = h->plan;
+  for (int part : {DEC, ENC}) {
+    Backward* bw = bws[part];
+    bw->ops.clear();
+    bw->jobs.clear();
+    bw->arena = arena;
+    bw->grads = grads;
+    B.bw = bw;
+    B.grad.clear(); B.skipgrad.clear(); B.csum_of.clear();
+    B.csum_used = 0;
+    BOp z{};
+    z.kind = BOp::MEMSET;
+    z.o0 = B.csum_arena; z.n = (long long)(B.csum_floats * sizeof(float));
+    bw->ops.push_back(z);
+    const std::vector<Block>& bl = part == ENC ? h->enc : h->dec;
+    auto tap = [&](int i) {
+      return i < 0 ? std::string() : (bl[i].kind == BK_CONV_IN || bl[i].kind == BK_LATENT_IN) ? bl[i].name + "conv_in" : bl[i].name;
+    };
+    for (int i = (int)bl.size() - 1; i >= 0; --i) {
+      const Block& k = bl[i];
+      const std::string in = tap(k.in);
+      switch (k.kind) {
+        case BK_CONV_OUT: B.conv_out_bwd(k, in, wflip, zbias); break;
+        case BK_LATENT_OUT: {   // g_moments -> quant_conv -> conv_out (C -> 2L, per output channel) -> conv_norm_out + SiLU
+          const Act x = B.fwd(in), eo = B.fwd(k.name + "conv_out");
+          const int C = x.C, H = x.H, W = x.W;
+          const size_t plane = (size_t)h->N * H * W;
+          float* gh_cn = gh ? gh + L2 * plane : nullptr;
+          BOp q{};
+          q.kind = BOp::QUANTBWD;
+          q.src = eo.p; q.f0 = B.P("quant_conv.weight"); q.o0 = B.PG("quant_conv.weight"); q.o1 = B.PG("quant_conv.bias");
+          q.o2 = gh; q.c = L2; q.H = H; q.W = W;
+          bw->ops.push_back(q);
+          Act A = B.gn_apply("A", x, nullptr, k.name + "conv_norm_out", true);
+          float* dw = B.PG(k.name + "conv_out.weight");
+          float* db = B.PG(k.name + "conv_out.bias");
+          for (int o = 0; o < L2; ++o) {
+            BOp w{};
+            w.kind = BOp::SCALAR_WGRAD;
+            w.src = A.p; w.f0 = gh_cn ? gh_cn + o * plane : nullptr; w.o0 = dw ? dw + (size_t)o * C * 9 : nullptr;
+            w.C = C; w.H = H; w.W = W; w.a = 1;
+            bw->ops.push_back(w);
+            BOp sb{};
+            sb.kind = BOp::SUMADD;
+            sb.f0 = w.f0; sb.n = (long long)plane; sb.o0 = db ? db + o : nullptr;
+            bw->ops.push_back(sb);
+          }
+          BOp fl{};
+          fl.kind = BOp::FLIP;
+          fl.f0 = B.P(k.name + "conv_out.weight"); fl.o0 = wflip; fl.C = C; fl.a = L2;
+          bw->ops.push_back(fl);
+          Act T1 = B.tmp("T1", C, H, W);
+          BOp ci{};
+          ci.kind = BOp::CONVIN;        // g_a[c] = sum_o sum_t g_h[o][p + s_t] * wflip[c][o][t]
+          ci.f2 = gh; ci.c = L2; ci.f0 = wflip; ci.f1 = zbias; ci.dst = T1.p; ci.C = C; ci.H = H; ci.W = W;
+          bw->ops.push_back(ci);
+          B.gn_bwd(T1, x, nullptr, k.name + "conv_norm_out", true, B.G(in), nullptr, nullptr, nullptr);
+          break;
+        }
+        case BK_RESNET: B.resnet_bwd(k, in, tap(k.skip)); break;
+        case BK_ATTN: B.attention_bwd(k.name, in); break;
+        case BK_DOWN_ASYM: B.downsample_bwd(k, in); break;
+        case BK_UP: B.upsample_bwd(k.name, in); break;
+        case BK_CONV_IN:        // encoder head: weight gradients only (no gradient w.r.t. the image)
+        case BK_LATENT_IN: {    // decoder head: conv_in on post_quant_conv(z), then the gradient w.r.t. z
+          const std::string n = tap(i);
+          const Act x = B.fwd(n);
+          const Act Gx = B.G(n);
+          BOp w{};
+          w.kind = BOp::SCALAR_WGRAD;
+          w.src = Gx.p; w.o0 = B.PG(n + ".weight"); w.C = x.C; w.H = x.H; w.W = x.W; w.a = 0;
+          if (k.kind == BK_CONV_IN) w.x_is_input = true;
+          else w.f0 = pl.zq;
+          bw->ops.push_back(w);
+          B.bias_grad(BwdBuilder::whole(Gx), n + ".bias");
+          if (k.kind == BK_LATENT_IN) {
+            BOp li{};
+            li.kind = BOp::LATENTINBWD;
+            li.src = Gx.p; li.f0 = B.P(n + ".weight"); li.f1 = B.P("post_quant_conv.weight"); li.f2 = pl.z_in;
+            li.o0 = B.PG("post_quant_conv.weight"); li.o1 = B.PG("post_quant_conv.bias");
+            li.C = x.C; li.c = k.cin; li.H = x.H; li.W = x.W;
+            bw->ops.push_back(li);
+          }
+          break;
+        }
+        default: return set_err("autoencoder backward: block %s has no backward", k.name.c_str());
+      }
+    }
+  }
+  if (bytes_out) *bytes_out = (B.mem.off + 255) & ~(size_t)255;
+  return 0;
+}
+
+void release_backward(b200ad_vae* h) {
+  for (Backward*& b : h->bwd) {
+    delete b;
+    b = nullptr;
+  }
+}
+
+}  // namespace b200ad
+
+extern "C" int b200ad_vae_set_training(b200ad_vae* h, int on) {
+  if (!h) return set_err("null handle");
+  if (h->training != (on != 0)) {
+    h->training = on != 0;
+    h->plan.lists.clear();    // the workspace layout changes: bind_workspace must be called again
+  }
+  return 0;
+}
+
+// The flat gradient buffer: encoder parameters (with quant_conv) first, then the decoder's (with post_quant_conv); each
+// part's plan zeroes only its own range.
+static void ensure_bwd(b200ad_vae* h) {
+  if (h->bwd[0]) return;
+  std::vector<size_t> goff;
+  size_t off = 0, dec_off = 0;
+  for (const auto& p : h->params) {
+    if (!dec_off && (p.name.rfind("decoder.", 0) == 0 || p.name.rfind("post_quant_conv.", 0) == 0)) dec_off = off;
+    size_t n = 1;
+    for (auto d : p.shape) n *= (size_t)d;
+    goff.push_back(off);
+    off += (n + 63) & ~(size_t)63;
+  }
+  for (int part : {ENC, DEC}) {
+    Backward* bw = new Backward();
+    bw->goff = goff;
+    bw->grad_floats = off;
+    bw->zero_off = part == ENC ? 0 : dec_off;
+    bw->zero_floats = part == ENC ? dec_off : off - dec_off;
+    h->bwd[part] = bw;
+  }
+}
+
+extern "C" size_t b200ad_vae_grad_floats(b200ad_vae* h) { ensure_bwd(h); return h->bwd[0]->grad_floats; }
+extern "C" size_t b200ad_vae_grad_offset(b200ad_vae* h, int i) { ensure_bwd(h); return h->bwd[0]->goff[i]; }
+
+static size_t vae_backward_size(b200ad_vae* h) {
+  ensure_bwd(h);
+  Backward t0, t1;
+  t0.goff = t1.goff = h->bwd[0]->goff;
+  Backward* tb[2] = {&t0, &t1};
+  size_t bytes = 0;
+  if (build_vae_backward(h, tb, nullptr, nullptr, &bytes)) return 0;
+  return bytes;
+}
+
+extern "C" size_t b200ad_vae_backward_bytes(b200ad_vae* h) { return vae_backward_size(h); }
+
+extern "C" int b200ad_vae_bind_backward(b200ad_vae* h, void* arena, size_t bytes, float* grads, void* stream) {
+  const size_t need = vae_backward_size(h);
+  if (!need) return -1;
+  if (bytes < need) return set_err("backward arena too small: %zu < %zu", bytes, need);
+  CK(cudaMemsetAsync(arena, 0, need, (cudaStream_t)stream));
+  size_t got = 0;
+  if (build_vae_backward(h, h->bwd, (uint8_t*)arena, grads, &got)) return -1;
+  for (Backward* b : h->bwd) b->arena_bytes = got;
+  return 0;
+}
+
+static int vae_backward(b200ad_vae* h, int part, const BwdArgs& a, int accumulate, cudaStream_t st) {
+  if (!h || !h->bwd[part] || h->bwd[part]->ops.empty()) return set_err("bind_backward must be called before backward");
+  return run_backward(h, h->bwd[part], a, accumulate, st);
+}
+
+extern "C" int b200ad_vae_decoder_backward(b200ad_vae* h, const float* g_x, float* g_z_out, int accumulate, void* stream) {
+  if (!g_x || !g_z_out) return set_err("decoder_backward: g_x and g_z_out are required");
+  BwdArgs a;
+  a.g_eps = g_x; a.g_z = g_z_out;
+  return vae_backward(h, DEC, a, accumulate, (cudaStream_t)stream);
+}
+
+extern "C" int b200ad_vae_encoder_backward(b200ad_vae* h, const float* x, const float* g_moments, int accumulate,
+                                           void* stream) {
+  if (!x || !g_moments) return set_err("encoder_backward: x and g_moments are required");
+  BwdArgs a;
+  a.x = x; a.g_mom = g_moments;
+  return vae_backward(h, ENC, a, accumulate, (cudaStream_t)stream);
+}
+
+extern "C" int b200ad_vae_backward_launch_count(const b200ad_vae* h) {
+  return h && h->bwd[0] ? h->bwd[0]->launches + h->bwd[1]->launches : 0;
+}

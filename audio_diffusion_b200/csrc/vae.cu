@@ -4,18 +4,11 @@
 //   audiodiffusion/pipeline_audio_diffusion.py:187-190   vqvae.decode(1 / scaling_factor * z)["sample"]
 // Parameter names are the diffusers state-dict keys that audiodiffusion/utils.py:156-303 (convert_ldm_to_hf_vae) emits.
 // The resnets, attention and up/down-samplers run on the same wgmma implicit-GEMM kernel as the U-Net (net.cuh).
-#include "net.cuh"
+#include "vae.cuh"
 
 using namespace b200ad;
 
-struct b200ad_vae : NetBase {
-  b200ad_vae_config cfg;
-  std::vector<Block> enc, dec;   // encoder, decoder
-};
-
 namespace b200ad {
-
-enum { ENC = 0, DEC = 1 };       // the two plans
 
 // AutoencoderKL as two block lists.  Transient activations ping-pong between two pooled buffers per (C, H, W): every block
 // reads its input from one and writes its output to the other (the shortcut K-segment re-reads the input while the output
@@ -62,7 +55,7 @@ static Plan vae_build_plan(const b200ad_vae* h, uint8_t* ws_base, int N, int H, 
   Builder B;
   B.h = h; B.built = &pl; B.N = N;
   B.single_head = true;
-  B.nopool = debug_nopool();
+  B.nopool = debug_nopool() || h->training;
   B.ws.base = ws_base;
   for (int pass = 0; pass < 2; ++pass) {
     enc.ops.clear(); dec.ops.clear();
@@ -112,7 +105,11 @@ extern "C" int b200ad_vae_create(const b200ad_vae_config* cfg, b200ad_vae** out)
   *out = h;
   return 0;
 }
-extern "C" void b200ad_vae_destroy(b200ad_vae* h) { delete h; }
+extern "C" void b200ad_vae_destroy(b200ad_vae* h) {
+  if (!h) return;
+  release_backward(h);
+  delete h;
+}
 extern "C" int b200ad_vae_num_params(const b200ad_vae* h) { return (int)h->params.size(); }
 extern "C" const char* b200ad_vae_param_name(const b200ad_vae* h, int i) { return h->params[i].name.c_str(); }
 extern "C" int b200ad_vae_param_shape(const b200ad_vae* h, int i, int64_t* dims) {

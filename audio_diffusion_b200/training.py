@@ -7,6 +7,11 @@ into one pass over all parameters (`b200ad_optim_step`, two launches).  `EMAMode
 
 `train_step` is the loop body of train_unet.py:238-267 on the engine (forward and backward in libb200ad.so through
 `UNet2DModel`'s autograd node); the unchanged reference script itself runs on `compat/accelerate`.
+
+`vae_loss` / `vae_train_step` are the autoencoder's objective and loop body (scripts/train_vae.py with
+config/ldm_autoencoder_kl.yaml): L1 reconstruction + kl_weight * KL, the generator loss of ldm's LPIPSWithDiscriminator
+before its discriminator starts, without the LPIPS term.  Encoder and decoder backward run in libb200ad.so through
+`AutoencoderKL`'s autograd nodes, so a perceptual term added in torch also reaches the decoder.
 """
 from __future__ import annotations
 
@@ -246,3 +251,30 @@ def mse_loss(pred: torch.Tensor, target: torch.Tensor, want_grad: bool = True):
                                                    grad.data_ptr() if grad is not None else None, scratch.data_ptr(),
                                                    _lib.stream_ptr()))
     return loss[0], grad
+
+
+def vae_loss(x: torch.Tensor, x_hat: torch.Tensor, posterior, kl_weight: float = 1e-6):
+    """(loss, rec, kl) of ldm's LPIPSWithDiscriminator before the discriminator starts, perceptual weight 0 and the
+    learned logvar at its initial 0 ([3P-recall] ldm.modules.losses.contperceptual):
+        nll  = sum(|x - x_hat| / exp(logvar) + logvar) / N,   kl = sum(posterior.kl()) / N,   loss = nll + kl_weight * kl.
+    `rec` is mean |x - x_hat| (what ldm logs as rec_loss)."""
+    rec = torch.abs(x.to(x_hat.dtype) - x_hat)
+    n = x_hat.shape[0]
+    nll = rec.sum() / n
+    kl = posterior.kl().sum() / n
+    return nll + kl_weight * kl, rec.mean(), kl
+
+
+def vae_train_step(vae, optimizer, images: torch.Tensor, generator: Optional[torch.Generator] = None,
+                   kl_weight: float = 1e-6):
+    """One iteration of the autoencoder's training loop: encode, sample the posterior, decode, `vae_loss`, backward
+    (CUDA), optimizer step, zero_grad.  ldm's optimizer is `FusedAdamW(vae.parameters(), lr=4.5e-6, betas=(0.5, 0.9),
+    weight_decay=0.0)`.  Returns (loss, rec, kl), detached."""
+    posterior = vae.encode(images).latent_dist
+    z = posterior.sample(generator=generator)
+    x_hat = vae.decode(z).sample
+    loss, rec, kl = vae_loss(images, x_hat, posterior, kl_weight)
+    loss.backward()
+    optimizer.step()
+    optimizer.zero_grad(set_to_none=True)
+    return loss.detach(), rec.detach(), kl.detach()

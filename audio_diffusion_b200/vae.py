@@ -6,6 +6,10 @@ config/ldm_autoencoder_kl.yaml:18-28 and with the state-dict keys audiodiffusion
 
 Encoder, decoder, quant/post-quant convs and the posterior sampling run in libb200ad.so (vae.cu); PyTorch owns the
 parameters (fp32 `nn.Parameter`s), the packed bf16 weights and the activation workspace.  No CPU fallback.
+
+Training (scripts/train_vae.py): with grad enabled, the module in train() mode and a parameter requiring grad, `encode`
+and `decode` are autograd nodes whose backward passes run in libb200ad.so (unet_bwd.cu); the posterior is then a torch
+expression on the differentiable moments, so autograd carries the reparameterisation, the logvar clamp and `kl()`.
 """
 from __future__ import annotations
 
@@ -27,27 +31,90 @@ class DecoderOutput(dict):
         self.sample = sample
 
 
-class DiagonalGaussianDistribution:
-    """Posterior returned by `encode(x).latent_dist`: `.sample(generator)`, `.mode()`, `.mean`, `.logvar`, `.std`, `.var`.
+class _VAEEncodeFunction(torch.autograd.Function):
+    """Autograd node of the training encoder: x -> moments; the backward pass is `b200ad_vae_encoder_backward` (the
+    encoder's and quant_conv's parameter gradients).  No gradient w.r.t. the image is produced."""
 
-    `sample()` draws its noise exactly as diffusers does (`randn_tensor(mean.shape, generator, device)`), then
+    @staticmethod
+    def forward(ctx, vae, x, *params):
+        m = vae._encode_train(x)
+        ctx.vae = vae
+        ctx.gen = vae._fwd_gen[0]
+        ctx.save_for_backward(x)
+        return m
+
+    @staticmethod
+    def backward(ctx, g):
+        (x,) = ctx.saved_tensors
+        ctx.vae._check_gen(0, ctx.gen)
+        ctx.vae._backward_part(0, x, g)
+        return (None, None) + (None,) * len(ctx.vae._pnames)
+
+
+class _VAEDecodeFunction(torch.autograd.Function):
+    """Autograd node of the training decoder: z -> image; the backward pass is `b200ad_vae_decoder_backward` (the
+    decoder's and post_quant_conv's parameter gradients, and the gradient w.r.t. z)."""
+
+    @staticmethod
+    def forward(ctx, vae, z, *params):
+        out = vae._decode_train(z)
+        ctx.vae = vae
+        ctx.gen = vae._fwd_gen[1]
+        ctx.zshape = z.shape
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        ctx.vae._check_gen(1, ctx.gen)
+        gz = ctx.vae._backward_part(1, None, g, ctx.zshape)
+        return (None, gz) + (None,) * len(ctx.vae._pnames)
+
+
+class _NoBackward(torch.autograd.Function):
+    """Marks an inference result computed while gradients were requested but training is not possible (the batch exceeds
+    max_batch, or a configuration without a backward): the forward values are today's, and backward() raises."""
+
+    @staticmethod
+    def forward(ctx, reason, t, *params):
+        ctx.reason = reason
+        return t.clone()
+
+    @staticmethod
+    def backward(ctx, g):
+        raise _lib.B200ADError(f"AutoencoderKL(b200): no backward for this call: {ctx.reason}")
+
+
+class DiagonalGaussianDistribution:
+    """Posterior returned by `encode(x).latent_dist`: `.sample(generator)`, `.mode()`, `.mean`, `.logvar`, `.std`, `.var`,
+    `.kl()`.
+
+    `sample()` draws its noise exactly as diffusers does (`randn_tensor(mean.shape, generator, device)`).  Inference: then
     mean + std * noise is evaluated by the encoder's tail kernel (vae_sample_kernel) — the moments never leave the device.
+    Training: the moments are the encoder node's differentiable output and every method is a torch expression on them.
     """
 
-    def __init__(self, vae: "AutoencoderKL", x: torch.Tensor):
+    def __init__(self, vae: "AutoencoderKL", x: torch.Tensor, train: bool = False, refuse: Optional[str] = None):
         self._vae = vae
         self._x = x
+        self._train = train
+        self._refuse = refuse
         self._moments: Optional[torch.Tensor] = None
 
     def _run(self, noise: Optional[torch.Tensor]) -> torch.Tensor:
         z, m = self._vae._encode(self._x, noise)
+        if self._refuse:
+            z, m = self._vae._no_backward(self._refuse, z), self._vae._no_backward(self._refuse, m)
         self._moments = m
         return z
 
     @property
     def parameters(self) -> torch.Tensor:
         if self._moments is None:
-            self._run(None)
+            if self._train:
+                named = self._vae._named()
+                self._moments = _VAEEncodeFunction.apply(self._vae, self._x, *[named[k] for k in self._vae._pnames])
+            else:
+                self._run(None)
         return self._moments
 
     @property
@@ -71,10 +138,18 @@ class DiagonalGaussianDistribution:
         shape = self._vae.latent_shape(x.shape)
         gdev = generator.device if generator is not None else x.device
         noise = torch.randn(shape, generator=generator, device=gdev, dtype=torch.float32).to(x.device)
+        if self._train:
+            return self.mean + self.std * noise
         return self._run(noise)
 
     def mode(self) -> torch.Tensor:
+        if self._train:
+            return self.mean
         return self._run(None)
+
+    def kl(self) -> torch.Tensor:
+        """KL(q(z|x) || N(0, I)) per sample, summed over the latent ([3P-recall] diffusers 0.24 / ldm `posterior.kl()`)."""
+        return 0.5 * torch.sum(torch.pow(self.mean, 2) + self.var - 1.0 - self.logvar, dim=[1, 2, 3])
 
 
 class AutoencoderKLOutput(dict):
@@ -150,6 +225,13 @@ class AutoencoderKL(nn.Module):
         self._packed_key = None
         self._ws = None
         self._ws_key = None
+        self._train_mode = False
+        self._fwd_gen = [0, 0]        # forwards run per part (encoder, decoder): a backward must see its own forward's
+        self._bwd_key = None
+        self._grad_flat = None
+        self._bwd_arena = None
+        self._grad_views = {}
+        self._grad_views_key = None
 
     # ------------------------------------------------------------------ diffusers directory layout
     _KEEP = ("in_channels", "out_channels", "down_block_types", "up_block_types", "block_out_channels",
@@ -252,6 +334,7 @@ class AutoencoderKL(nn.Module):
             self._ws_key = None
         wkey = (n, hh, ww, dev)
         if wkey != self._ws_key:
+            self._fwd_gen = [g + 1 for g in self._fwd_gen]     # the activations of both parts are gone
             need = L.b200ad_vae_workspace_bytes(self._h, n, hh, ww)
             if self._ws is None or self._ws.numel() < need or self._ws.device != dev:
                 self._ws = None
@@ -270,6 +353,7 @@ class AutoencoderKL(nn.Module):
 
     @torch.no_grad()
     def _encode(self, x: torch.Tensor, noise: Optional[torch.Tensor]):
+        self._set_training_mode(False)
         x = self._check(x, self.config.in_channels, "encode input")
         n, _, hh, ww = x.shape
         if hh % self._factor or ww % self._factor:
@@ -291,17 +375,155 @@ class AutoencoderKL(nn.Module):
                                                z[s:e].data_ptr(), m[s:e].data_ptr(), _lib.stream_ptr()))
         return z, m
 
+    # ------------------------------------------------------------------ training (backward in libb200ad)
+    def _needs_grad(self) -> bool:
+        return torch.is_grad_enabled() and self.training and any(p.requires_grad for p in self.parameters())
+
+    def _train_refusal(self, n: int) -> Optional[str]:
+        """Why a call that requests gradients cannot train (it then runs the inference path and its backward raises)."""
+        c = self.config
+        if (c.in_channels, c.out_channels, c.latent_channels) != (1, 1, 1):
+            return "the backward is implemented for in_channels = out_channels = latent_channels = 1"
+        if n > self.max_batch:
+            return (f"a training batch of {n} exceeds max_batch={self.max_batch} (training keeps the whole batch's "
+                    "activations; raise max_batch)")
+        return None
+
+    def _no_backward(self, reason: str, t: torch.Tensor) -> torch.Tensor:
+        named = self._named()
+        return _NoBackward.apply(reason, t, *[named[k] for k in self._pnames])
+
+    def _named(self) -> Dict[str, nn.Parameter]:
+        return dict(self.named_parameters())
+
+    def _set_training_mode(self, on: bool) -> None:
+        if self._train_mode != on:
+            _lib.check(_lib.lib().b200ad_vae_set_training(self._h, 1 if on else 0))
+            self._train_mode = on
+            self._ws_key = None        # the workspace layout differs (no buffer pooling when training)
+            self._bwd_key = None
+
+    def _check_gen(self, part: int, gen: int) -> None:
+        if gen != self._fwd_gen[part]:
+            what = ("encoder", "decoder")[part]
+            raise _lib.B200ADError(f"AutoencoderKL(b200): another forward ran on the {what} before backward(); the saved "
+                                   "activations of this graph were overwritten (one forward per backward)")
+
+    def _bind_train(self, n: int, hh: int, ww: int, dev) -> None:
+        if n > self.max_batch:
+            raise ValueError(f"AutoencoderKL(b200): a training batch of {n} exceeds max_batch={self.max_batch} (training "
+                             "keeps the whole batch's activations; raise max_batch)")
+        L = _lib.lib()
+        self._set_training_mode(True)
+        self._ensure_bound(n, hh, ww)
+        if self._bwd_key != self._ws_key:
+            nfl = L.b200ad_vae_grad_floats(self._h)
+            if self._grad_flat is None or self._grad_flat.numel() != nfl or self._grad_flat.device != dev:
+                self._grad_flat = torch.zeros(nfl, dtype=torch.float32, device=dev)
+            need = L.b200ad_vae_backward_bytes(self._h)
+            if need == 0:
+                _lib.check(-1)
+            if self._bwd_arena is None or self._bwd_arena.numel() < need or self._bwd_arena.device != dev:
+                self._bwd_arena = None
+                self._bwd_arena = torch.empty(need, dtype=torch.uint8, device=dev)
+            _lib.check(L.b200ad_vae_bind_backward(self._h, self._bwd_arena.data_ptr(), self._bwd_arena.numel(),
+                                                  self._grad_flat.data_ptr(), _lib.stream_ptr()))
+            self._bwd_key = self._ws_key
+
+    def _encode_train(self, x: torch.Tensor) -> torch.Tensor:
+        n, _, hh, ww = x.shape
+        if hh % self._factor or ww % self._factor:
+            raise ValueError(f"AutoencoderKL(b200): H and W must be multiples of {self._factor}")
+        lshape = self.latent_shape(x.shape)
+        with torch.cuda.device(x.device):
+            self._bind_train(n, hh, ww, x.device)
+            self._fwd_gen[0] += 1
+            z = torch.empty(lshape, dtype=torch.float32, device=x.device)
+            m = torch.empty((n, 2 * lshape[1], lshape[2], lshape[3]), dtype=torch.float32, device=x.device)
+            _lib.check(_lib.lib().b200ad_vae_encode(self._h, x.data_ptr(), None, z.data_ptr(), m.data_ptr(),
+                                                    _lib.stream_ptr()))
+        return m
+
+    def _decode_train(self, z: torch.Tensor) -> torch.Tensor:
+        z = z.detach().to(torch.float32).contiguous()
+        n, _, lh, lw = z.shape
+        hh, ww = lh * self._factor, lw * self._factor
+        with torch.cuda.device(z.device):
+            self._bind_train(n, hh, ww, z.device)
+            self._fwd_gen[1] += 1
+            out = torch.empty((n, self.config.out_channels, hh, ww), dtype=torch.float32, device=z.device)
+            _lib.check(_lib.lib().b200ad_vae_decode(self._h, z.data_ptr(), out.data_ptr(), _lib.stream_ptr()))
+        return out
+
+    def _backward_part(self, part: int, x: Optional[torch.Tensor], g: torch.Tensor, zshape=None):
+        """Backward of the encoder (part 0, from dL/dmoments) or the decoder (part 1, from dL/dimage; returns dL/dz)."""
+        L = _lib.lib()
+        g = g.to(torch.float32).contiguous()
+        named = self._named()
+        if self._grad_views_key != self._grad_flat.data_ptr():
+            self._grad_views = {0: [], 1: []}
+            for i, k in enumerate(self._pnames):
+                off = L.b200ad_vae_grad_offset(self._h, i)
+                p = named[k]
+                enc = k.startswith("encoder.") or k.startswith("quant_conv.")
+                self._grad_views[0 if enc else 1].append((p, self._grad_flat[off:off + p.numel()].view(p.shape)))
+            self._grad_views_key = self._grad_flat.data_ptr()
+        views = self._grad_views[part]
+        # torch semantics, per part: p.grad None -> start from zero; p.grad still our view -> add to what is there
+        have = [p.grad is not None for p, _ in views if p.requires_grad]
+        accumulate = bool(have) and all(have)
+        if any(have) and not accumulate:
+            raise _lib.B200ADError("AutoencoderKL(b200): either all of a part's parameter gradients are set (accumulate) "
+                                   "or none")
+        gz = None
+        with torch.cuda.device(g.device):
+            if part == 0:
+                _lib.check(L.b200ad_vae_encoder_backward(self._h, x.data_ptr(), g.data_ptr(), 1 if accumulate else 0,
+                                                         _lib.stream_ptr()))
+            else:
+                gz = torch.empty(zshape, dtype=torch.float32, device=g.device)
+                _lib.check(L.b200ad_vae_decoder_backward(self._h, g.data_ptr(), gz.data_ptr(), 1 if accumulate else 0,
+                                                         _lib.stream_ptr()))
+        for p, gv in views:
+            if p.grad is not None and p.grad.data_ptr() != gv.data_ptr():
+                raise _lib.B200ADError("AutoencoderKL(b200): p.grad must be None or the engine's own gradient view")
+            p.grad = gv
+        return gz
+
+    @property
+    def backward_launch_count(self) -> int:
+        """Kernel launches of the last decoder backward plus those of the last encoder backward."""
+        return _lib.lib().b200ad_vae_backward_launch_count(self._h)
+
     # ------------------------------------------------------------------ public calls
     def encode(self, x: torch.Tensor, return_dict: bool = True):
         """`vqvae.encode(x).latent_dist` — the encoder runs when the distribution is sampled / inspected."""
-        dist = DiagonalGaussianDistribution(self, self._check(x, self.config.in_channels, "encode input"))
+        x = self._check(x, self.config.in_channels, "encode input")
+        grad = self._needs_grad()
+        refuse = self._train_refusal(x.shape[0]) if grad else None
+        dist = DiagonalGaussianDistribution(self, x, train=grad and not refuse, refuse=refuse)
         if not return_dict:
             return (dist,)
         return AutoencoderKLOutput(dist)
 
-    @torch.no_grad()
     def decode(self, z: torch.Tensor, return_dict: bool = True):
         """`vqvae.decode(z)["sample"]` (pipeline_audio_diffusion.py:190)."""
+        grad = self._needs_grad()
+        refuse = self._train_refusal(z.shape[0]) if grad else None
+        if grad and not refuse:
+            self._check(z, self.config.latent_channels, "latents")
+            named = self._named()
+            out = _VAEDecodeFunction.apply(self, z, *[named[k] for k in self._pnames])
+            return (out,) if not return_dict else DecoderOutput(out)
+        with torch.no_grad():
+            res = self._decode_infer(z, return_dict)
+        if refuse:
+            out = self._no_backward(refuse, res[0] if not return_dict else res.sample)
+            return (out,) if not return_dict else DecoderOutput(out)
+        return res
+
+    def _decode_infer(self, z: torch.Tensor, return_dict: bool):
+        self._set_training_mode(False)
         z = self._check(z, self.config.latent_channels, "latents")
         n, _, lh, lw = z.shape
         hh, ww = lh * self._factor, lw * self._factor

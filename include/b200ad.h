@@ -164,6 +164,25 @@ int b200ad_vae_decode(b200ad_vae* h, const float* z, float* x_out, void* stream)
 int b200ad_vae_debug_tensor(b200ad_vae* h, const char* name, float* dst, int* dims, void* stream);
 int b200ad_vae_last_launch_count(const b200ad_vae* h);
 
+/* ---- Autoencoder backward (scripts/train_vae.py: the ldm reconstruction + KL objective) ----------------------------
+ * Protocol as for the U-Net: set_training(1) -> bind_workspace (every activation of both parts is kept, and the mid
+ * blocks' softmax) -> bind_backward -> per step: encode(x) -> decode(z) -> decoder_backward -> encoder_backward.
+ * Parameter i's gradient lives at float offset b200ad_vae_grad_offset(h, i) of one flat fp32 buffer.  Each backward
+ * writes only the slots of its own part: the decoder and post_quant_conv, or the encoder and quant_conv.  Implemented for
+ * in_channels = out_channels = latent_channels = 1; no gradient w.r.t. the input image is computed. */
+int b200ad_vae_set_training(b200ad_vae* h, int on);
+size_t b200ad_vae_grad_floats(b200ad_vae* h);
+size_t b200ad_vae_grad_offset(b200ad_vae* h, int i);
+size_t b200ad_vae_backward_bytes(b200ad_vae* h);
+int b200ad_vae_bind_backward(b200ad_vae* h, void* arena, size_t bytes, float* grads, void* stream);
+/* g_x: gradient of the loss w.r.t. the decoded image, fp32 [N, out, H, W] -> g_z_out: w.r.t. the decoder's input
+ * latents, fp32 [N, L, H/f, W/f] (written).  accumulate as for the U-Net. */
+int b200ad_vae_decoder_backward(b200ad_vae* h, const float* g_x, float* g_z_out, int accumulate, void* stream);
+/* x: the encoded image [N, in, H, W]; g_moments: gradient w.r.t. the moments (quant_conv's output) [N, 2L, H/f, W/f]. */
+int b200ad_vae_encoder_backward(b200ad_vae* h, const float* x, const float* g_moments, int accumulate, void* stream);
+/* Kernel launches of the last decoder_backward plus those of the last encoder_backward. */
+int b200ad_vae_backward_launch_count(const b200ad_vae* h);
+
 /* ---- Training step, optimizer side: replaces F.mse_loss, clip_grad_norm_(1.0), torch.optim.AdamW.step and
  * EMAModel.step of scripts/train_unet.py:258-266 (the U-Net backward itself is not built yet — DESIGN.md §6). -- */
 typedef struct {
