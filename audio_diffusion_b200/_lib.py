@@ -71,6 +71,7 @@ SYMBOLS = {
                                       C.POINTER(_I), C.POINTER(C.c_double), _I, _VP]),
     "b200ad_unet_debug_tensor": (_I, [_VP, C.c_char_p, _VP, C.POINTER(_I), _VP]),
     "b200ad_unet_last_launch_count": (_I, [_VP]),
+    "b200ad_unet_conv_plan": (_I, [_VP, _I, _I, _I, _I, C.POINTER(_I), _I]),
     "b200ad_unet_set_training": (_I, [_VP, _I]),
     "b200ad_unet_grad_floats": (_SZ, [_VP]),
     "b200ad_unet_grad_offset": (_SZ, [_VP, _I]),

@@ -12,11 +12,14 @@
 //     plus a halo of Wp+1 pixels on both sides) is bulk-copied (TMA engine) into shared memory; SBO = 128 B and every tap
 //     is a descriptor whose start address is shifted by (dh*Wp + dw) * 16 B.  (Few large copies: a bulk copy has a fixed
 //     cost however small it is.)
-//   - 2-D tile (ConvParams::tile2d): CONV_TW = 8 columns x CONV_TH = 32 rows.  Per 16 input channels one tensor-map copy
-//     lands the box [2 planes][32 + ht + hb rows][8 + hl + hr cols][8 ch]; each tile row is one core matrix, so SBO is the
-//     box row pitch (8 + hl + hr) * 16 B and a tap shifts the start address by (dh * pitch + dw) * 16 B.  At W = 256 the
-//     window is 10 x 34 pixels instead of 772, so each input pixel is loaded and normalised about once instead of three
-//     times.  Elements outside the image are zero-filled by the copy (the box is clipped at W, not at the pad column).
+//   - 2-D tile (ConvParams::tile2d): tw columns x th rows, 8 x 32 or 16 x 16.  Per 16 input channels one tensor-map copy
+//     lands the box [2 planes][th + ht + hb rows][tw + hl + hr cols][8 ch]; each 8-column row of a tile is one core matrix,
+//     so SBO is the box row pitch (tw + hl + hr) * 16 B and a tap shifts the start address by (dh * pitch + dw) * 16 B.
+//     8 x 32 is one N = 256 MMA per tap; 16 x 16 is two 8-column halves of 16 rows, one N = 128 MMA each (the second
+//     starts 8 pixels into the window), accumulating into the registers of flat tiles 0 and 1.  At W = 256 the window
+//     is 10 x 34 pixels instead of 772, so each input pixel is loaded and normalised about once instead of three times;
+//     at 16 x 16 and 32 x 32 an image is one or four whole items instead of 1.5 or 4.125 flat ones.  Elements outside
+//     the image are zero-filled by the copy (the box is clipped at W, not at the pad column).
 // Fused GroupNorm(+SiLU): the windows hold the RAW producer output; the transform warps rewrite them in place
 //   (x * scale[n][c] + shift[n][c], SiLU via one tanh.approx, zero on pad/guard positions) between the TMA landing and
 //   the MMA reading them, so the normalised tensor never exists in HBM.
@@ -29,9 +32,11 @@
 //   stmatrix.trans into a staging buffer ([plane][pixel][8 ch] = finished PF8 runs; the wgmma fragment puts the 8 channels
 //   of a plane in lanes 4 apart, which is exactly a transposed 8x8 matrix) -> bulk stores (TMA engine) draining while the
 //   next item is multiplied.  Flat items: one bulk store per plane and tile; pad columns and the run-off behind the image
-//   are stored as the zeros the layout requires there.  2-D tiles: the staging pixels are tile-row-major, and one
-//   tensor-map store writes the warpgroup's 8 planes; every pixel is inside the image, so pads and guards are never
-//   written (they are zero from the workspace memset at bind time and no writer of a PF8 tensor puts anything else there).
+//   are stored as the zeros the layout requires there.  2-D tiles: the staging pixels of a 128-pixel half are
+//   tile-row-major; 8 x 32: one tensor-map store writes the warpgroup's 8 planes, 16 x 16: one per (half, plane), like the
+//   flat runs; every pixel is inside the image, so pads and guards are never written (they are zero from the workspace
+//   memset at bind time and no writer of a PF8 tensor puts anything else there).  A folded upsample on 2-D tiles stores
+//   through a map of its output parity (a strided view of the 2x tensor); on flat items it scatters from the staging rows.
 // Small images (H * Wp + bottom halo <= 128 pixels: 8x8 and below): an item's tiles are the first tiles of CONSECUTIVE
 //   IMAGES, so one weight fetch and one N = 256 MMA serve two samples (ConvParams::pack).
 // Warp roles (12 warps): 0 activation producer, 1 weight producer, 2-3 transform, 4-7 and 8-11 the two consumer
@@ -45,21 +50,24 @@
 
 namespace b200ad {
 
-// Tensor maps of a 2-D-tiled launch (encoded by launch_conv_tc; unused by flat launches).  5-D over a PF8 tensor:
-// {8 channels, W columns, H rows, 8-channel planes, images}, based at pixel (0, 0) of plane 0.
+// Tensor maps of a 2-D-tiled launch (encoded by launch_conv_tc, see encode_pf8_map; unused by flat launches).  4-D over a
+// PF8 tensor: {8 W elements (a row's pixels, 8 channels each), H rows, 8-channel planes, images}, based at pixel (0, 0) of
+// plane 0.
 struct alignas(64) ConvMaps {
-  CUtensorMap src[CONV_MAXSEG];   // box {8, 8 + hl + hr, 32 + ht + hb, 2, 1}: one k-step's window of segment s
-  CUtensorMap out;                // box {8, 8, 32, 8, 1}: one consumer warpgroup's staging buffer
+  CUtensorMap src[CONV_MAXSEG];   // box {8 (tw + hl + hr), th + ht + hb, 2, 1}: one k-step's window of segment s
+  CUtensorMap out;                // 8 x 32: box {64, 32, 8, 1}, a consumer warpgroup's staging buffer; 16 x 16: box
+                                  // {64, 16, 1, 1}, one half-plane of it.  Folded upsample (16 x 16 only): 5-D over the
+                                  // columns / rows of the output parity (stride 2 in the 2x tensor), box {8, 8, 16, 1, 1}
 };
 
 // pixels per 8-channel plane of a segment's window (G: the item's 128-pixel tiles, flat items only)
 __host__ __device__ __forceinline__ int window_pixels(const ConvParams& p, const ConvSeg& sg, int G) {
-  return p.tile2d ? (CONV_TW + sg.hl + sg.hr) * (CONV_TH + sg.ht + sg.hb)
+  return p.tile2d ? (p.tw + sg.hl + sg.hr) * (p.th + sg.ht + sg.hb)
                   : G * CONV_TM + (sg.ht + sg.hb) * p.Wp + sg.hl + sg.hr;
 }
 // pixels from one window row to the next
 __host__ __device__ __forceinline__ int window_pitch(const ConvParams& p, const ConvSeg& sg) {
-  return p.tile2d ? CONV_TW + sg.hl + sg.hr : p.Wp;
+  return p.tile2d ? p.tw + sg.hl + sg.hr : p.Wp;
 }
 
 constexpr int CONV_THREADS = 384;     // 12 warps
@@ -68,6 +76,9 @@ constexpr int CONV_XF_THREADS = 64;   // transform warps 2, 3
 constexpr int CONV_SPLANE = CONV_MAXG * CONV_TM * 16;   // bytes per 8-channel plane of a buffer
 constexpr int CONV_STG_WG = 8 * CONV_SPLANE;
 constexpr int CONV_STAGING = 2 * CONV_STG_WG;
+static size_t conv_smem_bytes(const ConvParams& p) {
+  return (size_t)p.as * p.a_stage + (size_t)p.bs * CONV_B_SLOT + CONV_STAGING + 1024;
+}
 
 struct WorkItem {
   int n, ntile, m0, G;
@@ -81,8 +92,8 @@ __device__ __forceinline__ WorkItem decode_work(const ConvParams& p, int w) {
   if (p.tile2d) {   // tiles in column-major order: consecutive CTAs take vertically adjacent tiles, whose halos overlap in L2
     wi.n = gidx / p.groups_per_img;
     const int t = gidx - wi.n * p.groups_per_img, tx = t / p.tiles_y;
-    wi.r0 = (t - tx * p.tiles_y) * CONV_TH;
-    wi.c0 = tx * CONV_TW;
+    wi.r0 = (t - tx * p.tiles_y) * p.th;
+    wi.c0 = tx * p.tw;
     wi.m0 = 0;
     wi.G = CONV_MAXG;
     return wi;
@@ -120,6 +131,9 @@ __device__ __forceinline__ uint4 xform_vec(uint4 v, const f32x2_t (&sc)[4], cons
   return make_uint4(u[0], u[1], u[2], u[3]);
 }
 
+// SQUARE: the launch's items are 16 x 16 tiles.  A separate instantiation: with the N = 256 MMA of the other shapes and
+// the second N = 128 MMA (accumulators from acc[64]) in one function, ptxas serialises every wgmma (C7511).
+template <bool SQUARE>
 __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_constant__ ConvParams p,
                                                                   const __grid_constant__ ConvMaps maps) {
   constexpr int ASM = CONV_AS_MAX, BSM = CONV_BS_MAX;
@@ -188,7 +202,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_c
           const long long plane = (long long)(2 * ks + (lane & 1)) * p.PL;     // this lane's 8-channel plane of the k-step
           if (p.tile2d) {   // both planes in one box
             if (lane == 0)
-              tensor_g2s_5d(smem_base + stage * a_bytes, &maps.src[s], 0, wi.c0 - sg.hl, wi.r0 - sg.ht, 2 * ks, wi.n, full);
+              tensor_g2s_4d(smem_base + stage * a_bytes, &maps.src[s], 8 * (wi.c0 - sg.hl), wi.r0 - sg.ht, 2 * ks, wi.n, full);
           } else if (!p.pack) {
             const int pix0 = p.lead + wi.m0 - sg.ht * p.Wp - sg.hl;
             if (lane < 2)
@@ -284,8 +298,13 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_c
           for (int t = 0; t < nt; ++t) {
             const uint64_t wdesc = gmma_desc(bbase + (uint32_t)t * CONV_B_TAP, (CONV_NT / 8) * 128, 128);
             const uint64_t xdesc = gmma_desc(abase + (uint32_t)sg.aoff[t0 + t] * 16u, xlbo, xsbo);
-            if (wi.G == 2) wgmma_m64n256k16<0, 0>(acc, wdesc, xdesc);
-            else           wgmma_m64n128k16<0, 0>(acc, wdesc, xdesc);
+            if constexpr (SQUARE) {   // columns 0-7 into acc[0..63], columns 8-15 (8 pixels = 128 B on) into acc[64..127]
+              wgmma_m64n128k16_x2(acc, wdesc, xdesc, xdesc + (128u >> 4));
+            } else if (wi.G == 2) {
+              wgmma_m64n256k16<0, 0>(acc, wdesc, xdesc);
+            } else {
+              wgmma_m64n128k16<0, 0>(acc, wdesc, xdesc);
+            }
           }
           wgmma_commit();
           wgmma_wait<1>();   // the previous group has retired: its slots are free
@@ -369,8 +388,17 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_c
       if (p.tile2d) {
         fence_proxy_async_smem();   // staging rows written through the generic proxy -> visible to the TMA engine
         named_bar_sync(1 + cw, 128);
-        if (tid == 0 && !(p.dbg & 2)) {
-          tensor_s2g_5d(&maps.out, 0, wi.c0, wi.r0, wi.ntile * 16 + cw * 8, wi.n, stg_w);
+        if (SQUARE) {               // thread (half g, plane pl) = (tid >> 3, tid & 7) stores one 8 x 16 half-plane
+          const int g = tid >> 3, pl = tid & 7;
+          if (issuer && !(p.dbg & 2)) {
+            const uint32_t src = stg_w + (uint32_t)(pl * CONV_SPLANE + g * CONV_TM * 16);
+            const int c = wi.c0 + 8 * g, plane = wi.ntile * 16 + cw * 8 + pl;
+            if (p.up2) tensor_s2g_5d(&maps.out, 0, c, wi.r0, plane, wi.n, src);
+            else       tensor_s2g_4d(&maps.out, 8 * c, wi.r0, plane, wi.n, src);
+            bulk_commit();
+          }
+        } else if (tid == 0 && !(p.dbg & 2)) {
+          tensor_s2g_4d(&maps.out, 8 * wi.c0, wi.r0, wi.ntile * 16 + cw * 8, wi.n, stg_w);   // never an upsample
           bulk_commit();
         }
       } else if (!p.up2) {
@@ -385,7 +413,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_c
           bulk_commit();
         }
       } else {
-        // folded upsample: scatter into the 2x tensor at this launch's parity, straight from the staging rows
+        // folded upsample on flat items: scatter into the 2x tensor at this launch's parity, straight from the staging rows
         named_bar_sync(1 + cw, 128);
         const int npx = wi.G * CONV_TM;
         for (int i = tid; i < 8 * npx && !(p.dbg & 2); i += 128) {
@@ -567,10 +595,17 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_tc_kernel(const __grid_c
   }
 }
 
-// Tensor map over `planes` 8-channel planes of a PF8 tensor of the launch's geometry, images `img_stride` elements apart;
-// box {8, bw, bh, bplanes, 1}.  The driver's encoder is reached through the runtime, so the library links only cudart.
-static cudaError_t encode_pf8_map(CUtensorMap* m, const __nv_bfloat16* base, const ConvParams& p, int planes,
-                                  long long img_stride, int bw, int bh, int bplanes) {
+// Tensor map over `planes` 8-channel planes of a PF8 tensor: W x H pixels from pixel (0, 0) at `base`, `cs` / `rs` pixels
+// apart along a row / a column, planes `pl` pixels apart, images `img_stride` elements apart.
+// - cs == 1 (pixels of a row are contiguous): 4-D {8 W elements, H rows, planes, images}, box {8 bw, bh, bplanes, 1};
+//   coordinates (8 * column, row, plane, image).  A box row is then ONE run of 8 bw elements (128 - 288 B) for the TMA
+//   engine instead of bw separate 16-byte pixels, which it moves at a fraction of the rate.  Columns outside the image
+//   read as zeros and are not written, as whole pixels.
+// - otherwise (a folded upsample's output parity): 5-D {8, W, H, planes, images}, box {8, bw, bh, bplanes, 1};
+//   coordinates (0, column, row, plane, image).
+// The driver's encoder is reached through the runtime, so the library links only cudart.
+static cudaError_t encode_pf8_map(CUtensorMap* m, const __nv_bfloat16* base, const ConvParams& p, int cs, int rs, long long pl,
+                                  int planes, long long img_stride, int bw, int bh, int bplanes) {
   static PFN_cuTensorMapEncodeTiled_v12000 encode = nullptr;
   if (!encode) {
     void* fn = nullptr;
@@ -580,23 +615,32 @@ static cudaError_t encode_pf8_map(CUtensorMap* m, const __nv_bfloat16* base, con
     if (q != cudaDriverEntryPointSuccess || !fn) return cudaErrorNotSupported;
     encode = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(fn);
   }
-  const cuuint64_t dim[5] = {8, (cuuint64_t)p.W, (cuuint64_t)p.H, (cuuint64_t)planes, (cuuint64_t)p.N};
-  const cuuint64_t stride[4] = {16, (cuuint64_t)p.Wp * 16, (cuuint64_t)p.PL * 16, (cuuint64_t)img_stride * 2};
-  const cuuint32_t box[5] = {8, (cuuint32_t)bw, (cuuint32_t)bh, (cuuint32_t)bplanes, 1};
   const cuuint32_t estride[5] = {1, 1, 1, 1, 1};
-  const CUresult r = encode(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, (void*)(base + (long long)p.lead * 8), dim, stride, box,
-                            estride, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  CUresult r;
+  if (cs == 1) {
+    const cuuint64_t dim[4] = {(cuuint64_t)p.W * 8, (cuuint64_t)p.H, (cuuint64_t)planes, (cuuint64_t)p.N};
+    const cuuint64_t stride[3] = {(cuuint64_t)rs * 16, (cuuint64_t)pl * 16, (cuuint64_t)img_stride * 2};
+    const cuuint32_t box[4] = {(cuuint32_t)bw * 8, (cuuint32_t)bh, (cuuint32_t)bplanes, 1};
+    r = encode(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, (void*)base, dim, stride, box, estride, CU_TENSOR_MAP_INTERLEAVE_NONE,
+               CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  } else {
+    const cuuint64_t dim[5] = {8, (cuuint64_t)p.W, (cuuint64_t)p.H, (cuuint64_t)planes, (cuuint64_t)p.N};
+    const cuuint64_t stride[4] = {(cuuint64_t)cs * 16, (cuuint64_t)rs * 16, (cuuint64_t)pl * 16, (cuuint64_t)img_stride * 2};
+    const cuuint32_t box[5] = {8, (cuuint32_t)bw, (cuuint32_t)bh, (cuuint32_t)bplanes, 1};
+    r = encode(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, (void*)base, dim, stride, box, estride, CU_TENSOR_MAP_INTERLEAVE_NONE,
+               CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  }
   return r == CUDA_SUCCESS ? cudaSuccess : cudaErrorInvalidValue;
 }
 
-cudaError_t launch_conv_tc(const ConvParams& p_in, int num_sms, cudaStream_t stream) {
+int conv_dbg_env() {
   // timing experiments only; read on every launch so that one process can alternate settings (tools/ab_conv.py)
   const char* dbg_env = getenv("B200AD_CONV_DBG");
-  const int dbg = dbg_env ? atoi(dbg_env) : 0;
-  if (p_in.nseg < 1 || p_in.nseg > CONV_MAXSEG) return cudaErrorInvalidValue;
-  ConvParams p = p_in;
-  p.dbg = dbg;
+  return dbg_env ? atoi(dbg_env) : 0;
+}
+
+cudaError_t plan_conv_tc(ConvParams& p, int num_sms) {
+  if (p.nseg < 1 || p.nseg > CONV_MAXSEG) return cudaErrorInvalidValue;
   for (int s = 0; s < p.nseg; ++s) {
     ConvSeg& sg = p.seg[s];
     if (sg.ntaps > CONV_MAXTAPS || sg.ksteps < 1) return cudaErrorInvalidValue;
@@ -607,6 +651,9 @@ cudaError_t launch_conv_tc(const ConvParams& p_in, int num_sms, cudaStream_t str
       sg.hl |= sg.dw[t] < 0; sg.hr |= sg.dw[t] > 0;
     }
   }
+  p.tile2d = 0;
+  p.tw = p.th = 0;
+  p.tiles_y = 0;
   p.groups_per_img = (p.H * p.Wp + CONV_MAXG * CONV_TM - 1) / (CONV_MAXG * CONV_TM);
   p.ntiles_n = p.cout / CONV_NT;
   p.total_work = p.N * p.groups_per_img * p.ntiles_n;
@@ -636,22 +683,42 @@ cudaError_t launch_conv_tc(const ConvParams& p_in, int num_sms, cudaStream_t str
   }
   const int tiles_img = (p.H * p.Wp + CONV_TM - 1) / CONV_TM;
   const int max_g = p.pack ? p.pack : (tiles_img < CONV_MAXG ? tiles_img : CONV_MAXG);   // most tiles any item of this launch has
-  // 2-D tiles where their windows, summed over the segments, are smaller than the flat ones: W >= 64 for a 3x3 conv (the
-  // flat halo is two image rows, the tile's two rows of 8 + 2 pixels and two columns of 32 + 2).  The folded upsample
-  // scatters its output and packed small images are one tile each, so both stay flat.
-  p.tile2d = 0;
-  if (!p.pack && !p.up2 && !(dbg & 4096) && p.W % CONV_TW == 0 && p.H % CONV_TH == 0) {
-    ConvParams q = p;
-    q.tile2d = 1;
-    long long flat = 0, tiled = 0;
-    for (int s = 0; s < p.nseg; ++s) {
-      flat += window_pixels(p, p.seg[s], max_g);
-      tiled += window_pixels(q, p.seg[s], max_g);
+  // Item shape by cost per image and cout tile, compared in this order: MMA columns issued (a flat item whose second tile
+  // would be empty runs N = 128), items (each streams the cout tile's whole weight set from L2), window bytes loaded and
+  // normalised.  Flat items pay a halo of two image rows and, where H * Wp is not a multiple of 256, a part-empty last
+  // item (16 x 16: 1.5 items per image, 32 x 32: 4.125); a 2-D tile covers whole image rows and columns.  Packed small
+  // images are one tile each and stay flat.  Two exceptions, both measured (H100 80GB HBM3, 700 W, batch 64 at 256 x 256):
+  // - 16 x 16 and 8 x 32 tie on the first two wherever both fit, and 16 x 16's window is 5 % smaller; images of 64 rows
+  //   and more keep 8 x 32 (one N = 256 MMA per tap reads the weights from shared memory once, 16 x 16's two N = 128
+  //   MMAs twice; 16 x 16 there cost about 0.7 ms more per denoising step).
+  // - A folded upsample takes 16 x 16 tiles but not 8 x 32: its tile store through the parity map writes 16-byte pixels
+  //   32 bytes apart, and at 128 -> 256 that took 0.9 ms per step more than the flat items' scatter.
+  if (!p.pack && !(p.dbg & 4096)) {
+    auto window_cost = [&](const ConvParams& q, int G) {
+      long long c = 0;
+      for (int s = 0; s < q.nseg; ++s) c += (long long)window_pixels(q, q.seg[s], G) * q.seg[s].ksteps;
+      return c;
+    };
+    long long best[3] = {(long long)tiles_img * CONV_TM, p.groups_per_img, 0};
+    for (int i = 0; i < p.groups_per_img; ++i) best[2] += window_cost(p, min(CONV_MAXG, tiles_img - CONV_MAXG * i));
+    const int shapes[2][2] = {{8, 32}, {16, 16}};
+    for (const auto& sh : shapes) {
+      const int tw = sh[0], th = sh[1];
+      if (p.W % tw || p.H % th) continue;
+      if (tw == 16 && p.H >= 64 && p.H % 32 == 0 && p.W % 8 == 0) continue;
+      if (tw == 8 && p.up2) continue;
+      ConvParams q = p;
+      q.tile2d = 1; q.tw = tw; q.th = th;
+      const long long items = (long long)(p.W / tw) * (p.H / th);
+      const long long c[3] = {items * CONV_MAXG * CONV_TM, items, items * window_cost(q, CONV_MAXG)};
+      if (c[0] < best[0] || (c[0] == best[0] && (c[1] < best[1] || (c[1] == best[1] && c[2] < best[2])))) {
+        best[0] = c[0]; best[1] = c[1]; best[2] = c[2];
+        p.tile2d = 1; p.tw = tw; p.th = th;
+      }
     }
-    if (tiled < flat) {
-      p.tile2d = 1;
-      p.tiles_y = p.H / CONV_TH;
-      p.groups_per_img = (p.W / CONV_TW) * p.tiles_y;
+    if (p.tile2d) {
+      p.tiles_y = p.H / p.th;
+      p.groups_per_img = (p.W / p.tw) * p.tiles_y;
       p.total_work = p.N * p.groups_per_img * p.ntiles_n;
     }
   }
@@ -665,17 +732,6 @@ cudaError_t launch_conv_tc(const ConvParams& p_in, int num_sms, cudaStream_t str
     for (int t = 0; t < sg.ntaps; ++t) p.seg[s].aoff[t] = (sg.dh[t] + sg.ht) * pitch + sg.dw[t] + sg.hl;
   }
   p.a_stage = (a_stage + 255) & ~255;
-  ConvMaps maps{};
-  if (p.tile2d) {
-    for (int s = 0; s < p.nseg; ++s) {
-      const ConvSeg& sg = p.seg[s];
-      cudaError_t e = encode_pf8_map(&maps.src[s], sg.src, p, 2 * sg.ksteps, sg.img_stride, CONV_TW + sg.hl + sg.hr,
-                                     CONV_TH + sg.ht + sg.hb, 2);
-      if (e != cudaSuccess) return e;
-    }
-    cudaError_t e = encode_pf8_map(&maps.out, p.out, p, p.cout / 8, (long long)(p.cout / 8) * p.PL * 8, CONV_TW, CONV_TH, 8);
-    if (e != cudaSuccess) return e;
-  }
   // Ring depths: W = 256 fills shared memory with 3 activation stages + 5 weight slots.  Launches with smaller windows (narrow
   // images, packed small images, 1-tap convs) have SHORT k-steps, and the TMA -> transform -> MMA chain of a stage (a few
   // thousand cycles of L2 latency) is then covered only by more stages in flight: first up to 6 activation stages, then the
@@ -689,15 +745,45 @@ cudaError_t launch_conv_tc(const ConvParams& p_in, int num_sms, cudaStream_t str
   while (p.as < 6 && rings_fit(p.as + 1, p.bs)) ++p.as;
   while (p.bs < CONV_BS_MAX && rings_fit(p.as, p.bs + 1)) ++p.bs;
   while (p.as < CONV_AS_MAX && rings_fit(p.as + 1, p.bs)) ++p.as;
-  const size_t smem = (size_t)p.as * p.a_stage + (size_t)p.bs * CONV_B_SLOT + CONV_STAGING + 1024;
-  if (smem > (size_t)CONV_SMEM_MAX) return cudaErrorInvalidValue;  // image too wide for this tiling
+  if (conv_smem_bytes(p) > (size_t)CONV_SMEM_MAX) return cudaErrorInvalidValue;  // image too wide for this tiling
+  return cudaSuccess;
+}
+
+cudaError_t launch_conv_tc(const ConvParams& p_in, int num_sms, cudaStream_t stream) {
+  ConvParams p = p_in;
+  p.dbg = conv_dbg_env();
+  if (cudaError_t e = plan_conv_tc(p, num_sms)) return e;
+  ConvMaps maps{};
+  if (p.tile2d) {
+    for (int s = 0; s < p.nseg; ++s) {
+      const ConvSeg& sg = p.seg[s];
+      cudaError_t e = encode_pf8_map(&maps.src[s], sg.src + (long long)p.lead * 8, p, 1, p.Wp, p.PL, 2 * sg.ksteps,
+                                     sg.img_stride, p.tw + sg.hl + sg.hr, p.th + sg.ht + sg.hb, 2);
+      if (e != cudaSuccess) return e;
+    }
+    // 8 x 32: the warpgroup's 8 planes in one box; 16 x 16: one half-plane (8 columns x 16 rows) per box
+    const int bh = p.th, bplanes = p.tw == 16 ? 1 : 8;
+    cudaError_t e;
+    if (p.up2) {   // low-res pixel (h, w) -> (2h + oy, 2w + ox) of the 2x tensor: every second column and row
+      const Geom og = make_geom(p.N, 2 * p.H, 2 * p.W);
+      e = encode_pf8_map(&maps.out, p.out + (long long)(og.lead + p.oy * og.Wp + p.ox) * 8, p, 2, 2 * og.Wp, og.PL,
+                         p.cout / 8, (long long)(p.cout / 8) * og.PL * 8, 8, bh, bplanes);
+    } else {
+      e = encode_pf8_map(&maps.out, p.out + (long long)p.lead * 8, p, 1, p.Wp, p.PL, p.cout / 8,
+                         (long long)(p.cout / 8) * p.PL * 8, 8, bh, bplanes);
+    }
+    if (e != cudaSuccess) return e;
+  }
+  const size_t smem = conv_smem_bytes(p);
   const int grid = p.total_work < num_sms ? p.total_work : num_sms;
   if (grid <= 0) return cudaSuccess;
-  static size_t attr = 0;
-  if (smem > attr) {
-    cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  const bool square = p.tile2d && p.tw == 16;
+  void (*kernel)(ConvParams, ConvMaps) = square ? conv_tc_kernel<true> : conv_tc_kernel<false>;
+  static size_t attr[2] = {0, 0};
+  if (smem > attr[square]) {
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    attr = smem;
+    attr[square] = smem;
   }
   // launch with programmatic stream serialization: the grid may begin (prologue, weight prefetch) before its predecessor
   // has completed; it synchronises on the predecessor itself (griddepcontrol.wait) before touching anything it depends on
@@ -711,7 +797,7 @@ cudaError_t launch_conv_tc(const ConvParams& p_in, int num_sms, cudaStream_t str
   at[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = at;
   cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, conv_tc_kernel, p, maps);
+  return cudaLaunchKernelEx(&cfg, kernel, p, maps);
 }
 
 // ------------------------------------------------------------------------------------ identity weights

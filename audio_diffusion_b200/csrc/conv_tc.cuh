@@ -7,8 +7,6 @@ namespace b200ad {
 constexpr int CONV_NT = 128;        // output-channel tile = 2 x MMA M (one 64-row half per consumer warpgroup)
 constexpr int CONV_TM = 128;        // pixels per tile; an MMA covers up to two tiles (N = 256)
 constexpr int CONV_MAXG = 2;        // pixel tiles per work item: 64 x 256 fp32 accumulators = 128 registers per thread
-constexpr int CONV_TW = 8;          // 2-D item: CONV_TW columns (one core matrix of the MMA's N direction per tile row) ...
-constexpr int CONV_TH = CONV_MAXG * CONV_TM / CONV_TW;   // ... x 32 rows = 256 pixels
 constexpr int CONV_MAXSEG = 4;      // K-segments per launch
 constexpr int CONV_MAXTAPS = 9;
 constexpr int CONV_B_TAP = 16 * CONV_NT * 2;     // one tap, 16 input channels: 4096 B
@@ -38,7 +36,7 @@ struct ConvSeg {
   signed char dh[CONV_MAXTAPS];
   signed char dw[CONV_MAXTAPS];
   int aoff[CONV_MAXTAPS];      // (dh + ht) * pitch + dw + hl, filled in by launch_conv_tc: window offset of each tap (pitch:
-                               // Wp for flat items, CONV_TW + hl + hr for 2-D tiles)
+                               // Wp for flat items, tw + hl + hr for 2-D tiles)
   // Fused GroupNorm(+SiLU) of this source, applied to the A strips in shared memory before the MMAs read them:
   // value = silu?(x * ss[n][c].x + ss[n][c].y), forced to 0 on pad / guard positions. nullptr: source is used as is.
   const float2* ss;            // [N][ss_stride] (pointer already offset to this source's first channel)
@@ -65,9 +63,11 @@ struct ConvParams {
   int nseg;
   int N, H, W, Wp, lead, PL;
   int a_stage;          // bytes reserved for the A strips of one stage (set by the launcher)
-  // Item shape (set by the launcher): 0 = 256 consecutive flat pixels, 1 = a 2-D tile of CONV_TW columns x CONV_TH rows
+  // Item shape (set by the launcher): 0 = 256 consecutive flat pixels, 1 = a 2-D tile of tw columns x th rows, either
+  // 8 x 32 (one 8-column core-matrix strip, one N = 256 MMA per tap) or 16 x 16 (two 8-column halves, one N = 128 MMA each)
   int tile2d;
-  int tiles_y;          // 2-D tiles: H / CONV_TH (tiles per column of tiles)
+  int tw, th;           // 2-D tiles: the tile's columns and rows (0 for flat items)
+  int tiles_y;          // 2-D tiles: H / th (tiles per column of tiles)
   int groups_per_img;   // items per image and cout tile
   int ntiles_n;         // cout / 128
   int total_work;       // N * groups_per_img * ntiles_n  (packed: ceil(N / 4) * ntiles_n)
@@ -87,6 +87,11 @@ struct ConvParams {
   int dbg;                      // B200AD_CONV_DBG bit flags: 2 no stores, 8 no epilogue work, 32 no weight loads, 64 no transform (each removes a piece of work to measure its cost); 4096 flat items only (no 2-D tiles: the reference of the tiled path)
 };
 
+// The launcher's decisions for a launch, without launching (host only, no CUDA calls): halos and tap offsets, item shape
+// (flat, packed small images, 8 x 32 or 16 x 16 tiles), work items, activation stage bytes and ring depths.  `p.dbg` holds
+// the B200AD_CONV_DBG flags to plan with (conv_dbg_env() reads them as the launcher does).
+cudaError_t plan_conv_tc(ConvParams& p, int num_sms);
+int conv_dbg_env();
 cudaError_t launch_conv_tc(const ConvParams& p, int num_sms, cudaStream_t stream);
 
 // Identity weight blocks (W[co][ci] = delta) in the packed layout: a residual add is one extra 1-tap K-segment over the

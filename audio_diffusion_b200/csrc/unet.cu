@@ -243,6 +243,24 @@ extern "C" int b200ad_unet_profile_step(b200ad_unet* h, const float* x, const fl
   return nops;
 }
 
+extern "C" int b200ad_unet_conv_plan(const b200ad_unet* h, int N, int H, int W, int num_sms, int* rows, int max_rows) {
+  const Plan pl = build_plan(h, nullptr, N, H, W);
+  const int dbg = conv_dbg_env();
+  int n = 0;
+  for (const Op& op : pl.lists[0].ops) {
+    if (op.kind != OP_CONV) continue;
+    if (n >= max_rows) return set_err("conv_plan: more than %d conv launches", max_rows);
+    ConvParams p = op.conv;
+    p.dbg = dbg;
+    if (plan_conv_tc(p, num_sms) != cudaSuccess) return set_err("conv_plan: launch %d cannot be planned", n);
+    const int row[B200AD_CONV_PLAN_COLS] = {p.H, p.W, p.seg[0].ksteps * 16, p.cout, p.nseg, p.up2,
+                                             p.pack, p.tw, p.th, p.total_work, p.as, p.bs};
+    for (int c = 0; c < B200AD_CONV_PLAN_COLS; ++c) rows[n * B200AD_CONV_PLAN_COLS + c] = row[c];
+    ++n;
+  }
+  return n;
+}
+
 extern "C" int b200ad_unet_set_encoding(b200ad_unet* h, const float* enc, int S) {
   if (!h->cfg.cross_attention_dim) return set_err("set_encoding: this U-Net is unconditional");
   if (S < 1) return set_err("set_encoding: empty encoder sequence");

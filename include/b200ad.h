@@ -113,6 +113,15 @@ int b200ad_unet_profile_step(b200ad_unet* h, const float* x, const float* t, con
 /* Number of kernel launches the last forward enqueued. */
 int b200ad_unet_last_launch_count(const b200ad_unet* h);
 
+/* How the conv kernel would cut the work of every conv_tc launch of the forward plan at batch N, H x W, on a GPU with
+ * num_sms SMs; host only (no GPU needed), honouring B200AD_CONV_DBG as the launcher does.  Per launch, in plan order,
+ * B200AD_CONV_PLAN_COLS ints: H and W the launch runs at (a folded upsample: its low-res input), input channels of the
+ * first K-segment, cout, K-segments, folded upsample (0/1), packed images per item (0: not packed), tile columns and rows
+ * (0, 0: flat items; 8 x 32 or 16 x 16), work items, activation stages, weight-ring slots.  Returns the number of
+ * launches, or negative if there are more than max_rows. */
+#define B200AD_CONV_PLAN_COLS 12
+int b200ad_unet_conv_plan(const b200ad_unet* h, int N, int H, int W, int num_sms, int* rows, int max_rows);
+
 /* ---- U-Net backward (scripts/train_unet.py:259 `accelerator.backward(loss)`) ----------------------------
  * Protocol: set_training(1) -> bind_workspace (every activation is kept) -> bind_backward -> per step: forward(x, t),
  * then backward(x, dL/d eps). Parameter gradients land in ONE flat fp32 buffer; parameter i of the
