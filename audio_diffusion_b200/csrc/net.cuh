@@ -1,11 +1,12 @@
 // Shared host-side machinery of the model handles.  An architecture is one list of blocks (Block); the parameter table,
 // the packed-weight arena layout and the launch plan (ResnetBlock2D / attention with the GroupNorm apply fused into the
-// consuming conv) are each one loop over it, and one executor runs the plans of both models.
+// consuming conv) are each one loop over it, and one executor runs the forward and backward plans of both models.
 #pragma once
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <map>
 #include <string>
 #include <vector>
@@ -31,32 +32,53 @@ struct Act {  // PF8 activation tensor
   __nv_bfloat16* p = nullptr;
   int C = 0, H = 0, W = 0;
   stat_t* stats = nullptr;
+  size_t off = 0;  // byte offset of p in its arena: known in a size-only pass too, where p is null
 };
 
-// The values are reported per launch by b200ad_unet_profile_step (4 was the unfolded nearest-2x upsample).
+// The forward values are reported per launch by b200ad_unet_profile_step (4 was the unfolded nearest-2x upsample); the
+// backward's follow them.
 enum OpKind { OP_TEMB = 0, OP_CONV_IN = 1, OP_GN = 2, OP_CONV = 3, OP_PARITY = 5, OP_ATTN = 6, OP_CONV_OUT = 7,
               OP_ATTN1 = 8 /* single head of dim C */, OP_VAE_SAMPLE = 9, OP_MIX1X1 = 10,
               OP_LN = 11 /* LayerNorm over channels */, OP_GEGLU = 12, OP_MHA = 13 /* multi-head attention, head_dim 16/32/64 */,
               OP_XVEC = 14 /* cross-attention against a one-token encoding = per-sample vector */,
-              OP_GNAPPLY = 15 /* materialised GroupNorm (attention input: the q/k/v projection has 12 cout tiles) */ };
+              OP_GNAPPLY = 15 /* materialised GroupNorm (attention input: the q/k/v projection has 12 cout tiles) */,
+              OP_PACK_T /* transposed weight packs of a backward plan */, OP_DGRAD, OP_WGRAD, OP_GN_BWD, OP_CHANSUM,
+              OP_REDUCE_N, OP_SCATTER, OP_PF8ADD, OP_ATTN_BWD, OP_UNFOLD, OP_SCALAR_WGRAD, OP_CONV_IN_BWD, OP_FLIP, OP_SUMADD,
+              OP_LIN_IN, OP_LIN_W, OP_SILU_BWD, OP_SILU_FWD, OP_MEMSET, OP_LN_BWD, OP_GEGLU_BWD, OP_XVEC_BWD, OP_MHA_BWD,
+              OP_ATTN1_BWD, OP_QUANT_BWD, OP_LATENT_IN_BWD, OP_NKINDS };
+// by OpKind: error messages and the backward profile's keys (tools/cond_train_bench.py matches "mha_bwd x<count>")
+static const char* const op_names[] = {
+    "temb", "conv_in", "gn_finalize", "conv_tc", "", "parity_split", "attention", "conv_out", "attention_1head", "vae_sample",
+    "mix1x1", "layernorm", "geglu", "mha", "cross_attn_vec", "gn_apply", "pack_transposed", "conv_tc(dgrad)", "wgrad_tc",
+    "gn_bwd", "chan_sum", "reduce_n", "scatter", "pf8_add", "attention_bwd", "unfold_up2", "scalar_wgrad", "conv_in(dgrad)",
+    "flip", "sum_add", "lin_in", "lin_w", "silu_bwd", "silu_fwd", "memset", "layernorm_bwd", "geglu_bwd",
+    "cross_attn_vec_bwd", "mha_bwd", "attention_1head_bwd", "quant_conv_bwd", "latent_in_bwd"};
+static_assert(sizeof(op_names) / sizeof(op_names[0]) == OP_NKINDS, "one name per OpKind");
+
+struct RunArgs {                        // the per-call inputs of a plan
+  const float* in = nullptr;            // U-Net: the sample x; autoencoder: the image (encode) or the latents (decode)
+  const float* t = nullptr;             // U-Net: timesteps [N]
+  const float* noise = nullptr;         // U-Net: the scheduler's noise z; autoencoder encode: the sampling noise
+  float* out = nullptr;                 // U-Net: eps (optional); autoencoder: z (encode) or the image (decode)
+  float* moments = nullptr;             // autoencoder encode (optional)
+  float* x_out = nullptr;               // U-Net: the scheduler update (optional), with coef or coef_dev
+  const b200ad_step_coef* coef = nullptr;
+  const b200ad_step_coef* coef_dev = nullptr;
+  // backward (`in`: the forward's input)
+  const float* g_eps = nullptr;         // the gradient of the model output (U-Net: eps; autoencoder decoder: the image)
+  const float* g_mom = nullptr;         // autoencoder encoder: the gradient of the moments
+  float* g_z = nullptr;                 // autoencoder decoder: the gradient w.r.t. the latents (written)
+};
+
+using OpFn = std::function<cudaError_t(const RunArgs&, cudaStream_t)>;
+// One entry of a plan.  A closure must not capture its builder (a temporary that the plan outlives): op closures use
+// explicit capture lists, never [=] or [&].
 struct Op {
   OpKind kind;
-  ConvParams conv;
-  GnApplyParams gn;
-  // generic slots
-  const __nv_bfloat16* src = nullptr;
-  __nv_bfloat16* dst = nullptr;
-  int C = 0, H = 0, W = 0;
-  ConvOutParams co;
-  float2* ss = nullptr;  // OP_GN: output of gn_finalize
-  float* f0 = nullptr;   // OP_ATTN1: score scratch; OP_MIX1X1: fp32 destination; OP_CONV_IN: fp32 source (null: the caller's);
-                         // OP_MHA: row log-sum-exp for the backward (training; null: not kept)
-  const float* fw = nullptr;  // OP_CONV_IN / OP_VAE_SAMPLE / OP_MIX1X1 / OP_LN: fp32 weight and bias
-  const float* fb = nullptr;
-  const float* fc = nullptr;  // OP_XVEC: to_out bias
-  float* f1 = nullptr;        // OP_XVEC: destination [N][C]; OP_MIX1X1: copy of the input (training)
-  int cin = 0;                // OP_CONV_IN / OP_XVEC: input channels; OP_MHA: heads; OP_VAE_SAMPLE: latent channels
-  float eps = 0.f;            // OP_LN
+  int launches = 1;   // what this op adds to the plan's launch count
+  ConvParams conv;    // OP_CONV / OP_DGRAD (launch_conv_tc): data, because gn_attach edits the last conv of a forward plan
+                      // and b200ad_unet_conv_plan / b200ad_unet_profile_step read it
+  OpFn run;           // every other kind
 };
 
 struct Bump {  // two-pass bump allocator: base == nullptr computes sizes only
@@ -74,6 +96,13 @@ static size_t take_off(Bump& b, size_t bytes) {  // size-only pass: returns the 
   const size_t o = (b.off + 255) & ~(size_t)255;
   b.take(bytes);
   return o;
+}
+static Act take_act(Bump& b, int N, int C, int H, int W) {  // a PF8 tensor (no statistics)
+  Act a;
+  a.C = C; a.H = H; a.W = W;
+  a.off = take_off(b, (size_t)N * (C / 8) * make_geom(N, H, W).PL * 16);
+  a.p = b.base ? (__nv_bfloat16*)(b.base + a.off) : nullptr;
+  return a;
 }
 
 struct PackJob {  // one K-segment's packed weights
@@ -425,6 +454,28 @@ static int pack_common(NetBase* h, cudaStream_t st) {
 }
 
 // ================================================================================= launch plan
+// a conv writing `out` (its work decomposition, tiles per item and item count, is filled in by launch_conv_tc)
+static ConvParams conv_geom(int N, const Act& out) {
+  const Geom g = make_geom(N, out.H, out.W);
+  ConvParams p{};
+  p.N = N; p.H = out.H; p.W = out.W; p.Wp = g.Wp; p.lead = g.lead; p.PL = g.PL;
+  p.cout = out.C;
+  p.out = out.p;
+  p.stats = out.stats;
+  return p;
+}
+// GroupNorm(+SiLU) over cat(a, b) into dst; dst null: the parameters of the scale/shift finalize (gn_finalize)
+static GnApplyParams gn_params(const NetBase* h, int N, const Act& a, const Act* b, const std::string& norm,
+                               __nv_bfloat16* dst, bool silu, float eps = -1.f) {
+  GnApplyParams p{};
+  p.src[0] = a.p; p.stats[0] = a.stats; p.C[0] = a.C;
+  p.src[1] = b ? b->p : nullptr; p.stats[1] = b ? b->stats : nullptr; p.C[1] = b ? b->C : 0;
+  p.gamma = h->pptr[h->pidx.at(norm + ".weight")]; p.beta = h->pptr[h->pidx.at(norm + ".bias")];
+  p.dst = dst;
+  p.N = N; p.H = a.H; p.W = a.W; p.groups = h->norm_groups; p.eps = eps < 0.f ? h->norm_eps : eps; p.silu = silu ? 1 : 0;
+  return p;
+}
+
 struct Builder {
   const NetBase* h;
   Plan* built;
@@ -438,10 +489,7 @@ struct Builder {
   bool single_head = false;  // attention with one head of dim C (AutoencoderKL mid block) instead of head_dim 8
 
   Act alloc(int C, int H, int W, bool stats) {
-    Act a;
-    a.C = C; a.H = H; a.W = W;
-    const Geom g = make_geom(N, H, W);
-    a.p = (__nv_bfloat16*)ws.take((size_t)N * (C / 8) * g.PL * 16);
+    Act a = take_act(ws, N, C, H, W);
     if (stats) a.stats = (stat_t*)st.take((size_t)N * (C / 4) * 2 * sizeof(stat_t));
     return a;
   }
@@ -460,12 +508,11 @@ struct Builder {
   const float* P(const std::string& name) const { return h->pptr[h->pidx.at(name)]; }
   template <class T> const T* PK(size_t off) const { return h->packed ? (const T*)(h->packed + off) : nullptr; }
 
-  void conv_common(ConvParams& p, const Act& out) {
-    const Geom g = make_geom(N, out.H, out.W);
-    p.N = N; p.H = out.H; p.W = out.W; p.Wp = g.Wp; p.lead = g.lead; p.PL = g.PL;
-    p.cout = out.C;  // work decomposition (tiles per item, item count) is filled in by launch_conv_tc
-    p.out = out.p;
-    p.stats = out.stats;
+  void emit(OpKind kind, OpFn run, int launches = 1) { ops->push_back(Op{kind, launches, {}, std::move(run)}); }
+  void conv(const ConvParams& p) {
+    Op op{OP_CONV};
+    op.conv = p;
+    ops->push_back(op);
   }
   void seg(ConvSeg& s, const __nv_bfloat16* src, int C, int H, int W, size_t woff, const TapSet& t) {
     set_seg(s, src, C / 8, C, H, W, PK<__nv_bfloat16>(woff), t);
@@ -497,16 +544,8 @@ struct Builder {
     const int Ct = a.C + (b ? b->C : 0);
     float2* ss = (float2*)ws.take((size_t)N * Ct * sizeof(float2));
     if (gn_attach(a, b, norm, ss, eps)) return ss;
-    Op op{};
-    op.kind = OP_GN;
-    GnApplyParams& p = op.gn;
-    p.src[0] = a.p; p.stats[0] = a.stats; p.C[0] = a.C;
-    p.src[1] = b ? b->p : nullptr; p.stats[1] = b ? b->stats : nullptr; p.C[1] = b ? b->C : 0;
-    p.gamma = P(norm + ".weight"); p.beta = P(norm + ".bias");
-    p.dst = nullptr;
-    p.N = N; p.H = a.H; p.W = a.W; p.groups = h->norm_groups; p.eps = eps < 0.f ? h->norm_eps : eps; p.silu = 0;
-    op.ss = ss;
-    ops->push_back(op);
+    const GnApplyParams p = gn_params(h, N, a, b, norm, nullptr, false, eps);
+    emit(OP_GN, [p, ss](const RunArgs&, cudaStream_t s) { return launch_gn_finalize(p, ss, s); });
     return ss;
   }
   static void seg_norm(ConvSeg& s, const float2* ss, int stride, bool silu) {
@@ -514,15 +553,12 @@ struct Builder {
   }
 
   // conv_in of a model part, on the caller's fp32 input or on `src`
-  Act conv_in(const Block& k, float* src) {
+  Act conv_in(const Block& k, const float* src) {
     Act x = output(k, k.cout, H, W);
-    Op op{};
-    op.kind = OP_CONV_IN;
-    op.dst = x.p; op.C = k.cout; op.H = H; op.W = W; op.cin = k.cin;
-    op.f0 = src;
-    op.fw = P(k.name + "conv_in.weight"); op.fb = P(k.name + "conv_in.bias");
-    op.conv.stats = x.stats;
-    ops->push_back(op);
+    emit(OP_CONV_IN, [src, w = P(k.name + "conv_in.weight"), b = P(k.name + "conv_in.bias"), N = N, cin = k.cin, H = H,
+                      W = W, x](const RunArgs& a, cudaStream_t s) {
+      return launch_conv_in(src ? src : a.in, w, b, N, cin, H, W, x.C, x.p, x.stats, s);
+    });
     built->taps[k.name + "conv_in"] = x;
     return x;
   }
@@ -537,23 +573,31 @@ struct Builder {
       built->temb_u1 = (float*)ws.take((size_t)N * k.temb * 4);
       built->temb_u2 = (float*)ws.take((size_t)N * k.temb * 4);
     }
-    Op op{};
-    op.kind = OP_TEMB;
-    op.C = k.cout;
-    ops->push_back(op);
+    const Plan& pl = *built;
+    emit(OP_TEMB, [h = h, dim0 = k.cout, act = pl.temb_act, proj = pl.temb_proj, emb = pl.temb_emb, u1 = pl.temb_u1,
+                   u2 = pl.temb_u2, lead = h->training ? nullptr : pl.temb_lead](const RunArgs& a, cudaStream_t s) {
+      auto P = [h](const char* name) { return h->pptr[h->pidx.at(name)]; };
+      return launch_temb(a.t, h->N, dim0, P("time_embedding.linear_1.weight"), P("time_embedding.linear_1.bias"),
+                         P("time_embedding.linear_2.weight"), P("time_embedding.linear_2.bias"), act,
+                         (const float*)(h->packed + h->off_wcat), (const float*)(h->packed + h->off_bcat), h->temb_rows,
+                         proj, s, emb, u1, u2, lead);
+    }, 2);   // the MLP, then every resnet's projection
     return conv_in(k, nullptr);
   }
 
   // post_quant_conv on the caller's latents, then conv_in
   Act latent_in(const Block& k) {
-    built->zq = (float*)ws.take((size_t)N * k.cin * H * W * 4);
-    Op op{};
-    op.kind = OP_MIX1X1;
-    op.f0 = built->zq; op.C = k.cin; op.H = H; op.W = W;
-    op.fw = P("post_quant_conv.weight"); op.fb = P("post_quant_conv.bias");
-    if (h->training) op.f1 = built->z_in = (float*)ws.take((size_t)N * k.cin * H * W * 4);
-    ops->push_back(op);
-    return conv_in(k, built->zq);
+    float* zq = built->zq = (float*)ws.take((size_t)N * k.cin * H * W * 4);
+    float* z_in = h->training ? built->z_in = (float*)ws.take((size_t)N * k.cin * H * W * 4) : nullptr;
+    emit(OP_MIX1X1, [zq, z_in, w = P("post_quant_conv.weight"), b = P("post_quant_conv.bias"), N = N, L = k.cin, H = H,
+                     W = W](const RunArgs& a, cudaStream_t s) {
+      if (z_in) {   // training: the input is kept for the weight gradient
+        const cudaError_t e = cudaMemcpyAsync(z_in, a.in, (size_t)N * L * H * W * 4, cudaMemcpyDeviceToDevice, s);
+        if (e != cudaSuccess) return e;
+      }
+      return launch_mix1x1(a.in, w, b, zq, N, L, H * W, s);
+    });
+    return conv_in(k, zq);
   }
 
   // ResnetBlock2D on x = cat(a, b) (b optional) -> out (raw + stats)
@@ -564,10 +608,7 @@ struct Builder {
     const float2* ss1 = gn_finalize(a, b, n + ".norm1");
     Act h1 = pooled("h1", cout, H, W, true);
     {
-      Op op{};
-      op.kind = OP_CONV;
-      ConvParams& p = op.conv;
-      conv_common(p, h1);
+      ConvParams p = conv_geom(N, h1);
       p.nseg = 1;
       seg(p.seg[0], a, k.conv1[0], taps_conv(3));
       seg_norm(p.seg[0], ss1, cin, true);
@@ -581,15 +622,12 @@ struct Builder {
         p.temb = built->temb_proj + k.temb_row;
         p.temb_stride = h->temb_rows;
       }
-      ops->push_back(op);
+      conv(p);
     }
     const float2* ss2 = gn_finalize(h1, nullptr, n + ".norm2");
     Act out = output(k, cout, H, W);
     {
-      Op op{};
-      op.kind = OP_CONV;
-      ConvParams& p = op.conv;
-      conv_common(p, out);
+      ConvParams p = conv_geom(N, out);
       p.nseg = 1;
       seg(p.seg[0], h1, k.conv2, taps_conv(3));
       seg_norm(p.seg[0], ss2, cout, true);
@@ -606,7 +644,7 @@ struct Builder {
         p.nseg = 2;
         p.bias = P(n + ".conv2.bias");
       }
-      ops->push_back(op);
+      conv(p);
     }
     built->taps[n + ".h1"] = h1;
     built->taps[n] = out;
@@ -617,10 +655,7 @@ struct Builder {
   // and per-sample additive vector
   void linear(const Act& out, const Act& src, size_t woff, const float* bias, const float2* ss = nullptr,
               const Act* residual = nullptr, size_t ident = 0, const float* vec = nullptr, int vec_stride = 0) {
-    Op op{};
-    op.kind = OP_CONV;
-    ConvParams& p = op.conv;
-    conv_common(p, out);
+    ConvParams p = conv_geom(N, out);
     p.nseg = 1;
     seg(p.seg[0], src, woff, taps_conv(1));
     if (ss) seg_norm(p.seg[0], ss, src.C, false);
@@ -630,7 +665,7 @@ struct Builder {
     }
     p.bias = bias;
     p.temb = vec; p.temb_stride = vec_stride;
-    ops->push_back(op);
+    conv(p);
   }
 
   // Transformer2DModel with one BasicTransformerBlock (conditional U-Net), encoder sequence length 1:
@@ -643,35 +678,27 @@ struct Builder {
     const std::string t = n + ".transformer_blocks.0";
     const float2* ssx = gn_finalize(x, nullptr, n + ".norm", 1e-6f);
     float* vec = (float*)ws.take((size_t)N * C * sizeof(float));
-    {
-      Op op{};
-      op.kind = OP_XVEC;
-      op.C = C; op.cin = k.cross;
-      op.fw = P(t + ".attn2.to_v.weight"); op.fb = P(t + ".attn2.to_out.0.weight"); op.fc = P(t + ".attn2.to_out.0.bias");
-      op.f1 = vec;
-      ops->push_back(op);
-    }
+    emit(OP_XVEC, [h = h, wv = P(t + ".attn2.to_v.weight"), wo = P(t + ".attn2.to_out.0.weight"),
+                   bo = P(t + ".attn2.to_out.0.bias"), vec, N = N, C, X = k.cross](const RunArgs&, cudaStream_t s) {
+      return launch_cross_attn_vec(h->enc, wv, wo, bo, vec, N, C, X, s);
+    });
     Act h0 = pooled("tf_h0", C, H, W, false);
     linear(h0, x, k.proj_in, P(n + ".proj_in.bias"), ssx);
     Act n1 = pooled("tf_ln", C, H, W, false);
     auto layer_norm = [&](const Act& src, const Act& dst, const std::string& nm) {
-      Op op{};
-      op.kind = OP_LN;
-      op.src = src.p; op.dst = dst.p; op.C = C; op.H = H; op.W = W;
-      op.fw = P(nm + ".weight"); op.fb = P(nm + ".bias"); op.eps = 1e-5f;
-      ops->push_back(op);
+      emit(OP_LN, [x = src.p, y = dst.p, g = P(nm + ".weight"), b = P(nm + ".bias"), N = N, C, H, W](const RunArgs&,
+                                                                                                      cudaStream_t s) {
+        return launch_layernorm_pf8(x, y, g, b, N, C, H, W, 1e-5f, s);
+      });
     };
     layer_norm(h0, n1, t + ".norm1");
     Act qkv = pooled("tf_qkv", 3 * C, H, W, false);
     linear(qkv, n1, k.qkv, nullptr);
     Act ao = pooled("tf_ao", C, H, W, false);
-    {
-      Op op{};
-      op.kind = OP_MHA;
-      op.src = qkv.p; op.dst = ao.p; op.C = C; op.H = H; op.W = W; op.cin = heads;
-      if (h->training) op.f0 = built->lse[n] = (float*)ws.take((size_t)N * heads * H * W * sizeof(float));
-      ops->push_back(op);
-    }
+    float* lse = h->training ? built->lse[n] = (float*)ws.take((size_t)N * heads * H * W * sizeof(float)) : nullptr;
+    emit(OP_MHA, [q = qkv.p, o = ao.p, N = N, C, heads = heads, H, W, lse](const RunArgs&, cudaStream_t s) {
+      return launch_mha_flash(q, o, N, C, heads, H, W, s, lse);
+    });
     Act h2 = pooled("tf_h2", C, H, W, false);
     linear(h2, ao, k.out, P(t + ".attn1.to_out.0.bias"), nullptr, &h0, k.ident, vec, C);
     Act n3 = pooled("tf_ln", C, H, W, false);     // the same buffer as n1 unless training
@@ -679,12 +706,9 @@ struct Builder {
     Act ff1 = pooled("tf_ff1", 8 * C, H, W, false);
     linear(ff1, n3, k.ff1, P(t + ".ff.net.0.proj.bias"));
     Act gg = pooled("tf_gg", 4 * C, H, W, false);
-    {
-      Op op{};
-      op.kind = OP_GEGLU;
-      op.src = ff1.p; op.dst = gg.p; op.C = 4 * C; op.H = H; op.W = W;
-      ops->push_back(op);
-    }
+    emit(OP_GEGLU, [x = ff1.p, y = gg.p, N = N, C, H, W](const RunArgs&, cudaStream_t s) {
+      return launch_geglu_pf8(x, y, N, 4 * C, H, W, s);
+    });
     Act h3 = pooled("tf_h0", C, H, W, false);     // h0 is dead after h2
     linear(h3, gg, k.ff2, P(t + ".ff.net.2.bias"), nullptr, &h2, k.ident);
     Act out = output(k, C, H, W);
@@ -711,23 +735,17 @@ struct Builder {
     const size_t tsz = (size_t)N * (C / 8) * go.PL * 8;  // elements per parity tensor
     Act par = pooled("parity", 4 * C, Ho, Wo, false);     // 4 tensors back to back (same bytes as 4C channels)
     built->taps[k.name + ".parity"] = par;
-    {
-      Op op{};
-      op.kind = OP_PARITY;
-      op.src = x.p; op.dst = par.p; op.C = C; op.H = x.H; op.W = x.W;
-      ops->push_back(op);
-    }
+    emit(OP_PARITY, [x, par = par.p, N = N](const RunArgs&, cudaStream_t s) {
+      return launch_parity_split(x.p, par, N, x.C, x.H, x.W, s);
+    });
     Act y = output(k, C, Ho, Wo);
-    Op op{};
-    op.kind = OP_CONV;
-    ConvParams& p = op.conv;
-    conv_common(p, y);
+    ConvParams p = conv_geom(N, y);
     p.nseg = 4;
     for (int a = 0; a < 2; ++a)
       for (int b = 0; b < 2; ++b)
         seg(p.seg[a * 2 + b], par.p + (size_t)(a * 2 + b) * tsz, C, Ho, Wo, k.seg[a * 2 + b], down_taps(k, a, b));
     p.bias = P(k.name + ".bias");
-    ops->push_back(op);
+    conv(p);
     built->taps[k.name] = y;
     return y;
   }
@@ -738,17 +756,14 @@ struct Builder {
     Act y = output(k, C, hh * 2, ww * 2);
     for (int pa = 0; pa < 2; ++pa)
       for (int pb = 0; pb < 2; ++pb) {
-        Op op{};
-        op.kind = OP_CONV;
-        ConvParams& p = op.conv;
         Act lo = y;                       // item geometry = low-res input geometry, output tensor = y
         lo.H = hh; lo.W = ww;
-        conv_common(p, lo);
+        ConvParams p = conv_geom(N, lo);
         p.up2 = 1; p.oy = pa; p.ox = pb;
         p.nseg = 1;
         seg(p.seg[0], x, k.seg[pa * 2 + pb], taps_up2(pa, pb));
         p.bias = P(k.name + ".bias");
-        ops->push_back(op);
+        conv(p);
       }
     built->taps[k.name] = y;
     return y;
@@ -761,27 +776,21 @@ struct Builder {
     // the same window in its transform warps, and a 1-tap k-step (192 MMA cycles) cannot hide that (measured 187 us per
     // launch at 16x16, batch 64).  The normalised tensor is tiny here (16 MB): materialise it once, project the plain tensor.
     Act xn = pooled("attn_xn", C, H, W, false);
-    {
-      Op op{};
-      op.kind = OP_GNAPPLY;
-      GnApplyParams& g = op.gn;
-      g.src[0] = x.p; g.stats[0] = x.stats; g.C[0] = C;
-      g.src[1] = nullptr; g.stats[1] = nullptr; g.C[1] = 0;
-      g.gamma = P(n + ".group_norm.weight"); g.beta = P(n + ".group_norm.bias");
-      g.dst = xn.p;
-      g.N = N; g.H = H; g.W = W; g.groups = h->norm_groups; g.eps = h->norm_eps; g.silu = 0;
-      ops->push_back(op);
-    }
+    const GnApplyParams g = gn_params(h, N, x, nullptr, n + ".group_norm", xn.p, false);
+    emit(OP_GNAPPLY, [g](const RunArgs&, cudaStream_t s) { return launch_gn_apply(g, s); });
     Act qkv = pooled("qkv", 3 * C, H, W, false);
     linear(qkv, xn, k.qkv, PK<float>(k.bias));   // q|k|v blocks are contiguous
     Act ao = pooled("attn_o", C, H, W, false);
-    {
-      Op op{};
-      op.kind = single_head ? OP_ATTN1 : OP_ATTN;
-      op.src = qkv.p; op.dst = ao.p; op.C = C; op.H = H; op.W = W;
-      if (single_head) op.f0 = (float*)ws.take((size_t)N * H * W * H * W * sizeof(float));
-      if (single_head && h->training) built->probs[n] = op.f0;
-      ops->push_back(op);
+    if (single_head) {
+      float* scores = (float*)ws.take((size_t)N * H * W * H * W * sizeof(float));
+      if (h->training) built->probs[n] = scores;
+      emit(OP_ATTN1, [q = qkv.p, o = ao.p, scores, N = N, C, H, W](const RunArgs&, cudaStream_t s) {
+        return launch_attention_1head(q, o, scores, N, C, H, W, s);
+      }, 3);   // scores, softmax, output
+    } else {
+      emit(OP_ATTN, [q = qkv.p, o = ao.p, N = N, C, H, W](const RunArgs&, cudaStream_t s) {
+        return launch_attention(q, o, N, C, H, W, s);
+      });
     }
     Act out = output(k, C, H, W);
     linear(out, ao, k.out, P(n + ".to_out.0.bias"), nullptr, &x, k.ident);   // + residual
@@ -795,15 +804,21 @@ struct Builder {
   // CTA (null: in conv_out)
   Act conv_out(const Block& k, const Act& x) {
     const std::string& n = k.name;
-    Op op{};
-    op.kind = OP_CONV_OUT;
-    ConvOutParams& p = op.co;
+    ConvOutParams p{};
     p.src = x.p; p.stats = x.stats;
     p.ss = gn_attach(x, nullptr, n + "conv_norm_out");
     p.gamma = P(n + "conv_norm_out.weight"); p.beta = P(n + "conv_norm_out.bias");
     p.w = P(n + "conv_out.weight"); p.b = P(n + "conv_out.bias");
     p.N = N; p.C = x.C; p.H = x.H; p.W = x.W; p.cout = k.cout; p.groups = h->norm_groups; p.eps = h->norm_eps;
-    ops->push_back(op);
+    emit(OP_CONV_OUT, [p](const RunArgs& a, cudaStream_t s) {
+      ConvOutParams q = p;
+      q.eps_out = a.out;
+      q.x = a.in; q.z = a.noise; q.x_out = a.x_out;
+      static_assert(sizeof(b200ad_step_coef) == sizeof(StepCoef), "step-coefficient layouts differ");
+      q.coef_dev = reinterpret_cast<const StepCoef*>(a.coef_dev);
+      if (a.coef) memcpy(&q.coef, a.coef, sizeof(StepCoef));
+      return launch_conv_out(q, s);
+    });
     built->taps[n + "pre_out"] = x;
     return x;
   }
@@ -814,22 +829,18 @@ struct Builder {
     Act eo = pooled("enc_out", 128, x.H, x.W, false);
     {
       const float2* ss = gn_finalize(x, nullptr, n + "conv_norm_out");
-      Op op{};
-      op.kind = OP_CONV;
-      ConvParams& p = op.conv;
-      conv_common(p, eo);
+      ConvParams p = conv_geom(N, eo);
       p.nseg = 1;
       seg(p.seg[0], x, k.seg[0], taps_conv(3));
       seg_norm(p.seg[0], ss, x.C, true);
       p.bias = PK<float>(k.bias);
-      ops->push_back(op);
+      conv(p);
     }
     built->taps[n + "conv_out"] = eo;
-    Op op{};
-    op.kind = OP_VAE_SAMPLE;
-    op.src = eo.p; op.C = 128; op.H = x.H; op.W = x.W; op.cin = k.cout / 2;
-    op.fw = P("quant_conv.weight"); op.fb = P("quant_conv.bias");
-    ops->push_back(op);
+    emit(OP_VAE_SAMPLE, [eo = eo.p, w = P("quant_conv.weight"), b = P("quant_conv.bias"), N = N, L = k.cout / 2, H = x.H,
+                         W = x.W](const RunArgs& a, cudaStream_t s) {
+      return launch_vae_sample(eo, w, b, a.noise, a.out, a.moments, N, 128, L, H, W, s);
+    });
     return eo;
   }
 
@@ -862,74 +873,36 @@ static bool debug_nopool() {
 }
 
 // ================================================================================= plan executor
-struct RunArgs {                        // the per-call inputs of a plan
-  const float* in = nullptr;            // U-Net: the sample x; autoencoder: the image (encode) or the latents (decode)
-  const float* t = nullptr;             // U-Net: timesteps [N]
-  const float* noise = nullptr;         // U-Net: the scheduler's noise z; autoencoder encode: the sampling noise
-  float* out = nullptr;                 // U-Net: eps (optional); autoencoder: z (encode) or the image (decode)
-  float* moments = nullptr;             // autoencoder encode (optional)
-  float* x_out = nullptr;               // U-Net: the scheduler update (optional), with coef or coef_dev
-  const b200ad_step_coef* coef = nullptr;
-  const b200ad_step_coef* coef_dev = nullptr;
+struct OpEvents {   // per-op timing: an event before the first op of a run and one after every op
+  std::vector<cudaEvent_t> ev;
+  ~OpEvents() {
+    for (cudaEvent_t e : ev)
+      if (e) cudaEventDestroy(e);
+  }
+  int ms(size_t i, float* out) const {   // device time of op i (after the stream has synchronised)
+    CK(cudaEventElapsedTime(out, ev[i], ev[i + 1]));
+    return 0;
+  }
 };
 
-static int run_ops(NetBase* h, const OpList& l, const RunArgs& a, cudaStream_t st) {
-  const Plan& pl = h->plan;
-  int launches = 0;
-  CK(cudaMemsetAsync(l.stats, 0, l.stats_bytes, st));
-  for (const Op& op : l.ops) {
-    switch (op.kind) {
-      case OP_TEMB:      // two launches: the MLP, then every resnet's projection
-        CK(launch_temb(a.t, h->N, op.C, h->pptr[h->pidx.at("time_embedding.linear_1.weight")],
-                       h->pptr[h->pidx.at("time_embedding.linear_1.bias")],
-                       h->pptr[h->pidx.at("time_embedding.linear_2.weight")],
-                       h->pptr[h->pidx.at("time_embedding.linear_2.bias")], pl.temb_act,
-                       (const float*)(h->packed + h->off_wcat), (const float*)(h->packed + h->off_bcat), h->temb_rows,
-                       pl.temb_proj, st, h->training ? pl.temb_emb : nullptr, h->training ? pl.temb_u1 : nullptr,
-                       h->training ? pl.temb_u2 : nullptr, h->training ? nullptr : pl.temb_lead));
-        launches += 1;
-        break;
-      case OP_CONV_IN:
-        CK(launch_conv_in(op.f0 ? op.f0 : a.in, op.fw, op.fb, h->N, op.cin, op.H, op.W, op.C, op.dst, op.conv.stats, st));
-        break;
-      case OP_GN: CK(launch_gn_finalize(op.gn, op.ss, st)); break;
-      case OP_GNAPPLY: CK(launch_gn_apply(op.gn, st)); break;
-      case OP_CONV: CK(launch_conv_tc(op.conv, h->num_sms, st)); break;
-      case OP_PARITY: CK(launch_parity_split(op.src, op.dst, h->N, op.C, op.H, op.W, st)); break;
-      case OP_ATTN: CK(launch_attention(op.src, op.dst, h->N, op.C, op.H, op.W, st)); break;
-      case OP_ATTN1:     // three launches: scores, softmax, output
-        CK(launch_attention_1head(op.src, op.dst, op.f0, h->N, op.C, op.H, op.W, st));
-        launches += 2;
-        break;
-      case OP_LN: CK(launch_layernorm_pf8(op.src, op.dst, op.fw, op.fb, h->N, op.C, op.H, op.W, op.eps, st)); break;
-      case OP_GEGLU: CK(launch_geglu_pf8(op.src, op.dst, h->N, op.C, op.H, op.W, st)); break;
-      case OP_MHA: CK(launch_mha_flash(op.src, op.dst, h->N, op.C, op.cin, op.H, op.W, st, op.f0)); break;
-      case OP_XVEC:
-        if (!h->enc) return set_err("conditional U-Net: call b200ad_unet_set_encoding before forward");
-        if (h->enc_S != 1) return set_err("conditional U-Net: encoder sequence length %d (only 1 is implemented)", h->enc_S);
-        CK(launch_cross_attn_vec(h->enc, op.fw, op.fb, op.fc, op.f1, h->N, op.C, op.cin, st));
-        break;
-      case OP_VAE_SAMPLE:
-        CK(launch_vae_sample(op.src, op.fw, op.fb, a.noise, a.out, a.moments, h->N, op.C, op.cin, op.H, op.W, st));
-        break;
-      case OP_MIX1X1:    // training: the input is kept for the weight gradient
-        if (op.f1) CK(cudaMemcpyAsync(op.f1, a.in, (size_t)h->N * op.C * op.H * op.W * 4, cudaMemcpyDeviceToDevice, st));
-        CK(launch_mix1x1(a.in, op.fw, op.fb, op.f0, h->N, op.C, op.H * op.W, st));
-        break;
-      case OP_CONV_OUT: {
-        ConvOutParams p = op.co;
-        p.eps_out = a.out;
-        p.x = a.in; p.z = a.noise; p.x_out = a.x_out;
-        static_assert(sizeof(b200ad_step_coef) == sizeof(StepCoef), "step-coefficient layouts differ");
-        p.coef_dev = reinterpret_cast<const StepCoef*>(a.coef_dev);
-        if (a.coef) memcpy(&p.coef, a.coef, sizeof(StepCoef));
-        CK(launch_conv_out(p, st));
-        break;
-      }
-    }
-    ++launches;
+// Zeroes the plan's GroupNorm statistics and launches its ops in order; on success stores the launch count.
+static int run_ops(const NetBase* h, const OpList& l, const RunArgs& a, cudaStream_t st, int* launches,
+                   OpEvents* timing = nullptr) {
+  if (l.stats_bytes) CK(cudaMemsetAsync(l.stats, 0, l.stats_bytes, st));
+  if (timing) {
+    timing->ev.assign(l.ops.size() + 1, nullptr);
+    for (cudaEvent_t& e : timing->ev) CK(cudaEventCreate(&e));
+    CK(cudaEventRecord(timing->ev[0], st));
   }
-  h->last_launches = launches;
+  int n = 0;
+  for (size_t i = 0; i < l.ops.size(); ++i) {
+    const Op& op = l.ops[i];
+    const cudaError_t e = op.run ? op.run(a, st) : launch_conv_tc(op.conv, h->num_sms, st);
+    if (e != cudaSuccess) return set_err("%s: %s", op_names[op.kind], cudaGetErrorString(e));
+    if (timing) CK(cudaEventRecord(timing->ev[i + 1], st));
+    n += op.launches;
+  }
+  *launches = n;
   return 0;
 }
 

@@ -191,9 +191,13 @@ extern "C" int b200ad_unet_bind_workspace(b200ad_unet* h, void* workspace, size_
   return 0;
 }
 
-static int run_plan(b200ad_unet* h, const RunArgs& a, cudaStream_t st) {
+static int run_plan(b200ad_unet* h, const RunArgs& a, cudaStream_t st, OpEvents* timing = nullptr) {
   if (h->plan.lists.empty()) return set_err("bind_workspace must be called before forward");
-  return run_ops(h, h->plan.lists[0], a, st);
+  if (h->cfg.cross_attention_dim) {   // the transformer blocks read the encoding
+    if (!h->enc) return set_err("conditional U-Net: call b200ad_unet_set_encoding before forward");
+    if (h->enc_S != 1) return set_err("conditional U-Net: encoder sequence length %d (only 1 is implemented)", h->enc_S);
+  }
+  return run_ops(h, h->plan.lists[0], a, st, &h->last_launches, timing);
 }
 
 // One step with a CUDA event pair around every launch of the plan (device time per op, on `stream`).
@@ -202,30 +206,20 @@ extern "C" int b200ad_unet_profile_step(b200ad_unet* h, const float* x, const fl
                                         double* op_flops, int max_ops, void* stream) {
   if (h->plan.lists.empty()) return set_err("bind_workspace must be called before profile_step");
   cudaStream_t st = (cudaStream_t)stream;
-  const OpList& l = h->plan.lists[0];
-  const std::vector<Op>& saved = l.ops;
-  const int nops = (int)saved.size();
+  const std::vector<Op>& ops = h->plan.lists[0].ops;
+  const int nops = (int)ops.size();
   if (nops > max_ops) return set_err("profile_step: %d ops > max_ops %d", nops, max_ops);
-  std::vector<cudaEvent_t> ev(nops + 1);
-  for (auto& e : ev) CK(cudaEventCreate(&e));
-  CK(cudaMemsetAsync(l.stats, 0, l.stats_bytes, st));
   RunArgs a;
   a.in = x; a.t = t; a.noise = z; a.coef = coef; a.x_out = x_out;
-  OpList one;                  // a one-op plan between two events (no stats to clear: stats_bytes 0)
-  one.stats = l.stats;
-  for (int i = 0; i < nops; ++i) {
-    CK(cudaEventRecord(ev[i], st));
-    one.ops.assign(1, saved[i]);
-    if (const int rc = run_ops(h, one, a, st)) return rc;
-  }
-  CK(cudaEventRecord(ev[nops], st));
+  OpEvents ev;
+  if (run_plan(h, a, st, &ev)) return -1;
   CK(cudaStreamSynchronize(st));
   for (int i = 0; i < nops; ++i) {
-    CK(cudaEventElapsedTime(&op_ms[i], ev[i], ev[i + 1]));
-    op_kind[i] = (int)saved[i].kind;
+    if (ev.ms(i, &op_ms[i])) return -1;
+    op_kind[i] = (int)ops[i].kind;
     double fl = 0;
-    if (saved[i].kind == OP_CONV) {
-      const ConvParams& p = saved[i].conv;
+    if (ops[i].kind == OP_CONV) {
+      const ConvParams& p = ops[i].conv;
       double k = 0;
       // algorithmic taps: a folded upsample launch stands for the 3x3 conv on its quarter of the output pixels; a residual
       // add carried as an identity-weight K-segment is an addition, not a convolution: no algorithmic FLOPs
@@ -239,7 +233,6 @@ extern "C" int b200ad_unet_profile_step(b200ad_unet* h, const float* x, const fl
     }
     op_flops[i] = fl;
   }
-  for (auto& e : ev) cudaEventDestroy(e);
   return nops;
 }
 

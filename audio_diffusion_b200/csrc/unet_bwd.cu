@@ -8,7 +8,8 @@
 //     as four scatter launches, the folded upsampling convs as one gather launch over the parity planes of the gradient);
 //   * weight gradients run on wgrad_tc_kernel (wgmma, pixels as the reduction dimension, MN-major operands);
 //   * GroupNorm(+SiLU), attention core, biases / time embedding, conv_in / conv_out are memory-bound kernels (bwd_kernels.cu).
-// This first version materialises the normalised activations for the weight gradients (no fusion yet) — DESIGN.md §6.
+// The normalised activations the weight gradients read are materialised (no fusion yet).
+// A backward plan is an OpList of net.cuh, run by the forward's executor (run_ops).
 #include "bwd_kernels.cuh"
 #include "unet.cuh"
 #include "vae.cuh"
@@ -20,45 +21,13 @@ namespace b200ad {
 struct View {            // channel range of a PF8 tensor
   const __nv_bfloat16* p = nullptr;   // first plane of the view (image 0)
   int C = 0, img_planes = 0, H = 0, W = 0;
-};
-
-struct BOp {
-  enum Kind { CONV, WGRAD, GNBWD, GNAPPLY, CHANSUM, REDUCE_N, SCATTER, PF8ADD, ATTNBWD, PARITY, UNFOLD, SCALAR_WGRAD, CONVIN,
-              FLIP, SUMADD, LIN_IN, LIN_W, SILU_BWD, SILU_FWD, MEMSET,
-              LNBWD, GEGLUBWD, XVECBWD, MHABWD, ATTN1BWD, QUANTBWD, LATENTINBWD, NKINDS } kind;
-  ConvParams conv;
-  WgradDesc wg;
-  GnBwdParams gb;
-  GnApplyParams ga;
-  UnfoldMasks um;
-  const __nv_bfloat16* src = nullptr;
-  const __nv_bfloat16* src2 = nullptr;
-  const __nv_bfloat16* src3 = nullptr;
-  __nv_bfloat16* dst = nullptr;
-  __nv_bfloat16* dst2 = nullptr;  // bf16 scratch
-  const float* f0 = nullptr;
-  const float* f1 = nullptr;
-  const float* f2 = nullptr;
-  float* o0 = nullptr;
-  float* o1 = nullptr;
-  float* o2 = nullptr;        // scratch (never a parameter gradient)
-  int C = 0, H = 0, W = 0, a = 0, b = 0, c = 0, d = 0;
-  long long n = 0;
-  bool x_is_input = false;    // SCALAR_WGRAD: X = the forward input image passed to backward()
-  bool x_is_geps = false;     // X / source = the output gradient passed to backward()
-};
-
-struct BwdArgs {              // the per-call inputs of a backward plan
-  const float* x = nullptr;   // the forward's input image (SCALAR_WGRAD x_is_input)
-  const float* g_eps = nullptr;   // the gradient of the model output (U-Net: eps; autoencoder decoder: the image)
-  const float* g_mom = nullptr;   // autoencoder encoder: the gradient of the moments
-  float* g_z = nullptr;           // autoencoder decoder: the gradient w.r.t. the latents (written)
+  size_t off = 0;                     // byte offset of p in its arena (Act::off)
 };
 
 }  // namespace b200ad
 
 struct Backward {
-  std::vector<BOp> ops;
+  OpList list;                       // the ops (no GroupNorm statistics)
   std::vector<PackJob> jobs;         // transposed weight packs, redone at every backward (the weights move every step)
   std::vector<size_t> goff;          // float offset of every parameter's gradient in the flat buffer
   size_t grad_floats = 0;
@@ -86,19 +55,14 @@ struct BwdBuilder {
   int heads = 8;                              // conditional U-Net: attention heads of the transformer blocks
   bool single_head = false;                   // attention with one head of dim C (the autoencoder) instead of head_dim 8
   // per-sample channel sums produced by the GroupNorm-backward apply pass for the gradient tensor it writes (keyed by that
-  // tensor): the producer's bias gradient then is a reduction over N of a [N][C] array instead of a pass over the tensor
+  // tensor's arena offset, the same in the size pass): the producer's bias gradient then is a reduction over N of a [N][C]
+  // array instead of a pass over the tensor
   float* csum_arena = nullptr;
   size_t csum_floats = 0, csum_used = 0;
-  std::map<const __nv_bfloat16*, float*> csum_of;
+  std::map<size_t, float*> csum_of;
   const float* last_cs = nullptr;             // [N][C] sums of the latest bias_grad (the time-embedding rows are read from it)
 
-  Act act_alloc(int C, int H, int W) {
-    Act a;
-    a.C = C; a.H = H; a.W = W;
-    const Geom g = make_geom(N, H, W);
-    a.p = (__nv_bfloat16*)mem.take((size_t)N * (C / 8) * g.PL * 16);
-    return a;
-  }
+  Act act_alloc(int C, int H, int W) { return take_act(mem, N, C, H, W); }
   Act tmp(const std::string& tag, int C, int H, int W) {
     const std::string key = S("%s:%d:%d:%d", tag.c_str(), C, H, W);
     auto it = pool.find(key);
@@ -123,9 +87,15 @@ struct BwdBuilder {
     const Geom g = make_geom(1, a.H, a.W);
     v.p = a.p ? a.p + (long long)(c0 / 8) * g.PL * 8 : nullptr;
     v.C = C; v.img_planes = a.C / 8; v.H = a.H; v.W = a.W;
+    v.off = a.off + (size_t)(c0 / 8) * g.PL * 16;
     return v;
   }
   static View whole(const Act& a) { return view(a, 0, a.C); }
+
+  void emit(OpKind kind, OpFn run, int launches = 1) { bw->list.ops.push_back(Op{kind, launches, {}, std::move(run)}); }
+  void zero(void* p, size_t bytes) {
+    emit(OP_MEMSET, [p, bytes](const RunArgs&, cudaStream_t s) { return cudaMemsetAsync(p, 0, bytes, s); });
+  }
 
   // ---- transposed weight packing jobs ----------------------------------------------------------------------------
   // GEMM out channels = the layer's input channels [i0, i0 + I) ... the kernel reads W[o][i][kh][kw] with i = co.
@@ -140,13 +110,21 @@ struct BwdBuilder {
     bw->jobs.push_back(j);
     return bw->arena ? (const __nv_bfloat16*)(bw->arena + j.off) : nullptr;
   }
+  // the plan's first op: all of its transposed packs in one launch
+  void pack_op() {
+    emit(OP_PACK_T, [h = h, bw = bw](const RunArgs&, cudaStream_t s) {
+      std::vector<PackItem> items;
+      items.reserve(bw->jobs.size());
+      for (const PackJob& j : bw->jobs) items.push_back(make_pack_item(h, j, bw->arena));
+      return launch_pack_batch(bw->pack_batch, items, s);
+    });
+  }
 
   // ---- op emitters ------------------------------------------------------------------------------------------------
-  void conv_base(ConvParams& p, const Act& out) {
-    const Geom g = make_geom(N, out.H, out.W);
-    p = ConvParams{};
-    p.N = N; p.H = out.H; p.W = out.W; p.Wp = g.Wp; p.lead = g.lead; p.PL = g.PL;
-    p.cout = out.C; p.out = out.p;
+  void conv(const ConvParams& p) {
+    Op op{OP_DGRAD};
+    op.conv = p;
+    bw->list.ops.push_back(op);
   }
   static void seg(ConvSeg& s, const View& src, const __nv_bfloat16* wpack, const TapSet& t) {
     set_seg(s, src.p, src.img_planes, src.C, src.H, src.W, wpack, t);
@@ -154,64 +132,49 @@ struct BwdBuilder {
   // data gradient of a stride-1 KxK conv: out (I channels) = conv^T(gy (O channels))
   void dgrad(const std::string& wname, const View& gy, const Act& out, int K) {
     const TapSet t = taps_mirrored(K);
-    BOp op{};
-    op.kind = BOp::CONV;
-    conv_base(op.conv, out);
-    seg(op.conv.seg[0], gy, tjob(wname, gy.C, out.C, K, t), t);
-    op.conv.nseg = 1;
-    bw->ops.push_back(op);
+    ConvParams p = conv_geom(N, out);
+    seg(p.seg[0], gy, tjob(wname, gy.C, out.C, K, t), t);
+    p.nseg = 1;
+    conv(p);
   }
   // weight gradient of the forward K-segment with tap set t (of ntaps_total taps of the weight) that read `act`
   void wgrad(const View& gy, const View& act, float* dw, int cin_total, int ci_off, int ntaps_total, const TapSet& t) {
-    BOp op{};
-    op.kind = BOp::WGRAD;
-    WgradDesc& d = op.wg;
+    WgradDesc d{};
     d.gy = gy.p; d.act = act.p; d.dw = dw; d.N = N; d.H = gy.H; d.W = gy.W; d.cout = gy.C; d.cin = act.C;
     d.gy_img_planes = gy.img_planes; d.act_img_planes = act.img_planes;
     d.cin_total = cin_total; d.ci_off = ci_off; d.ntaps_total = ntaps_total; d.ntaps = t.pack.ntaps;
     for (int k = 0; k < t.pack.ntaps; ++k) { d.dh[k] = t.dh[k]; d.dw_[k] = t.dw[k]; d.tapidx[k] = t.wtap[k]; }
-    bw->ops.push_back(op);
+    emit(OP_WGRAD, [h = h, d](const RunArgs&, cudaStream_t s) { return launch_wgrad_tc(d, h->num_sms, s); });
   }
   void wgrad_conv(const View& gy, const View& act, const std::string& wname, int K) {   // plain stride-1 conv
     wgrad(gy, act, PG(wname), act.C, 0, K * K, taps_conv(K));
   }
-  // per-channel sums of a gradient -> bias gradient(s); returns the [N][C] scratch (valid until the next chan_sum)
+  // per-channel sums of a gradient -> bias gradient(s); last_cs: the [N][C] sums (valid until the next chan_sum)
   void bias_grad(const View& g, const std::string& bname, const std::string& bname2 = "") {
-    BOp op{};
-    auto it = csum_of.find(g.p);
+    float* db = PG(bname);
+    float* db2 = bname2.empty() ? nullptr : PG(bname2);
+    auto it = csum_of.find(g.off);
     if (it != csum_of.end() && g.img_planes * 8 == g.C) {     // whole tensor, sums already made by the pass that wrote it
-      op.kind = BOp::REDUCE_N;
-      op.f0 = it->second; op.o0 = PG(bname); op.o1 = bname2.empty() ? nullptr : PG(bname2); op.C = g.C;
       last_cs = it->second;
-      bw->ops.push_back(op);
+      emit(OP_REDUCE_N, [sums = it->second, db, db2, N = N, C = g.C](const RunArgs&, cudaStream_t s) {
+        return launch_reduce_n_add(sums, db, db2, N, C, s);
+      });
       return;
     }
-    op.kind = BOp::CHANSUM;
-    op.src = g.p; op.o0 = cs; op.C = g.C; op.a = g.img_planes; op.H = g.H; op.W = g.W;
-    op.o1 = PG(bname);                                        // bias gradient(s) accumulated by the same kernel
-    op.f1 = bname2.empty() ? nullptr : PG(bname2);
     last_cs = cs;
-    bw->ops.push_back(op);
+    emit(OP_CHANSUM, [g, sums = cs, db, db2, N = N](const RunArgs&, cudaStream_t s) {   // bias gradients by the same kernel
+      return launch_chan_sum(g.p, sums, N, g.C, g.img_planes, g.H, g.W, s, db, db2);
+    });
   }
   Act gn_apply(const std::string& tag, const Act& a, const Act* b, const std::string& norm, bool silu, float eps = -1.f) {
-    const int Ct = a.C + (b ? b->C : 0);
-    Act out = tmp(tag, Ct, a.H, a.W);
-    BOp op{};
-    op.kind = BOp::GNAPPLY;
-    GnApplyParams& p = op.ga;
-    p.src[0] = a.p; p.stats[0] = a.stats; p.C[0] = a.C;
-    p.src[1] = b ? b->p : nullptr; p.stats[1] = b ? b->stats : nullptr; p.C[1] = b ? b->C : 0;
-    p.gamma = P(norm + ".weight"); p.beta = P(norm + ".bias");
-    p.dst = out.p; p.N = N; p.H = a.H; p.W = a.W; p.groups = h->norm_groups; p.eps = eps < 0.f ? h->norm_eps : eps;
-    p.silu = silu ? 1 : 0;
-    bw->ops.push_back(op);
+    Act out = tmp(tag, a.C + (b ? b->C : 0), a.H, a.W);
+    const GnApplyParams p = gn_params(h, N, a, b, norm, out.p, silu, eps);
+    emit(OP_GNAPPLY, [p](const RunArgs&, cudaStream_t s) { return launch_gn_apply(p, s); });
     return out;
   }
   void gn_bwd(const Act& ga, const Act& a, const Act* b, const std::string& norm, bool silu, const Act& d0, const Act* d1,
               const __nv_bfloat16* addS, const __nv_bfloat16* add0, float eps = -1.f) {
-    BOp op{};
-    op.kind = BOp::GNBWD;
-    GnBwdParams& p = op.gb;
+    GnBwdParams p{};
     p.ga = ga.p;
     p.src[0] = a.p; p.stats[0] = a.stats; p.C[0] = a.C;
     p.src[1] = b ? b->p : nullptr; p.stats[1] = b ? b->stats : nullptr; p.C[1] = b ? b->C : 0;
@@ -224,16 +187,35 @@ struct BwdBuilder {
     const size_t need = (size_t)N * a.C;
     if (csum_used + need <= csum_floats) {
       p.csum0 = csum_arena ? csum_arena + csum_used : nullptr;
-      csum_of[d0.p] = p.csum0;
+      csum_of[d0.off] = p.csum0;
       csum_used += need;
-      if (!csum_arena) csum_of[d0.p] = (float*)1;             // size pass: the plan must have the same shape as the real one
     }
     p.N = N; p.H = a.H; p.W = a.W; p.groups = h->norm_groups; p.eps = eps < 0.f ? h->norm_eps : eps; p.silu = silu ? 1 : 0;
-    bw->ops.push_back(op);
+    emit(OP_GN_BWD, [p](const RunArgs&, cudaStream_t s) { return launch_gn_bwd(p, s); }, 2);
   }
   const __nv_bfloat16* skip_of(const std::string& name) const {
     auto it = skipgrad.find(name);
     return it == skipgrad.end() ? nullptr : it->second.p;
+  }
+  // conv_out's data gradient (3x3, O -> C channels) as the conv_in kernel over the fp32 output gradient gy (null: the
+  // gradient passed to backward()): g_a[c] = sum_o sum_t gy[o][p + s_t] * wflip[c][o][t]
+  void conv_out_dgrad(const std::string& wname, const float* gy, int O, float* wflip, const float* zbias, const Act& out) {
+    emit(OP_FLIP, [w = P(wname), wflip, C = out.C, O](const RunArgs&, cudaStream_t s) {
+      return launch_flip_taps(w, wflip, C, s, O);
+    });
+    emit(OP_CONV_IN_BWD, [gy, wflip, zbias, out, N = N, O](const RunArgs& a, cudaStream_t s) {
+      return launch_conv_in(gy ? gy : a.g_eps, wflip, zbias, N, O, out.H, out.W, out.C, out.p, nullptr, s);
+    });
+  }
+  // weight gradient of a 3x3 conv with one fp32 output channel x (null: the gradient passed to backward(); flip: x is
+  // that output's gradient, `g` the conv's input) or one fp32 input channel x (the conv's output gradient is `g`)
+  void scalar_wgrad(const Act& g, const float* x, bool x_is_input, float* dw, int flip) {
+    emit(OP_SCALAR_WGRAD, [g, x, x_is_input, dw, flip, N = N](const RunArgs& a, cudaStream_t s) {
+      return launch_scalar_conv_wgrad(g.p, x ? x : x_is_input ? a.in : a.g_eps, dw, N, g.C, g.H, g.W, flip, s);
+    });
+  }
+  void sum_add(const float* x, long long n, float* dst) {   // x null: the gradient passed to backward()
+    emit(OP_SUMADD, [x, n, dst](const RunArgs& a, cudaStream_t s) { return launch_sum_add(x ? x : a.g_eps, n, dst, s); });
   }
 
   // ---- blocks -----------------------------------------------------------------------------------------------------
@@ -259,12 +241,11 @@ struct BwdBuilder {
     gn_bwd(T1, h1, nullptr, n + ".norm2", true, Gh1, nullptr, nullptr, nullptr);
     // conv1 bias + time embedding projection rows of this block
     bias_grad(whole(Gh1), n + ".conv1.bias");
-    if (k.temb_row >= 0) {
-      BOp op{};
-      op.kind = BOp::SCATTER;
-      op.f0 = last_cs; op.o0 = gproj; op.C = co; op.a = h->temb_rows; op.b = k.temb_row;
-      bw->ops.push_back(op);
-    }
+    if (k.temb_row >= 0)
+      emit(OP_SCATTER, [sums = last_cs, gproj = gproj, N = N, co, rows = h->temb_rows, row = k.temb_row](const RunArgs&,
+                                                                                                         cudaStream_t s) {
+        return launch_scatter_rows(sums, gproj, N, co, rows, row, s);
+      });
     // conv1
     Act T2 = tmp("T2", Ct, H, W);
     dgrad(n + ".conv1.weight", whole(Gh1), T2, 3);
@@ -300,20 +281,18 @@ struct BwdBuilder {
     wgrad_conv(whole(Gout), whole(ao), n + ".to_out.0.weight", 1);
     bias_grad(whole(Gout), n + ".to_out.0.bias");
     Act Gqkv = tmp("Gqkv", 3 * C, H, W);
-    if (single_head) {   // the forward's softmax P is kept: four GEMMs on the tensor cores
+    if (single_head) {   // the forward's softmax P is kept: row dot products, then the dS, dV, dQ, dK GEMMs
       const long long S = (long long)H * W;
-      BOp op{};
-      op.kind = BOp::ATTN1BWD;
-      op.src = qkv.p; op.src2 = T1.p; op.src3 = ao.p; op.dst = Gqkv.p; op.f0 = h->plan.probs.at(n);
-      op.o2 = (float*)mem.take((size_t)N * S * sizeof(float));
-      op.dst2 = (__nv_bfloat16*)mem.take((size_t)N * S * S * sizeof(__nv_bfloat16));
-      op.C = C; op.H = H; op.W = W;
-      bw->ops.push_back(op);
+      float* D = (float*)mem.take((size_t)N * S * sizeof(float));
+      __nv_bfloat16* dS = (__nv_bfloat16*)mem.take((size_t)N * S * S * sizeof(__nv_bfloat16));
+      emit(OP_ATTN1_BWD, [q = qkv.p, o = ao.p, go = T1.p, probs = h->plan.probs.at(n), D, dS, gq = Gqkv.p, N = N, C, H,
+                          W](const RunArgs&, cudaStream_t s) {
+        return launch_attention_1head_bwd(q, o, go, probs, D, dS, gq, N, C, H, W, s);
+      }, 5);
     } else {
-      BOp op{};
-      op.kind = BOp::ATTNBWD;
-      op.src = qkv.p; op.src2 = T1.p; op.dst = Gqkv.p; op.C = C; op.H = H; op.W = W;
-      bw->ops.push_back(op);
+      emit(OP_ATTN_BWD, [q = qkv.p, go = T1.p, gq = Gqkv.p, N = N, C, H, W](const RunArgs&, cudaStream_t s) {
+        return launch_attention_bwd(q, go, gq, N, C, H, W, s);
+      });
     }
     Act XN = gn_apply("A", x, nullptr, n + ".group_norm", false);
     const char* names[3] = {"to_q", "to_k", "to_v"};
@@ -325,26 +304,22 @@ struct BwdBuilder {
     // g(norm(x)) = sum over q, k, v of W^T g: one launch, three K-segments
     Act T2 = tmp("T2", C, H, W);
     {
-      BOp op{};
-      op.kind = BOp::CONV;
-      conv_base(op.conv, T2);
+      ConvParams p = conv_geom(N, T2);
       const TapSet t = taps_mirrored(1);
       for (int k = 0; k < 3; ++k)
-        seg(op.conv.seg[k], view(Gqkv, k * C, C), tjob(n + "." + names[k] + ".weight", C, C, 1, t), t);
-      op.conv.nseg = 3;
-      bw->ops.push_back(op);
+        seg(p.seg[k], view(Gqkv, k * C, C), tjob(n + "." + names[k] + ".weight", C, C, 1, t), t);
+      p.nseg = 3;
+      conv(p);
     }
     gn_bwd(T2, x, nullptr, n + ".group_norm", false, G(xn), nullptr, Gout.p, skip_of(xn));
   }
 
   // LayerNorm over channels (eps 1e-5, as the forward): gx = LN-backward(gy; x) + add, gamma / beta gradients
   void layer_norm_bwd(const Act& gy, const Act& x, const std::string& norm, const Act& gx, const Act& add) {
-    BOp op{};
-    op.kind = BOp::LNBWD;
-    op.src = x.p; op.src2 = gy.p; op.src3 = add.p; op.dst = gx.p;
-    op.f0 = P(norm + ".weight"); op.o0 = PG(norm + ".weight"); op.o1 = PG(norm + ".bias");
-    op.C = x.C; op.H = x.H; op.W = x.W;
-    bw->ops.push_back(op);
+    emit(OP_LN_BWD, [x, gy = gy.p, add = add.p, gx = gx.p, gamma = P(norm + ".weight"), dgamma = PG(norm + ".weight"),
+                     dbeta = PG(norm + ".bias"), N = N](const RunArgs&, cudaStream_t s) {
+      return launch_layernorm_bwd_pf8(x.p, gy, add, gx, gamma, dgamma, dbeta, N, x.C, x.H, x.W, 1e-5f, s);
+    });
   }
 
   // Transformer2DModel with one BasicTransformerBlock (Builder::transformer) in reverse, from G(out) to G(x):
@@ -371,12 +346,9 @@ struct BwdBuilder {
     bias_grad(whole(Gh3), t + ".ff.net.2.bias");
     // GEGLU
     Act Gff1 = tmp("tf_Gff1", 8 * C, H, W);
-    {
-      BOp op{};
-      op.kind = BOp::GEGLUBWD;
-      op.src = ff1.p; op.src2 = Ggg.p; op.dst = Gff1.p; op.C = 4 * C; op.H = H; op.W = W;
-      bw->ops.push_back(op);
-    }
+    emit(OP_GEGLU_BWD, [src = ff1.p, gy = Ggg.p, gx = Gff1.p, N = N, C, H, W](const RunArgs&, cudaStream_t s) {
+      return launch_geglu_bwd_pf8(src, gy, gx, N, 4 * C, H, W, s);
+    });
     // ff.net.0.proj
     Act Gn = tmp("tf_Gn", C, H, W);
     dgrad(t + ".ff.net.0.proj.weight", whole(Gff1), Gn, 1);
@@ -390,38 +362,30 @@ struct BwdBuilder {
     dgrad(t + ".attn1.to_out.0.weight", whole(Gh2), Gao, 1);
     wgrad_conv(whole(Gh2), whole(ao), t + ".attn1.to_out.0.weight", 1);
     bias_grad(whole(Gh2), t + ".attn1.to_out.0.bias", t + ".attn2.to_out.0.bias");
-    {
-      BOp op{};
-      op.kind = BOp::XVECBWD;   // dvec[n] = per-sample channel sums of G(h2) (last_cs, made just above)
-      op.f0 = last_cs; op.f1 = P(t + ".attn2.to_v.weight"); op.f2 = P(t + ".attn2.to_out.0.weight");
-      op.o0 = PG(t + ".attn2.to_out.0.weight"); op.o1 = PG(t + ".attn2.to_v.weight");
-      op.o2 = (float*)mem.take((size_t)2 * N * C * sizeof(float));
-      op.C = C; op.a = k.cross;
-      bw->ops.push_back(op);
-    }
+    // dvec[n] = per-sample channel sums of G(h2) (last_cs, made just above)
+    emit(OP_XVEC_BWD, [h = h, dvec = last_cs, wv = P(t + ".attn2.to_v.weight"), wo = P(t + ".attn2.to_out.0.weight"),
+                       dwo = PG(t + ".attn2.to_out.0.weight"), dwv = PG(t + ".attn2.to_v.weight"),
+                       scratch = (float*)mem.take((size_t)2 * N * C * sizeof(float)), N = N, C,
+                       X = k.cross](const RunArgs&, cudaStream_t s) {
+      return launch_cross_attn_vec_bwd(h->enc, dvec, wv, wo, dwo, dwv, scratch, N, C, X, s);
+    }, 2);
     // attention core (P recomputed from the forward's row log-sum-exp)
     Act Gqkv = tmp("tf_Gqkv", 3 * C, H, W);
-    {
-      BOp op{};
-      op.kind = BOp::MHABWD;
-      op.src = qkv.p; op.src2 = Gao.p; op.src3 = ao.p; op.dst = Gqkv.p;
-      op.f0 = h->plan.lse.at(n);
-      op.o2 = (float*)mem.take((size_t)N * heads * H * W * sizeof(float));
-      op.C = C; op.H = H; op.W = W; op.a = heads;
-      bw->ops.push_back(op);
-    }
+    emit(OP_MHA_BWD, [q = qkv.p, o = ao.p, go = Gao.p, lse = h->plan.lse.at(n),
+                      dsum = (float*)mem.take((size_t)N * heads * H * W * sizeof(float)), gq = Gqkv.p, N = N, C,
+                      heads = heads, H, W](const RunArgs&, cudaStream_t s) {
+      return launch_mha_bwd(q, o, go, lse, dsum, gq, N, C, heads, H, W, s);
+    }, 3);
     // q / k / v projections (no bias); g(n1) = sum over q, k, v of W^T g: one launch, three K-segments
     const char* names[3] = {"to_q", "to_k", "to_v"};
     for (int j = 0; j < 3; ++j) wgrad_conv(view(Gqkv, j * C, C), whole(n1), t + ".attn1." + names[j] + ".weight", 1);
     {
-      BOp op{};
-      op.kind = BOp::CONV;
-      conv_base(op.conv, Gn);
+      ConvParams p = conv_geom(N, Gn);
       const TapSet ts = taps_mirrored(1);
       for (int j = 0; j < 3; ++j)
-        seg(op.conv.seg[j], view(Gqkv, j * C, C), tjob(t + ".attn1." + names[j] + ".weight", C, C, 1, ts), ts);
-      op.conv.nseg = 3;
-      bw->ops.push_back(op);
+        seg(p.seg[j], view(Gqkv, j * C, C), tjob(t + ".attn1." + names[j] + ".weight", C, C, 1, ts), ts);
+      p.nseg = 3;
+      conv(p);
     }
     // norm1 (+ residual) -> G(h0)
     Act Gh0 = tmp("tf_Gh0", C, H, W);
@@ -457,22 +421,18 @@ struct BwdBuilder {
     for (int a = 0; a < 2; ++a)
       for (int b = 0; b < 2; ++b) {
         const TapSet t = k.kind == BK_DOWN ? taps_scatter2(a, b) : taps_scatter2_asym(a, b);
-        BOp op{};
-        op.kind = BOp::CONV;
         Act lo = Gx;
         lo.H = Ho; lo.W = Wo;
-        conv_base(op.conv, lo);
-        op.conv.up2 = 1; op.conv.oy = a; op.conv.ox = b;
-        seg(op.conv.seg[0], whole(Gy), tjob(n + ".weight", C, C, 3, t), t);
-        op.conv.nseg = 1;
-        bw->ops.push_back(op);
+        ConvParams p = conv_geom(N, lo);
+        p.up2 = 1; p.oy = a; p.ox = b;
+        seg(p.seg[0], whole(Gy), tjob(n + ".weight", C, C, 3, t), t);
+        p.nseg = 1;
+        conv(p);
       }
-    if (skipgrad.count(xn)) {
-      BOp op{};
-      op.kind = BOp::PF8ADD;
-      op.dst = Gx.p; op.src = skip_of(xn); op.C = C; op.H = x.H; op.W = x.W;
-      bw->ops.push_back(op);
-    }
+    if (skipgrad.count(xn))
+      emit(OP_PF8ADD, [gx = Gx.p, add = skip_of(xn), N = N, C, H = x.H, W = x.W](const RunArgs&, cudaStream_t s) {
+        return launch_pf8_add(gx, add, N, C, H, W, s);
+      });
   }
 
   // Upsample2D folded into four 2x2 convs (forward taps_up2): x (low) -> y (2x)
@@ -484,23 +444,13 @@ struct BwdBuilder {
     const Geom gl = make_geom(N, H, W);
     const size_t tsz = (size_t)N * (C / 8) * gl.PL * 8;
     Act gpar = tmp("gpar", 4 * C, H, W);          // parity planes of the gradient, 4 tensors back to back
-    {
-      BOp op{};
-      op.kind = BOp::PARITY;
-      op.src = Gy.p; op.dst = gpar.p; op.C = C; op.H = y.H; op.W = y.W;
-      bw->ops.push_back(op);
-    }
+    emit(OP_PARITY, [gy = Gy.p, gpar = gpar.p, N = N, C, H = y.H, W = y.W](const RunArgs&, cudaStream_t s) {
+      return launch_parity_split(gy, gpar, N, C, H, W, s);
+    });
     float* dwf = (float*)mem.take((size_t)4 * C * C * 4 * sizeof(float));
-    {
-      BOp op{};
-      op.kind = BOp::MEMSET;
-      op.o0 = dwf; op.n = (long long)4 * C * C * 4 * sizeof(float);
-      bw->ops.push_back(op);
-    }
-    BOp dg{};
-    dg.kind = BOp::CONV;
+    zero(dwf, (size_t)4 * C * C * 4 * sizeof(float));
     Act Gx = G(xn);
-    conv_base(dg.conv, Gx);
+    ConvParams dg = conv_geom(N, Gx);
     UnfoldMasks um{};
     for (int oy = 0; oy < 2; ++oy)
       for (int ox = 0; ox < 2; ++ox) {
@@ -511,40 +461,23 @@ struct BwdBuilder {
         plane.p = gpar.p ? gpar.p + (size_t)pidx * tsz : nullptr;
         wgrad(whole(plane), whole(x), dwf ? dwf + (size_t)pidx * C * C * 4 : nullptr, C, 0, 4, fwd_taps);
         for (int t = 0; t < 4; ++t) um.mask[pidx][t] = fwd_taps.pack.fold_mask[t];
-        seg(dg.conv.seg[pidx], whole(plane), tjob(n + ".weight", C, C, 3, bwd_taps), bwd_taps);
+        seg(dg.seg[pidx], whole(plane), tjob(n + ".weight", C, C, 3, bwd_taps), bwd_taps);
       }
-    dg.conv.nseg = 4;
-    {
-      BOp op{};
-      op.kind = BOp::UNFOLD;
-      op.f0 = dwf; op.o0 = PG(n + ".weight"); op.n = (long long)C * C; op.um = um;
-      bw->ops.push_back(op);
-    }
-    bw->ops.push_back(dg);
+    dg.nseg = 4;
+    emit(OP_UNFOLD, [dwf, dw = PG(n + ".weight"), nco_ci = (long long)C * C, um](const RunArgs&, cudaStream_t s) {
+      return launch_unfold_up2(dwf, dw, nco_ci, um, s);
+    });
+    conv(dg);
   }
 
   // conv_norm_out + SiLU + conv_out (C -> 1) on the last activation `in`, from the output gradient passed to backward()
   void conv_out_bwd(const Block& k, const std::string& in, float* wflip, const float* zbias) {
     const Act x = fwd(in);
-    const int C = x.C;
     Act A = gn_apply("A", x, nullptr, k.name + "conv_norm_out", true);
-    BOp w{};
-    w.kind = BOp::SCALAR_WGRAD;
-    w.src = A.p; w.x_is_geps = true; w.o0 = PG(k.name + "conv_out.weight"); w.C = C; w.H = x.H; w.W = x.W; w.a = 1;
-    bw->ops.push_back(w);
-    BOp sb{};
-    sb.kind = BOp::SUMADD;
-    sb.x_is_geps = true; sb.n = (long long)N * x.H * x.W; sb.o0 = PG(k.name + "conv_out.bias");
-    bw->ops.push_back(sb);
-    BOp f{};
-    f.kind = BOp::FLIP;
-    f.f0 = P(k.name + "conv_out.weight"); f.o0 = wflip; f.C = C;
-    bw->ops.push_back(f);
-    Act T1 = tmp("T1", C, x.H, x.W);
-    BOp ci{};
-    ci.kind = BOp::CONVIN;        // conv_in kernel: g_a[c] = sum_t g_eps[p + s_t] * wflip[c][t]
-    ci.x_is_geps = true; ci.f0 = wflip; ci.f1 = zbias; ci.dst = T1.p; ci.C = C; ci.H = x.H; ci.W = x.W;
-    bw->ops.push_back(ci);
+    scalar_wgrad(A, nullptr, false, PG(k.name + "conv_out.weight"), 1);
+    sum_add(nullptr, (long long)N * x.H * x.W, PG(k.name + "conv_out.bias"));
+    Act T1 = tmp("T1", x.C, x.H, x.W);
+    conv_out_dgrad(k.name + "conv_out.weight", nullptr, 1, wflip, zbias, T1);
     gn_bwd(T1, x, nullptr, k.name + "conv_norm_out", true, G(in), nullptr, nullptr, nullptr);
   }
 };
@@ -552,7 +485,7 @@ struct BwdBuilder {
 static int build_backward(b200ad_unet* h, Backward* bw, uint8_t* arena, float* grads, size_t* bytes_out) {
   const b200ad_unet_config& c = h->cfg;
   if (!h->training || h->plan.lists.empty()) return set_err("backward needs set_training(1) before bind_workspace");
-  bw->ops.clear();
+  bw->list.ops.clear();
   bw->jobs.clear();
   bw->arena = arena;
   bw->grads = grads;
@@ -560,6 +493,7 @@ static int build_backward(b200ad_unet* h, Backward* bw, uint8_t* arena, float* g
   B.h = h; B.bw = bw; B.N = h->N;
   B.heads = c.attention_head_dim;
   B.mem.base = arena;
+  B.pack_op();
   int maxC = c.block_out_channels[0];
   for (const auto& kv : h->plan.taps) maxC = kv.second.C > maxC ? kv.second.C : maxC;
   const int D = c.block_out_channels[0] * 4;
@@ -568,17 +502,30 @@ static int build_backward(b200ad_unet* h, Backward* bw, uint8_t* arena, float* g
   B.gproj = (float*)B.mem.take((size_t)h->N * h->temb_rows * sizeof(float));
   B.csum_floats = (size_t)h->N * 65536;       // all GroupNorm-backward outputs of the reference architecture: 16 K channels
   B.csum_arena = (float*)B.mem.take(B.csum_floats * sizeof(float));
-  {
-    BOp z{};
-    z.kind = BOp::MEMSET;
-    z.o0 = B.csum_arena; z.n = (long long)(B.csum_floats * sizeof(float));
-    bw->ops.push_back(z);
-  }
+  B.zero(B.csum_arena, B.csum_floats * sizeof(float));
   float* g_act = (float*)B.mem.take((size_t)h->N * D * sizeof(float));   // gradient w.r.t. silu(linear_2)
   float* g_h1 = (float*)B.mem.take((size_t)h->N * D * sizeof(float));
   float* h1v = (float*)B.mem.take((size_t)h->N * D * sizeof(float));
   float* wflip = (float*)B.mem.take((size_t)c.block_out_channels[0] * 9 * sizeof(float));
   const float* zbias = (const float*)B.mem.take((size_t)c.block_out_channels[0] * sizeof(float));   // never written: zeros
+
+  // linear layers of the timestep embedding: dW, db from the output gradient g (row stride gs) and the input x;
+  // gin = g W; u: SiLU pre-activation
+  const int N = h->N;
+  auto lin_w = [&](const float* g, int gs, const float* x, int O, int I, const std::string& name) {
+    B.emit(OP_LIN_W, [g, gs, x, O, I, dw = B.PG(name + ".weight"), db = B.PG(name + ".bias"), N](const RunArgs&,
+                                                                                                 cudaStream_t s) {
+      return launch_lin_bwd_weight(g, gs, x, O, I, dw, db, N, s);
+    });
+  };
+  auto lin_in = [&](const float* g, int gs, const float* w, int O, int I, float* gin) {
+    B.emit(OP_LIN_IN, [g, gs, w, O, I, gin, N](const RunArgs&, cudaStream_t s) {
+      return launch_lin_bwd_input(g, gs, w, O, I, gin, N, 0, s);
+    });
+  };
+  auto silu_bwd = [&](float* g, const float* u) {
+    B.emit(OP_SILU_BWD, [g, u, n = N * D](const RunArgs&, cudaStream_t s) { return launch_silu_bwd(g, u, n, s); });
+  };
 
   // the forward's blocks in reverse; a block's output is the forward tap of its name (the head's: conv_in)
   const std::vector<Block>& bl = h->blocks;
@@ -587,15 +534,11 @@ static int build_backward(b200ad_unet* h, Backward* bw, uint8_t* arena, float* g
     const Block& k = bl[i];
     const std::string in = tap(k.in);
     switch (k.kind) {
-      case BK_CONV_OUT: {    // g_eps -> gradient of the last activation
+      case BK_CONV_OUT:      // g_eps -> gradient of the last activation
         if (c.out_channels != 1) return set_err("backward: out_channels != 1 is not implemented");
         B.conv_out_bwd(k, in, wflip, zbias);
-        BOp z{};
-        z.kind = BOp::MEMSET;
-        z.o0 = B.gproj; z.n = (long long)h->N * h->temb_rows * sizeof(float);
-        bw->ops.push_back(z);
+        B.zero(B.gproj, (size_t)h->N * h->temb_rows * sizeof(float));
         break;
-      }
       case BK_RESNET: B.resnet_bwd(k, in, tap(k.skip)); break;
       case BK_ATTN: B.attention_bwd(k.name, in); break;
       case BK_TRANSFORMER: B.transformer_bwd(k, in); break;
@@ -604,55 +547,24 @@ static int build_backward(b200ad_unet* h, Backward* bw, uint8_t* arena, float* g
       case BK_UNET_HEAD: {   // conv_in, then the timestep embedding MLP and the per-resnet projections
         if (c.in_channels != 1) return set_err("backward: in_channels != 1 is not implemented");
         const std::string n = tap(i);
-        const Act x = B.fwd(n);
         const Act Gx = B.G(n);
         if (!B.skipgrad.count(n)) return set_err("backward: conv_in skip gradient missing");
         // (the first resnet's GroupNorm backward already added the skip contribution)
-        BOp w{};
-        w.kind = BOp::SCALAR_WGRAD;
-        w.src = Gx.p; w.x_is_input = true; w.o0 = B.PG(n + ".weight"); w.C = x.C; w.H = x.H; w.W = x.W; w.a = 0;
-        bw->ops.push_back(w);
+        B.scalar_wgrad(Gx, nullptr, true, B.PG(n + ".weight"), 0);
         B.bias_grad(BwdBuilder::whole(Gx), n + ".bias");
         const Plan& pl = h->plan;
-        for (const Block& r : bl) {     // time_emb_proj of every resnet: dW = g_proj_rows^T temb_act
-          if (r.temb_row < 0) continue;
-          BOp op{};
-          op.kind = BOp::LIN_W;
-          op.f0 = B.gproj + r.temb_row; op.a = h->temb_rows; op.f1 = pl.temb_act; op.b = r.cout; op.c = D;
-          op.o0 = B.PG(r.name + ".time_emb_proj.weight"); op.o1 = B.PG(r.name + ".time_emb_proj.bias");
-          bw->ops.push_back(op);
-        }
-        BOp gi{};
-        gi.kind = BOp::LIN_IN;   // g(temb_act) = g_proj Wcat
-        gi.f0 = B.gproj; gi.a = h->temb_rows; gi.f1 = h->packed ? (const float*)(h->packed + h->off_wcat) : nullptr;
-        gi.b = h->temb_rows; gi.c = D; gi.o0 = g_act;
-        bw->ops.push_back(gi);
-        BOp s2{};
-        s2.kind = BOp::SILU_BWD;
-        s2.o0 = g_act; s2.f0 = pl.temb_u2; s2.n = (long long)h->N * D;
-        bw->ops.push_back(s2);
-        BOp hf{};
-        hf.kind = BOp::SILU_FWD;
-        hf.f0 = pl.temb_u1; hf.o0 = h1v; hf.n = (long long)h->N * D;
-        bw->ops.push_back(hf);
-        BOp w2{};
-        w2.kind = BOp::LIN_W;
-        w2.f0 = g_act; w2.a = D; w2.f1 = h1v; w2.b = D; w2.c = D;
-        w2.o0 = B.PG("time_embedding.linear_2.weight"); w2.o1 = B.PG("time_embedding.linear_2.bias");
-        bw->ops.push_back(w2);
-        BOp g1{};
-        g1.kind = BOp::LIN_IN;
-        g1.f0 = g_act; g1.a = D; g1.f1 = B.P("time_embedding.linear_2.weight"); g1.b = D; g1.c = D; g1.o0 = g_h1;
-        bw->ops.push_back(g1);
-        BOp s1{};
-        s1.kind = BOp::SILU_BWD;
-        s1.o0 = g_h1; s1.f0 = pl.temb_u1; s1.n = (long long)h->N * D;
-        bw->ops.push_back(s1);
-        BOp w1{};
-        w1.kind = BOp::LIN_W;
-        w1.f0 = g_h1; w1.a = D; w1.f1 = pl.temb_emb; w1.b = D; w1.c = k.cout;
-        w1.o0 = B.PG("time_embedding.linear_1.weight"); w1.o1 = B.PG("time_embedding.linear_1.bias");
-        bw->ops.push_back(w1);
+        for (const Block& r : bl)        // time_emb_proj of every resnet: dW = g_proj_rows^T temb_act
+          if (r.temb_row >= 0) lin_w(B.gproj + r.temb_row, h->temb_rows, pl.temb_act, r.cout, D, r.name + ".time_emb_proj");
+        // g(temb_act) = g_proj Wcat
+        lin_in(B.gproj, h->temb_rows, h->packed ? (const float*)(h->packed + h->off_wcat) : nullptr, h->temb_rows, D, g_act);
+        silu_bwd(g_act, pl.temb_u2);
+        B.emit(OP_SILU_FWD, [u = pl.temb_u1, h1v, n = N * D](const RunArgs&, cudaStream_t s) {
+          return launch_silu_fwd(u, h1v, n, s);
+        });
+        lin_w(g_act, D, h1v, D, D, "time_embedding.linear_2");
+        lin_in(g_act, D, B.P("time_embedding.linear_2.weight"), D, D, g_h1);
+        silu_bwd(g_h1, pl.temb_u1);
+        lin_w(g_h1, D, pl.temb_emb, D, k.cout, "time_embedding.linear_1");
         break;
       }
       default: return set_err("backward: block %s has no backward", k.name.c_str());
@@ -662,13 +574,50 @@ static int build_backward(b200ad_unet* h, Backward* bw, uint8_t* arena, float* g
   return 0;
 }
 
-}  // namespace b200ad
+// The size pass (null arena) must plan the ops the bound pass plans, or the arena size it found may be wrong.
+static int check_same_plan(const Backward& sized, Backward* bound) {
+  bool same = sized.list.ops.size() == bound->list.ops.size();
+  for (size_t i = 0; same && i < sized.list.ops.size(); ++i) same = sized.list.ops[i].kind == bound->list.ops[i].kind;
+  if (same) return 0;
+  bound->list.ops.clear();
+  return set_err("bind_backward: the size pass and the bound pass planned different ops");
+}
 
-namespace b200ad {
+// Runs a bound backward plan: zeroes its gradient slots (unless accumulating), then its ops.
+static int run_backward(NetBase* h, Backward* bw, const RunArgs& a, int accumulate, cudaStream_t st) {
+  // B200AD_BWD_PROFILE=1: CUDA events around every op, per-kind totals printed to stderr (tools/train_bench.py)
+  static const bool prof = [] { const char* e = getenv("B200AD_BWD_PROFILE"); return e && e[0] == '1'; }();
+  if (!accumulate) CK(cudaMemsetAsync(bw->grads + bw->zero_off, 0, bw->zero_floats * sizeof(float), st));   // every kernel below ADDS
+  OpEvents ev;
+  if (run_ops(h, bw->list, a, st, &bw->launches, prof ? &ev : nullptr)) return -1;
+  if (prof) {
+    CK(cudaStreamSynchronize(st));
+    double tot[OP_NKINDS] = {0};
+    int cnt[OP_NKINDS] = {0};
+    for (size_t i = 0; i < bw->list.ops.size(); ++i) {
+      float ms = 0.f;
+      if (ev.ms(i, &ms)) return -1;
+      tot[bw->list.ops[i].kind] += ms;
+      cnt[bw->list.ops[i].kind]++;
+    }
+    fprintf(stderr, "{\"backward_profile_ms\": {");
+    const char* sep = "";
+    for (int k = 0; k < OP_NKINDS; ++k) {
+      if (!cnt[k]) continue;
+      if (k == OP_PACK_T) fprintf(stderr, "%s\"%s\": %.3f", sep, op_names[k], tot[k]);   // one per plan
+      else fprintf(stderr, "%s\"%s x%d\": %.3f", sep, op_names[k], cnt[k], tot[k]);
+      sep = ", ";
+    }
+    fprintf(stderr, "}}\n");
+  }
+  return 0;
+}
+
 void release_backward(b200ad_unet* h) {
   delete h->bwd;
   h->bwd = nullptr;
 }
+
 }  // namespace b200ad
 
 // ================================================================================= C ABI
@@ -711,131 +660,23 @@ extern "C" size_t b200ad_unet_backward_bytes(b200ad_unet* h) {
 extern "C" int b200ad_unet_bind_backward(b200ad_unet* h, void* arena, size_t bytes, float* grads, void* stream) {
   ensure_bwd(h);
   size_t need = 0;
-  {
-    Backward tmp;
-    tmp.goff = h->bwd->goff;
-    if (build_backward(h, &tmp, nullptr, nullptr, &need)) return -1;
-  }
+  Backward sized;
+  sized.goff = h->bwd->goff;
+  if (build_backward(h, &sized, nullptr, nullptr, &need)) return -1;
   if (bytes < need) return set_err("backward arena too small: %zu < %zu", bytes, need);
   CK(cudaMemsetAsync(arena, 0, need, (cudaStream_t)stream));
-  if (build_backward(h, h->bwd, (uint8_t*)arena, grads, &need)) return -1;
+  if (build_backward(h, h->bwd, (uint8_t*)arena, grads, &need) || check_same_plan(sized, h->bwd)) return -1;
   h->bwd->arena_bytes = need;
   return 0;
 }
 
-// Runs a bound backward plan.
-static int run_backward(NetBase* h, Backward* bw, const BwdArgs& a, int accumulate, cudaStream_t st) {
-  const int N = h->N;
-  const float* x = a.x;
-  const float* g_eps = a.g_eps;
-  int launches = 0;
-  // B200AD_BWD_PROFILE=1: CUDA events around every op, per-kind totals printed to stderr (tools/train_bench.py)
-  static const bool prof = [] { const char* e = getenv("B200AD_BWD_PROFILE"); return e && e[0] == '1'; }();
-  std::vector<cudaEvent_t> ev;
-  if (prof) {
-    ev.resize(bw->ops.size() + 2);
-    for (auto& e : ev) CK(cudaEventCreate(&e));
-    CK(cudaEventRecord(ev[0], st));
-  }
-  if (!accumulate) CK(cudaMemsetAsync(bw->grads + bw->zero_off, 0, bw->zero_floats * sizeof(float), st));   // every kernel below ADDS
-  {
-    std::vector<PackItem> items;
-    items.reserve(bw->jobs.size());
-    for (const PackJob& j : bw->jobs) items.push_back(make_pack_item(h, j, bw->arena));
-    CK(launch_pack_batch(bw->pack_batch, items, st));
-  }
-  launches += 1;
-  if (prof) CK(cudaEventRecord(ev[1], st));
-  size_t opi = 0;
-  for (BOp& op : bw->ops) {
-    switch (op.kind) {
-      case BOp::CONV: CK(launch_conv_tc(op.conv, h->num_sms, st)); break;
-      case BOp::WGRAD: CK(launch_wgrad_tc(op.wg, h->num_sms, st)); break;
-      case BOp::GNBWD: CK(launch_gn_bwd(op.gb, st)); launches += 1; break;
-      case BOp::GNAPPLY: CK(launch_gn_apply(op.ga, st)); break;
-      case BOp::CHANSUM:
-        CK(launch_chan_sum(op.src, op.o0, N, op.C, op.a, op.H, op.W, st, op.o1, const_cast<float*>(op.f1)));
-        break;
-      case BOp::REDUCE_N: CK(launch_reduce_n_add(op.f0, op.o0, op.o1, N, op.C, st)); break;
-      case BOp::SCATTER: CK(launch_scatter_rows(op.f0, op.o0, N, op.C, op.a, op.b, st)); break;
-      case BOp::PF8ADD: CK(launch_pf8_add(op.dst, op.src, N, op.C, op.H, op.W, st)); break;
-      case BOp::ATTNBWD: CK(launch_attention_bwd(op.src, op.src2, op.dst, N, op.C, op.H, op.W, st)); break;
-      case BOp::PARITY: CK(launch_parity_split(op.src, op.dst, N, op.C, op.H, op.W, st)); break;
-      case BOp::UNFOLD: CK(launch_unfold_up2(op.f0, op.o0, op.n, op.um, st)); break;
-      case BOp::SCALAR_WGRAD:     // X: f0, or an input of the call
-        CK(launch_scalar_conv_wgrad(op.src, op.f0 ? op.f0 : op.x_is_geps ? g_eps : x, op.o0, N, op.C, op.H, op.W, op.a, st));
-        break;
-      case BOp::CONVIN:           // source: f2 (c channels), or the output gradient (1 channel)
-        CK(launch_conv_in(op.f2 ? op.f2 : g_eps, op.f0, op.f1, N, op.c ? op.c : 1, op.H, op.W, op.C, op.dst, nullptr, st));
-        break;
-      case BOp::FLIP: CK(launch_flip_taps(op.f0, op.o0, op.C, st, op.a ? op.a : 1)); break;
-      case BOp::SUMADD: CK(launch_sum_add(op.f0 ? op.f0 : g_eps, op.n, op.o0, st)); break;
-      case BOp::LIN_IN: CK(launch_lin_bwd_input(op.f0, op.a, op.f1, op.b, op.c, op.o0, N, 0, st)); break;
-      case BOp::LIN_W: CK(launch_lin_bwd_weight(op.f0, op.a, op.f1, op.b, op.c, op.o0, op.o1, N, st)); break;
-      case BOp::SILU_BWD: CK(launch_silu_bwd(op.o0, op.f0, (int)op.n, st)); break;
-      case BOp::SILU_FWD: CK(launch_silu_fwd(op.f0, op.o0, (int)op.n, st)); break;
-      case BOp::MEMSET: CK(cudaMemsetAsync(op.o0, 0, (size_t)op.n, st)); break;
-      case BOp::LNBWD:
-        CK(launch_layernorm_bwd_pf8(op.src, op.src2, op.src3, op.dst, op.f0, op.o0, op.o1, N, op.C, op.H, op.W, 1e-5f, st));
-        break;
-      case BOp::GEGLUBWD: CK(launch_geglu_bwd_pf8(op.src, op.src2, op.dst, N, op.C, op.H, op.W, st)); break;
-      case BOp::XVECBWD:
-        if (!h->enc || h->enc_S != 1) return set_err("backward: the conditional U-Net needs the forward's encoding (S = 1) bound");
-        CK(launch_cross_attn_vec_bwd(h->enc, op.f0, op.f1, op.f2, op.o0, op.o1, op.o2, N, op.C, op.a, st));
-        launches += 1;
-        break;
-      case BOp::MHABWD:
-        CK(launch_mha_bwd(op.src, op.src3, op.src2, op.f0, op.o2, op.dst, N, op.C, op.a, op.H, op.W, st));
-        launches += 2;
-        break;
-      case BOp::ATTN1BWD:   // row dot products, then the dS, dV, dQ, dK GEMMs
-        CK(launch_attention_1head_bwd(op.src, op.src3, op.src2, op.f0, op.o2, op.dst2, op.dst, N, op.C, op.H, op.W, st));
-        launches += 4;
-        break;
-      case BOp::QUANTBWD:
-        CK(launch_quant_conv_bwd(a.g_mom, op.src, op.f0, op.o2, op.o2 + (size_t)N * op.c * op.H * op.W, op.o0, op.o1, N,
-                                 op.c, op.H, op.W, st));
-        break;
-      case BOp::LATENTINBWD:
-        CK(launch_latent_in_bwd(op.src, op.f0, op.f1, op.f2, a.g_z, op.o0, op.o1, N, op.C, op.c, op.H, op.W, st));
-        break;
-      case BOp::NKINDS: break;
-    }
-    ++launches;
-    if (prof) CK(cudaEventRecord(ev[2 + opi], st));
-    ++opi;
-  }
-  bw->launches = launches;
-  if (prof) {
-    static const char* names[BOp::NKINDS] = {
-        "conv_tc(dgrad)", "wgrad_tc", "gn_bwd", "gn_apply", "chan_sum", "reduce_n", "scatter", "pf8_add", "attention_bwd",
-        "parity_split", "unfold_up2", "scalar_wgrad", "conv_in(dgrad)", "flip", "sum_add", "lin_in", "lin_w", "silu_bwd",
-        "silu_fwd", "memset", "layernorm_bwd", "geglu_bwd", "cross_attn_vec_bwd", "mha_bwd", "attention_1head_bwd",
-        "quant_conv_bwd", "latent_in_bwd"};
-    CK(cudaStreamSynchronize(st));
-    double tot[BOp::NKINDS] = {0};
-    int cnt[BOp::NKINDS] = {0};
-    float ms = 0.f;
-    CK(cudaEventElapsedTime(&ms, ev[0], ev[1]));
-    fprintf(stderr, "{\"backward_profile_ms\": {\"pack_transposed\": %.3f", ms);
-    for (size_t i = 0; i < bw->ops.size(); ++i) {
-      CK(cudaEventElapsedTime(&ms, ev[1 + i], ev[2 + i]));
-      tot[bw->ops[i].kind] += ms;
-      cnt[bw->ops[i].kind]++;
-    }
-    for (int k = 0; k < BOp::NKINDS; ++k)
-      if (cnt[k]) fprintf(stderr, ", \"%s x%d\": %.3f", names[k], cnt[k], tot[k]);
-    fprintf(stderr, "}}\n");
-    for (auto& e : ev) cudaEventDestroy(e);
-  }
-  return 0;
-}
-
 extern "C" int b200ad_unet_backward(b200ad_unet* h, const float* x, const float* g_eps, int accumulate, void* stream) {
-  if (!h || !h->bwd || h->bwd->ops.empty()) return set_err("bind_backward must be called before backward");
+  if (!h || !h->bwd || h->bwd->list.ops.empty()) return set_err("bind_backward must be called before backward");
   if (!x || !g_eps) return set_err("backward: x and g_eps are required");
-  BwdArgs a;
-  a.x = x; a.g_eps = g_eps;
+  if (h->cfg.cross_attention_dim && (!h->enc || h->enc_S != 1))
+    return set_err("backward: the conditional U-Net needs the forward's encoding (S = 1) bound");
+  RunArgs a;
+  a.in = x; a.g_eps = g_eps;
   return run_backward(h, h->bwd, a, accumulate, (cudaStream_t)stream);
 }
 
@@ -870,17 +711,15 @@ static int build_vae_backward(b200ad_vae* h, Backward* const* bws, uint8_t* aren
   const Plan& pl = h->plan;
   for (int part : {DEC, ENC}) {
     Backward* bw = bws[part];
-    bw->ops.clear();
+    bw->list.ops.clear();
     bw->jobs.clear();
     bw->arena = arena;
     bw->grads = grads;
     B.bw = bw;
     B.grad.clear(); B.skipgrad.clear(); B.csum_of.clear();
     B.csum_used = 0;
-    BOp z{};
-    z.kind = BOp::MEMSET;
-    z.o0 = B.csum_arena; z.n = (long long)(B.csum_floats * sizeof(float));
-    bw->ops.push_back(z);
+    B.pack_op();
+    B.zero(B.csum_arena, B.csum_floats * sizeof(float));
     const std::vector<Block>& bl = part == ENC ? h->enc : h->dec;
     auto tap = [&](int i) {
       return i < 0 ? std::string() : (bl[i].kind == BK_CONV_IN || bl[i].kind == BK_LATENT_IN) ? bl[i].name + "conv_in" : bl[i].name;
@@ -895,34 +734,20 @@ static int build_vae_backward(b200ad_vae* h, Backward* const* bws, uint8_t* aren
           const int C = x.C, H = x.H, W = x.W;
           const size_t plane = (size_t)h->N * H * W;
           float* gh_cn = gh ? gh + L2 * plane : nullptr;
-          BOp q{};
-          q.kind = BOp::QUANTBWD;
-          q.src = eo.p; q.f0 = B.P("quant_conv.weight"); q.o0 = B.PG("quant_conv.weight"); q.o1 = B.PG("quant_conv.bias");
-          q.o2 = gh; q.c = L2; q.H = H; q.W = W;
-          bw->ops.push_back(q);
+          B.emit(OP_QUANT_BWD, [eo = eo.p, w = B.P("quant_conv.weight"), gh, gh_cn, dw = B.PG("quant_conv.weight"),
+                                db = B.PG("quant_conv.bias"), N = h->N, L2, H, W](const RunArgs& a, cudaStream_t s) {
+            return launch_quant_conv_bwd(a.g_mom, eo, w, gh, gh_cn, dw, db, N, L2, H, W, s);
+          });
           Act A = B.gn_apply("A", x, nullptr, k.name + "conv_norm_out", true);
           float* dw = B.PG(k.name + "conv_out.weight");
           float* db = B.PG(k.name + "conv_out.bias");
           for (int o = 0; o < L2; ++o) {
-            BOp w{};
-            w.kind = BOp::SCALAR_WGRAD;
-            w.src = A.p; w.f0 = gh_cn ? gh_cn + o * plane : nullptr; w.o0 = dw ? dw + (size_t)o * C * 9 : nullptr;
-            w.C = C; w.H = H; w.W = W; w.a = 1;
-            bw->ops.push_back(w);
-            BOp sb{};
-            sb.kind = BOp::SUMADD;
-            sb.f0 = w.f0; sb.n = (long long)plane; sb.o0 = db ? db + o : nullptr;
-            bw->ops.push_back(sb);
+            const float* g = gh_cn ? gh_cn + o * plane : nullptr;
+            B.scalar_wgrad(A, g, false, dw ? dw + (size_t)o * C * 9 : nullptr, 1);
+            B.sum_add(g, (long long)plane, db ? db + o : nullptr);
           }
-          BOp fl{};
-          fl.kind = BOp::FLIP;
-          fl.f0 = B.P(k.name + "conv_out.weight"); fl.o0 = wflip; fl.C = C; fl.a = L2;
-          bw->ops.push_back(fl);
           Act T1 = B.tmp("T1", C, H, W);
-          BOp ci{};
-          ci.kind = BOp::CONVIN;        // g_a[c] = sum_o sum_t g_h[o][p + s_t] * wflip[c][o][t]
-          ci.f2 = gh; ci.c = L2; ci.f0 = wflip; ci.f1 = zbias; ci.dst = T1.p; ci.C = C; ci.H = H; ci.W = W;
-          bw->ops.push_back(ci);
+          B.conv_out_dgrad(k.name + "conv_out.weight", gh, L2, wflip, zbias, T1);
           B.gn_bwd(T1, x, nullptr, k.name + "conv_norm_out", true, B.G(in), nullptr, nullptr, nullptr);
           break;
         }
@@ -935,21 +760,14 @@ static int build_vae_backward(b200ad_vae* h, Backward* const* bws, uint8_t* aren
           const std::string n = tap(i);
           const Act x = B.fwd(n);
           const Act Gx = B.G(n);
-          BOp w{};
-          w.kind = BOp::SCALAR_WGRAD;
-          w.src = Gx.p; w.o0 = B.PG(n + ".weight"); w.C = x.C; w.H = x.H; w.W = x.W; w.a = 0;
-          if (k.kind == BK_CONV_IN) w.x_is_input = true;
-          else w.f0 = pl.zq;
-          bw->ops.push_back(w);
+          B.scalar_wgrad(Gx, k.kind == BK_CONV_IN ? nullptr : pl.zq, true, B.PG(n + ".weight"), 0);
           B.bias_grad(BwdBuilder::whole(Gx), n + ".bias");
-          if (k.kind == BK_LATENT_IN) {
-            BOp li{};
-            li.kind = BOp::LATENTINBWD;
-            li.src = Gx.p; li.f0 = B.P(n + ".weight"); li.f1 = B.P("post_quant_conv.weight"); li.f2 = pl.z_in;
-            li.o0 = B.PG("post_quant_conv.weight"); li.o1 = B.PG("post_quant_conv.bias");
-            li.C = x.C; li.c = k.cin; li.H = x.H; li.W = x.W;
-            bw->ops.push_back(li);
-          }
+          if (k.kind == BK_LATENT_IN)
+            B.emit(OP_LATENT_IN_BWD, [gy = Gx.p, win = B.P(n + ".weight"), wpq = B.P("post_quant_conv.weight"), z = pl.z_in,
+                                      dw = B.PG("post_quant_conv.weight"), db = B.PG("post_quant_conv.bias"), N = h->N,
+                                      C = x.C, L = k.cin, H = x.H, W = x.W](const RunArgs& a, cudaStream_t s) {
+              return launch_latent_in_bwd(gy, win, wpq, z, a.g_z, dw, db, N, C, L, H, W, s);
+            });
           break;
         }
         default: return set_err("autoencoder backward: block %s has no backward", k.name.c_str());
@@ -1004,37 +822,43 @@ static void ensure_bwd(b200ad_vae* h) {
 extern "C" size_t b200ad_vae_grad_floats(b200ad_vae* h) { ensure_bwd(h); return h->bwd[0]->grad_floats; }
 extern "C" size_t b200ad_vae_grad_offset(b200ad_vae* h, int i) { ensure_bwd(h); return h->bwd[0]->goff[i]; }
 
-static size_t vae_backward_size(b200ad_vae* h) {
+// Builds both plans with a null arena into sized[ENC], sized[DEC]; returns the arena bytes (0: error).
+static size_t vae_backward_size(b200ad_vae* h, Backward* sized) {
   ensure_bwd(h);
-  Backward t0, t1;
-  t0.goff = t1.goff = h->bwd[0]->goff;
-  Backward* tb[2] = {&t0, &t1};
+  sized[0].goff = sized[1].goff = h->bwd[0]->goff;
+  Backward* tb[2] = {&sized[0], &sized[1]};
   size_t bytes = 0;
   if (build_vae_backward(h, tb, nullptr, nullptr, &bytes)) return 0;
   return bytes;
 }
 
-extern "C" size_t b200ad_vae_backward_bytes(b200ad_vae* h) { return vae_backward_size(h); }
+extern "C" size_t b200ad_vae_backward_bytes(b200ad_vae* h) {
+  Backward sized[2];
+  return vae_backward_size(h, sized);
+}
 
 extern "C" int b200ad_vae_bind_backward(b200ad_vae* h, void* arena, size_t bytes, float* grads, void* stream) {
-  const size_t need = vae_backward_size(h);
+  Backward sized[2];
+  const size_t need = vae_backward_size(h, sized);
   if (!need) return -1;
   if (bytes < need) return set_err("backward arena too small: %zu < %zu", bytes, need);
   CK(cudaMemsetAsync(arena, 0, need, (cudaStream_t)stream));
   size_t got = 0;
   if (build_vae_backward(h, h->bwd, (uint8_t*)arena, grads, &got)) return -1;
+  for (int part : {ENC, DEC})
+    if (check_same_plan(sized[part], h->bwd[part])) return -1;
   for (Backward* b : h->bwd) b->arena_bytes = got;
   return 0;
 }
 
-static int vae_backward(b200ad_vae* h, int part, const BwdArgs& a, int accumulate, cudaStream_t st) {
-  if (!h || !h->bwd[part] || h->bwd[part]->ops.empty()) return set_err("bind_backward must be called before backward");
+static int vae_backward(b200ad_vae* h, int part, const RunArgs& a, int accumulate, cudaStream_t st) {
+  if (!h || !h->bwd[part] || h->bwd[part]->list.ops.empty()) return set_err("bind_backward must be called before backward");
   return run_backward(h, h->bwd[part], a, accumulate, st);
 }
 
 extern "C" int b200ad_vae_decoder_backward(b200ad_vae* h, const float* g_x, float* g_z_out, int accumulate, void* stream) {
   if (!g_x || !g_z_out) return set_err("decoder_backward: g_x and g_z_out are required");
-  BwdArgs a;
+  RunArgs a;
   a.g_eps = g_x; a.g_z = g_z_out;
   return vae_backward(h, DEC, a, accumulate, (cudaStream_t)stream);
 }
@@ -1042,8 +866,8 @@ extern "C" int b200ad_vae_decoder_backward(b200ad_vae* h, const float* g_x, floa
 extern "C" int b200ad_vae_encoder_backward(b200ad_vae* h, const float* x, const float* g_moments, int accumulate,
                                            void* stream) {
   if (!x || !g_moments) return set_err("encoder_backward: x and g_moments are required");
-  BwdArgs a;
-  a.x = x; a.g_mom = g_moments;
+  RunArgs a;
+  a.in = x; a.g_mom = g_moments;
   return vae_backward(h, ENC, a, accumulate, (cudaStream_t)stream);
 }
 

@@ -152,7 +152,7 @@ extern "C" int b200ad_vae_encode(b200ad_vae* h, const float* x, const float* noi
   if (!x || !z) return set_err("x and z are required");
   RunArgs a;
   a.in = x; a.noise = noise; a.out = z; a.moments = moments;
-  return run_ops(h, h->plan.lists[ENC], a, (cudaStream_t)stream);
+  return run_ops(h, h->plan.lists[ENC], a, (cudaStream_t)stream, &h->last_launches);
 }
 
 extern "C" int b200ad_vae_decode(b200ad_vae* h, const float* z, float* x_out, void* stream) {
@@ -160,7 +160,7 @@ extern "C" int b200ad_vae_decode(b200ad_vae* h, const float* z, float* x_out, vo
   if (!z || !x_out) return set_err("z and x_out are required");
   RunArgs a;
   a.in = z; a.out = x_out;
-  return run_ops(h, h->plan.lists[DEC], a, (cudaStream_t)stream);
+  return run_ops(h, h->plan.lists[DEC], a, (cudaStream_t)stream, &h->last_launches);
 }
 
 extern "C" int b200ad_vae_last_launch_count(const b200ad_vae* h) { return h->last_launches; }
