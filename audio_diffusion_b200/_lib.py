@@ -79,6 +79,7 @@ SYMBOLS = {
     "b200ad_unet_bind_backward": (_I, [_VP, _VP, _SZ, _VP, _VP]),
     "b200ad_unet_backward": (_I, [_VP, _VP, _VP, _I, _VP]),
     "b200ad_unet_backward_launch_count": (_I, [_VP]),
+    "b200ad_unet_debug_grad": (_I, [_VP, C.c_char_p, _I, _VP, C.POINTER(_I), _VP]),
     "b200ad_vae_set_training": (_I, [_VP, _I]),
     "b200ad_vae_grad_floats": (_SZ, [_VP]),
     "b200ad_vae_grad_offset": (_SZ, [_VP, _I]),
@@ -87,6 +88,7 @@ SYMBOLS = {
     "b200ad_vae_decoder_backward": (_I, [_VP, _VP, _VP, _I, _VP]),
     "b200ad_vae_encoder_backward": (_I, [_VP, _VP, _VP, _I, _VP]),
     "b200ad_vae_backward_launch_count": (_I, [_VP]),
+    "b200ad_vae_debug_grad": (_I, [_VP, C.c_char_p, _I, _VP, C.POINTER(_I), _VP]),
     "b200ad_vae_create": (_I, [C.POINTER(VAEConfigC), C.POINTER(_VP)]),
     "b200ad_vae_destroy": (None, [_VP]),
     "b200ad_vae_num_params": (_I, [_VP]),

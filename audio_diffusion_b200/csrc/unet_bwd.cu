@@ -37,6 +37,9 @@ struct Backward {
   float* grads = nullptr;
   int launches = 0;
   PackBatch pack_batch;              // one launch for all transposed packs
+  // the builder's gradient tensors by forward tap name (arena tensors of their own, final once the plan has run):
+  // the whole gradient, and the share of it a skip connection brought (debug_grad)
+  std::map<std::string, Act> grad, skipgrad;
 };
 
 namespace b200ad {
@@ -570,8 +573,26 @@ static int build_backward(b200ad_unet* h, Backward* bw, uint8_t* arena, float* g
       default: return set_err("backward: block %s has no backward", k.name.c_str());
     }
   }
+  bw->grad = B.grad;
+  bw->skipgrad = B.skipgrad;
   if (bytes_out) *bytes_out = (B.mem.off + 255) & ~(size_t)255;
   return 0;
+}
+
+// fp32 NCHW copy of a gradient tensor of a bound backward plan (skip: the skip connection's share); as debug_tensor
+static int debug_grad(const NetBase* h, const Backward* const* bws, int nbw, const char* name, int skip, float* dst,
+                      int* dims, cudaStream_t st) {
+  for (int i = 0; i < nbw; ++i) {
+    if (!bws[i] || bws[i]->list.ops.empty()) return set_err("debug_grad: bind_backward must be called first");
+    const std::map<std::string, Act>& m = skip ? bws[i]->skipgrad : bws[i]->grad;
+    auto it = m.find(name);
+    if (it == m.end()) continue;
+    const Act& a = it->second;
+    if (dims) { dims[0] = a.C; dims[1] = a.H; dims[2] = a.W; }
+    if (dst) CK(launch_pf8_to_nchw(a.p, dst, h->N, a.C, a.H, a.W, st));
+    return a.C;
+  }
+  return set_err("debug_grad: no %sgradient for '%s'", skip ? "skip " : "", name);
 }
 
 // The size pass (null arena) must plan the ops the bound pass plans, or the arena size it found may be wrong.
@@ -682,6 +703,12 @@ extern "C" int b200ad_unet_backward(b200ad_unet* h, const float* x, const float*
 
 extern "C" int b200ad_unet_backward_launch_count(const b200ad_unet* h) { return h && h->bwd ? h->bwd->launches : 0; }
 
+extern "C" int b200ad_unet_debug_grad(b200ad_unet* h, const char* name, int skip, float* dst, int* dims, void* stream) {
+  if (!h || !name) return set_err("null argument");
+  const Backward* bws[1] = {h->bwd};
+  return debug_grad(h, bws, 1, name, skip, dst, dims, (cudaStream_t)stream);
+}
+
 // ================================================================================= autoencoder backward
 namespace b200ad {
 
@@ -773,6 +800,8 @@ static int build_vae_backward(b200ad_vae* h, Backward* const* bws, uint8_t* aren
         default: return set_err("autoencoder backward: block %s has no backward", k.name.c_str());
       }
     }
+    bw->grad = B.grad;         // the maps are cleared for the next part
+    bw->skipgrad = B.skipgrad;
   }
   if (bytes_out) *bytes_out = (B.mem.off + 255) & ~(size_t)255;
   return 0;
@@ -873,4 +902,10 @@ extern "C" int b200ad_vae_encoder_backward(b200ad_vae* h, const float* x, const 
 
 extern "C" int b200ad_vae_backward_launch_count(const b200ad_vae* h) {
   return h && h->bwd[0] ? h->bwd[0]->launches + h->bwd[1]->launches : 0;
+}
+
+extern "C" int b200ad_vae_debug_grad(b200ad_vae* h, const char* name, int skip, float* dst, int* dims, void* stream) {
+  if (!h || !name) return set_err("null argument");
+  const Backward* bws[2] = {h->bwd[DEC], h->bwd[ENC]};
+  return debug_grad(h, bws, 2, name, skip, dst, dims, (cudaStream_t)stream);
 }

@@ -427,6 +427,18 @@ class UNet2DModel(nn.Module):
         _lib.check(min(0, L.b200ad_unet_debug_tensor(self._h, name.encode(), out.data_ptr(), dims, _lib.stream_ptr())))
         return out
 
+    def debug_grad(self, name: str, skip: bool = False) -> torch.Tensor:
+        """fp32 NCHW copy of the last backward's gradient w.r.t. the activation `debug_tensor(name)` (skip=True: the share
+        of it that the skip connection brought) (per-block backward tests)."""
+        L = _lib.lib()
+        dims = (C.c_int * 3)()
+        _lib.check(min(0, L.b200ad_unet_debug_grad(self._h, name.encode(), int(skip), None, dims, _lib.stream_ptr())))
+        n = self._ws_key[0]
+        out = torch.empty((n, dims[0], dims[1], dims[2]), dtype=torch.float32, device=self.device)
+        _lib.check(min(0, L.b200ad_unet_debug_grad(self._h, name.encode(), int(skip), out.data_ptr(), dims,
+                                                   _lib.stream_ptr())))
+        return out
+
     @property
     def last_launch_count(self) -> int:
         return _lib.lib().b200ad_unet_last_launch_count(self._h)

@@ -553,6 +553,18 @@ class AutoencoderKL(nn.Module):
         _lib.check(min(0, L.b200ad_vae_debug_tensor(self._h, name.encode(), out.data_ptr(), dims, _lib.stream_ptr())))
         return out
 
+    def debug_grad(self, name: str, skip: bool = False) -> torch.Tensor:
+        """fp32 NCHW copy of the last decoder / encoder backward's gradient w.r.t. the activation `debug_tensor(name)`
+        (skip=True: the share of it a skip connection brought; the autoencoder has none) (per-block backward tests)."""
+        L = _lib.lib()
+        dims = (C.c_int * 3)()
+        _lib.check(min(0, L.b200ad_vae_debug_grad(self._h, name.encode(), int(skip), None, dims, _lib.stream_ptr())))
+        n = self._ws_key[0]
+        out = torch.empty((n, dims[0], dims[1], dims[2]), dtype=torch.float32, device=self.device)
+        _lib.check(min(0, L.b200ad_vae_debug_grad(self._h, name.encode(), int(skip), out.data_ptr(), dims,
+                                                  _lib.stream_ptr())))
+        return out
+
     @property
     def last_launch_count(self) -> int:
         return _lib.lib().b200ad_vae_last_launch_count(self._h)

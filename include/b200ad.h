@@ -138,6 +138,10 @@ int b200ad_unet_bind_backward(b200ad_unet* h, void* arena, size_t bytes, float* 
  * accumulate = 0 zeroes the gradient buffer first; != 0 adds to it (gradient accumulation, `accelerator.accumulate`). */
 int b200ad_unet_backward(b200ad_unet* h, const float* x, const float* g_eps, int accumulate, void* stream);
 int b200ad_unet_backward_launch_count(const b200ad_unet* h);
+/* Debug / parity, after a backward: copy the gradient of the loss w.r.t. the forward tap `name` to fp32 NCHW (skip = 0),
+ * or the share of it that a skip connection brought (skip = 1).  Returns the number of channels, or negative (unknown
+ * name, or no such gradient).  dst may be NULL to query (dims[0..2] = C, H, W). */
+int b200ad_unet_debug_grad(b200ad_unet* h, const char* name, int skip, float* dst, int* dims, void* stream);
 
 /* ---- Latent autoencoder: replaces diffusers.AutoencoderKL as the pipeline drives it ---------------------
  * (audiodiffusion/pipeline_audio_diffusion.py:143-147 encode + sample, :187-190 decode; architecture
@@ -191,6 +195,8 @@ int b200ad_vae_decoder_backward(b200ad_vae* h, const float* g_x, float* g_z_out,
 int b200ad_vae_encoder_backward(b200ad_vae* h, const float* x, const float* g_moments, int accumulate, void* stream);
 /* Kernel launches of the last decoder_backward plus those of the last encoder_backward. */
 int b200ad_vae_backward_launch_count(const b200ad_vae* h);
+/* As b200ad_unet_debug_grad, over the last decoder and encoder backward. */
+int b200ad_vae_debug_grad(b200ad_vae* h, const char* name, int skip, float* dst, int* dims, void* stream);
 
 /* ---- Training step, optimizer side: replaces F.mse_loss, clip_grad_norm_(1.0), torch.optim.AdamW.step and
  * EMAModel.step of scripts/train_unet.py:258-266 (the U-Net backward itself is not built yet — DESIGN.md §6). -- */
