@@ -183,7 +183,10 @@ struct Plan {    // everything a plan builder derives from the workspace and (N,
   size_t ws_bytes = 0;
 };
 
-// State shared by the model handles (U-Net, VAE): parameter table, packed-weight arena layout, workspace plan.
+struct Backward;   // a backward plan (unet_bwd.cu)
+
+// State shared by the model handles (U-Net, VAE): parameter table, packed-weight arena layout, workspace plan, backward
+// plans.
 struct NetBase {
   int norm_groups = 32;
   float norm_eps = 1e-5f;
@@ -209,7 +212,11 @@ struct NetBase {
   int enc_S = 0;
   int last_launches = 0;
   PackBatch pack_batch;             // device job table of the weight packing (one launch for all K-segments)
+  // backward: one plan per part (U-Net: the whole model; autoencoder: encoder, decoder), built by bind_backward
+  int nparts = 1;
+  Backward* bwd[2] = {};
 };
+void release_backward(NetBase* h);   // frees h->bwd (unet_bwd.cu)
 
 static PackItem make_pack_item(const NetBase* h, const PackJob& j, uint8_t* arena) {
   PackItem it;
@@ -223,11 +230,17 @@ static PackItem make_pack_item(const NetBase* h, const PackJob& j, uint8_t* aren
   return it;
 }
 
-static const char* check_groups(const int* ch, int n, int groups) {
-  if (groups < 1 || groups > 64) return "norm_num_groups must be in 1..64";
-  for (int i = 0; i < n; ++i)   // GroupNorm partial sums are kept per 4-channel quad: a group must be whole quads
-    if (ch[i] % groups || (ch[i] / groups) % 4) return "channels per GroupNorm group must be a multiple of 4 for every block";
-  return nullptr;
+// The configuration checks of both models' create; 0, or -1 with the error set.
+static int check_net_config(int num_blocks, const int* ch, int out_channels, int groups) {
+  if (num_blocks < 1 || num_blocks > B200AD_MAX_BLOCKS) return set_err("num_blocks out of range");
+  for (int i = 0; i < num_blocks; ++i)
+    if (ch[i] % 128) return set_err("block_out_channels must be multiples of 128");
+  if (out_channels > 4) return set_err("out_channels > 4 not implemented");
+  if (groups < 1 || groups > 64) return set_err("norm_num_groups must be in 1..64");
+  for (int i = 0; i < num_blocks; ++i)   // GroupNorm partial sums are kept per 4-channel quad: a group must be whole quads
+    if (ch[i] % groups || (ch[i] / groups) % 4)
+      return set_err("channels per GroupNorm group must be a multiple of 4 for every block");
+  return 0;
 }
 
 static std::string S(const char* fmt, ...) {
@@ -240,6 +253,11 @@ static std::string S(const char* fmt, ...) {
 }
 
 // ================================================================================= parameter table
+static int param_shape(const NetBase* h, int i, int64_t* dims) {
+  const auto& s = h->params[i].shape;
+  for (size_t k = 0; k < s.size(); ++k) dims[k] = s[k];
+  return (int)s.size();
+}
 static void add_param(NetBase* h, const std::string& name, std::vector<int64_t> shape) {
   h->pidx[name] = (int)h->params.size();
   h->params.push_back({name, std::move(shape)});
@@ -870,6 +888,34 @@ struct Builder {
 static bool debug_nopool() {
   const char* e = getenv("B200AD_DEBUG_NOPOOL");
   return e && e[0] == '1';
+}
+
+// Binds the plan `build` makes for (N, H, W) over a caller-owned workspace: a size pass, the workspace zeroed, the bound pass.
+template <class Net>
+static int bind_workspace(Net* h, Plan (*build)(const Net*, uint8_t*, int, int, int), void* workspace, size_t bytes, int N,
+                          int H, int W, cudaStream_t st) {
+  if (!h->packed) return set_err("set_params must be called before bind_workspace");
+  const int down = 1 << (h->cfg.num_blocks - 1);
+  if (H % down || W % down) return set_err("H and W must be multiples of %d", down);
+  const size_t need = build(h, nullptr, N, H, W).ws_bytes;
+  if (bytes < need) return set_err("workspace too small: %zu < %zu", bytes, need);
+  CK(cudaMemsetAsync(workspace, 0, need, st));
+  h->plan = build(h, (uint8_t*)workspace, N, H, W);
+  h->N = N; h->H = H; h->W = W;
+  h->ws = (uint8_t*)workspace; h->ws_bytes = need;
+  int dev = 0;
+  CK(cudaGetDevice(&dev));
+  CK(cudaDeviceGetAttribute(&h->num_sms, cudaDevAttrMultiProcessorCount, dev));
+  return 0;
+}
+
+static int set_training(NetBase* h, int on) {
+  if (!h) return set_err("null handle");
+  if (h->training != (on != 0)) {
+    h->training = on != 0;
+    h->plan.lists.clear();    // the workspace layout changes: bind_workspace must be called again
+  }
+  return 0;
 }
 
 // ================================================================================= plan executor

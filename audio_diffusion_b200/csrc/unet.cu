@@ -77,7 +77,7 @@ extern "C" int b200ad_version(void) { return 1; }
 
 extern "C" int b200ad_unet_create(const b200ad_unet_config* cfg, b200ad_unet** out) {
   if (!cfg || !out) return set_err("null argument");
-  if (cfg->num_blocks < 1 || cfg->num_blocks > B200AD_MAX_BLOCKS) return set_err("num_blocks out of range");
+  if (check_net_config(cfg->num_blocks, cfg->block_out_channels, cfg->out_channels, cfg->norm_num_groups)) return -1;
   if (cfg->attention_head_dim != 8) return set_err("only attention_head_dim == 8 is implemented");
   if (cfg->cross_attention_dim < 0 || cfg->cross_attention_dim > 4096) return set_err("cross_attention_dim out of range");
   for (int i = 0; i < cfg->num_blocks; ++i) {
@@ -86,10 +86,6 @@ extern "C" int b200ad_unet_create(const b200ad_unet_config* cfg, b200ad_unet** o
     const int d = cfg->block_out_channels[i] / 8;    // conditional model: 8 heads, head_dim = channels / 8
     if ((cfg->down_cross[i] || cfg->up_cross[i]) && d != 16 && d != 32 && d != 64) return set_err("cross-attention blocks need channels / 8 in {16, 32, 64}");
   }
-  for (int i = 0; i < cfg->num_blocks; ++i)
-    if (cfg->block_out_channels[i] % 128) return set_err("block_out_channels must be multiples of 128");
-  if (cfg->out_channels > 4) return set_err("out_channels > 4 not implemented");
-  if (const char* e = check_groups(cfg->block_out_channels, cfg->num_blocks, cfg->norm_num_groups)) return set_err("%s", e);
   b200ad_unet* h = new b200ad_unet();
   h->cfg = *cfg;
   h->norm_groups = cfg->norm_num_groups;
@@ -113,11 +109,7 @@ extern "C" void b200ad_unet_destroy(b200ad_unet* h) {
 }
 extern "C" int b200ad_unet_num_params(const b200ad_unet* h) { return (int)h->params.size(); }
 extern "C" const char* b200ad_unet_param_name(const b200ad_unet* h, int i) { return h->params[i].name.c_str(); }
-extern "C" int b200ad_unet_param_shape(const b200ad_unet* h, int i, int64_t* dims) {
-  const auto& s = h->params[i].shape;
-  for (size_t k = 0; k < s.size(); ++k) dims[k] = s[k];
-  return (int)s.size();
-}
+extern "C" int b200ad_unet_param_shape(const b200ad_unet* h, int i, int64_t* dims) { return param_shape(h, i, dims); }
 extern "C" size_t b200ad_unet_packed_bytes(const b200ad_unet* h) { return h->packed_bytes; }
 
 extern "C" int b200ad_unet_set_params(b200ad_unet* h, const float* const* params, void* packed, size_t packed_bytes,
@@ -176,19 +168,7 @@ extern "C" size_t b200ad_unet_workspace_bytes(const b200ad_unet* h, int N, int H
 }
 
 extern "C" int b200ad_unet_bind_workspace(b200ad_unet* h, void* workspace, size_t bytes, int N, int H, int W, void* stream) {
-  if (!h->packed) return set_err("set_params must be called before bind_workspace");
-  const int down = 1 << (h->cfg.num_blocks - 1);
-  if (H % down || W % down) return set_err("H and W must be multiples of %d", down);
-  const size_t need = build_plan(h, nullptr, N, H, W).ws_bytes;
-  if (bytes < need) return set_err("workspace too small: %zu < %zu", bytes, need);
-  CK(cudaMemsetAsync(workspace, 0, need, (cudaStream_t)stream));
-  h->plan = build_plan(h, (uint8_t*)workspace, N, H, W);
-  h->N = N; h->H = H; h->W = W;
-  h->ws = (uint8_t*)workspace; h->ws_bytes = need;
-  int dev = 0;
-  CK(cudaGetDevice(&dev));
-  CK(cudaDeviceGetAttribute(&h->num_sms, cudaDevAttrMultiProcessorCount, dev));
-  return 0;
+  return bind_workspace(h, build_plan, workspace, bytes, N, H, W, (cudaStream_t)stream);
 }
 
 static int run_plan(b200ad_unet* h, const RunArgs& a, cudaStream_t st, OpEvents* timing = nullptr) {

@@ -5,9 +5,4 @@
 struct b200ad_unet : b200ad::NetBase {
   b200ad_unet_config cfg;
   std::vector<b200ad::Block> blocks;
-  struct Backward* bwd = nullptr;   // built lazily by b200ad_unet_backward (unet_bwd.cu)
 };
-
-namespace b200ad {
-void release_backward(b200ad_unet* h);   // frees h->bwd (defined next to the Backward type, unet_bwd.cu)
-}

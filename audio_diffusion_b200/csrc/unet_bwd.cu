@@ -24,8 +24,6 @@ struct View {            // channel range of a PF8 tensor
   size_t off = 0;                     // byte offset of p in its arena (Act::off)
 };
 
-}  // namespace b200ad
-
 struct Backward {
   OpList list;                       // the ops (no GroupNorm statistics)
   std::vector<PackJob> jobs;         // transposed weight packs, redone at every backward (the weights move every step)
@@ -41,8 +39,6 @@ struct Backward {
   // the whole gradient, and the share of it a skip connection brought (debug_grad)
   std::map<std::string, Act> grad, skipgrad;
 };
-
-namespace b200ad {
 
 struct BwdBuilder {
   NetBase* h;
@@ -485,9 +481,10 @@ struct BwdBuilder {
   }
 };
 
-static int build_backward(b200ad_unet* h, Backward* bw, uint8_t* arena, float* grads, size_t* bytes_out) {
+static int build_unet_backward(b200ad_unet* h, Backward* const* bws, uint8_t* arena, float* grads, size_t* bytes_out) {
   const b200ad_unet_config& c = h->cfg;
   if (!h->training || h->plan.lists.empty()) return set_err("backward needs set_training(1) before bind_workspace");
+  Backward* bw = bws[0];
   bw->list.ops.clear();
   bw->jobs.clear();
   bw->arena = arena;
@@ -579,138 +576,7 @@ static int build_backward(b200ad_unet* h, Backward* bw, uint8_t* arena, float* g
   return 0;
 }
 
-// fp32 NCHW copy of a gradient tensor of a bound backward plan (skip: the skip connection's share); as debug_tensor
-static int debug_grad(const NetBase* h, const Backward* const* bws, int nbw, const char* name, int skip, float* dst,
-                      int* dims, cudaStream_t st) {
-  for (int i = 0; i < nbw; ++i) {
-    if (!bws[i] || bws[i]->list.ops.empty()) return set_err("debug_grad: bind_backward must be called first");
-    const std::map<std::string, Act>& m = skip ? bws[i]->skipgrad : bws[i]->grad;
-    auto it = m.find(name);
-    if (it == m.end()) continue;
-    const Act& a = it->second;
-    if (dims) { dims[0] = a.C; dims[1] = a.H; dims[2] = a.W; }
-    if (dst) CK(launch_pf8_to_nchw(a.p, dst, h->N, a.C, a.H, a.W, st));
-    return a.C;
-  }
-  return set_err("debug_grad: no %sgradient for '%s'", skip ? "skip " : "", name);
-}
-
-// The size pass (null arena) must plan the ops the bound pass plans, or the arena size it found may be wrong.
-static int check_same_plan(const Backward& sized, Backward* bound) {
-  bool same = sized.list.ops.size() == bound->list.ops.size();
-  for (size_t i = 0; same && i < sized.list.ops.size(); ++i) same = sized.list.ops[i].kind == bound->list.ops[i].kind;
-  if (same) return 0;
-  bound->list.ops.clear();
-  return set_err("bind_backward: the size pass and the bound pass planned different ops");
-}
-
-// Runs a bound backward plan: zeroes its gradient slots (unless accumulating), then its ops.
-static int run_backward(NetBase* h, Backward* bw, const RunArgs& a, int accumulate, cudaStream_t st) {
-  // B200AD_BWD_PROFILE=1: CUDA events around every op, per-kind totals printed to stderr (tools/train_bench.py)
-  static const bool prof = [] { const char* e = getenv("B200AD_BWD_PROFILE"); return e && e[0] == '1'; }();
-  if (!accumulate) CK(cudaMemsetAsync(bw->grads + bw->zero_off, 0, bw->zero_floats * sizeof(float), st));   // every kernel below ADDS
-  OpEvents ev;
-  if (run_ops(h, bw->list, a, st, &bw->launches, prof ? &ev : nullptr)) return -1;
-  if (prof) {
-    CK(cudaStreamSynchronize(st));
-    double tot[OP_NKINDS] = {0};
-    int cnt[OP_NKINDS] = {0};
-    for (size_t i = 0; i < bw->list.ops.size(); ++i) {
-      float ms = 0.f;
-      if (ev.ms(i, &ms)) return -1;
-      tot[bw->list.ops[i].kind] += ms;
-      cnt[bw->list.ops[i].kind]++;
-    }
-    fprintf(stderr, "{\"backward_profile_ms\": {");
-    const char* sep = "";
-    for (int k = 0; k < OP_NKINDS; ++k) {
-      if (!cnt[k]) continue;
-      if (k == OP_PACK_T) fprintf(stderr, "%s\"%s\": %.3f", sep, op_names[k], tot[k]);   // one per plan
-      else fprintf(stderr, "%s\"%s x%d\": %.3f", sep, op_names[k], cnt[k], tot[k]);
-      sep = ", ";
-    }
-    fprintf(stderr, "}}\n");
-  }
-  return 0;
-}
-
-void release_backward(b200ad_unet* h) {
-  delete h->bwd;
-  h->bwd = nullptr;
-}
-
-}  // namespace b200ad
-
-// ================================================================================= C ABI
-extern "C" int b200ad_unet_set_training(b200ad_unet* h, int on) {
-  if (!h) return set_err("null handle");
-  if (h->training != (on != 0)) {
-    h->training = on != 0;
-    h->plan.lists.clear();    // the workspace layout changes: bind_workspace must be called again
-  }
-  return 0;
-}
-
-static void ensure_bwd(b200ad_unet* h) {
-  if (h->bwd) return;
-  Backward* bw = new Backward();
-  size_t off = 0;
-  for (const auto& p : h->params) {
-    size_t n = 1;
-    for (auto d : p.shape) n *= (size_t)d;
-    bw->goff.push_back(off);
-    off += (n + 63) & ~(size_t)63;
-  }
-  bw->grad_floats = off;
-  bw->zero_floats = off;
-  h->bwd = bw;
-}
-
-extern "C" size_t b200ad_unet_grad_floats(b200ad_unet* h) { ensure_bwd(h); return h->bwd->grad_floats; }
-extern "C" size_t b200ad_unet_grad_offset(b200ad_unet* h, int i) { ensure_bwd(h); return h->bwd->goff[i]; }
-
-extern "C" size_t b200ad_unet_backward_bytes(b200ad_unet* h) {
-  ensure_bwd(h);
-  Backward tmp;
-  tmp.goff = h->bwd->goff;
-  size_t bytes = 0;
-  if (build_backward(h, &tmp, nullptr, nullptr, &bytes)) return 0;
-  return bytes;
-}
-
-extern "C" int b200ad_unet_bind_backward(b200ad_unet* h, void* arena, size_t bytes, float* grads, void* stream) {
-  ensure_bwd(h);
-  size_t need = 0;
-  Backward sized;
-  sized.goff = h->bwd->goff;
-  if (build_backward(h, &sized, nullptr, nullptr, &need)) return -1;
-  if (bytes < need) return set_err("backward arena too small: %zu < %zu", bytes, need);
-  CK(cudaMemsetAsync(arena, 0, need, (cudaStream_t)stream));
-  if (build_backward(h, h->bwd, (uint8_t*)arena, grads, &need) || check_same_plan(sized, h->bwd)) return -1;
-  h->bwd->arena_bytes = need;
-  return 0;
-}
-
-extern "C" int b200ad_unet_backward(b200ad_unet* h, const float* x, const float* g_eps, int accumulate, void* stream) {
-  if (!h || !h->bwd || h->bwd->list.ops.empty()) return set_err("bind_backward must be called before backward");
-  if (!x || !g_eps) return set_err("backward: x and g_eps are required");
-  if (h->cfg.cross_attention_dim && (!h->enc || h->enc_S != 1))
-    return set_err("backward: the conditional U-Net needs the forward's encoding (S = 1) bound");
-  RunArgs a;
-  a.in = x; a.g_eps = g_eps;
-  return run_backward(h, h->bwd, a, accumulate, (cudaStream_t)stream);
-}
-
-extern "C" int b200ad_unet_backward_launch_count(const b200ad_unet* h) { return h && h->bwd ? h->bwd->launches : 0; }
-
-extern "C" int b200ad_unet_debug_grad(b200ad_unet* h, const char* name, int skip, float* dst, int* dims, void* stream) {
-  if (!h || !name) return set_err("null argument");
-  const Backward* bws[1] = {h->bwd};
-  return debug_grad(h, bws, 1, name, skip, dst, dims, (cudaStream_t)stream);
-}
-
 // ================================================================================= autoencoder backward
-namespace b200ad {
 
 // Both parts' plans over one arena: the decoder first, then the encoder (the order of a training step's backward).
 static int build_vae_backward(b200ad_vae* h, Backward* const* bws, uint8_t* arena, float* grads, size_t* bytes_out) {
@@ -807,89 +673,167 @@ static int build_vae_backward(b200ad_vae* h, Backward* const* bws, uint8_t* aren
   return 0;
 }
 
-void release_backward(b200ad_vae* h) {
+// ================================================================================= the handle protocol of both models
+// fp32 NCHW copy of a gradient tensor of a bound backward plan (skip: the skip connection's share); as debug_tensor.  The
+// parts are searched in order: the autoencoder's tap names all start with "encoder." or "decoder.", so a name is found in
+// one part only.
+static int debug_grad(const NetBase* h, const char* name, int skip, float* dst, int* dims, cudaStream_t st) {
+  if (!h || !name) return set_err("null argument");
+  for (int i = 0; i < h->nparts; ++i) {
+    const Backward* bw = h->bwd[i];
+    if (!bw || bw->list.ops.empty()) return set_err("debug_grad: bind_backward must be called first");
+    const std::map<std::string, Act>& m = skip ? bw->skipgrad : bw->grad;
+    auto it = m.find(name);
+    if (it == m.end()) continue;
+    const Act& a = it->second;
+    if (dims) { dims[0] = a.C; dims[1] = a.H; dims[2] = a.W; }
+    if (dst) CK(launch_pf8_to_nchw(a.p, dst, h->N, a.C, a.H, a.W, st));
+    return a.C;
+  }
+  return set_err("debug_grad: no %sgradient for '%s'", skip ? "skip " : "", name);
+}
+
+// The size pass (null arena) must plan the ops the bound pass plans, or the arena size it found may be wrong.
+static int check_same_plan(const Backward& sized, Backward* bound) {
+  bool same = sized.list.ops.size() == bound->list.ops.size();
+  for (size_t i = 0; same && i < sized.list.ops.size(); ++i) same = sized.list.ops[i].kind == bound->list.ops[i].kind;
+  if (same) return 0;
+  bound->list.ops.clear();
+  return set_err("bind_backward: the size pass and the bound pass planned different ops");
+}
+
+// Runs the bound backward plan of `part`: zeroes its gradient slots (unless accumulating), then its ops.
+static int run_backward(NetBase* h, int part, const RunArgs& a, int accumulate, cudaStream_t st) {
+  if (!h || !h->bwd[part] || h->bwd[part]->list.ops.empty()) return set_err("bind_backward must be called before backward");
+  Backward* bw = h->bwd[part];
+  // B200AD_BWD_PROFILE=1: CUDA events around every op, per-kind totals printed to stderr (tools/train_bench.py)
+  static const bool prof = [] { const char* e = getenv("B200AD_BWD_PROFILE"); return e && e[0] == '1'; }();
+  if (!accumulate) CK(cudaMemsetAsync(bw->grads + bw->zero_off, 0, bw->zero_floats * sizeof(float), st));   // every kernel below ADDS
+  OpEvents ev;
+  if (run_ops(h, bw->list, a, st, &bw->launches, prof ? &ev : nullptr)) return -1;
+  if (prof) {
+    CK(cudaStreamSynchronize(st));
+    double tot[OP_NKINDS] = {0};
+    int cnt[OP_NKINDS] = {0};
+    for (size_t i = 0; i < bw->list.ops.size(); ++i) {
+      float ms = 0.f;
+      if (ev.ms(i, &ms)) return -1;
+      tot[bw->list.ops[i].kind] += ms;
+      cnt[bw->list.ops[i].kind]++;
+    }
+    fprintf(stderr, "{\"backward_profile_ms\": {");
+    const char* sep = "";
+    for (int k = 0; k < OP_NKINDS; ++k) {
+      if (!cnt[k]) continue;
+      if (k == OP_PACK_T) fprintf(stderr, "%s\"%s\": %.3f", sep, op_names[k], tot[k]);   // one per plan
+      else fprintf(stderr, "%s\"%s x%d\": %.3f", sep, op_names[k], cnt[k], tot[k]);
+      sep = ", ";
+    }
+    fprintf(stderr, "}}\n");
+  }
+  return 0;
+}
+
+void release_backward(NetBase* h) {
   for (Backward*& b : h->bwd) {
     delete b;
     b = nullptr;
   }
 }
 
-}  // namespace b200ad
-
-extern "C" int b200ad_vae_set_training(b200ad_vae* h, int on) {
-  if (!h) return set_err("null handle");
-  if (h->training != (on != 0)) {
-    h->training = on != 0;
-    h->plan.lists.clear();    // the workspace layout changes: bind_workspace must be called again
-  }
-  return 0;
-}
-
-// The flat gradient buffer: encoder parameters (with quant_conv) first, then the decoder's (with post_quant_conv); each
-// part's plan zeroes only its own range.
-static void ensure_bwd(b200ad_vae* h) {
+// The flat gradient buffer: every parameter's gradient at a 64-float-aligned offset, in table order.  Each part's plan
+// zeroes only its own range: the autoencoder's decoder part starts at its first decoder. / post_quant_conv. parameter.
+static void ensure_bwd(NetBase* h) {
   if (h->bwd[0]) return;
   std::vector<size_t> goff;
-  size_t off = 0, dec_off = 0;
+  size_t off = 0, split = 0;
   for (const auto& p : h->params) {
-    if (!dec_off && (p.name.rfind("decoder.", 0) == 0 || p.name.rfind("post_quant_conv.", 0) == 0)) dec_off = off;
+    if (!split && (p.name.rfind("decoder.", 0) == 0 || p.name.rfind("post_quant_conv.", 0) == 0)) split = off;
     size_t n = 1;
     for (auto d : p.shape) n *= (size_t)d;
     goff.push_back(off);
     off += (n + 63) & ~(size_t)63;
   }
-  for (int part : {ENC, DEC}) {
+  for (int part = 0; part < h->nparts; ++part) {
     Backward* bw = new Backward();
     bw->goff = goff;
     bw->grad_floats = off;
-    bw->zero_off = part == ENC ? 0 : dec_off;
-    bw->zero_floats = part == ENC ? dec_off : off - dec_off;
+    bw->zero_off = part == 0 ? 0 : split;
+    bw->zero_floats = (part == h->nparts - 1 ? off : split) - bw->zero_off;
     h->bwd[part] = bw;
   }
 }
 
-extern "C" size_t b200ad_vae_grad_floats(b200ad_vae* h) { ensure_bwd(h); return h->bwd[0]->grad_floats; }
-extern "C" size_t b200ad_vae_grad_offset(b200ad_vae* h, int i) { ensure_bwd(h); return h->bwd[0]->goff[i]; }
+// A model's backward plan builder: the plans of all its parts over one arena (null: size pass), into bws[0..nparts).
+template <class Net> using BuildBackward = int (*)(Net*, Backward* const*, uint8_t*, float*, size_t*);
 
-// Builds both plans with a null arena into sized[ENC], sized[DEC]; returns the arena bytes (0: error).
-static size_t vae_backward_size(b200ad_vae* h, Backward* sized) {
+// Size pass of every part into sized[]; returns the arena bytes (0: error).
+template <class Net> static size_t backward_size(Net* h, BuildBackward<Net> build, Backward* sized) {
   ensure_bwd(h);
-  sized[0].goff = sized[1].goff = h->bwd[0]->goff;
-  Backward* tb[2] = {&sized[0], &sized[1]};
+  Backward* parts[2] = {&sized[0], &sized[1]};
+  for (Backward* b : parts) b->goff = h->bwd[0]->goff;
   size_t bytes = 0;
-  if (build_vae_backward(h, tb, nullptr, nullptr, &bytes)) return 0;
-  return bytes;
+  return build(h, parts, nullptr, nullptr, &bytes) ? 0 : bytes;
 }
 
-extern "C" size_t b200ad_vae_backward_bytes(b200ad_vae* h) {
+template <class Net> static size_t backward_bytes(Net* h, BuildBackward<Net> build) {
   Backward sized[2];
-  return vae_backward_size(h, sized);
+  return backward_size(h, build, sized);
 }
 
-extern "C" int b200ad_vae_bind_backward(b200ad_vae* h, void* arena, size_t bytes, float* grads, void* stream) {
+template <class Net>
+static int bind_backward(Net* h, BuildBackward<Net> build, void* arena, size_t bytes, float* grads, cudaStream_t st) {
   Backward sized[2];
-  const size_t need = vae_backward_size(h, sized);
+  const size_t need = backward_size(h, build, sized);
   if (!need) return -1;
   if (bytes < need) return set_err("backward arena too small: %zu < %zu", bytes, need);
-  CK(cudaMemsetAsync(arena, 0, need, (cudaStream_t)stream));
+  CK(cudaMemsetAsync(arena, 0, need, st));
   size_t got = 0;
-  if (build_vae_backward(h, h->bwd, (uint8_t*)arena, grads, &got)) return -1;
-  for (int part : {ENC, DEC})
+  if (build(h, h->bwd, (uint8_t*)arena, grads, &got)) return -1;
+  for (int part = 0; part < h->nparts; ++part)
     if (check_same_plan(sized[part], h->bwd[part])) return -1;
-  for (Backward* b : h->bwd) b->arena_bytes = got;
+  for (int part = 0; part < h->nparts; ++part) h->bwd[part]->arena_bytes = got;
   return 0;
 }
 
-static int vae_backward(b200ad_vae* h, int part, const RunArgs& a, int accumulate, cudaStream_t st) {
-  if (!h || !h->bwd[part] || h->bwd[part]->list.ops.empty()) return set_err("bind_backward must be called before backward");
-  return run_backward(h, h->bwd[part], a, accumulate, st);
+static int backward_launch_count(const NetBase* h) {   // the last backward of every part
+  int n = 0;
+  for (int part = 0; h && part < h->nparts; ++part) n += h->bwd[part] ? h->bwd[part]->launches : 0;
+  return n;
+}
+
+}  // namespace b200ad
+
+// ================================================================================= C ABI: the handle protocol
+extern "C" int b200ad_unet_set_training(b200ad_unet* h, int on) { return set_training(h, on); }
+extern "C" size_t b200ad_unet_grad_floats(b200ad_unet* h) { ensure_bwd(h); return h->bwd[0]->grad_floats; }
+extern "C" size_t b200ad_unet_grad_offset(b200ad_unet* h, int i) { ensure_bwd(h); return h->bwd[0]->goff[i]; }
+extern "C" size_t b200ad_unet_backward_bytes(b200ad_unet* h) { return backward_bytes(h, build_unet_backward); }
+extern "C" int b200ad_unet_bind_backward(b200ad_unet* h, void* arena, size_t bytes, float* grads, void* stream) {
+  return bind_backward(h, build_unet_backward, arena, bytes, grads, (cudaStream_t)stream);
+}
+extern "C" int b200ad_unet_backward_launch_count(const b200ad_unet* h) { return backward_launch_count(h); }
+extern "C" int b200ad_unet_debug_grad(b200ad_unet* h, const char* name, int skip, float* dst, int* dims, void* stream) {
+  return debug_grad(h, name, skip, dst, dims, (cudaStream_t)stream);
+}
+
+extern "C" int b200ad_vae_set_training(b200ad_vae* h, int on) { return set_training(h, on); }
+extern "C" size_t b200ad_vae_grad_floats(b200ad_vae* h) { ensure_bwd(h); return h->bwd[0]->grad_floats; }
+extern "C" size_t b200ad_vae_grad_offset(b200ad_vae* h, int i) { ensure_bwd(h); return h->bwd[0]->goff[i]; }
+extern "C" size_t b200ad_vae_backward_bytes(b200ad_vae* h) { return backward_bytes(h, build_vae_backward); }
+extern "C" int b200ad_vae_bind_backward(b200ad_vae* h, void* arena, size_t bytes, float* grads, void* stream) {
+  return bind_backward(h, build_vae_backward, arena, bytes, grads, (cudaStream_t)stream);
+}
+extern "C" int b200ad_vae_backward_launch_count(const b200ad_vae* h) { return backward_launch_count(h); }
+extern "C" int b200ad_vae_debug_grad(b200ad_vae* h, const char* name, int skip, float* dst, int* dims, void* stream) {
+  return debug_grad(h, name, skip, dst, dims, (cudaStream_t)stream);
 }
 
 extern "C" int b200ad_vae_decoder_backward(b200ad_vae* h, const float* g_x, float* g_z_out, int accumulate, void* stream) {
   if (!g_x || !g_z_out) return set_err("decoder_backward: g_x and g_z_out are required");
   RunArgs a;
   a.g_eps = g_x; a.g_z = g_z_out;
-  return vae_backward(h, DEC, a, accumulate, (cudaStream_t)stream);
+  return run_backward(h, DEC, a, accumulate, (cudaStream_t)stream);
 }
 
 extern "C" int b200ad_vae_encoder_backward(b200ad_vae* h, const float* x, const float* g_moments, int accumulate,
@@ -897,15 +841,14 @@ extern "C" int b200ad_vae_encoder_backward(b200ad_vae* h, const float* x, const 
   if (!x || !g_moments) return set_err("encoder_backward: x and g_moments are required");
   RunArgs a;
   a.in = x; a.g_mom = g_moments;
-  return vae_backward(h, ENC, a, accumulate, (cudaStream_t)stream);
+  return run_backward(h, ENC, a, accumulate, (cudaStream_t)stream);
 }
 
-extern "C" int b200ad_vae_backward_launch_count(const b200ad_vae* h) {
-  return h && h->bwd[0] ? h->bwd[0]->launches + h->bwd[1]->launches : 0;
-}
-
-extern "C" int b200ad_vae_debug_grad(b200ad_vae* h, const char* name, int skip, float* dst, int* dims, void* stream) {
-  if (!h || !name) return set_err("null argument");
-  const Backward* bws[2] = {h->bwd[DEC], h->bwd[ENC]};
-  return debug_grad(h, bws, 2, name, skip, dst, dims, (cudaStream_t)stream);
+extern "C" int b200ad_unet_backward(b200ad_unet* h, const float* x, const float* g_eps, int accumulate, void* stream) {
+  if (!x || !g_eps) return set_err("backward: x and g_eps are required");
+  if (h && h->cfg.cross_attention_dim && (!h->enc || h->enc_S != 1))
+    return set_err("backward: the conditional U-Net needs the forward's encoding (S = 1) bound");
+  RunArgs a;
+  a.in = x; a.g_eps = g_eps;
+  return run_backward(h, 0, a, accumulate, (cudaStream_t)stream);
 }

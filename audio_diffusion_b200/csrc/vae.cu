@@ -84,14 +84,11 @@ static Plan vae_build_plan(const b200ad_vae* h, uint8_t* ws_base, int N, int H, 
 // ================================================================================= C ABI: AutoencoderKL
 extern "C" int b200ad_vae_create(const b200ad_vae_config* cfg, b200ad_vae** out) {
   if (!cfg || !out) return set_err("null argument");
-  if (cfg->num_blocks < 1 || cfg->num_blocks > B200AD_MAX_BLOCKS) return set_err("num_blocks out of range");
-  for (int i = 0; i < cfg->num_blocks; ++i)
-    if (cfg->block_out_channels[i] % 128) return set_err("block_out_channels must be multiples of 128");
+  if (check_net_config(cfg->num_blocks, cfg->block_out_channels, cfg->out_channels, cfg->norm_num_groups)) return -1;
   if (cfg->latent_channels < 1 || cfg->latent_channels > 4) return set_err("latent_channels must be 1..4");
-  if (cfg->out_channels > 4) return set_err("out_channels > 4 not implemented");
-  if (const char* e = check_groups(cfg->block_out_channels, cfg->num_blocks, cfg->norm_num_groups)) return set_err("%s", e);
   b200ad_vae* h = new b200ad_vae();
   h->cfg = *cfg;
+  h->nparts = 2;
   h->norm_groups = cfg->norm_num_groups;
   h->norm_eps = cfg->norm_eps;
   vae_blocks(h);
@@ -112,11 +109,7 @@ extern "C" void b200ad_vae_destroy(b200ad_vae* h) {
 }
 extern "C" int b200ad_vae_num_params(const b200ad_vae* h) { return (int)h->params.size(); }
 extern "C" const char* b200ad_vae_param_name(const b200ad_vae* h, int i) { return h->params[i].name.c_str(); }
-extern "C" int b200ad_vae_param_shape(const b200ad_vae* h, int i, int64_t* dims) {
-  const auto& s = h->params[i].shape;
-  for (size_t k = 0; k < s.size(); ++k) dims[k] = s[k];
-  return (int)s.size();
-}
+extern "C" int b200ad_vae_param_shape(const b200ad_vae* h, int i, int64_t* dims) { return param_shape(h, i, dims); }
 extern "C" size_t b200ad_vae_packed_bytes(const b200ad_vae* h) { return h->packed_bytes; }
 
 extern "C" int b200ad_vae_set_params(b200ad_vae* h, const float* const* params, void* packed, size_t packed_bytes,
@@ -132,19 +125,7 @@ extern "C" size_t b200ad_vae_workspace_bytes(const b200ad_vae* h, int N, int H, 
 }
 
 extern "C" int b200ad_vae_bind_workspace(b200ad_vae* h, void* workspace, size_t bytes, int N, int H, int W, void* stream) {
-  if (!h->packed) return set_err("set_params must be called before bind_workspace");
-  const int f = 1 << (h->cfg.num_blocks - 1);
-  if (H % f || W % f) return set_err("H and W must be multiples of %d", f);
-  const size_t need = vae_build_plan(h, nullptr, N, H, W).ws_bytes;
-  if (bytes < need) return set_err("workspace too small: %zu < %zu", bytes, need);
-  CK(cudaMemsetAsync(workspace, 0, need, (cudaStream_t)stream));
-  h->plan = vae_build_plan(h, (uint8_t*)workspace, N, H, W);
-  h->N = N; h->H = H; h->W = W;
-  h->ws = (uint8_t*)workspace; h->ws_bytes = need;
-  int dev = 0;
-  CK(cudaGetDevice(&dev));
-  CK(cudaDeviceGetAttribute(&h->num_sms, cudaDevAttrMultiProcessorCount, dev));
-  return 0;
+  return bind_workspace(h, vae_build_plan, workspace, bytes, N, H, W, (cudaStream_t)stream);
 }
 
 extern "C" int b200ad_vae_encode(b200ad_vae* h, const float* x, const float* noise, float* z, float* moments, void* stream) {

@@ -5,10 +5,8 @@
 struct b200ad_vae : b200ad::NetBase {
   b200ad_vae_config cfg;
   std::vector<b200ad::Block> enc, dec;   // encoder, decoder
-  struct Backward* bwd[2] = {};          // encoder, decoder backward plans (unet_bwd.cu)
 };
 
 namespace b200ad {
-enum { ENC = 0, DEC = 1 };               // the two plans
-void release_backward(b200ad_vae* h);    // frees h->bwd (defined next to the Backward type, unet_bwd.cu)
+enum { ENC = 0, DEC = 1 };               // the two plans (forward and backward)
 }

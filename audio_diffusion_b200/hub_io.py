@@ -43,16 +43,19 @@ def load_weights(sub: str):
     return fixed
 
 
-def model_from_dir(cls, sub: str):
+def model_from_dir(cls, sub: str, keep=None):
     """EVERY constructor argument present in config.json is handed to `cls`, whose own validation rejects what the engine
     does not implement (a silently dropped `freq_shift` or `downsample_padding` would load fine and sample garbage);
-    keys the constructor does not know are an error too."""
+    keys the constructor does not know are an error too.  `keep`: hand over these keys only, and ignore the rest."""
     cfgp = os.path.join(sub, "config.json")
     if not os.path.exists(cfgp):
         raise EnvironmentError(f"{sub} does not contain a {cls.__name__} (config.json missing)")
     with open(cfgp) as f:
         cfg = json.load(f)
-    kwargs = {k: v for k, v in cfg.items() if not k.startswith("_")}
+    if keep is not None:
+        kwargs = {k: cfg[k] for k in keep if k in cfg}
+    else:
+        kwargs = {k: v for k, v in cfg.items() if not k.startswith("_")}
     try:
         model = cls(**kwargs)
     except TypeError as e:

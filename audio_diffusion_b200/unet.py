@@ -2,21 +2,20 @@
 (scripts/train_unet.py:115-137; audiodiffusion/pipeline_audio_diffusion.py:118-126,160-163,237).
 
 Same constructor kwargs, same state-dict key layout (SURVEY §8b) and the same call convention
-`unet(sample, timestep)["sample"]`; the forward runs entirely in libb200ad.so (tcgen05 implicit-GEMM
-convs, fused GroupNorm statistics, fused scheduler step).  PyTorch owns every tensor: parameters are
-ordinary fp32 `nn.Parameter`s, the packed bf16 weights and the activation workspace are torch byte tensors.
+`unet(sample, timestep)["sample"]`; the forward runs entirely in libb200ad.so (wgmma implicit-GEMM convs, fused GroupNorm
+statistics, fused scheduler step).  Training: with grad enabled and the module in train() mode, the forward is an autograd
+node whose backward runs in libb200ad.so too (unet_bwd.cu).  The engine plumbing is `EngineModel`'s (engine.py).
 """
 from __future__ import annotations
 
 import ctypes as C
-import math
-from typing import Dict, Optional, Sequence, Tuple, Union
+from typing import Optional, Sequence, Tuple, Union
 
 import torch
-from torch import nn
 
 from . import _lib
 from ._lib import MAX_BLOCKS, StepCoefC, UNetConfigC
+from .engine import EngineModel, _Cfg
 
 
 class UNet2DOutput(dict):
@@ -27,18 +26,22 @@ class UNet2DOutput(dict):
         self.sample = sample
 
 
-class _Cfg(dict):
-    __getattr__ = dict.__getitem__
-
-
-def _set_deep(root: nn.Module, dotted: str, p: nn.Parameter) -> None:
-    parts = dotted.split(".")
-    m = root
-    for name in parts[:-1]:
-        if name not in m._modules:
-            m.add_module(name, nn.Module())
-        m = m._modules[name]
-    m.register_parameter(parts[-1], p)
+def _unet_config(in_channels: int, out_channels: int, layers_per_block: int, block_out_channels: Sequence[int],
+                 down_block_types: Sequence[str], up_block_types: Sequence[str], norm_num_groups: int, norm_eps: float,
+                 attention_head_dim: int, cross_attention_dim: int = 0) -> UNetConfigC:
+    c = UNetConfigC()
+    c.in_channels, c.out_channels = in_channels, out_channels
+    c.layers_per_block, c.num_blocks = layers_per_block, len(block_out_channels)
+    for i, v in enumerate(block_out_channels):
+        c.block_out_channels[i] = int(v)
+        c.down_attn[i] = 1 if down_block_types[i] == "AttnDownBlock2D" else 0
+        c.up_attn[i] = 1 if up_block_types[i] == "AttnUpBlock2D" else 0
+        c.down_cross[i] = 1 if down_block_types[i] == "CrossAttnDownBlock2D" else 0
+        c.up_cross[i] = 1 if up_block_types[i] == "CrossAttnUpBlock2D" else 0
+    c.norm_num_groups, c.norm_eps = norm_num_groups, norm_eps
+    c.attention_head_dim = attention_head_dim
+    c.cross_attention_dim = cross_attention_dim
+    return c
 
 
 class _UNetFunction(torch.autograd.Function):
@@ -49,23 +52,32 @@ class _UNetFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, model, x, t, enc, *params):
-        out = model._forward_train(x, t, enc)
+        out = model._run(x, t, enc, train=True)
         ctx.model = model
-        ctx.gen = model._fwd_gen         # the activations live in the model's single workspace: backward must see THIS forward
+        ctx.gen = model._fwd_gen[0]     # the activations live in the model's single workspace: backward must see THIS forward
         ctx.save_for_backward(x, enc)
         return out
 
     @staticmethod
     def backward(ctx, g):
         x, enc = ctx.saved_tensors
-        if ctx.gen != ctx.model._fwd_gen:
-            raise _lib.B200ADError("UNet2DModel(b200): another forward ran on this model before backward(); the saved "
-                                   "activations of this graph were overwritten (one forward per backward)")
-        ctx.model._backward_train(x, g, enc)     # fills p.grad (views of the flat gradient buffer)
-        return (None, None, None, None) + (None,) * len(ctx.model._pnames)
+        m = ctx.model
+        m._check_gen(0, ctx.gen)
+        g = g.to(torch.float32).contiguous()
+
+        def launch(accumulate):
+            m._set_encoding(enc)      # another call may have bound a different encoding since the forward
+            _lib.check(m._fn("backward")(m._h, x.data_ptr(), g.data_ptr(), accumulate, _lib.stream_ptr()))
+            if not m._no_sync:
+                m._allreduce_gradients()
+        m._backward_part(0, launch)     # fills p.grad (views of the flat gradient buffer)
+        return (None, None, None, None) + (None,) * len(m._pnames)
 
 
-class UNet2DModel(nn.Module):
+class UNet2DModel(EngineModel):
+    _prefix = "unet"
+    _no_sync = False
+
     def __init__(
         self,
         sample_size: Optional[Union[int, Tuple[int, int]]] = None,
@@ -132,115 +144,9 @@ class UNet2DModel(nn.Module):
             add_attention=add_attention, downsample_type=downsample_type, upsample_type=upsample_type, dropout=dropout,
             attn_norm_num_groups=attn_norm_num_groups, class_embed_type=class_embed_type,
             num_class_embeds=num_class_embeds, num_train_timesteps=num_train_timesteps, _class_name="UNet2DModel")
-
-        c = UNetConfigC()
-        c.in_channels, c.out_channels = in_channels, out_channels
-        c.layers_per_block, c.num_blocks = layers_per_block, len(block_out_channels)
-        for i, v in enumerate(block_out_channels):
-            c.block_out_channels[i] = int(v)
-            c.down_attn[i] = 1 if down_block_types[i] == "AttnDownBlock2D" else 0
-            c.up_attn[i] = 1 if up_block_types[i] == "AttnUpBlock2D" else 0
-        c.norm_num_groups, c.norm_eps = norm_num_groups, norm_eps
-        c.attention_head_dim = attention_head_dim if attention_head_dim is not None else -1
-        self._init_engine(c, seed)
-
-    def _init_engine(self, c: UNetConfigC, seed: Optional[int]) -> None:
-        """Create the library handle and the fp32 master parameters (table and naming come from the library)."""
-        self._c = c
-        L = _lib.lib()
-        h = C.c_void_p()
-        _lib.check(L.b200ad_unet_create(C.byref(c), C.byref(h)))
-        self._h = h
-        # parameter table comes from the library (diffusers naming); PyTorch default init
-        g = torch.Generator().manual_seed(seed) if seed is not None else None
-        self._pnames = []
-        dims = (C.c_int64 * 4)()
-        shapes: Dict[str, Tuple[int, ...]] = {}
-        for i in range(L.b200ad_unet_num_params(h)):
-            name = L.b200ad_unet_param_name(h, i).decode()
-            nd = L.b200ad_unet_param_shape(h, i, dims)
-            shapes[name] = tuple(int(dims[k]) for k in range(nd))
-            self._pnames.append(name)
-        for name in self._pnames:
-            shape = shapes[name]
-            leaf = name.rsplit(".", 2)[-2]
-            is_norm = leaf.startswith("norm") or leaf == "group_norm" or leaf == "conv_norm_out"
-            if is_norm:
-                t = torch.ones(shape) if name.endswith(".weight") else torch.zeros(shape)
-            else:
-                wshape = shapes[name[: name.rfind(".")] + ".weight"]
-                bound = 1.0 / math.sqrt(int(math.prod(wshape[1:])))
-                t = (torch.rand(shape, generator=g) * 2 - 1) * bound
-            _set_deep(self, name, nn.Parameter(t))
-        self._packed = None
-        self._packed_key = None
-        self._ws = None
-        self._ws_key = None
-        self._plist = None
-        self._fwd_gen = 0                # bumped by every forward that writes the workspace
-
-    # ------------------------------------------------------------------ diffusers ModelMixin persistence
-    @classmethod
-    def from_pretrained(cls, path: str, subfolder: Optional[str] = None, **_unused) -> "UNet2DModel":
-        """`<path>/config.json` + `diffusion_pytorch_model.{safetensors,bin}`; older hub files' attention key names
-        (query/key/value/proj_attn) are renamed on the way in."""
-        import os
-        from .hub_io import model_from_dir
-        return model_from_dir(cls, os.path.join(path, subfolder) if subfolder else path)
-
-    def save_pretrained(self, path: str, safe_serialization: bool = True, **_unused) -> None:
-        from .hub_io import save_model
-        save_model(self, path, safe_serialization=safe_serialization)
-
-    # ------------------------------------------------------------------ engine plumbing
-    def __del__(self):
-        try:
-            if getattr(self, "_h", None):
-                _lib.lib().b200ad_unet_destroy(self._h)
-                self._h = None
-        except Exception:
-            pass
-
-    def _named(self) -> Dict[str, nn.Parameter]:
-        return dict(self.named_parameters())
-
-    @property
-    def device(self) -> torch.device:
-        return next(self.parameters()).device
-
-    def _ensure_bound(self, n: int, hh: int, ww: int) -> None:
-        _lib.require_cuda()
-        L = _lib.lib()
-        if self._plist is None:            # Parameter objects are stable (module.to() swaps .data); resolve the names once
-            named = self._named()
-            self._plist = [named[k] for k in self._pnames]
-        params = self._plist
-        dev = params[0].device
-        if dev.type != "cuda":
-            raise _lib.B200ADError("UNet2DModel(b200): parameters must live on a CUDA device (call .to('cuda'))")
-        for p in params:
-            if p.dtype != torch.float32 or not p.is_contiguous():
-                raise _lib.B200ADError("UNet2DModel(b200): parameters must be contiguous fp32 (master weights)")
-        key = tuple((p.data_ptr(), p._version) for p in params)
-        if self._packed is None or self._packed.device != dev:
-            self._packed = torch.empty(L.b200ad_unet_packed_bytes(self._h), dtype=torch.uint8, device=dev)
-            self._packed_key = None
-            self._ws_key = None
-        if key != self._packed_key:
-            arr = (C.c_void_p * len(params))(*[p.data_ptr() for p in params])
-            _lib.check(L.b200ad_unet_set_params(self._h, arr, self._packed.data_ptr(), self._packed.numel(),
-                                                _lib.stream_ptr()))
-            self._packed_key = key
-            self._ws_key = None  # plan holds parameter pointers
-        wkey = (n, hh, ww, dev)
-        if wkey != self._ws_key:
-            need = L.b200ad_unet_workspace_bytes(self._h, n, hh, ww)
-            if self._ws is None or self._ws.numel() < need or self._ws.device != dev:
-                self._ws = None
-                self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
-            _lib.check(L.b200ad_unet_bind_workspace(self._h, self._ws.data_ptr(), self._ws.numel(), n, hh, ww,
-                                                    _lib.stream_ptr()))
-            self._ws_key = wkey
+        self._init_engine(_unet_config(in_channels, out_channels, layers_per_block, block_out_channels, down_block_types,
+                                       up_block_types, norm_num_groups, norm_eps,
+                                       attention_head_dim if attention_head_dim is not None else -1), seed)
 
     def _timesteps(self, timestep, n: int, dev) -> torch.Tensor:
         t = timestep
@@ -256,99 +162,49 @@ class UNet2DModel(nn.Module):
     def _check_input(self, sample: torch.Tensor) -> torch.Tensor:
         _lib.require_cuda()
         if sample.device.type != "cuda":
-            raise _lib.B200ADError("UNet2DModel(b200): input must be a CUDA tensor (no CPU fallback)")
+            raise self._err("input must be a CUDA tensor (no CPU fallback)")
         return sample.to(torch.float32).contiguous()
+
+    def _encoding(self, enc, n: int, dev) -> Optional[torch.Tensor]:
+        """The conditional model's validated encoding; None here."""
+        return None
+
+    def _set_encoding(self, enc: Optional[torch.Tensor]) -> None:
+        if enc is not None:
+            _lib.check(self._fn("set_encoding")(self._h, enc.data_ptr(), enc.shape[1]))
 
     # ------------------------------------------------------------------ public call
     def forward(self, sample: torch.Tensor, timestep, return_dict: bool = True):
         """ε = unet(sample, timestep)["sample"] — pipeline_audio_diffusion.py:163."""
         if sample.requires_grad:
-            raise NotImplementedError("UNet2DModel(b200): gradients w.r.t. the input sample are not computed")
-        needs_grad = torch.is_grad_enabled() and self.training and any(p.requires_grad for p in self.parameters())
+            raise NotImplementedError(f"{type(self).__name__}(b200): gradients w.r.t. the input sample are not computed")
+        return self._forward(sample, timestep, None, return_dict)
+
+    def _forward(self, sample: torch.Tensor, timestep, enc, return_dict: bool):
         x = self._check_input(sample)
-        n, _, hh, ww = x.shape
-        if needs_grad:      # training step (scripts/train_unet.py:257-259): forward keeps every activation, backward in CUDA
-            t = self._timesteps(timestep, n, x.device)
-            named = self._named()
-            out = _UNetFunction.apply(self, x, t, None, *[named[k] for k in self._pnames])
-            return UNet2DOutput(out) if return_dict else (out,)
-        with torch.cuda.device(x.device):
-            self._fwd_gen += 1
-            self._set_training_mode(False)
-            self._ensure_bound(n, hh, ww)
-            t = self._timesteps(timestep, n, x.device)
-            out = torch.empty((n, self.out_channels, hh, ww), dtype=torch.float32, device=x.device)
-            _lib.check(_lib.lib().b200ad_unet_forward(self._h, x.data_ptr(), t.data_ptr(), out.data_ptr(),
-                                                      _lib.stream_ptr()))
-        if not return_dict:
-            return (out,)
-        return UNet2DOutput(out)
+        if self._needs_grad():    # training step (scripts/train_unet.py:257-259): forward keeps every activation
+            n = x.shape[0]
+            t, e = self._timesteps(timestep, n, x.device), self._encoding(enc, n, x.device)
+            out = _UNetFunction.apply(self, x, t, e, *self._plist)
+        else:
+            out = self._run(x, timestep, enc, train=False)
+        return UNet2DOutput(out) if return_dict else (out,)
 
-    # ------------------------------------------------------------------ training (backward in libb200ad)
-    def _set_training_mode(self, on: bool) -> None:
-        if getattr(self, "_train_mode", False) != on:
-            _lib.check(_lib.lib().b200ad_unet_set_training(self._h, 1 if on else 0))
-            self._train_mode = on
-            self._ws_key = None        # the workspace layout differs (no buffer pooling when training)
-            self._bwd_key = None
-
-    def _forward_train(self, x: torch.Tensor, t: torch.Tensor, enc: Optional[torch.Tensor] = None) -> torch.Tensor:
-        L = _lib.lib()
+    def _run(self, x: torch.Tensor, timestep, enc, train: bool) -> torch.Tensor:
+        """One forward into a new output tensor; timestep and encoding are converted after binding (already converted
+        ones, as the training node passes them, are left as they are)."""
         n, _, hh, ww = x.shape
         with torch.cuda.device(x.device):
-            self._fwd_gen += 1
-            self._set_training_mode(True)
-            self._ensure_bound(n, hh, ww)
-            if getattr(self, "_bwd_key", None) != self._ws_key:
-                nfl = L.b200ad_unet_grad_floats(self._h)
-                if getattr(self, "_grad_flat", None) is None or self._grad_flat.numel() != nfl or self._grad_flat.device != x.device:
-                    self._grad_flat = torch.zeros(nfl, dtype=torch.float32, device=x.device)
-                need = L.b200ad_unet_backward_bytes(self._h)
-                if need == 0:
-                    _lib.check(-1)
-                if getattr(self, "_bwd_arena", None) is None or self._bwd_arena.numel() < need or self._bwd_arena.device != x.device:
-                    self._bwd_arena = None
-                    self._bwd_arena = torch.empty(need, dtype=torch.uint8, device=x.device)
-                _lib.check(L.b200ad_unet_bind_backward(self._h, self._bwd_arena.data_ptr(), self._bwd_arena.numel(),
-                                                       self._grad_flat.data_ptr(), _lib.stream_ptr()))
-                self._bwd_key = self._ws_key
+            self._fwd_gen[0] += 1
+            self._bind(n, hh, ww, train, x.device)
+            t = self._timesteps(timestep, n, x.device)
+            e = self._encoding(enc, n, x.device)
             out = torch.empty((n, self.out_channels, hh, ww), dtype=torch.float32, device=x.device)
-            if enc is not None:
-                _lib.check(L.b200ad_unet_set_encoding(self._h, enc.data_ptr(), enc.shape[1]))
-            _lib.check(L.b200ad_unet_forward(self._h, x.data_ptr(), t.data_ptr(), out.data_ptr(), _lib.stream_ptr()))
+            self._set_encoding(e)
+            _lib.check(self._fn("forward")(self._h, x.data_ptr(), t.data_ptr(), out.data_ptr(), _lib.stream_ptr()))
         return out
 
-    def _backward_train(self, x: torch.Tensor, g: torch.Tensor, enc: Optional[torch.Tensor] = None):
-        L = _lib.lib()
-        g = g.to(torch.float32).contiguous()
-        # torch semantics: gradients accumulate until they are zeroed. p.grad is None (zero_grad(set_to_none=True), the
-        # default) -> start from zero; p.grad still our view (not zeroed, or zeroed in place) -> add to what is there.
-        views = getattr(self, "_grad_views", None)
-        params = [p for p in self.parameters() if p.requires_grad]
-        have = [p.grad is not None for p in params]
-        accumulate = bool(views) and all(have)
-        if any(have) and not accumulate:
-            raise _lib.B200ADError("UNet2DModel(b200): either all parameter gradients are set (accumulate) or none")
-        with torch.cuda.device(x.device):
-            if enc is not None:          # another call may have bound a different encoding since the forward
-                _lib.check(L.b200ad_unet_set_encoding(self._h, enc.data_ptr(), enc.shape[1]))
-            _lib.check(L.b200ad_unet_backward(self._h, x.data_ptr(), g.data_ptr(), 1 if accumulate else 0, _lib.stream_ptr()))
-        if not getattr(self, "_no_sync", False):
-            self._allreduce_gradients()
-        # Parameter gradients are VIEWS of the flat buffer, assigned directly (no 700-tensor clone / accumulate pass).
-        if getattr(self, "_grad_views_key", None) != self._grad_flat.data_ptr():
-            named = self._named()
-            self._grad_views = []
-            for i, k in enumerate(self._pnames):
-                off = L.b200ad_unet_grad_offset(self._h, i)
-                p = named[k]
-                self._grad_views.append((p, self._grad_flat[off:off + p.numel()].view(p.shape)))
-            self._grad_views_key = self._grad_flat.data_ptr()
-        for p, gv in self._grad_views:
-            if p.grad is not None and p.grad.data_ptr() != gv.data_ptr():
-                raise _lib.B200ADError("UNet2DModel(b200): p.grad must be None or the engine's own gradient view")
-            p.grad = gv
-
+    # ------------------------------------------------------------------ data parallel
     def _allreduce_gradients(self) -> None:
         """Data parallel (accelerate's DDP, scripts/train_unet.py:181): mean of the flat gradient buffer over the ranks, ONE
         collective after the backward pass.  It is not overlapped with the backward pass: an all-reduce in four buckets,
@@ -365,7 +221,7 @@ class UNet2DModel(nn.Module):
 
         @contextlib.contextmanager
         def ctx():
-            old = getattr(self, "_no_sync", False)
+            old = self._no_sync
             self._no_sync = True
             try:
                 yield
@@ -373,26 +229,28 @@ class UNet2DModel(nn.Module):
                 self._no_sync = old
         return ctx()
 
-    @property
-    def last_backward_launch_count(self) -> int:
-        return _lib.lib().b200ad_unet_backward_launch_count(self._h)
-
-    @torch.no_grad()
+    # ------------------------------------------------------------------ sampling
     def forward_step(self, sample: torch.Tensor, timestep, coef: StepCoefC, noise: Optional[torch.Tensor] = None,
                      out: Optional[torch.Tensor] = None, want_eps: bool = False):
         """Fused `scheduler.step(unet(sample, t), t, sample)["prev_sample"]` (pipeline_audio_diffusion.py:163-179)."""
+        return self._forward_step(sample, timestep, coef, None, noise, out, want_eps)
+
+    @torch.no_grad()
+    def _forward_step(self, sample: torch.Tensor, timestep, coef: StepCoefC, enc, noise: Optional[torch.Tensor],
+                      out: Optional[torch.Tensor], want_eps: bool):
         x = self._check_input(sample)
         n, _, hh, ww = x.shape
         with torch.cuda.device(x.device):
-            self._fwd_gen += 1
-            self._set_training_mode(False)
-            self._ensure_bound(n, hh, ww)
+            self._fwd_gen[0] += 1
+            self._bind(n, hh, ww, False, x.device)
             t = self._timesteps(timestep, n, x.device)
+            e = self._encoding(enc, n, x.device)
             if out is None:
                 out = torch.empty_like(x)
             eps = torch.empty_like(x) if want_eps else None
             z = noise.to(torch.float32).contiguous() if noise is not None else None
-            _lib.check(_lib.lib().b200ad_unet_forward_step(
+            self._set_encoding(e)
+            _lib.check(self._fn("forward_step")(
                 self._h, x.data_ptr(), t.data_ptr(), z.data_ptr() if z is not None else None, C.byref(coef),
                 out.data_ptr(), eps.data_ptr() if eps is not None else None, _lib.stream_ptr()))
         return (out, eps) if want_eps else out
@@ -408,40 +266,13 @@ class UNet2DModel(nn.Module):
         st = cache.get(key)
         if st is not None:
             with torch.cuda.device(x.device):
-                self._set_training_mode(False)
-                self._ensure_bound(n, hh, ww)
+                self._bind(n, hh, ww, False, x.device)
             if st._bound == (self._packed_key, self._ws_key):
                 st.x.copy_(x)
                 return st
         st = GraphStepper(self, x.clone())
         cache[key] = st
         return st
-
-    def debug_tensor(self, name: str) -> torch.Tensor:
-        """fp32 NCHW copy of a named internal activation of the last forward (parity tests)."""
-        L = _lib.lib()
-        dims = (C.c_int * 3)()
-        _lib.check(min(0, L.b200ad_unet_debug_tensor(self._h, name.encode(), None, dims, _lib.stream_ptr())))
-        n = self._ws_key[0]
-        out = torch.empty((n, dims[0], dims[1], dims[2]), dtype=torch.float32, device=self.device)
-        _lib.check(min(0, L.b200ad_unet_debug_tensor(self._h, name.encode(), out.data_ptr(), dims, _lib.stream_ptr())))
-        return out
-
-    def debug_grad(self, name: str, skip: bool = False) -> torch.Tensor:
-        """fp32 NCHW copy of the last backward's gradient w.r.t. the activation `debug_tensor(name)` (skip=True: the share
-        of it that the skip connection brought) (per-block backward tests)."""
-        L = _lib.lib()
-        dims = (C.c_int * 3)()
-        _lib.check(min(0, L.b200ad_unet_debug_grad(self._h, name.encode(), int(skip), None, dims, _lib.stream_ptr())))
-        n = self._ws_key[0]
-        out = torch.empty((n, dims[0], dims[1], dims[2]), dtype=torch.float32, device=self.device)
-        _lib.check(min(0, L.b200ad_unet_debug_grad(self._h, name.encode(), int(skip), out.data_ptr(), dims,
-                                                   _lib.stream_ptr())))
-        return out
-
-    @property
-    def last_launch_count(self) -> int:
-        return _lib.lib().b200ad_unet_last_launch_count(self._h)
 
 
 class GraphStepper:
@@ -466,9 +297,8 @@ class GraphStepper:
         self.coef = torch.zeros(32, dtype=torch.uint8, device=dev)          # one b200ad_step_coef
         L = _lib.lib()
         with torch.cuda.device(dev), torch.no_grad():
-            model._fwd_gen += 1
-            model._set_training_mode(False)
-            model._ensure_bound(n, hh, ww)
+            model._fwd_gen[0] += 1
+            model._bind(n, hh, ww, False, dev)
             scratch = torch.empty_like(sample)
 
             def enqueue(out):
@@ -498,6 +328,6 @@ class GraphStepper:
                                                              self.t.numel(), _lib.stream_ptr()))
         if noise is not None:
             self.z.copy_(noise)
-        m._fwd_gen += 1
+        m._fwd_gen[0] += 1
         self.graph.replay()
         return self.x

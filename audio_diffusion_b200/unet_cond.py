@@ -16,14 +16,13 @@ reference's encodings are precomputed data), so an encoding with `requires_grad`
 """
 from __future__ import annotations
 
-import ctypes as C
 from typing import Optional, Sequence, Tuple, Union
 
 import torch
 
-from . import _lib
-from ._lib import MAX_BLOCKS, StepCoefC, UNetConfigC
-from .unet import UNet2DModel, UNet2DOutput, _Cfg, _UNetFunction
+from ._lib import MAX_BLOCKS, StepCoefC
+from .engine import _Cfg
+from .unet import UNet2DModel, _unet_config
 
 
 class UNet2DConditionModel(UNet2DModel):
@@ -87,17 +86,8 @@ class UNet2DConditionModel(UNet2DModel):
             block_out_channels=tuple(block_out_channels), layers_per_block=layers_per_block,
             cross_attention_dim=cross_attention_dim, attention_head_dim=attention_head_dim,
             norm_num_groups=norm_num_groups, norm_eps=norm_eps, _class_name="UNet2DConditionModel")
-        c = UNetConfigC()
-        c.in_channels, c.out_channels = in_channels, out_channels
-        c.layers_per_block, c.num_blocks = layers_per_block, len(block_out_channels)
-        for i, v in enumerate(block_out_channels):
-            c.block_out_channels[i] = int(v)
-            c.down_cross[i] = 1 if down_block_types[i] == "CrossAttnDownBlock2D" else 0
-            c.up_cross[i] = 1 if up_block_types[i] == "CrossAttnUpBlock2D" else 0
-        c.norm_num_groups, c.norm_eps = norm_num_groups, norm_eps
-        c.attention_head_dim = heads
-        c.cross_attention_dim = cross_attention_dim
-        self._init_engine(c, seed)
+        self._init_engine(_unet_config(in_channels, out_channels, layers_per_block, block_out_channels, down_block_types,
+                                       up_block_types, norm_num_groups, norm_eps, heads, cross_attention_dim), seed)
 
     def _encoding(self, enc: torch.Tensor, n: int, dev) -> torch.Tensor:
         if enc is None:
@@ -114,55 +104,18 @@ class UNet2DConditionModel(UNet2DModel):
     def forward(self, sample: torch.Tensor, timestep, encoder_hidden_states: torch.Tensor = None, return_dict: bool = True):
         """ε = unet(sample, timestep, encoding)["sample"] — pipeline_audio_diffusion.py:161 (inference) and
         scripts/train_unet.py:255 (training: in train mode with grad enabled, backward() fills the parameter gradients)."""
-        if torch.is_grad_enabled() and self.training and any(p.requires_grad for p in self.parameters()):
+        if self._needs_grad():
             if sample.requires_grad:
                 raise NotImplementedError("UNet2DConditionModel(b200): gradients w.r.t. the input sample are not computed")
             if torch.is_tensor(encoder_hidden_states) and encoder_hidden_states.requires_grad:
                 raise NotImplementedError("UNet2DConditionModel(b200): gradients w.r.t. encoder_hidden_states are not computed "
                                           "(pass precomputed encodings, e.g. .detach())")
-            x = self._check_input(sample)
-            n = x.shape[0]
-            t = self._timesteps(timestep, n, x.device)
-            e = self._encoding(encoder_hidden_states, n, x.device)
-            named = self._named()
-            out = _UNetFunction.apply(self, x, t, e, *[named[k] for k in self._pnames])
-            return UNet2DOutput(out) if return_dict else (out,)
-        x = self._check_input(sample)
-        n, _, hh, ww = x.shape
-        with torch.cuda.device(x.device):
-            self._fwd_gen += 1
-            self._set_training_mode(False)
-            self._ensure_bound(n, hh, ww)
-            t = self._timesteps(timestep, n, x.device)
-            e = self._encoding(encoder_hidden_states, n, x.device)
-            out = torch.empty((n, self.out_channels, hh, ww), dtype=torch.float32, device=x.device)
-            L = _lib.lib()
-            _lib.check(L.b200ad_unet_set_encoding(self._h, e.data_ptr(), e.shape[1]))
-            _lib.check(L.b200ad_unet_forward(self._h, x.data_ptr(), t.data_ptr(), out.data_ptr(), _lib.stream_ptr()))
-        return UNet2DOutput(out) if return_dict else (out,)
+        return self._forward(sample, timestep, encoder_hidden_states, return_dict)
 
-    @torch.no_grad()
     def forward_step(self, sample: torch.Tensor, timestep, coef: StepCoefC, encoder_hidden_states: torch.Tensor = None,
                      noise: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None, want_eps: bool = False):
         """Fused `scheduler.step(unet(sample, t, encoding), t, sample)["prev_sample"]` (pipeline_audio_diffusion.py:161-179)."""
-        x = self._check_input(sample)
-        n, _, hh, ww = x.shape
-        with torch.cuda.device(x.device):
-            self._fwd_gen += 1
-            self._set_training_mode(False)
-            self._ensure_bound(n, hh, ww)
-            t = self._timesteps(timestep, n, x.device)
-            e = self._encoding(encoder_hidden_states, n, x.device)
-            if out is None:
-                out = torch.empty_like(x)
-            eps = torch.empty_like(x) if want_eps else None
-            z = noise.to(torch.float32).contiguous() if noise is not None else None
-            L = _lib.lib()
-            _lib.check(L.b200ad_unet_set_encoding(self._h, e.data_ptr(), e.shape[1]))
-            _lib.check(L.b200ad_unet_forward_step(
-                self._h, x.data_ptr(), t.data_ptr(), z.data_ptr() if z is not None else None, C.byref(coef),
-                out.data_ptr(), eps.data_ptr() if eps is not None else None, _lib.stream_ptr()))
-        return (out, eps) if want_eps else out
+        return self._forward_step(sample, timestep, coef, encoder_hidden_states, noise, out, want_eps)
 
 
 def load_cond_unet(sub: str) -> UNet2DConditionModel:

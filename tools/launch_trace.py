@@ -144,7 +144,7 @@ def vae_train(dev):
         vae_loss(x, y, posterior)[0].backward()
         return y.detach()
     y, seq = traced(step)
-    rec = {"launches": seq, "last_launch_count": vae.last_launch_count, "backward_launch_count": vae.backward_launch_count,
+    rec = {"launches": seq, "last_launch_count": vae.last_launch_count, "backward_launch_count": vae.last_backward_launch_count,
            "backward_bytes": _lib.lib().b200ad_vae_backward_bytes(vae._h)}
     return rec, {"image": y, "grad_flat": vae._grad_flat.clone()}
 

@@ -61,7 +61,7 @@ def engine(batch: int, steps: int, warmup: int = 2):
         y = model.decode(post.sample()).sample
         loss = torch.abs(x - y).sum() / batch + 1e-6 * post.kl().sum() / batch
         loss.backward()
-        launches.append(model.backward_launch_count)
+        launches.append(model.last_backward_launch_count)
         opt.step()
         opt.zero_grad(set_to_none=True)
 
