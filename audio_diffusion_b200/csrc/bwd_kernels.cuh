@@ -65,12 +65,11 @@ cudaError_t launch_mha_bwd(const __nv_bfloat16* qkv, const __nv_bfloat16* o, con
                            float* dsum, __nv_bfloat16* gqkv, int N, int C, int heads, int H, int W, cudaStream_t s);
 
 // Autoencoder layers (vae_bwd_kernels.cu).
-// single-head attention (one head of dim C, S = H * W tokens, S % 64 == 0, C % 64 == 0): qkv and o as the forward read /
-// wrote them, go = dL/do (PF8, C channels), P the forward's softmax (fp32 [N][S][S]) -> gqkv (PF8, 3C channels).
+// single-head attention (one head of dim C, S = H * W tokens, S % 64 == 0, C % 64 == 0): qkv as the forward read it,
+// go = dL/do (PF8, C channels), P the forward's softmax (fp32 [N][S][S]) -> gqkv (PF8, 3C channels).
 // Scratch: D (N * S floats), dS (N * S * S bf16).
-cudaError_t launch_attention_1head_bwd(const __nv_bfloat16* qkv, const __nv_bfloat16* o, const __nv_bfloat16* go,
-                                       const float* P, float* D, __nv_bfloat16* dS, __nv_bfloat16* gqkv, int N, int C, int H,
-                                       int W, cudaStream_t s);
+cudaError_t launch_attention_1head_bwd(const __nv_bfloat16* qkv, const __nv_bfloat16* go, const float* P, float* D,
+                                       __nv_bfloat16* dS, __nv_bfloat16* gqkv, int N, int C, int H, int W, cudaStream_t s);
 // quant_conv (1x1, L2 -> L2) on the first L2 channels of h (PF8, 128 channels), from gm (fp32 [N][L2][H][W]) -> g_h as
 // fp32 [N][L2][H][W] (gh_nc) and [L2][N][H][W] (gh_cn); dwq / dbq accumulated.  L2 <= 8.
 cudaError_t launch_quant_conv_bwd(const float* gm, const __nv_bfloat16* h, const float* wq, float* gh_nc, float* gh_cn,

@@ -280,14 +280,14 @@ struct BwdBuilder {
     wgrad_conv(whole(Gout), whole(ao), n + ".to_out.0.weight", 1);
     bias_grad(whole(Gout), n + ".to_out.0.bias");
     Act Gqkv = tmp("Gqkv", 3 * C, H, W);
-    if (single_head) {   // the forward's softmax P is kept: row dot products, then the dS, dV, dQ, dK GEMMs
+    if (single_head) {   // the forward's softmax P is kept: dP GEMM for the row sums of P o dP, then dS, dV, dQ, dK
       const long long S = (long long)H * W;
       float* D = (float*)mem.take((size_t)N * S * sizeof(float));
       __nv_bfloat16* dS = (__nv_bfloat16*)mem.take((size_t)N * S * S * sizeof(__nv_bfloat16));
-      emit(OP_ATTN1_BWD, [q = qkv.p, o = ao.p, go = T1.p, probs = h->plan.probs.at(n), D, dS, gq = Gqkv.p, N = N, C, H,
+      emit(OP_ATTN1_BWD, [q = qkv.p, go = T1.p, probs = h->plan.probs.at(n), D, dS, gq = Gqkv.p, N = N, C, H,
                           W](const RunArgs&, cudaStream_t s) {
-        return launch_attention_1head_bwd(q, o, go, probs, D, dS, gq, N, C, H, W, s);
-      }, 5);
+        return launch_attention_1head_bwd(q, go, probs, D, dS, gq, N, C, H, W, s);
+      }, 6);
     } else {
       emit(OP_ATTN_BWD, [q = qkv.p, go = T1.p, gq = Gqkv.p, N = N, C, H, W](const RunArgs&, cudaStream_t s) {
         return launch_attention_bwd(q, go, gq, N, C, H, W, s);

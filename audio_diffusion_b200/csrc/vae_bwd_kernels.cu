@@ -12,34 +12,28 @@ __device__ __forceinline__ float warp_sum_v(float v) {
   for (int sh = 16; sh >= 1; sh >>= 1) v += __shfl_xor_sync(0xffffffffu, v, sh);
   return v;
 }
-__device__ __forceinline__ float dot8(const uint4& a, const uint4& b) {
-  const uint32_t ua[4] = {a.x, a.y, a.z, a.w}, ub[4] = {b.x, b.y, b.z, b.w};
-  float s = 0.f;
-#pragma unroll
-  for (int e = 0; e < 4; ++e) {
-    const float2 x = unpack_bf16x2(ua[e]), y = unpack_bf16x2(ub[e]);
-    s = fmaf(x.x, y.x, s);
-    s = fmaf(x.y, y.y, s);
-  }
-  return s;
-}
 }  // namespace
 
 // ---------------------------------------------------------------------------------------------------------------------
 // Single-head attention backward (one head of dim C over S = H*W tokens).  The forward kept P = softmax(scale Q K^T)
-// (fp32 [N][S][S]).  With dO the gradient of the attention output O:
-//   D[q] = sum_c dO[q][c] O[q][c]
-//   dS   = P o (dO V^T - D) * scale       (bf16 [N][S][S] scratch)
+// (fp32 [N][S][S]).  With dO the gradient of the attention output O and dP = dO V^T:
+//   D[q] = sum_k P[q][k] dP[q][k]
+//   dS   = P o (dP - D) * scale           (bf16 [N][S][S] scratch)
 //   dV   = P^T dO,  dQ = dS K,  dK = dS^T Q   -> PF8 gqkv (q | k | v), the layout the q/k/v projections' backward reads.
-// The four GEMMs run on one kernel: CTA tile 64 x 64, K step 32, four warps of 32 x 32 on mma.sync m16n8k16 (bf16
+// D equals sum_c dO[q][c] O[q][c] in exact arithmetic, but formed from the stored bf16 O it does not match the fp32 P and
+// dP that dS is made of: over S = 1024 tokens with a near-uniform P, dP - D cancels to a few percent of dP and O's
+// rounding alone put 1.5 % into the to_q / to_k weight gradients.  So D is summed from P and dP themselves: a first dP
+// GEMM writes each 64-key tile's partial row sums, one pass adds them in a fixed order, and the dS GEMM recomputes dP.
+// The five GEMMs run on one kernel: CTA tile 64 x 64, K step 32, four warps of 32 x 32 on mma.sync m16n8k16 (bf16
 // operands, fp32 accumulation).  Every operand tile is staged in shared memory as [row][k] with k contiguous, so the A
 // and B fragments are plain 32-bit loads; the loaders transpose where the global layout runs the other way.
-enum { A1_DV = 0, A1_DS = 1, A1_DQ = 2, A1_DK = 3 };
+enum { A1_DV = 0, A1_DS = 1, A1_DQ = 2, A1_DK = 3, A1_DP = 4 };
 struct Attn1Bwd {
   const __nv_bfloat16* qkv;   // PF8, 3C channels
   const __nv_bfloat16* go;    // PF8, C channels
   const float* P;
   const float* D;             // [N][S]
+  float* Dp;                  // [N][S][S / 64] partial row sums of P o dP, in the dS scratch until the dS GEMM runs
   __nv_bfloat16* dS;
   __nv_bfloat16* gqkv;        // PF8, 3C channels
   int C, H, W, S;
@@ -47,22 +41,14 @@ struct Attn1Bwd {
 };
 constexpr int A1_BK = 32, A1_LD = A1_BK + 8;   // row pitch 80 B: the fragment loads of a warp hit 32 distinct banks
 
-__global__ void __launch_bounds__(256) attn1_rowdot_kernel(const __nv_bfloat16* __restrict__ o,
-                                                           const __nv_bfloat16* __restrict__ go, float* __restrict__ D,
-                                                           int N, int C, int H, int W) {
-  const Geom g = make_geom(N, H, W);
-  const int S = H * W, lane = threadIdx.x & 31;
-  const int tok = blockIdx.x * 8 + (threadIdx.x >> 5);
-  if (tok >= N * S) return;
-  const int n = tok / S, q = tok - n * S;
-  const long long pix = pf8_pixel(g, q, W);
+// D[token] = the A1_DP partials of its S / 64 key tiles, added in tile order
+__global__ void __launch_bounds__(256) attn1_rowdot_kernel(const float* __restrict__ Dp, float* __restrict__ D, int NS,
+                                                           int tiles) {
+  const int tok = blockIdx.x * 256 + threadIdx.x;
+  if (tok >= NS) return;
   float s = 0.f;
-  for (int pl = lane; pl < C / 8; pl += 32) {
-    const long long off = ((long long)n * (C / 8) + pl) * g.PL * 8 + pix;
-    s += dot8(*reinterpret_cast<const uint4*>(o + off), *reinterpret_cast<const uint4*>(go + off));
-  }
-  s = warp_sum_v(s);
-  if (lane == 0) D[tok] = s;
+  for (int t = 0; t < tiles; ++t) s += Dp[(long long)tok * tiles + t];
+  D[tok] = s;
 }
 
 // X[r][0..7 of vector v] <- 8 channels of token `tok` (rows = tokens, k = channels)
@@ -98,7 +84,7 @@ __global__ void __launch_bounds__(128) attn1_gemm_kernel(const Attn1Bwd a, int N
   const __nv_bfloat16* go = a.go + (long long)n * planes * g.PL * 8;
   const float* P = a.P + (long long)n * S * S;
   __nv_bfloat16* dS = a.dS + (long long)n * S * S;
-  const int K = MODE == A1_DS ? C : S;
+  const int K = MODE == A1_DS || MODE == A1_DP ? C : S;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, gr = lane >> 2, tq = lane & 3;
   const int wm = (warp >> 1) * 32, wn = (warp & 1) * 32;
   float acc[2][4][4] = {};
@@ -113,7 +99,7 @@ __global__ void __launch_bounds__(128) attn1_gemm_kernel(const Attn1Bwd a, int N
         As[4 * j + 3][q] = __float2bfloat16_rn(f.w);
       }
       a1_cols_pf8(Bs, go, g, W, k0, n0);
-    } else if (MODE == A1_DS) {   // A[q][c] = dO[q][c];  B[key][c] = V[key][c]
+    } else if (MODE == A1_DS || MODE == A1_DP) {   // A[q][c] = dO[q][c];  B[key][c] = V[key][c]
       a1_rows_pf8(As, go, g, W, m0, k0);
       a1_rows_pf8(Bs, qkv + (long long)2 * planes * g.PL * 8, g, W, n0, k0);
     } else if (MODE == A1_DQ) {   // A[q][key] = dS[q][key];  B[c][key] = K[key][c]
@@ -158,6 +144,28 @@ __global__ void __launch_bounds__(128) attn1_gemm_kernel(const Attn1Bwd a, int N
     __syncthreads();
   }
   // epilogue: lane holds rows (gr, gr + 8) x columns (2 tq, 2 tq + 1) of every 16 x 8 tile
+  if (MODE == A1_DP) {   // sum over this tile's 64 keys of P dP per row: lanes of one row, then the two column warps
+    __shared__ float red[2][64];
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int r = wm + i * 16 + gr + 8 * h;
+        float s = 0.f;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const float2 p = *reinterpret_cast<const float2*>(P + (long long)(m0 + r) * S + n0 + wn + j * 8 + 2 * tq);
+          s += p.x * acc[i][j][2 * h] + p.y * acc[i][j][2 * h + 1];
+        }
+        s += __shfl_xor_sync(0xffffffffu, s, 1);
+        s += __shfl_xor_sync(0xffffffffu, s, 2);
+        if (tq == 0) red[warp & 1][r] = s;
+      }
+    __syncthreads();
+    if (threadIdx.x < 64)
+      a.Dp[((long long)n * S + m0 + threadIdx.x) * (S / 64) + blockIdx.x] = red[0][threadIdx.x] + red[1][threadIdx.x];
+    return;
+  }
   const float* D = a.D + (long long)n * S;
   __nv_bfloat16* gout = a.gqkv + ((long long)n * 3 * planes + (MODE == A1_DV ? 2 * planes : MODE == A1_DK ? planes : 0)) *
                                      g.PL * 8;
@@ -182,15 +190,16 @@ __global__ void __launch_bounds__(128) attn1_gemm_kernel(const Attn1Bwd a, int N
       }
 }
 
-cudaError_t launch_attention_1head_bwd(const __nv_bfloat16* qkv, const __nv_bfloat16* o, const __nv_bfloat16* go,
-                                       const float* P, float* D, __nv_bfloat16* dS, __nv_bfloat16* gqkv, int N, int C, int H,
-                                       int W, cudaStream_t s) {
+cudaError_t launch_attention_1head_bwd(const __nv_bfloat16* qkv, const __nv_bfloat16* go, const float* P, float* D,
+                                       __nv_bfloat16* dS, __nv_bfloat16* gqkv, int N, int C, int H, int W, cudaStream_t s) {
   const int S = H * W;
   if (S % 64 || C % 64) return cudaErrorInvalidValue;
-  attn1_rowdot_kernel<<<(N * S + 7) / 8, 256, 0, s>>>(o, go, D, N, C, H, W);
+  Attn1Bwd a{qkv, go, P, D, reinterpret_cast<float*>(dS), dS, gqkv, C, H, W, S, rsqrtf((float)C)};
+  attn1_gemm_kernel<A1_DP><<<dim3(S / 64, S / 64, N), 128, 0, s>>>(a, N);   // partial row sums of P o dP
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;
-  Attn1Bwd a{qkv, go, P, D, dS, gqkv, C, H, W, S, rsqrtf((float)C)};
+  attn1_rowdot_kernel<<<(N * S + 255) / 256, 256, 0, s>>>(a.Dp, D, N * S, S / 64);
+  if ((e = cudaGetLastError()) != cudaSuccess) return e;
   attn1_gemm_kernel<A1_DS><<<dim3(S / 64, S / 64, N), 128, 0, s>>>(a, N);   // dS first: dQ and dK read it
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
   attn1_gemm_kernel<A1_DV><<<dim3(C / 64, S / 64, N), 128, 0, s>>>(a, N);

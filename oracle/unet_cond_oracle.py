@@ -191,10 +191,10 @@ def unet_cond_forward(w: Dict[str, torch.Tensor], cfg: CondUNetConfig, sample: t
     g, eps = cfg.norm_num_groups, cfg.norm_eps
     t = timestep
     if not torch.is_tensor(t):
-        t = torch.tensor([t], dtype=torch.long)
+        t = torch.tensor([t], dtype=torch.long, device=sample.device)
     elif t.ndim == 0:
         t = t[None]
-    t = t * torch.ones(sample.shape[0], dtype=t.dtype)
+    t = t * torch.ones(sample.shape[0], dtype=t.dtype, device=t.device)
     emb = timestep_embedding(t, boc[0]).to(sample.dtype)
     emb = F.linear(F.silu(F.linear(emb, w["time_embedding.linear_1.weight"], w["time_embedding.linear_1.bias"])),
                    w["time_embedding.linear_2.weight"], w["time_embedding.linear_2.bias"])

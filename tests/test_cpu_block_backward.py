@@ -35,10 +35,10 @@ def _check_params(grads, ref, expect):
     assert worst[0] < 1e-9      # fp64 rounding; a wrong decomposition or skip share is off by O(1)
 
 
-def _unet_case(size, n, seed):
+def _unet_case(size, n, seed, arch=TRAIN_CFG):
     from oracle.schedulers_oracle import OracleDDPM
     from oracle.unet_oracle import UNetConfig, init_weights, unet_forward
-    cfg = UNetConfig(sample_size=size, **TRAIN_CFG)
+    cfg = UNetConfig(sample_size=size, **arch)
     w = _d(init_weights(cfg, seed=seed))
     g = torch.Generator().manual_seed(seed + 1)
     clean = (torch.rand(n, 1, *size, generator=g) * 2 - 1).double()
@@ -60,29 +60,60 @@ def test_unet_block_chain_reproduces_autograd():
     _check_params(grads, ref, [k for k in w if not k.startswith("time_embedding.")])
 
 
-def test_cond_unet_block_chain_reproduces_autograd():
+def _cond_chain(cfg_kw, size, n, transformers):
+    """The conditional U-Net's block references chained over the oracle's activations against whole-model autograd."""
     from oracle.schedulers_oracle import OracleDDPM
     from oracle.unet_cond_oracle import CondUNetConfig, init_weights, unet_cond_forward
-    cfg = CondUNetConfig(sample_size=(16, 16), **COND_CFG)
+    cfg = CondUNetConfig(sample_size=size, **cfg_kw)
     w = _d(init_weights(cfg, seed=3))
     g = torch.Generator().manual_seed(4)
-    clean = (torch.rand(3, 1, 16, 16, generator=g) * 2 - 1).double()
-    noise = torch.randn(3, 1, 16, 16, generator=g).double()
-    enc = torch.randn(3, 1, 100, generator=g).double()
-    noisy = OracleDDPM().add_noise(clean, noise, T3)
+    clean = (torch.rand(n, 1, *size, generator=g) * 2 - 1).double()
+    noise = torch.randn(n, 1, *size, generator=g).double()
+    enc = torch.randn(n, 1, 100, generator=g).double()
+    t = T3[:n]
+    noisy = OracleDDPM().add_noise(clean, noise, t)
     wl = {k: v.clone().requires_grad_(True) for k, v in w.items()}
-    pred = unet_cond_forward(wl, cfg, noisy, T3, enc)
+    pred = unet_cond_forward(wl, cfg, noisy, t, enc)
     ref = dict(zip(wl, torch.autograd.grad(((pred - noise) ** 2).mean(), list(wl.values()), allow_unused=True)))
     taps = {}
-    pred = unet_cond_forward(w, cfg, noisy, T3, enc, taps)
+    pred = unet_cond_forward(w, cfg, noisy, t, enc, taps)
     blocks = bg.unet_blocks(cfg)
-    assert sum(b.kind == "transformer" for b in blocks) == 6
-    _, grads, _ = bg.chain(blocks, taps, noisy, 2 * (pred - noise) / pred.numel(), w, cfg, bg.temb_act(w, cfg, T3), enc)
+    assert sum(b.kind == "transformer" for b in blocks) == transformers
+    _, grads, _ = bg.chain(blocks, taps, noisy, 2 * (pred - noise) / pred.numel(), w, cfg, bg.temb_act(w, cfg, t), enc)
     for k in grads:      # attn2.to_q / to_k and norm2 do not reach the output: exactly zero
         if ref[k] is None:
             ref[k] = torch.zeros_like(w[k])
             assert torch.count_nonzero(grads[k]) == 0, k
     _check_params(grads, ref, [k for k in w if not k.startswith("time_embedding.")])
+
+
+def test_cond_unet_block_chain_reproduces_autograd():
+    _cond_chain(COND_CFG, (16, 16), 3, 6)
+
+
+@pytest.mark.timeout(300)
+def test_published_unet_block_chain_reproduces_autograd():
+    """The six-level UNet2DModel the GPU tests train at 64x64 and 256x256: attention at down block 4 and up block 1, skip
+    connections across six levels, at 64x64 so that the last level is 2x2."""
+    from oracle.train_oracle import loss_and_grads
+    from test_gpu_fullconfig import REF_ARCH
+    cfg, w, clean, noise, t, noisy, taps, g_eps = _unet_case((64, 64), 2, 2, REF_ARCH)
+    _, ref, _ = loss_and_grads(w, cfg, clean, noise, t)
+    blocks = bg.unet_blocks(cfg)
+    assert [b.name for b in blocks if b.kind == "attn"] == (
+        ["down_blocks.4.attentions.0", "down_blocks.4.attentions.1", "mid_block.attentions.0"]
+        + [f"up_blocks.1.attentions.{j}" for j in range(3)])
+    assert sum(b.skip is not None for b in blocks) == 6 * 3
+    _, grads, _ = bg.chain(blocks, taps, noisy, g_eps, w, cfg, taps["temb_act"])
+    _check_params(grads, ref, [k for k in w if not k.startswith("time_embedding.")])
+
+
+@pytest.mark.timeout(300)
+def test_published_cond_unet_block_chain_reproduces_autograd():
+    """The four-level UNet2DConditionModel the GPU tests train at 64x64 (transformers in three down and three up blocks
+    and the mid block), at 32x32."""
+    from test_gpu_cond_train import ARCH
+    _cond_chain({k: ARCH[k] for k in ("block_out_channels", "down_block_types", "up_block_types")}, (32, 32), 2, 16)
 
 
 def test_vae_block_chain_reproduces_autograd():
