@@ -14,6 +14,13 @@ the decomposition reproduces autograd through the whole model.
 `bf16_storage()` rounds, inside a reference, every conv / linear operand, weight and output to bf16 and every gradient
 that flows back through those operands and outputs: the points where the engine stores a tensor or a gradient in bf16.
 Comparing a reference run under it with the exact one gives the bf16 floor of a block's gradients.
+
+The forward: `block_forward` is the same `_forward` evaluated in fp64 without autograd; `sub_forward` splits a resnet, an
+attention block and a transformer into the steps whose outputs the engine keeps as taps (`.h1`; `.qkv`, `.ao`; `.h0` ..
+`.h3`), each step computed from the given values of the steps before it, so that a per-step comparison on the engine's
+own taps pins an error to one step.  tests/test_cpu_block_forward.py shows that both restate the model.  Their rounded
+forms add the bf16 points only the forward has (bf16_storage(forward=True), the stored outputs), which give the forward
+floors; the backward floors do not use them.
 """
 from __future__ import annotations
 
@@ -180,11 +187,25 @@ class _Store(torch.autograd.Function):
         return (bf16(g) if ctx.bwd else g), None, None
 
 
+def _softmax_bf16_probs(x, dim=-1, **_):
+    """softmax whose numerators exp(s - max) are rounded to bf16 while the denominator sums them exact: the P.V MMA of
+    attention_mma_kernel (csrc/small_ops.cu) and mha_flash_kernel (csrc/cond_ops.cu) reads the unnormalised exp(S) packed
+    to bf16 and divides by the fp32 row sum afterwards."""
+    e = torch.exp(x - x.amax(dim, keepdim=True))
+    return bf16(e) / e.sum(dim, keepdim=True)
+
+
 @contextlib.contextmanager
-def bf16_storage():
+def bf16_storage(forward: bool = False, bf16_probs: bool = False):
     """Inside: conv / linear operands and outputs are stored in bf16 both ways, weights are bf16 (their gradients are not
-    rounded: the engine accumulates them in fp32).  Linear layers over [N, D] vectors (the time embedding) stay exact."""
-    conv, lin = F.conv2d, F.linear
+    rounded: the engine accumulates them in fp32).  Linear layers over [N, D] vectors (the time embedding) stay exact.
+
+    forward: also the bf16 roundings only the forward makes (the forward floors; the backward floors leave it off):
+    conv_out's weights over a wide input are bf16 (conv_out_kernel in csrc/elementwise.cu builds bf16 MMA fragments from
+    them; the autoencoder's encoder conv_out runs on conv_tc_kernel with packed bf16 weights).  bf16_probs: the attention
+    probabilities' numerators are bf16 (_softmax_bf16_probs); the SIMT attention_kernel and the single-head attention keep
+    fp32 probabilities."""
+    conv, lin, smax = F.conv2d, F.linear, torch.softmax
     st = lambda t: _Store.apply(t, True, True)
     wq = lambda t: _Store.apply(t, True, False)
 
@@ -194,20 +215,25 @@ def bf16_storage():
         # stored in bf16 (the autoencoder's encoder tail reads it back for quant_conv's weight gradient)
         if min(wt.shape[:2]) <= 4:
             a = a if wt.shape[1] <= 4 else st(a)
+            if forward and wt.shape[1] > 4:
+                wt = wq(wt)
             y = conv(a, wt, b, *args, **kw)
             return st(y) if wt.shape[0] > 4 else y if wt.shape[1] <= 4 else _Store.apply(y, True, False)
         return st(conv(st(a), wq(wt), b, *args, **kw))
 
     def l(a, wt, b=None):
-        if a.dim() == 2:
+        # forward: the cross-attention over a one-token encoding is a per-sample vector in fp32 (cross_attn_vec_kernel)
+        if a.dim() == 2 or (forward and a.shape[-2] == 1):
             return lin(a, wt, b)
         return st(lin(st(a), wq(wt), b))
 
     F.conv2d, F.linear = c, l
+    if bf16_probs:
+        torch.softmax = _softmax_bf16_probs
     try:
         yield
     finally:
-        F.conv2d, F.linear = conv, lin
+        F.conv2d, F.linear, torch.softmax = conv, lin, smax
 
 
 def block_backward(blk: Block, w: Dict[str, torch.Tensor], xs: Sequence[torch.Tensor], gout: torch.Tensor, cfg,
@@ -230,6 +256,158 @@ def block_backward(blk: Block, w: Dict[str, torch.Tensor], xs: Sequence[torch.Te
     if rounded:
         gi = [bf16(g) for g in gi]
     return gi, dict(zip(pw.keys(), gr[len(xl):]))
+
+
+def _probs_rounded(blk: Block, x: torch.Tensor) -> bool:
+    """Whether the block's attention core packs its probabilities to bf16 (launch_attention picks attention_mma_kernel
+    for seq % 16 == 0 and seq <= 1536; the transformers always run mha_flash_kernel)."""
+    seq = x.shape[2] * x.shape[3]
+    return blk.kind == "transformer" or (blk.kind == "attn" and seq % 16 == 0 and seq * 32 <= 48 * 1024)
+
+
+def _stored(blk: Block, t: torch.Tensor) -> torch.Tensor:
+    """The value as the engine stores the block's output: bf16, except the model outputs (eps, image, moments: fp32)."""
+    return t if blk.kind in ("tail", "enc_tail") else bf16(t)
+
+
+@torch.no_grad()
+def block_forward(blk: Block, w: Dict[str, torch.Tensor], xs: Sequence[torch.Tensor], cfg,
+                  temb_act: Optional[torch.Tensor] = None, enc: Optional[torch.Tensor] = None, rounded: bool = False):
+    """fp64 forward of one block from its inputs xs ([input] or [input, skip]): the `_forward` that block_backward
+    differentiates.  rounded: under bf16_storage(forward=True) with the forward's own bf16 points, output stored as the
+    engine stores it."""
+    dev = xs[0].device
+    d = lambda t: None if t is None else t.detach().to(device=dev, dtype=torch.float64)
+    pw = {k: d(v) for k, v in w.items() if k.startswith(blk.prefixes)}
+    xl = [d(x) for x in xs]
+    if not rounded:
+        return _forward(blk, pw, xl, cfg, d(temb_act), d(enc))
+    with bf16_storage(forward=True, bf16_probs=_probs_rounded(blk, xl[0])):
+        return _stored(blk, _forward(blk, pw, xl, cfg, d(temb_act), d(enc)))
+
+
+def _lnc(x, w, p, eps=1e-5):
+    """LayerNorm over the channels of an NCHW tensor."""
+    return F.layer_norm(x.permute(0, 2, 3, 1), (x.shape[1],), w[p + ".weight"], w[p + ".bias"], eps).permute(0, 3, 1, 2)
+
+
+def _c1(x, wt, b=None):
+    """A linear layer over the pixel tokens of an NCHW tensor (the engine's 1-tap conv)."""
+    return F.conv2d(x, wt[:, :, None, None] if wt.dim() == 2 else wt, b)
+
+
+def _attn_core(qkv, heads, bf16_probs):
+    """softmax(q k^T / sqrt(d)) v per head over the pixel tokens of the q | k | v tensor [N, 3C, H, W] -> [N, C, H, W]."""
+    n, c3, hh, ww = qkv.shape
+    c = c3 // 3
+    q, k, v = (t.reshape(n, heads, c // heads, hh * ww).transpose(-1, -2) for t in qkv.split(c, dim=1))
+    s = (q @ k.transpose(-1, -2)) * (c // heads) ** -0.5
+    p = _softmax_bf16_probs(s) if bf16_probs else torch.softmax(s, dim=-1)
+    return (p @ v).transpose(-1, -2).reshape(n, c, hh, ww)
+
+
+def _stages(blk: Block, w, x, cfg, temb_act, enc, bf16_probs):
+    """The sub-block steps of a block as (tap suffix, step) pairs in order; a step maps the values so far (by suffix; ""
+    is the block input, "out" the output) to its own value.  Sub-taps the engine exposes are exactly these suffixes."""
+    n = blk.name
+    G = cfg.norm_num_groups
+    if blk.kind in ("resnet", "resnet_vae"):
+        eps = cfg.norm_eps if blk.kind == "resnet" else vo.EPS
+
+        def h1(v):
+            h = F.conv2d(F.silu(F.group_norm(v[""], G, w[n + ".norm1.weight"], w[n + ".norm1.bias"], eps)),
+                         w[n + ".conv1.weight"], w[n + ".conv1.bias"], padding=1)
+            if temb_act is not None and n + ".time_emb_proj.weight" in w:
+                h = h + F.linear(temb_act, w[n + ".time_emb_proj.weight"], w[n + ".time_emb_proj.bias"])[:, :, None, None]
+            return h
+
+        def out(v):
+            h = F.silu(F.group_norm(v[".h1"], G, w[n + ".norm2.weight"], w[n + ".norm2.bias"], eps))
+            h = F.conv2d(h, w[n + ".conv2.weight"], w[n + ".conv2.bias"], padding=1)
+            sc = v[""]
+            if n + ".conv_shortcut.weight" in w:
+                sc = F.conv2d(sc, w[n + ".conv_shortcut.weight"], w[n + ".conv_shortcut.bias"])
+            return sc + h
+        return [(".h1", h1), ("out", out)]
+    if blk.kind in ("attn", "attn1"):
+        eps = cfg.norm_eps if blk.kind == "attn" else vo.EPS
+        heads = x.shape[1] // cfg.attention_head_dim if blk.kind == "attn" else 1
+
+        def qkv(v):
+            h = F.group_norm(v[""], G, w[n + ".group_norm.weight"], w[n + ".group_norm.bias"], eps)
+            wt = torch.cat([w[n + ".to_q.weight"], w[n + ".to_k.weight"], w[n + ".to_v.weight"]])
+            return _c1(h, wt, torch.cat([w[n + ".to_q.bias"], w[n + ".to_k.bias"], w[n + ".to_v.bias"]]))
+        return [(".qkv", qkv), (".ao", lambda v: _attn_core(v[".qkv"], heads, bf16_probs)),
+                ("out", lambda v: _c1(v[".ao"], w[n + ".to_out.0.weight"], w[n + ".to_out.0.bias"]) + v[""])]
+    if blk.kind == "transformer":
+        t = n + ".transformer_blocks.0"
+        heads = cfg.attention_head_dim
+
+        def attn2(v):
+            h = _c1(v[".ao"], w[t + ".attn1.to_out.0.weight"], w[t + ".attn1.to_out.0.bias"]) + v[".h0"]
+            b, c, hh, ww = h.shape
+            tok = h.permute(0, 2, 3, 1).reshape(b, hh * ww, c)
+            n2 = F.layer_norm(tok, (c,), w[t + ".norm2.weight"], w[t + ".norm2.bias"], 1e-5)
+            a = uco._mha(F.linear(n2, w[t + ".attn2.to_q.weight"]), F.linear(enc, w[t + ".attn2.to_k.weight"]),
+                         F.linear(enc, w[t + ".attn2.to_v.weight"]), heads)
+            a = F.linear(a, w[t + ".attn2.to_out.0.weight"], w[t + ".attn2.to_out.0.bias"])
+            return h + a.reshape(b, hh, ww, c).permute(0, 3, 1, 2)
+
+        def gg(v):
+            u, gate = v[".ff1"].chunk(2, dim=1)
+            return u * F.gelu(gate)
+        return [
+            (".h0", lambda v: _c1(F.group_norm(v[""], G, w[n + ".norm.weight"], w[n + ".norm.bias"], 1e-6),
+                                  w[n + ".proj_in.weight"], w[n + ".proj_in.bias"])),
+            (".n1", lambda v: _lnc(v[".h0"], w, t + ".norm1")),
+            (".qkv", lambda v: _c1(v[".n1"], torch.cat([w[t + f".attn1.to_{p}.weight"] for p in "qkv"]))),
+            (".ao", lambda v: _attn_core(v[".qkv"], heads, bf16_probs)),
+            (".attn2", attn2),
+            (".n3", lambda v: _lnc(v[".attn2"], w, t + ".norm3")),
+            (".ff1", lambda v: _c1(v[".n3"], w[t + ".ff.net.0.proj.weight"], w[t + ".ff.net.0.proj.bias"])),
+            (".gg", gg),
+            (".h3", lambda v: _c1(v[".gg"], w[t + ".ff.net.2.weight"], w[t + ".ff.net.2.bias"]) + v[".attn2"]),
+            ("out", lambda v: _c1(v[".h3"], w[n + ".proj_out.weight"], w[n + ".proj_out.bias"]) + v[""]),
+        ]
+    return [("out", lambda v: _forward(blk, w, [v[""]], cfg, temb_act, enc))]
+
+
+# the sub-taps the engine keeps in eval mode (training keeps every one of a transformer's)
+EVAL_SUBTAPS = {"resnet": (".h1",), "resnet_vae": (".h1",), "attn": (".qkv", ".ao"), "attn1": (".qkv", ".ao"),
+                "transformer": (".attn2",)}
+
+
+@torch.no_grad()
+def sub_forward(blk: Block, w: Dict[str, torch.Tensor], xs: Sequence[torch.Tensor], cfg,
+                temb_act: Optional[torch.Tensor] = None, enc: Optional[torch.Tensor] = None, get=None,
+                taps: Optional[Sequence[str]] = None, rounded: bool = False) -> Dict[str, torch.Tensor]:
+    """fp64 references of a block's sub-taps and output, each step computed from the given values of the steps before it:
+    get(suffix) for the suffixes in `taps` (the engine's own sub-taps, so that an error is pinned to one step; default:
+    those the engine keeps in eval mode, "all": every step), the reference's own value of the steps the engine does not
+    expose.  Returns {suffix: reference} for the suffixes in taps
+    and "out".  rounded: every step under bf16_storage(forward=True) and stored in bf16, as the engine stores them."""
+    dev = xs[0].device
+    d = lambda t: None if t is None else t.detach().to(device=dev, dtype=torch.float64)
+    pw = {k: d(v) for k, v in w.items() if k.startswith(blk.prefixes)}
+    xl = [d(x) for x in xs]
+    x = torch.cat(xl, dim=1) if len(xl) > 1 else xl[0]
+    probs = _probs_rounded(blk, x)
+    vals = {"": x}
+    res = {}
+    with bf16_storage(forward=True, bf16_probs=probs) if rounded else contextlib.nullcontext():
+        steps = _stages(blk, pw, x, cfg, d(temb_act), d(enc), probs and rounded)
+        if taps is None:
+            taps = EVAL_SUBTAPS.get(blk.kind, ())
+        elif taps == "all":
+            taps = [s for s, _ in steps[:-1]]
+        for name, fn in steps:
+            y = fn(vals)
+            if rounded:
+                y = _stored(blk, y) if name == "out" else bf16(y)
+            if name in taps or name == "out":
+                res[name] = y
+            vals[name] = d(get(name)) if get is not None and name in taps else y
+    return res
 
 
 def chain(blocks: Sequence[Block], acts: Dict[str, torch.Tensor], model_in: torch.Tensor, g_out: torch.Tensor, w, cfg,

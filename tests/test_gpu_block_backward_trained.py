@@ -32,6 +32,8 @@ import torch
 from oracle import block_grads as bg
 from test_cpu_block_backward import _floors
 from test_gpu_block_backward import _run_checks, _w64
+from test_gpu_block_forward import _floors as _fwd_floors
+from test_gpu_block_forward import check_against_floors, forward_checks
 from test_gpu_cond_train import ARCH as COND_ARCH
 from test_gpu_fullconfig import REF_ARCH
 
@@ -77,6 +79,84 @@ COND64_BARS = {
     "tail": ((0.0072, 0.0117, 0.0066), (0.005, 0.005, 0.005)),   # floor (0.0024, 0.0039, 0.0022) | (0.0002, 0.0003, 0.0002)
 }
 
+# the training forward (no timestep dedupe; every transformer tap kept: .h0, .n1, .qkv, .ao, .attn2, .n3, .ff1, .gg, .h3),
+# block by block on the same run's activations as tests/test_gpu_block_forward.py checks the eval forward, bars by its
+# rule: key -> (a, b, c), three times the floor printed beside it.  The fp64 times in the docstrings below include this
+# work (measured with it: 256x256 11.3 s, 64x64 1.9 s, autoencoder 3.9 s, conditional 2.8 s; peak memory unchanged).
+UNET256_FWD_BARS = {
+    "attn": (0.00735, 0.01269, 0.00768),   # floor (0.00245, 0.00423, 0.00256)
+    "attn.ao": (0.0051, 0.01056, 0.00561),   # floor (0.0017, 0.00352, 0.00187)
+    "attn.out": (0.00636, 0.01224, 0.00678),   # floor (0.00212, 0.00408, 0.00226)
+    "attn.qkv": (0.00882, 0.01251, 0.00873),   # floor (0.00294, 0.00417, 0.00291)
+    "down": (0.00732, 0.01041, 0.00777),   # floor (0.00244, 0.00347, 0.00259)
+    "head": (0.00498, 0.00606, 0.00462),   # floor (0.00166, 0.00202, 0.00154)
+    "resnet": (0.01299, 0.01983, 0.01371),   # floor (0.00433, 0.00661, 0.00457)
+    "resnet.h1": (0.0102, 0.02118, 0.01125),   # floor (0.0034, 0.00706, 0.00375)
+    "resnet.out": (0.01017, 0.01722, 0.01053),   # floor (0.00339, 0.00574, 0.00351)
+    "tail": (0.00924, 0.01008, 0.00885),   # floor (0.00308, 0.00336, 0.00295)
+    "up": (0.00732, 0.01131, 0.00795),   # floor (0.00244, 0.00377, 0.00265)
+    "resnet.h1:mean": (0.01971, 0.01971, 0.01971),   # floor (0.00657, 0.00657, 0.00657)
+}
+UNET64_FWD_BARS = {
+    "attn": (0.00726, 0.01038, 0.00825),   # floor (0.00242, 0.00346, 0.00275)
+    "attn.ao": (0.00549, 0.01044, 0.00612),   # floor (0.00183, 0.00348, 0.00204)
+    "attn.out": (0.00621, 0.00981, 0.00699),   # floor (0.00207, 0.00327, 0.00233)
+    "attn.qkv": (0.00876, 0.01242, 0.00939),   # floor (0.00292, 0.00414, 0.00313)
+    "down": (0.00729, 0.01041, 0.00864),   # floor (0.00243, 0.00347, 0.00288)
+    "head": (0.00498, 0.00738, 0.00468),   # floor (0.00166, 0.00246, 0.00156)
+    "resnet": (0.01287, 0.018, 0.01503),   # floor (0.00429, 0.006, 0.00501)
+    "resnet.h1": (0.01032, 0.01965, 0.01197),   # floor (0.00344, 0.00655, 0.00399)
+    "resnet.out": (0.01002, 0.01725, 0.01098),   # floor (0.00334, 0.00575, 0.00366)
+    "tail": (0.0084, 0.01176, 0.00771),   # floor (0.0028, 0.00392, 0.00257)
+    "up": (0.00723, 0.01044, 0.00846),   # floor (0.00241, 0.00348, 0.00282)
+    "resnet.h1:mean": (0.02574, 0.02574, 0.02574),   # floor (0.00858, 0.00858, 0.00858)
+}
+VAE256_FWD_BARS = {
+    "decoder:attn1": (0.00579, 0.00942, 0.00579),   # floor (0.00193, 0.00314, 0.00193)
+    "decoder:attn1.ao": (0.00495, 0.00906, 0.00531),   # floor (0.00165, 0.00302, 0.00177)
+    "decoder:attn1.out": (0.00549, 0.00954, 0.00528),   # floor (0.00183, 0.00318, 0.00176)
+    "decoder:attn1.qkv": (0.00876, 0.00993, 0.0087),   # floor (0.00292, 0.00331, 0.0029)
+    "decoder:dec_head": (0.00498, 0.00594, 0.00462),   # floor (0.00166, 0.00198, 0.00154)
+    "decoder:resnet_vae": (0.01233, 0.01788, 0.0135),   # floor (0.00411, 0.00596, 0.0045)
+    "decoder:resnet_vae.h1": (0.00888, 0.01377, 0.00966),   # floor (0.00296, 0.00459, 0.00322)
+    "decoder:resnet_vae.out": (0.00993, 0.01434, 0.01068),   # floor (0.00331, 0.00478, 0.00356)
+    "decoder:tail": (0.00711, 0.00951, 0.00711),   # floor (0.00237, 0.00317, 0.00237)
+    "decoder:up": (0.00711, 0.01098, 0.00729),   # floor (0.00237, 0.00366, 0.00243)
+    "encoder:attn1": (0.00588, 0.0084, 0.00591),   # floor (0.00196, 0.0028, 0.00197)
+    "encoder:attn1.ao": (0.00504, 0.00975, 0.00513),   # floor (0.00168, 0.00325, 0.00171)
+    "encoder:attn1.out": (0.00555, 0.00861, 0.00528),   # floor (0.00185, 0.00287, 0.00176)
+    "encoder:attn1.qkv": (0.00879, 0.01089, 0.00843),   # floor (0.00293, 0.00363, 0.00281)
+    "encoder:down_asym": (0.00714, 0.00951, 0.00798),   # floor (0.00238, 0.00317, 0.00266)
+    "encoder:enc_tail": (0.00501, 0.00756, 0.00501),   # floor (0.00167, 0.00252, 0.00167)
+    "encoder:head": (0.00498, 0.01062, 0.00459),   # floor (0.00166, 0.00354, 0.00153)
+    "encoder:resnet_vae": (0.01287, 0.01719, 0.01281),   # floor (0.00429, 0.00573, 0.00427)
+    "encoder:resnet_vae.h1": (0.00885, 0.01176, 0.00915),   # floor (0.00295, 0.00392, 0.00305)
+    "encoder:resnet_vae.out": (0.0099, 0.01554, 0.00963),   # floor (0.0033, 0.00518, 0.00321)
+    "decoder:resnet_vae.h1:mean": (0.01281, 0.01281, 0.01281),   # floor (0.00427, 0.00427, 0.00427)
+    "encoder:resnet_vae.h1:mean": (0.01101, 0.01101, 0.01101),   # floor (0.00367, 0.00367, 0.00367)
+}
+COND64_FWD_BARS = {
+    "down": (0.00714, 0.01077, 0.00771),   # floor (0.00238, 0.00359, 0.00257)
+    "head": (0.00498, 0.0069, 0.00465),   # floor (0.00166, 0.0023, 0.00155)
+    "resnet": (0.0123, 0.01875, 0.01332),   # floor (0.0041, 0.00625, 0.00444)
+    "resnet.h1": (0.01023, 0.02082, 0.01131),   # floor (0.00341, 0.00694, 0.00377)
+    "resnet.out": (0.00987, 0.01749, 0.01062),   # floor (0.00329, 0.00583, 0.00354)
+    "tail": (0.00915, 0.01083, 0.00915),   # floor (0.00305, 0.00361, 0.00305)
+    "transformer": (0.01047, 0.01485, 0.01155),   # floor (0.00349, 0.00495, 0.00385)
+    "transformer.ao": (0.00507, 0.01125, 0.00564),   # floor (0.00169, 0.00375, 0.00188)
+    "transformer.attn2": (0.00702, 0.01137, 0.01086),   # floor (0.00234, 0.00379, 0.00362)
+    "transformer.ff1": (0.00726, 0.01233, 0.00765),   # floor (0.00242, 0.00411, 0.00255)
+    "transformer.gg": (0.00495, 0.009, 0.00498),   # floor (0.00165, 0.003, 0.00166)
+    "transformer.h0": (0.00885, 0.01302, 0.00993),   # floor (0.00295, 0.00434, 0.00331)
+    "transformer.h3": (0.00522, 0.00831, 0.00516),   # floor (0.00174, 0.00277, 0.00172)
+    "transformer.n1": (0.00501, 0.01014, 0.00483),   # floor (0.00167, 0.00338, 0.00161)
+    "transformer.n3": (0.00501, 0.01062, 0.00477),   # floor (0.00167, 0.00354, 0.00159)
+    "transformer.out": (0.00738, 0.01272, 0.00768),   # floor (0.00246, 0.00424, 0.00256)
+    "transformer.qkv": (0.00732, 0.01146, 0.00747),   # floor (0.00244, 0.00382, 0.00249)
+    "up": (0.00708, 0.00939, 0.00789),   # floor (0.00236, 0.00313, 0.00263)
+    "resnet.h1:mean": (0.01806, 0.01806, 0.01806),   # floor (0.00602, 0.00602, 0.00602)
+}
+
 
 def _report(name, floors, bars, t0):
     """Prints the floors as a bar table (three times the floor, no lower than 0.5 %), the time and the peak memory of the
@@ -96,7 +176,7 @@ def _report(name, floors, bars, t0):
     return bad
 
 
-def _unet_case(cuda, size, n, seed, bars):
+def _unet_case(cuda, size, n, seed, bars, fwd_bars):
     from audio_diffusion_b200.unet import UNet2DModel
     from oracle.schedulers_oracle import OracleDDPM
     from oracle.unet_oracle import UNetConfig, init_weights, unet_forward
@@ -114,6 +194,7 @@ def _unet_case(cuda, size, n, seed, bars):
     noise = noise.to(cuda)
     torch.nn.functional.mse_loss(pred, noise).backward()
     g_eps = 2 * (pred.detach() - noise) / pred.numel()
+    eps = pred.detach()
     del pred
     blocks = bg.unet_blocks(cfg)
     assert [b.name for b in blocks if b.kind == "attn"] == (
@@ -128,8 +209,12 @@ def _unet_case(cuda, size, n, seed, bars):
         pred = unet_forward(w64, cfg, noisy.double(), t.to(cuda), taps)
     floors = _floors(blocks, taps, noisy.double(), 2 * (pred - noise.double()) / pred.numel(), w64, cfg, taps["temb_act"])
     bad = _report(f"UNet2DModel {size[0]}x{size[1]} batch {n}", floors, bars, t0)
+    temb = bg.temb_act(w64, cfg, t.to(cuda))
+    frows = forward_checks(model.debug_tensor, blocks, noisy, eps, w64, cfg, temb, taps="all")
+    ffl = _fwd_floors(blocks, taps, noisy.double(), w64, cfg, temb, taps="all")
     assert not fails, fails
     assert not bad, bad
+    check_against_floors(f"UNet2DModel {size[0]}x{size[1]} batch {n}, training forward", frows, ffl, fwd_bars, t0)
 
 
 @pytest.mark.timeout(900)
@@ -138,7 +223,7 @@ def test_unet_256_backward_per_block(cuda):
     every level from 256x256 to 8x8, the 8x32 and 16x16 data-gradient tiles, the parity-scatter data gradient of every
     downsampler, the folded upsamplers' data gradients, and per-sample bias / time-embedding sums over an odd batch.
     fp64 work: 10 s, 28.6 GiB peak."""
-    _unet_case(cuda, (256, 256), 5, 7, UNET256_BARS)
+    _unet_case(cuda, (256, 256), 5, 7, UNET256_BARS, UNET256_FWD_BARS)
 
 
 @pytest.mark.timeout(600)
@@ -146,7 +231,7 @@ def test_unet_64_packed_backward_per_block(cuda):
     """The published UNet2DModel at 64x64, batch 5: the 8x8, 4x4 and 2x2 levels pack up to four images per conv work
     item, so the last item holds one image; a gradient leaking across the halo between packed images shows here and not
     at batch 1.  Attention at 4x4.  fp64 work: 1.2 s, 4.9 GiB peak."""
-    _unet_case(cuda, (64, 64), 5, 9, UNET64_BARS)
+    _unet_case(cuda, (64, 64), 5, 9, UNET64_BARS, UNET64_FWD_BARS)
 
 
 @pytest.mark.timeout(600)
@@ -170,24 +255,31 @@ def test_vae_256_backward_per_block(cuda):
     z = torch.randn(2, 1, 32, 32, generator=g).to(cuda)
     gx = torch.randn(2, 1, 256, 256, generator=g).to(cuda)
     gm = torch.randn(2, 2, 32, 32, generator=g).to(cuda)
-    model.encode(x).latent_dist.parameters.backward(gm)
+    mom = model.encode(x).latent_dist.parameters
+    mom.backward(gm)
     zz = z.clone().requires_grad_(True)
-    model.decode(zz).sample.backward(gx)
+    img = model.decode(zz).sample
+    img.backward(gx)
     w64 = _w64(w, cuda)
     torch.cuda.reset_peak_memory_stats()
     t0 = time.perf_counter()
     fails = _run_checks(model, bg.vae_blocks(cfg, "decoder"), z, gx, w64, cfg, VAE256_BARS, "decoder:", g_in=zz.grad)
     fails += _run_checks(model, bg.vae_blocks(cfg, "encoder"), x, gm, w64, cfg, VAE256_BARS, "encoder:")
-    floors = {}
-    for part, inp, gout, fwd in (("decoder", z, gx, vo.decode), ("encoder", x, gm, vo.encode_moments)):
+    floors, frows, ffl = {}, [], {}
+    for part, inp, gout, fwd, out in (("decoder", z, gx, vo.decode, img.detach()),
+                                      ("encoder", x, gm, vo.encode_moments, mom.detach())):
         taps = {}
         with torch.no_grad():
             fwd(w64, cfg, inp.double(), taps)
-        for k, v in _floors(bg.vae_blocks(cfg, part), taps, inp.double(), gout.double(), w64, cfg).items():
+        blocks = bg.vae_blocks(cfg, part)
+        for k, v in _floors(blocks, taps, inp.double(), gout.double(), w64, cfg).items():
             floors[part + ":" + k] = v
+        frows += forward_checks(model.debug_tensor, blocks, inp.double(), out, w64, cfg, prefix=part + ":", taps="all")
+        ffl.update(_fwd_floors(blocks, taps, inp.double(), w64, cfg, prefix=part + ":", taps="all"))
     bad = _report("AutoencoderKL 256x256 batch 2", floors, VAE256_BARS, t0)
     assert not fails, fails
     assert not bad, bad
+    check_against_floors("AutoencoderKL 256x256 batch 2, training forward", frows, ffl, VAE256_FWD_BARS, t0)
 
 
 @pytest.mark.timeout(600)
@@ -215,6 +307,7 @@ def test_cond_unet_64_backward_per_block(cuda):
     noise = noise.to(cuda)
     torch.nn.functional.mse_loss(pred, noise).backward()
     g_eps = 2 * (pred.detach() - noise) / pred.numel()
+    eps = pred.detach()
     del pred
     blocks = bg.unet_blocks(cfg)
     assert sum(b.kind == "transformer" for b in blocks) == 16
@@ -229,8 +322,11 @@ def test_cond_unet_64_backward_per_block(cuda):
     floors = _floors(blocks, taps, noisy.double(), 2 * (pred - noise.double()) / pred.numel(), w64, cfg, temb,
                      enc.double())
     bad = _report("UNet2DConditionModel 64x64 batch 2", floors, COND64_BARS, t0)
+    frows = forward_checks(model.debug_tensor, blocks, noisy, eps, w64, cfg, temb, enc.double(), taps="all")
+    ffl = _fwd_floors(blocks, taps, noisy.double(), w64, cfg, temb, enc.double(), taps="all")
     assert not fails, fails
     assert not bad, bad
+    check_against_floors("UNet2DConditionModel 64x64 batch 2, training forward", frows, ffl, COND64_FWD_BARS, t0)
 
 
 @pytest.mark.timeout(600)
