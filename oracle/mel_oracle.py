@@ -81,18 +81,29 @@ def stft(y: np.ndarray, n_fft: int, hop: int) -> np.ndarray:
     return scipy.fft.rfft(frames, axis=0).astype(cdtype, copy=False)
 
 
-def istft(S: np.ndarray, n_fft: int, hop: int, dtype=np.float32) -> np.ndarray:
-    """librosa.istft(center=True, length=None, window='hann'): overlap-add / window-sumsquare."""
+def istft(S: np.ndarray, n_fft: int, hop: int, dtype=np.float32, rounded: bool = False) -> np.ndarray:
+    """librosa.istft(center=True, length=None, window='hann'): overlap-add / window-sumsquare.
+
+    rounded=True applies the storage roundings of the CUDA decode (mel.cu gl_istft_kernel / ola_sample) and only those:
+    the windowed frames are stored as float32, summed in float64, the sum is cast to float32 and divided in float32 by
+    the float32 window sum-square where that is above FLT_MIN (left unnormalised elsewhere).  Returns float32."""
     n_frames = S.shape[-1]
     win = _hann(n_fft)
     expected = n_fft + hop * (n_frames - 1)
     ytmp = scipy.fft.irfft(S, n=n_fft, axis=0) * win[:, None]
+    if rounded:
+        ytmp = ytmp.astype(np.float32).astype(np.float64)
     y = np.zeros(expected, dtype=np.float64)
     wss = np.zeros(expected, dtype=np.float64)
     wsq = win ** 2
     for f in range(n_frames):
         y[f * hop: f * hop + n_fft] += ytmp[:, f]
         wss[f * hop: f * hop + n_fft] += wsq
+    if rounded:
+        y32, w32 = y.astype(np.float32), wss.astype(np.float32)
+        nz = w32 > np.finfo(np.float32).tiny
+        y32[nz] /= w32[nz]
+        return y32[n_fft // 2: expected - n_fft // 2]
     tiny = np.finfo(np.float32 if dtype == np.float32 else np.float64).tiny
     nz = wss > tiny
     y[nz] /= wss[nz]
@@ -106,6 +117,14 @@ def melspectrogram(y: np.ndarray, sr: int, n_fft: int, hop: int, n_mels: int) ->
     S = np.abs(stft(y, n_fft, hop)) ** 2
     M = mel_filterbank(sr, n_fft, n_mels)
     return np.einsum("ft,mf->mt", S, M, optimize=True)
+
+
+def mel_power64(y: np.ndarray, basis: np.ndarray, n_fft: int, hop: int) -> np.ndarray:
+    """The mel power spectrogram (n_mels, frames) in float64: the float64 STFT power of `y` times `basis` promoted to
+    float64.  Given the float32 basis the CUDA encode multiplies by, this is the exact value of what that kernel
+    computes, with no rounding of the basis in between."""
+    S = np.abs(stft(np.asarray(y, dtype=np.float64), n_fft, hop)) ** 2
+    return basis.astype(np.float64) @ S
 
 
 def power_to_db(S: np.ndarray, ref=np.max, amin: float = 1e-10, top_db: float = 80.0) -> np.ndarray:
@@ -175,25 +194,65 @@ def mel_to_stft(M: np.ndarray, sr: int, n_fft: int) -> np.ndarray:
 
 
 def griffinlim(S: np.ndarray, n_iter: int, hop: int, n_fft: int, momentum: float = 0.99,
-               rng: np.random.Generator | None = None, dtype=np.float32) -> np.ndarray:
+               rng: np.random.Generator | None = None, dtype=np.float32, angles0: np.ndarray | None = None,
+               rounded: bool = False) -> np.ndarray:
     """librosa.griffinlim(init='random', random_state=None).  The reference leaves the RNG unseeded
-    (non-deterministic); pass `rng` to make the oracle reproducible."""
-    rng = rng or np.random.default_rng()
+    (non-deterministic); pass `rng` to make the oracle reproducible, or `angles0`, the initial complex spectrum
+    (magnitude included), to start where another implementation starts.
+
+    With S float64 and dtype=float64 every step runs in float64 (the exact Griffin-Lim).  rounded=True (S float64)
+    applies the storage roundings of the CUDA decode and only those: the float32 frames and overlap-add of
+    istft(rounded=True), `rebuilt` and `tprev` stored as complex64, the momentum step and the phase normalisation in
+    float64, the latter only where |angles| > 0."""
     cdtype = np.complex64 if S.dtype == np.float32 else np.complex128
     eps = np.finfo(S.dtype).tiny
-    angles = np.exp(2j * np.pi * rng.random(size=S.shape)).astype(cdtype)
-    angles *= S
+    if angles0 is None:
+        rng = rng or np.random.default_rng()
+        angles = np.exp(2j * np.pi * rng.random(size=S.shape)).astype(cdtype)
+        angles *= S
+    else:
+        angles = np.array(angles0, dtype=cdtype)
     tprev = None
     for _ in range(n_iter):
-        inverse = istft(angles, n_fft, hop, dtype=dtype)
+        inverse = istft(angles, n_fft, hop, dtype=dtype, rounded=rounded)
         rebuilt = stft(inverse, n_fft, hop)
-        angles = rebuilt.astype(cdtype, copy=True)
-        if tprev is not None:
-            angles -= (momentum / (1 + momentum)) * tprev
-        angles /= np.abs(angles) + eps
-        angles *= S
+        if rounded:
+            angles = rebuilt.astype(np.complex128)
+            if tprev is not None:
+                angles -= (momentum / (1 + momentum)) * tprev.astype(np.complex128)
+            a = np.abs(angles)
+            nz = a > 0
+            angles[nz] *= S[nz] / a[nz]
+        else:
+            angles = rebuilt.astype(cdtype, copy=True)
+            if tprev is not None:
+                angles -= (momentum / (1 + momentum)) * tprev
+            angles /= np.abs(angles) + eps
+            angles *= S
         tprev = rebuilt
-    return istft(angles, n_fft, hop, dtype=dtype)
+    return istft(angles, n_fft, hop, dtype=dtype, rounded=rounded)
+
+
+def phase_u01(seed: int, idx) -> np.ndarray:
+    """mel.cu `u01`: splitmix64 of state seed + (idx + 1) * 0x9E3779B97F4A7C15, top 53 bits scaled to [0, 1)."""
+    idx = np.asarray(idx, dtype=np.uint64)
+    with np.errstate(over="ignore"):
+        z = np.uint64(seed) + np.uint64(0x9E3779B97F4A7C15) * (idx + np.uint64(1))
+        z = (z ^ (z >> np.uint64(30))) * np.uint64(0xBF58476D1CE4E5B9)
+        z = (z ^ (z >> np.uint64(27))) * np.uint64(0x94D049BB133111EB)
+        z = z ^ (z >> np.uint64(31))
+    return (z >> np.uint64(11)).astype(np.float64) * 2.0 ** -53
+
+
+def initial_spectrum(images: np.ndarray, pinv: np.ndarray, seed: int, top_db: float = 80.0) -> np.ndarray:
+    """The CUDA decode's Griffin-Lim starting point for a batch of (n, n_mels, frames) uint8 images, as (n, bins,
+    frames) complex128: sqrt(max(pinv @ db_to_power(image), 0)) (the inverse mel transform, see
+    test_mel_nnls_is_initial_point_on_image_domain) times exp(2 pi i u), u = phase_u01(seed, (n * frames + t) * bins + f)."""
+    n, _, T = images.shape
+    F = pinv.shape[0]
+    mag = np.sqrt(np.maximum(pinv @ u8_to_power(images, top_db), 0.0))
+    o = (np.arange(n)[:, None, None] * T + np.arange(T)[None, None, :]) * F + np.arange(F)[None, :, None]
+    return mag * np.exp(2j * np.pi * phase_u01(seed, o))
 
 
 def bytes_to_audio(b: np.ndarray, sr=22050, n_fft=2048, hop=512, top_db=80, n_iter=32,

@@ -204,11 +204,70 @@ def test_mel_roundtrip_in_mel_domain():
     assert np.abs(b2.astype(int) - b.astype(int)).mean() < 12.0
 
 
+def test_mel_phase_u01_known_answers():
+    """oracle.phase_u01 is mel.cu's u01: from state 0, splitmix64's published first outputs, top 53 bits over 2^53."""
+    from oracle import mel_oracle as mo
+    first = [0xe220a8397b1dcdaf, 0x6e789e6aa1b965f4, 0x06c45d188009454f, 0xf88bb8a8724c81ec]
+    u = mo.phase_u01(0, np.arange(4))
+    assert u.tolist() == [(z >> 11) * 2.0 ** -53 for z in first]
+    assert np.allclose(u, [0.8833108082136426, 0.43152799704850997, 0.026433771592597743, 0.9708819781538285], rtol=0, atol=1e-16)
+    # the seed offsets the state: seed s at index i is state s + (i + 1) * golden gamma
+    assert mo.phase_u01(0x9E3779B97F4A7C15, 0) == u[1]
+
+
+def test_mel_griffinlim_from_given_spectrum():
+    """griffinlim(angles0=...) starts from the given spectrum: in float64 with n_iter = 0 it is istft of that spectrum;
+    the rounded model (the CUDA decode's float32 frames and overlap-add) differs from it, by far less than 1e-6."""
+    from audio_diffusion_b200.mel import slaney_mel_basis
+    from oracle import mel_oracle as mo
+    n_fft, hop = 512, 128
+    img = mo.audio_slice_to_bytes(_tone(n=64 * hop - 1, noise=0.1), n_fft=n_fft, hop=hop, n_mels=64)
+    pinv = np.linalg.pinv(slaney_mel_basis(22050, n_fft, 64, np.float64))
+    A0 = mo.initial_spectrum(img[None], pinv, 12345)[0]
+    mag = np.abs(A0)
+    exact = mo.griffinlim(mag, 0, hop, n_fft, dtype=np.float64, angles0=A0)
+    assert exact.dtype == np.float64 and np.array_equal(exact, mo.istft(A0, n_fft, hop, dtype=np.float64))
+    rd = mo.griffinlim(mag, 0, hop, n_fft, dtype=np.float32, angles0=A0, rounded=True)
+    assert rd.dtype == np.float32 and rd.shape == exact.shape
+    rel = np.linalg.norm(rd - exact) / np.linalg.norm(exact)
+    assert 0 < rel < 1e-6, rel
+    # the seeded magnitude is the inverse mel transform of the image; the phase changes with the seed
+    assert np.allclose(mag, np.sqrt(np.clip(pinv @ mo.u8_to_power(img), 0, None)), rtol=1e-12, atol=0)
+    assert not np.allclose(A0, mo.initial_spectrum(img[None], pinv, 12346)[0])
+
+
+def test_mel_config_validation_without_gpu():
+    """b200ad_mel_scratch_bytes (host code) rejects every n_fft outside the powers of two in [64, 4096] and every hop
+    outside [1, n_fft], naming the rule; Mel refuses such a configuration before it allocates."""
+    import ctypes as C
+
+    from audio_diffusion_b200 import _lib
+    from audio_diffusion_b200.mel import Mel
+    L = _lib.lib()
+    for n_fft, hop, rule in [(32, 8, "n_fft must be a power of two"), (1000, 250, "n_fft must be a power of two"),
+                             (3000, 512, "n_fft must be a power of two"), (8192, 512, "n_fft must be a power of two"),
+                             (2048, 0, "hop_length out of range"), (2048, 2049, "hop_length out of range"),
+                             (64, 65, "hop_length out of range")]:
+        cfg = _lib.MelConfigC(64, 64, 22050, n_fft, hop, 80, 32)
+        assert L.b200ad_mel_scratch_bytes(C.byref(cfg), 1) == 0, (n_fft, hop)
+        assert rule in L.b200ad_last_error().decode(), (n_fft, hop)
+    for n_fft in (64, 128, 256, 512, 1024, 2048, 4096):
+        for hop in (1, n_fft // 4, n_fft):
+            assert L.b200ad_mel_scratch_bytes(C.byref(_lib.MelConfigC(64, 64, 22050, n_fft, hop, 80, 32)), 2) > 0
+    with pytest.raises(_lib.B200ADError, match="n_fft must be a power of two"):
+        Mel(n_fft=1000)._scratch(1, "cpu")
+
+
 def test_product_mel_constants_equal_oracle():
     from audio_diffusion_b200.mel import Mel, slaney_mel_basis
     from oracle import mel_oracle as mo
     for dt in (np.float32, np.float64):
         assert np.array_equal(slaney_mel_basis(22050, 2048, 256, dt), mo.mel_filterbank(22050, 2048, 256, dtype=dt))
+    # every accepted n_fft, at the mel counts tests/test_gpu_mel_fp64.py runs it with
+    for n_fft, n_mels in [(64, 48), (128, 32), (256, 40), (512, 64), (1024, 80), (2048, 128), (4096, 128)]:
+        for dt in (np.float32, np.float64):
+            assert np.array_equal(slaney_mel_basis(22050, n_fft, n_mels, dt),
+                                  mo.mel_filterbank(22050, n_fft, n_mels, dtype=dt)), (n_fft, n_mels, dt)
     m = Mel(x_res=64, y_res=64, hop_length=1024)
     assert m.slice_size == 64 * 1024 - 1 and m.n_mels == 64
     m.load_audio(raw_audio=np.ones(10, dtype=np.float32))

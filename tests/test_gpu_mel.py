@@ -20,16 +20,19 @@ def _audio(n, seed=0, f=440.0):
     return (y * np.linspace(0.2, 1.0, n)).astype(np.float32)
 
 
-@pytest.mark.parametrize("x_res,y_res,hop", [(256, 256, 512), (64, 64, 1024)])
-def test_encode_matches_oracle(cuda, x_res, y_res, hop):
+# every n_fft the codec accepts and the edges of tests/test_gpu_mel_fp64.py's table, plus the 64 x 64 default-size case
+@pytest.mark.parametrize("n_fft,hop,x_res,y_res", [(64, 16, 64, 48), (128, 128, 32, 32), (256, 100, 64, 40),
+                                                   (512, 128, 96, 64), (1024, 256, 128, 80), (2048, 512, 256, 256),
+                                                   (2048, 1024, 64, 64), (2048, 2048, 64, 128), (4096, 1024, 128, 128)])
+def test_encode_matches_oracle(cuda, n_fft, hop, x_res, y_res):
     from audio_diffusion_b200.mel import Mel
     from oracle import mel_oracle as mo
-    mel = Mel(x_res=x_res, y_res=y_res, hop_length=hop)
+    mel = Mel(x_res=x_res, y_res=y_res, n_fft=n_fft, hop_length=hop)
     L = mel.slice_size
     ys = np.stack([_audio(L, seed=s, f=220.0 * (s + 1)) for s in range(3)] + [np.zeros(L, np.float32)])
     got = mel.audio_slices_to_images(ys, device=cuda).cpu().numpy()
     for i in range(len(ys)):
-        ref = mo.audio_slice_to_bytes(ys[i], n_fft=2048, hop=hop, n_mels=y_res)
+        ref = mo.audio_slice_to_bytes(ys[i], n_fft=n_fft, hop=hop, n_mels=y_res)
         diff = np.abs(got[i].astype(int) - ref.astype(int))
         assert diff.max() <= 1, f"slice {i}: max grey diff {diff.max()}"
         assert (diff == 0).mean() >= 0.995, f"slice {i}: only {(diff == 0).mean():.4f} identical"
