@@ -64,6 +64,7 @@ SYMBOLS = {
     "b200ad_unet_bind_workspace": (_I, [_VP, _VP, _SZ, _I, _I, _I, _VP]),
     "b200ad_unet_forward": (_I, [_VP, _VP, _VP, _VP, _VP]),
     "b200ad_unet_set_encoding": (_I, [_VP, _VP, _I]),
+    "b200ad_unet_set_encoder_len": (_I, [_VP, _I]),
     "b200ad_unet_forward_step": (_I, [_VP, _VP, _VP, _VP, C.POINTER(StepCoefC), _VP, _VP, _VP]),
     "b200ad_unet_forward_step_dev": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _VP]),
     "b200ad_step_scalars_upload": (_I, [C.POINTER(StepCoefC), C.c_float, _VP, _VP, C.c_int, _VP]),
@@ -116,6 +117,8 @@ SYMBOLS = {
     "b200ad_group_norm": (_I, [_VP] * 4 + [_I] * 5 + [C.c_float, _I, _VP, _SZ, _VP]),
     "b200ad_mha_scratch_bytes": (_SZ, [_I] * 5),
     "b200ad_mha_forward_backward": (_I, [_VP] * 8 + [_I] * 5 + [_VP, _SZ, _VP]),
+    "b200ad_xattn_scratch_bytes": (_SZ, [_I] * 6),
+    "b200ad_xattn_forward_backward": (_I, [_VP] * 8 + [_I] * 6 + [_VP, _SZ, _VP]),
     "b200ad_mel_scratch_bytes": (_SZ, [C.POINTER(MelConfigC), _I]),
     "b200ad_mel_encode": (_I, [C.POINTER(MelConfigC), _VP, _VP, _VP, _I, _VP, _SZ, _VP]),
     "b200ad_mel_encode_ref": (_I, [C.POINTER(MelConfigC), _VP, _VP, _VP, _I, _VP, _VP, _VP, _SZ, _VP]),

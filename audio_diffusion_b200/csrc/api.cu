@@ -296,6 +296,62 @@ extern "C" int b200ad_mha_forward_backward(const float* q, const float* k, const
   return 0;
 }
 
+// Cross-attention against S > 1 encoder tokens, forward and backward, on fp32 tensors: the training forward kernel (with
+// its row log-sum-exp) and the backward launches the model runs (without the K / V projections).
+struct XattnScratch {
+  size_t q, o, go, gq, k, v, lse, dsum, part, total;
+};
+static XattnScratch xattn_scratch_layout(int N, int C, int heads, int H, int W, int S) {
+  XattnScratch s{};
+  const Geom g = make_geom(N, H, W);
+  const size_t pf = (size_t)N * (C / 8) * g.PL * 16, rows = (size_t)N * heads * H * W * sizeof(float);
+  const size_t kv = (size_t)N * S * C * sizeof(__nv_bfloat16);
+  size_t off = 0;
+  s.q = off; off = al(off + pf);
+  s.o = off; off = al(off + pf);
+  s.go = off; off = al(off + pf);
+  s.gq = off; off = al(off + pf);
+  s.k = off; off = al(off + kv);
+  s.v = off; off = al(off + kv);
+  s.lse = off; off = al(off + rows);
+  s.dsum = off; off = al(off + rows);
+  s.part = off; off = al(off + xattn_part_floats(N, C, heads, H, W, S) * sizeof(float));
+  s.total = off;
+  return s;
+}
+extern "C" size_t b200ad_xattn_scratch_bytes(int N, int C, int heads, int H, int W, int S) {
+  return xattn_scratch_layout(N, C, heads, H, W, S).total;
+}
+extern "C" int b200ad_xattn_forward_backward(const float* q, const float* k, const float* v, const float* dout, float* out,
+                                             float* dq, float* dk, float* dv, int N, int C, int heads, int H, int W, int S,
+                                             void* scratch, size_t scratch_bytes, void* stream) {
+  if (heads < 1 || C % heads || (C / heads != 16 && C / heads != 32 && C / heads != 64))
+    return set_err("xattn_forward_backward: head_dim C / heads must be 16, 32 or 64");
+  if (S < 1 || S > XATTN_MAX_S) return set_err("xattn_forward_backward: S = %d outside [1, %d]", S, XATTN_MAX_S);
+  const XattnScratch L = xattn_scratch_layout(N, C, heads, H, W, S);
+  if (scratch_bytes < L.total) return set_err("xattn_forward_backward: scratch too small (%zu < %zu)", scratch_bytes, L.total);
+  cudaStream_t st = (cudaStream_t)stream;
+  uint8_t* sb = (uint8_t*)scratch;
+  CK(cudaMemsetAsync(sb, 0, L.total, st));
+  __nv_bfloat16* qp = (__nv_bfloat16*)(sb + L.q);
+  __nv_bfloat16* op = (__nv_bfloat16*)(sb + L.o);
+  __nv_bfloat16* gop = (__nv_bfloat16*)(sb + L.go);
+  __nv_bfloat16* gqp = (__nv_bfloat16*)(sb + L.gq);
+  __nv_bfloat16* kp = (__nv_bfloat16*)(sb + L.k);
+  __nv_bfloat16* vp = (__nv_bfloat16*)(sb + L.v);
+  float* lse = (float*)(sb + L.lse);
+  CK(launch_nchw_to_pf8(q, qp, N, C, H, W, st));
+  CK(launch_nchw_to_pf8(dout, gop, N, C, H, W, st));
+  CK(launch_f32_to_bf16(k, kp, (long long)N * S * C, st));
+  CK(launch_f32_to_bf16(v, vp, (long long)N * S * C, st));
+  CK(launch_xattn(qp, kp, vp, op, N, C, heads, H, W, S, st, lse));
+  CK(launch_xattn_bwd(qp, kp, vp, op, gop, lse, (float*)(sb + L.dsum), (float*)(sb + L.part), gqp, dk, dv, N, C, heads, H, W,
+                      S, st));
+  CK(launch_pf8_to_nchw(op, out, N, C, H, W, st));
+  CK(launch_pf8_to_nchw(gqp, dq, N, C, H, W, st));
+  return 0;
+}
+
 extern "C" int b200ad_sample_to_u8(const float* x, uint8_t* img, size_t n, void* stream) {
   CK(launch_sample_to_u8(x, img, n, (cudaStream_t)stream));
   return 0;

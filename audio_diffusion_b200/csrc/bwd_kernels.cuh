@@ -63,6 +63,17 @@ cudaError_t launch_cross_attn_vec_bwd(const float* enc, const float* dvec, const
 // (PF8, C channels), lse from launch_mha_flash -> gqkv (PF8, 3C channels).  dsum: N * heads * H * W floats of scratch.
 cudaError_t launch_mha_bwd(const __nv_bfloat16* qkv, const __nv_bfloat16* o, const __nv_bfloat16* go, const float* lse,
                            float* dsum, __nv_bfloat16* gqkv, int N, int C, int heads, int H, int W, cudaStream_t s);
+// cross-attention against S > 1 encoder tokens: q, o as the forward read / wrote them (PF8, C channels), k, v bf16
+// [N][S][C], go = dL/do (PF8, C channels), lse from launch_xattn -> gq (PF8, C channels) and dk, dv fp32 [N][S][C]
+// (overwritten).  Scratch: dsum (N * heads * H * W floats) and part (xattn_part_floats floats): per query split fp32
+// partial sums of dK and dV, added in split order (no atomics: the result is deterministic).
+size_t xattn_part_floats(int N, int C, int heads, int H, int W, int S);
+cudaError_t launch_xattn_bwd(const __nv_bfloat16* q, const __nv_bfloat16* k, const __nv_bfloat16* v, const __nv_bfloat16* o,
+                             const __nv_bfloat16* go, const float* lse, float* dsum, float* part, __nv_bfloat16* gq, float* dk,
+                             float* dv, int N, int C, int heads, int H, int W, int S, cudaStream_t s);
+// the K / V projections' weight gradients: dwk[c][x] += sum over the M = N * S tokens of dk[m][c] enc[m][x], dwv the same
+cudaError_t launch_xattn_kv_wgrad(const float* dk, const float* dv, const float* enc, float* dwk, float* dwv, int M, int C,
+                                  int X, cudaStream_t s);
 
 // Autoencoder layers (vae_bwd_kernels.cu).
 // single-head attention (one head of dim C, S = H * W tokens, S % 64 == 0, C % 64 == 0): qkv as the forward read it,

@@ -492,4 +492,352 @@ cudaError_t launch_mha_bwd(const __nv_bfloat16* qkv, const __nv_bfloat16* o, con
   return cudaErrorInvalidValue;
 }
 
+// ------------------------------------------------------------------------------------ cross-attention, S > 1 keys, backward
+// The forward is xattn_fwd_kernel (cond_ops.cu): q and O are PF8 tensors of C channels, K and V bf16 [N][S][C].  The same
+// identities as the self-attention backward above, in four launches: D = rowsum(dO o O) (mha_bwd_dot_kernel); dQ
+// (query-parallel, K and V staged once per CTA); dK and dV as fp32 partial sums per split of the queries (65 536 queries
+// of one sample meet at most 256 keys, so the key-parallel form alone would leave most SMs idle); the partials added in
+// split order.
+
+// B fragment (k16 x n8, "col") by transposing ldmatrix from a [plane][SP rows] tile whose rows run along k
+__device__ __forceinline__ void ldsm_b_trans_sp(uint32_t& b0, uint32_t& b1, uint32_t tile_addr, int plane, int SP, int row0,
+                                                int lane) {
+  const uint32_t a = tile_addr + (uint32_t)((plane * SP + row0 + (lane & 15)) * 16);
+  asm volatile("ldmatrix.sync.aligned.m8n8.x2.trans.shared.b16 {%0,%1}, [%2];" : "=r"(b0), "=r"(b1) : "r"(a));
+}
+
+// dQ: one CTA = one (sample, head), K / V staged once, XATTN_BWD_QT tiles of 64 queries; per 64-key tile and warp:
+// S = Q K^T, dP = dO V^T, dS = P o (dP - D) (keys beyond S masked), dQ += dS K.
+constexpr int XATTN_BWD_QT = 4;
+template <int D>
+// (minimum 1 CTA per SM: without it ptxas caps the D = 16 / 32 instantiations below their needs and spills)
+__global__ void __launch_bounds__(128, 1) xattn_bwd_dq_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
+                                                           const __nv_bfloat16* __restrict__ v, const __nv_bfloat16* __restrict__ go,
+                                                           const float* __restrict__ lse, const float* __restrict__ dsum,
+                                                           __nv_bfloat16* __restrict__ gq, int N, int C, int H, int W, int S,
+                                                           float scale_log2, float scale) {
+  constexpr int DP = D / 8, KS = D / 16;
+  extern __shared__ __align__(16) uint4 xsm[];
+  const int SP = (S + 63) & ~63;
+  uint4* ks = xsm;
+  uint4* vs = xsm + DP * SP;
+  const Geom g = make_geom(N, H, W);
+  const int seq = H * W, planes = C >> 3, heads = gridDim.y;
+  const int head = blockIdx.y, n = blockIdx.z;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, gq8 = lane >> 2, tq = lane & 3;
+  xattn_stage_kv<D>(ks, vs, k, v, n, head, C, S, SP);
+  __syncthreads();
+  const uint32_t* ks32 = reinterpret_cast<const uint32_t*>(ks);
+  const uint32_t* vs32 = reinterpret_cast<const uint32_t*>(vs);
+  const uint32_t ks_addr = smem_u32(ks);
+  const long long hoff = ((long long)n * planes + head * DP) * g.PL * 8;
+  const __nv_bfloat16* qb = q + hoff;
+  const __nv_bfloat16* gob = go + hoff;
+  __nv_bfloat16* qd = gq + hoff;
+  const long long rowb = ((long long)n * heads + head) * seq;
+  const int ntiles = (seq + 63) / 64;
+  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    const int q0 = tile * 64;
+    const int r0 = min(q0 + warp * 16 + gq8, seq - 1), r1 = min(q0 + warp * 16 + gq8 + 8, seq - 1);
+    const long long o0 = pf8_pixel(g, r0, W), o1 = pf8_pixel(g, r1, W);
+    uint32_t qa[KS][4], oa[KS][4];
+    load_rows_a<KS>(qa, qb, g, o0, o1, tq);
+    load_rows_a<KS>(oa, gob, g, o0, o1, tq);
+    const float l0 = lse[rowb + r0], l1 = lse[rowb + r1], d0 = dsum[rowb + r0], d1 = dsum[rowb + r1];
+    float dq[DP][4];
+#pragma unroll
+    for (int i = 0; i < DP; ++i) { dq[i][0] = dq[i][1] = dq[i][2] = dq[i][3] = 0.f; }
+    for (int k0 = 0; k0 < S; k0 += 64) {
+      float sc[8][4], dp[8][4];
+#pragma unroll
+      for (int t = 0; t < 8; ++t) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) { sc[t][e] = 0.f; dp[t][e] = 0.f; }
+        if (k0 + t * 8 < S) {
+#pragma unroll
+          for (int j = 0; j < KS; ++j) {
+            const int w0 = ((2 * j) * SP + k0 + t * 8 + gq8) * 4 + tq, w1 = ((2 * j + 1) * SP + k0 + t * 8 + gq8) * 4 + tq;
+            mma_bf16_16x8x16(sc[t], qa[j][0], qa[j][1], qa[j][2], qa[j][3], ks32[w0], ks32[w1]);
+            mma_bf16_16x8x16(dp[t], oa[j][0], oa[j][1], oa[j][2], oa[j][3], vs32[w0], vs32[w1]);
+          }
+        }
+      }
+#pragma unroll
+      for (int t = 0; t < 8; ++t) {
+        const int key = k0 + t * 8 + 2 * tq;
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const float p = (key + (e & 1) < S) ? exp2f(sc[t][e] * scale_log2 - (e < 2 ? l0 : l1)) : 0.f;
+          dp[t][e] = p * (dp[t][e] - (e < 2 ? d0 : d1));
+        }
+      }
+#pragma unroll
+      for (int k16 = 0; k16 < 4; ++k16) {
+        if (k0 + k16 * 16 < S) {
+          const float* s0 = dp[2 * k16];
+          const float* s1 = dp[2 * k16 + 1];
+          const uint32_t sa0 = pack_bf16x2(s0[0], s0[1]), sa1 = pack_bf16x2(s0[2], s0[3]), sa2 = pack_bf16x2(s1[0], s1[1]),
+                         sa3 = pack_bf16x2(s1[2], s1[3]);
+#pragma unroll
+          for (int i = 0; i < DP; ++i) {
+            uint32_t b0, b1;
+            ldsm_b_trans_sp(b0, b1, ks_addr, i, SP, k0 + k16 * 16, lane);
+            mma_bf16_16x8x16(dq[i], sa0, sa1, sa2, sa3, b0, b1);
+          }
+        }
+      }
+    }
+    const int qa_row = q0 + warp * 16 + gq8, qb_row = qa_row + 8;
+#pragma unroll
+    for (int i = 0; i < DP; ++i) {
+      if (qa_row < seq) *reinterpret_cast<uint32_t*>(qd + (long long)i * g.PL * 8 + o0 + 2 * tq) = pack_bf16x2(dq[i][0] * scale, dq[i][1] * scale);
+      if (qb_row < seq) *reinterpret_cast<uint32_t*>(qd + (long long)i * g.PL * 8 + o1 + 2 * tq) = pack_bf16x2(dq[i][2] * scale, dq[i][3] * scale);
+    }
+  }
+}
+
+// How the queries of one (sample, head) are split for the dK / dV partial sums: a function of the shapes only (not of
+// the GPU), so the summation order, and with it every bit of the result, is the same on any device.
+struct XattnSplit {
+  int SP, ntiles, per_split, nsplit;
+};
+static XattnSplit xattn_split(int N, int heads, int H, int W, int S) {
+  XattnSplit x;
+  x.SP = (S + 63) & ~63;
+  x.ntiles = (H * W + 63) / 64;
+  const int base = (x.SP / 64) * heads * N;                 // CTAs without splitting
+  int want = (1024 + base - 1) / base;                      // about 8 CTAs per SM of an H100
+  want = want < 1 ? 1 : want > x.ntiles ? x.ntiles : want;
+  x.per_split = (x.ntiles + want - 1) / want;
+  x.nsplit = (x.ntiles + x.per_split - 1) / x.per_split;
+  return x;
+}
+size_t xattn_part_floats(int N, int C, int heads, int H, int W, int S) {
+  const XattnSplit x = xattn_split(N, heads, H, W, S);
+  return (size_t)2 * x.nsplit * N * x.SP * C;               // dK | dV, [split][n][head][key][D]
+}
+
+// dK, dV partials: one CTA = 64 keys of one (sample, head) (4 warps x 16 keys, K / V rows as A fragments) and the query
+// tiles of one split, streamed through shared memory as in mha_bwd_kv_kernel.  Writes every one of its SP key rows (rows
+// beyond S read key S - 1 and are never summed).
+template <int D>
+__global__ void __launch_bounds__(128) xattn_bwd_kv_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
+                                                           const __nv_bfloat16* __restrict__ v, const __nv_bfloat16* __restrict__ go,
+                                                           const float* __restrict__ lse, const float* __restrict__ dsum,
+                                                           float* __restrict__ part, int N, int C, int heads, int H, int W, int S,
+                                                           int per_split, float scale_log2) {
+  constexpr int DP = D / 8, KS = D / 16;
+  __shared__ __align__(16) uint4 qs[DP][64];
+  __shared__ __align__(16) uint4 dos[DP][64];
+  __shared__ float ls[64], dd[64];
+  const Geom g = make_geom(N, H, W);
+  const int seq = H * W, planes = C >> 3, SP = (S + 63) & ~63, nsplit = gridDim.y;
+  const int k0 = blockIdx.x * 64, split = blockIdx.y, n = blockIdx.z / heads, head = blockIdx.z - n * heads;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, gq8 = lane >> 2, tq = lane & 3;
+  const long long hoff = ((long long)n * planes + head * DP) * g.PL * 8;
+  const __nv_bfloat16* qb = q + hoff;
+  const __nv_bfloat16* gob = go + hoff;
+  const float* lrow = lse + ((long long)n * heads + head) * seq;
+  const float* drow = dsum + ((long long)n * heads + head) * seq;
+  const int r0 = min(k0 + warp * 16 + gq8, S - 1), r1 = min(k0 + warp * 16 + gq8 + 8, S - 1);
+  const __nv_bfloat16* kr0 = k + ((long long)n * S + r0) * C + head * D;
+  const __nv_bfloat16* kr1 = k + ((long long)n * S + r1) * C + head * D;
+  const __nv_bfloat16* vr0 = v + ((long long)n * S + r0) * C + head * D;
+  const __nv_bfloat16* vr1 = v + ((long long)n * S + r1) * C + head * D;
+  uint32_t ka[KS][4], va[KS][4];
+#pragma unroll
+  for (int j = 0; j < KS; ++j) {
+    ka[j][0] = *reinterpret_cast<const uint32_t*>(kr0 + 16 * j + 2 * tq);
+    ka[j][1] = *reinterpret_cast<const uint32_t*>(kr1 + 16 * j + 2 * tq);
+    ka[j][2] = *reinterpret_cast<const uint32_t*>(kr0 + 16 * j + 8 + 2 * tq);
+    ka[j][3] = *reinterpret_cast<const uint32_t*>(kr1 + 16 * j + 8 + 2 * tq);
+    va[j][0] = *reinterpret_cast<const uint32_t*>(vr0 + 16 * j + 2 * tq);
+    va[j][1] = *reinterpret_cast<const uint32_t*>(vr1 + 16 * j + 2 * tq);
+    va[j][2] = *reinterpret_cast<const uint32_t*>(vr0 + 16 * j + 8 + 2 * tq);
+    va[j][3] = *reinterpret_cast<const uint32_t*>(vr1 + 16 * j + 8 + 2 * tq);
+  }
+  float dk[DP][4], dv[DP][4];
+#pragma unroll
+  for (int i = 0; i < DP; ++i)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) { dk[i][e] = 0.f; dv[i][e] = 0.f; }
+  const uint32_t* qs32 = reinterpret_cast<const uint32_t*>(qs);
+  const uint32_t* do32 = reinterpret_cast<const uint32_t*>(dos);
+  const uint32_t qs_addr = smem_u32(qs), do_addr = smem_u32(dos);
+  const int t_end = min((split + 1) * per_split, (seq + 63) / 64);
+  for (int tile = split * per_split; tile < t_end; ++tile) {
+    const int q0 = tile * 64;
+    __syncthreads();
+    for (int i = threadIdx.x; i < DP * 64; i += 128) {
+      const int pl = i >> 6, qq = i & 63, qi = q0 + qq;
+      uint4 a = make_uint4(0, 0, 0, 0), b = make_uint4(0, 0, 0, 0);
+      if (qi < seq) {
+        const long long off = pf8_pixel(g, qi, W);
+        a = *reinterpret_cast<const uint4*>(qb + (long long)pl * g.PL * 8 + off);
+        b = *reinterpret_cast<const uint4*>(gob + (long long)pl * g.PL * 8 + off);
+      }
+      qs[pl][qq] = a;
+      dos[pl][qq] = b;
+    }
+    if (threadIdx.x < 64) {   // queries beyond seq: lse = +inf -> P = 0
+      const int qi = q0 + threadIdx.x;
+      ls[threadIdx.x] = qi < seq ? lrow[qi] : INFINITY;
+      dd[threadIdx.x] = qi < seq ? drow[qi] : 0.f;
+    }
+    __syncthreads();
+    float st[8][4], dpt[8][4];
+#pragma unroll
+    for (int t = 0; t < 8; ++t) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) { st[t][e] = 0.f; dpt[t][e] = 0.f; }
+#pragma unroll
+      for (int j = 0; j < KS; ++j) {
+        const int w0 = ((2 * j) * 64 + t * 8 + gq8) * 4 + tq, w1 = ((2 * j + 1) * 64 + t * 8 + gq8) * 4 + tq;
+        mma_bf16_16x8x16(st[t], ka[j][0], ka[j][1], ka[j][2], ka[j][3], qs32[w0], qs32[w1]);
+        mma_bf16_16x8x16(dpt[t], va[j][0], va[j][1], va[j][2], va[j][3], do32[w0], do32[w1]);
+      }
+    }
+#pragma unroll
+    for (int t = 0; t < 8; ++t)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int col = t * 8 + 2 * tq + (e & 1);
+        const float p = exp2f(st[t][e] * scale_log2 - ls[col]);
+        st[t][e] = p;
+        dpt[t][e] = p * (dpt[t][e] - dd[col]);
+      }
+#pragma unroll
+    for (int k16 = 0; k16 < 4; ++k16) {
+      const float* p0 = st[2 * k16];
+      const float* p1 = st[2 * k16 + 1];
+      const float* s0 = dpt[2 * k16];
+      const float* s1 = dpt[2 * k16 + 1];
+      const uint32_t pa0 = pack_bf16x2(p0[0], p0[1]), pa1 = pack_bf16x2(p0[2], p0[3]), pa2 = pack_bf16x2(p1[0], p1[1]),
+                     pa3 = pack_bf16x2(p1[2], p1[3]);
+      const uint32_t sa0 = pack_bf16x2(s0[0], s0[1]), sa1 = pack_bf16x2(s0[2], s0[3]), sa2 = pack_bf16x2(s1[0], s1[1]),
+                     sa3 = pack_bf16x2(s1[2], s1[3]);
+#pragma unroll
+      for (int i = 0; i < DP; ++i) {
+        uint32_t b0, b1;
+        ldsm_b_trans(b0, b1, do_addr, i, k16, lane);
+        mma_bf16_16x8x16(dv[i], pa0, pa1, pa2, pa3, b0, b1);
+        ldsm_b_trans(b0, b1, qs_addr, i, k16, lane);
+        mma_bf16_16x8x16(dk[i], sa0, sa1, sa2, sa3, b0, b1);
+      }
+    }
+  }
+  // accumulator (c0, c1) = (key row gq8, channels 8i + 2tq, +1), (c2, c3) = key row gq8 + 8
+  const size_t half = (size_t)nsplit * N * SP * C;
+  float* pk = part + (((size_t)split * N + n) * heads + head) * SP * D;
+  float* pv = pk + half;
+  const int ra = k0 + warp * 16 + gq8, rb = ra + 8;
+#pragma unroll
+  for (int i = 0; i < DP; ++i) {
+    *reinterpret_cast<float2*>(pk + (size_t)ra * D + 8 * i + 2 * tq) = make_float2(dk[i][0], dk[i][1]);
+    *reinterpret_cast<float2*>(pk + (size_t)rb * D + 8 * i + 2 * tq) = make_float2(dk[i][2], dk[i][3]);
+    *reinterpret_cast<float2*>(pv + (size_t)ra * D + 8 * i + 2 * tq) = make_float2(dv[i][0], dv[i][1]);
+    *reinterpret_cast<float2*>(pv + (size_t)rb * D + 8 * i + 2 * tq) = make_float2(dv[i][2], dv[i][3]);
+  }
+}
+
+// dk[n][s][c] = scale * sum over the splits (in order) of the dK partials; dv the same without the scale
+__global__ void __launch_bounds__(256) xattn_kv_reduce_kernel(const float* __restrict__ part, float* __restrict__ dk,
+                                                              float* __restrict__ dv, int N, int C, int heads, int S, int SP,
+                                                              int nsplit, float scale) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (long long)N * S * C) return;
+  const int D = C / heads;
+  const int c = (int)(idx % C), s = (int)((idx / C) % S), n = (int)(idx / ((long long)C * S));
+  const int head = c / D, d = c - head * D;
+  const size_t half = (size_t)nsplit * N * SP * C;
+  const size_t stride = (size_t)N * SP * C;   // one split
+  const float* pk = part + (((size_t)n * heads + head) * SP + s) * D + d;
+  float a = 0.f, b = 0.f;
+  for (int j = 0; j < nsplit; ++j) {
+    a += pk[j * stride];
+    b += pk[half + j * stride];
+  }
+  dk[idx] = a * scale;
+  dv[idx] = b;
+}
+
+template <int D>
+static cudaError_t xattn_bwd_launch(const __nv_bfloat16* q, const __nv_bfloat16* k, const __nv_bfloat16* v, const __nv_bfloat16* o,
+                                    const __nv_bfloat16* go, const float* lse, float* dsum, float* part, __nv_bfloat16* gq,
+                                    float* dk, float* dv, int N, int C, int heads, int H, int W, int S, cudaStream_t s) {
+  const int seq = H * W;
+  const float scale = 1.0f / sqrtf((float)D), sl2 = 1.4426950408889634f * scale;
+  const XattnSplit x = xattn_split(N, heads, H, W, S);
+  static const cudaError_t attr = cudaFuncSetAttribute(xattn_bwd_dq_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                       2 * (D / 8) * XATTN_MAX_S * (int)sizeof(uint4));
+  if (attr != cudaSuccess) return attr;
+  mha_bwd_dot_kernel<D><<<dim3((seq + 255) / 256, heads, N), 256, 0, s>>>(o, go, dsum, N, C, H, W);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  const size_t smem = (size_t)2 * (D / 8) * x.SP * sizeof(uint4);
+  xattn_bwd_dq_kernel<D><<<dim3((x.ntiles + XATTN_BWD_QT - 1) / XATTN_BWD_QT, heads, N), 128, smem, s>>>(
+      q, k, v, go, lse, dsum, gq, N, C, H, W, S, sl2, scale);
+  if ((e = cudaGetLastError()) != cudaSuccess) return e;
+  xattn_bwd_kv_kernel<D><<<dim3(x.SP / 64, x.nsplit, N * heads), 128, 0, s>>>(q, k, v, go, lse, dsum, part, N, C, heads, H, W,
+                                                                               S, x.per_split, sl2);
+  if ((e = cudaGetLastError()) != cudaSuccess) return e;
+  const long long tot = (long long)N * S * C;
+  xattn_kv_reduce_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, s>>>(part, dk, dv, N, C, heads, S, x.SP, x.nsplit, scale);
+  return cudaGetLastError();
+}
+cudaError_t launch_xattn_bwd(const __nv_bfloat16* q, const __nv_bfloat16* k, const __nv_bfloat16* v, const __nv_bfloat16* o,
+                             const __nv_bfloat16* go, const float* lse, float* dsum, float* part, __nv_bfloat16* gq, float* dk,
+                             float* dv, int N, int C, int heads, int H, int W, int S, cudaStream_t s) {
+  if (S < 1 || S > XATTN_MAX_S || C % heads) return cudaErrorInvalidValue;
+  const int D = C / heads;
+  if (D == 16) return xattn_bwd_launch<16>(q, k, v, o, go, lse, dsum, part, gq, dk, dv, N, C, heads, H, W, S, s);
+  if (D == 32) return xattn_bwd_launch<32>(q, k, v, o, go, lse, dsum, part, gq, dk, dv, N, C, heads, H, W, S, s);
+  if (D == 64) return xattn_bwd_launch<64>(q, k, v, o, go, lse, dsum, part, gq, dk, dv, N, C, heads, H, W, S, s);
+  return cudaErrorInvalidValue;
+}
+
+// dW[c][x] += sum_m G[m][c] E[m][x] for the K (blockIdx.z = 0) and V (1) projections: 64 x 64 output tiles, 256 threads
+// of 4 x 4 outputs, the token dimension in steps of 16 through shared memory (fixed order: deterministic).
+__global__ void __launch_bounds__(256) xattn_kv_wgrad_kernel(const float* __restrict__ dk, const float* __restrict__ dv,
+                                                             const float* __restrict__ enc, float* __restrict__ dwk,
+                                                             float* __restrict__ dwv, int M, int C, int X) {
+  __shared__ float gs[16][64], es[16][64];
+  const float* G = blockIdx.z ? dv : dk;
+  float* dw = blockIdx.z ? dwv : dwk;
+  const int c0 = blockIdx.y * 64, x0 = blockIdx.x * 64;
+  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+  float acc[4][4] = {};
+  for (int m0 = 0; m0 < M; m0 += 16) {
+    for (int i = threadIdx.x; i < 16 * 64; i += 256) {
+      const int r = i >> 6, col = i & 63, m = m0 + r;
+      gs[r][col] = (m < M && c0 + col < C) ? G[(long long)m * C + c0 + col] : 0.f;
+      es[r][col] = (m < M && x0 + col < X) ? enc[(long long)m * X + x0 + col] : 0.f;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int r = 0; r < 16; ++r) {
+      float a[4], b[4];
+#pragma unroll
+      for (int u = 0; u < 4; ++u) { a[u] = gs[r][ty * 4 + u]; b[u] = es[r][tx * 4 + u]; }
+#pragma unroll
+      for (int u = 0; u < 4; ++u)
+#pragma unroll
+        for (int w = 0; w < 4; ++w) acc[u][w] = fmaf(a[u], b[w], acc[u][w]);
+    }
+    __syncthreads();
+  }
+#pragma unroll
+  for (int u = 0; u < 4; ++u)
+#pragma unroll
+    for (int w = 0; w < 4; ++w) {
+      const int c = c0 + ty * 4 + u, x = x0 + tx * 4 + w;
+      if (c < C && x < X) dw[(long long)c * X + x] += acc[u][w];
+    }
+}
+cudaError_t launch_xattn_kv_wgrad(const float* dk, const float* dv, const float* enc, float* dwk, float* dwv, int M, int C,
+                                  int X, cudaStream_t s) {
+  xattn_kv_wgrad_kernel<<<dim3((X + 63) / 64, (C + 63) / 64, 2), 256, 0, s>>>(dk, dv, enc, dwk, dwv, M, C, X);
+  return cudaGetLastError();
+}
+
 }  // namespace b200ad

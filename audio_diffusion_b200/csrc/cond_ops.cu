@@ -247,4 +247,186 @@ cudaError_t launch_mha_flash(const __nv_bfloat16* qkv, __nv_bfloat16* out, int N
   return cudaGetLastError();
 }
 
+// ------------------------------------------------------------------------------------ cross-attention, S > 1 keys
+// attn2(x, enc) = to_out(softmax(q K^T / sqrt(D)) V) with q = to_q(LN2(x)) (a 1x1 conv of the plan), K = enc Wk^T and
+// V = enc Wv^T over the S tokens of the same sample.
+
+// K / V projections: one CTA = XKV_ROWS tokens (their encodings in shared memory), one thread per output channel of K | V;
+// each weight element is read once per CTA.  bf16 [N][S][C] out.
+constexpr int XKV_ROWS = 8;
+__global__ void __launch_bounds__(256) xattn_kv_kernel(const float* __restrict__ enc, const float* __restrict__ wk,
+                                                       const float* __restrict__ wv, __nv_bfloat16* __restrict__ k,
+                                                       __nv_bfloat16* __restrict__ v, int M, int C, int X) {
+  extern __shared__ float es[];   // [XKV_ROWS][X]
+  const int m0 = blockIdx.x * XKV_ROWS, rows = min(XKV_ROWS, M - m0);
+  for (int i = threadIdx.x; i < XKV_ROWS * X; i += blockDim.x) es[i] = i < rows * X ? enc[(long long)m0 * X + i] : 0.f;
+  __syncthreads();
+  for (int c = threadIdx.x; c < 2 * C; c += blockDim.x) {
+    const float* w = c < C ? wk + (long long)c * X : wv + (long long)(c - C) * X;
+    float a[XKV_ROWS];
+#pragma unroll
+    for (int r = 0; r < XKV_ROWS; ++r) a[r] = 0.f;
+    for (int x = 0; x < X; ++x) {
+      const float wx = __ldg(w + x);
+#pragma unroll
+      for (int r = 0; r < XKV_ROWS; ++r) a[r] = fmaf(wx, es[r * X + x], a[r]);
+    }
+    __nv_bfloat16* dst = c < C ? k + c : v + (c - C);
+#pragma unroll
+    for (int r = 0; r < XKV_ROWS; ++r)
+      if (r < rows) dst[(long long)(m0 + r) * C] = __float2bfloat16(a[r]);
+  }
+}
+cudaError_t launch_xattn_kv(const float* enc, const float* wk, const float* wv, __nv_bfloat16* k, __nv_bfloat16* v, int N, int S,
+                            int C, int X, cudaStream_t s) {
+  const int M = N * S;
+  xattn_kv_kernel<<<(M + XKV_ROWS - 1) / XKV_ROWS, 256, (size_t)XKV_ROWS * X * sizeof(float), s>>>(enc, wk, wv, k, v, M, C, X);
+  return cudaGetLastError();
+}
+
+__global__ void f32_to_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ dst, long long n) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) dst[i] = __float2bfloat16(src[i]);
+}
+cudaError_t launch_f32_to_bf16(const float* src, __nv_bfloat16* dst, long long n, cudaStream_t s) {
+  f32_to_bf16_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(src, dst, n);
+  return cudaGetLastError();
+}
+
+// Forward: one CTA = one (sample, head), K and V staged once, then XATTN_QT tiles of 64 queries (4 warps x 16 rows); keys
+// in tiles of 64 with the online softmax of mha_flash_kernel (exp2 domain, P V by transposing ldmatrix).  Keys S..SP-1
+// are masked; 8-key column tiles and 16-key P V steps wholly beyond S are skipped (warp-uniform).
+constexpr int XATTN_QT = 4;
+template <int D, bool LSE>
+__global__ void __launch_bounds__(128) xattn_fwd_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
+                                                        const __nv_bfloat16* __restrict__ v, __nv_bfloat16* __restrict__ out,
+                                                        int N, int C, int H, int W, int S, float scale_log2,
+                                                        float* __restrict__ lse) {
+  constexpr int DP = D / 8, KS = D / 16;
+  extern __shared__ __align__(16) uint4 xsm[];
+  const int SP = (S + 63) & ~63;
+  uint4* ks = xsm;
+  uint4* vs = xsm + DP * SP;
+  const Geom g = make_geom(N, H, W);
+  const int seq = H * W, planes = C >> 3, heads = gridDim.y;
+  const int head = blockIdx.y, n = blockIdx.z;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, gq = lane >> 2, tq = lane & 3;
+  xattn_stage_kv<D>(ks, vs, k, v, n, head, C, S, SP);
+  __syncthreads();
+  const uint32_t* ks32 = reinterpret_cast<const uint32_t*>(ks);
+  const uint32_t vs_addr = smem_u32(vs);
+  const __nv_bfloat16* qb = q + ((long long)n * planes + head * DP) * g.PL * 8;
+  __nv_bfloat16* ob = out + ((long long)n * planes + head * DP) * g.PL * 8;
+  const int ntiles = (seq + 63) / 64;
+  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    const int q0 = tile * 64;
+    const int r0 = min(q0 + warp * 16 + gq, seq - 1), r1 = min(q0 + warp * 16 + gq + 8, seq - 1);
+    const long long o0 = pf8_pixel(g, r0, W), o1 = pf8_pixel(g, r1, W);
+    uint32_t qa[KS][4];
+#pragma unroll
+    for (int j = 0; j < KS; ++j) {
+      qa[j][0] = *reinterpret_cast<const uint32_t*>(qb + (long long)(2 * j) * g.PL * 8 + o0 + 2 * tq);
+      qa[j][1] = *reinterpret_cast<const uint32_t*>(qb + (long long)(2 * j) * g.PL * 8 + o1 + 2 * tq);
+      qa[j][2] = *reinterpret_cast<const uint32_t*>(qb + (long long)(2 * j + 1) * g.PL * 8 + o0 + 2 * tq);
+      qa[j][3] = *reinterpret_cast<const uint32_t*>(qb + (long long)(2 * j + 1) * g.PL * 8 + o1 + 2 * tq);
+    }
+    float oacc[DP][4];
+#pragma unroll
+    for (int i = 0; i < DP; ++i) { oacc[i][0] = oacc[i][1] = oacc[i][2] = oacc[i][3] = 0.f; }
+    float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+    for (int k0 = 0; k0 < S; k0 += 64) {
+      float sc[8][4];
+#pragma unroll
+      for (int t = 0; t < 8; ++t) {
+        sc[t][0] = sc[t][1] = sc[t][2] = sc[t][3] = 0.f;
+        if (k0 + t * 8 < S) {
+#pragma unroll
+          for (int j = 0; j < KS; ++j) {
+            const uint32_t b0 = ks32[((2 * j) * SP + k0 + t * 8 + gq) * 4 + tq];
+            const uint32_t b1 = ks32[((2 * j + 1) * SP + k0 + t * 8 + gq) * 4 + tq];
+            mma_bf16_16x8x16(sc[t], qa[j][0], qa[j][1], qa[j][2], qa[j][3], b0, b1);
+          }
+        }
+      }
+      float mx0 = m0, mx1 = m1;
+#pragma unroll
+      for (int t = 0; t < 8; ++t) {
+        const int key = k0 + t * 8 + 2 * tq;
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const float x = (key + (e & 1) < S) ? sc[t][e] * scale_log2 : -INFINITY;
+          sc[t][e] = x;
+          if (e < 2) mx0 = fmaxf(mx0, x); else mx1 = fmaxf(mx1, x);
+        }
+      }
+      mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1)); mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+      mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1)); mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+      const float c0 = exp2f(m0 - mx0), c1 = exp2f(m1 - mx1);
+      m0 = mx0; m1 = mx1;
+      l0 *= c0; l1 *= c1;
+#pragma unroll
+      for (int i = 0; i < DP; ++i) { oacc[i][0] *= c0; oacc[i][1] *= c0; oacc[i][2] *= c1; oacc[i][3] *= c1; }
+#pragma unroll
+      for (int kb16 = 0; kb16 < 4; ++kb16) {
+        if (k0 + kb16 * 16 >= S) continue;
+        float* s0 = sc[2 * kb16];
+        float* s1 = sc[2 * kb16 + 1];
+        const float e00 = exp2f(s0[0] - m0), e01 = exp2f(s0[1] - m0), e02 = exp2f(s0[2] - m1), e03 = exp2f(s0[3] - m1);
+        const float e10 = exp2f(s1[0] - m0), e11 = exp2f(s1[1] - m0), e12 = exp2f(s1[2] - m1), e13 = exp2f(s1[3] - m1);
+        l0 += (e00 + e01) + (e10 + e11);
+        l1 += (e02 + e03) + (e12 + e13);
+        const uint32_t pa0 = pack_bf16x2(e00, e01), pa1 = pack_bf16x2(e02, e03), pa2 = pack_bf16x2(e10, e11),
+                       pa3 = pack_bf16x2(e12, e13);
+#pragma unroll
+        for (int i = 0; i < DP; ++i) {
+          uint32_t vb0, vb1;
+          const uint32_t va = vs_addr + (uint32_t)((i * SP + k0 + kb16 * 16 + (lane & 15)) * 16);
+          asm volatile("ldmatrix.sync.aligned.m8n8.x2.trans.shared.b16 {%0,%1}, [%2];" : "=r"(vb0), "=r"(vb1) : "r"(va));
+          mma_bf16_16x8x16(oacc[i], pa0, pa1, pa2, pa3, vb0, vb1);
+        }
+      }
+    }
+    l0 += __shfl_xor_sync(0xffffffffu, l0, 1); l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+    l1 += __shfl_xor_sync(0xffffffffu, l1, 1); l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+    const float i0 = 1.0f / l0, i1 = 1.0f / l1;
+    const int q_a = q0 + warp * 16 + gq, q_b = q_a + 8;
+#pragma unroll
+    for (int i = 0; i < DP; ++i) {
+      if (q_a < seq) *reinterpret_cast<uint32_t*>(ob + (long long)i * g.PL * 8 + o0 + 2 * tq) = pack_bf16x2(oacc[i][0] * i0, oacc[i][1] * i0);
+      if (q_b < seq) *reinterpret_cast<uint32_t*>(ob + (long long)i * g.PL * 8 + o1 + 2 * tq) = pack_bf16x2(oacc[i][2] * i1, oacc[i][3] * i1);
+    }
+    if (LSE && tq == 0) {
+      float* lr = lse + ((long long)n * heads + head) * seq;
+      if (q_a < seq) lr[q_a] = m0 + __log2f(l0);
+      if (q_b < seq) lr[q_b] = m1 + __log2f(l1);
+    }
+  }
+}
+
+template <int D, bool LSE>
+static cudaError_t xattn_launch(const __nv_bfloat16* q, const __nv_bfloat16* k, const __nv_bfloat16* v, __nv_bfloat16* out, int N,
+                                int C, int heads, int H, int W, int S, cudaStream_t s, float* lse) {
+  const size_t smem = (size_t)2 * (D / 8) * ((S + 63) & ~63) * sizeof(uint4);
+  static const cudaError_t attr = cudaFuncSetAttribute(xattn_fwd_kernel<D, LSE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                       2 * (D / 8) * XATTN_MAX_S * (int)sizeof(uint4));
+  if (attr != cudaSuccess) return attr;
+  const int ntiles = (H * W + 63) / 64;
+  const dim3 grid((ntiles + XATTN_QT - 1) / XATTN_QT, heads, N);
+  xattn_fwd_kernel<D, LSE><<<grid, 128, smem, s>>>(q, k, v, out, N, C, H, W, S, 1.4426950408889634f / sqrtf((float)D), lse);
+  return cudaGetLastError();
+}
+cudaError_t launch_xattn(const __nv_bfloat16* q, const __nv_bfloat16* k, const __nv_bfloat16* v, __nv_bfloat16* out, int N,
+                         int C, int heads, int H, int W, int S, cudaStream_t s, float* lse) {
+  if (S < 1 || S > XATTN_MAX_S || C % heads) return cudaErrorInvalidValue;
+  const int D = C / heads;
+  // inference (lse null) runs an instantiation without the log-sum-exp store
+  if (D == 16) return lse ? xattn_launch<16, true>(q, k, v, out, N, C, heads, H, W, S, s, lse)
+                          : xattn_launch<16, false>(q, k, v, out, N, C, heads, H, W, S, s, nullptr);
+  if (D == 32) return lse ? xattn_launch<32, true>(q, k, v, out, N, C, heads, H, W, S, s, lse)
+                          : xattn_launch<32, false>(q, k, v, out, N, C, heads, H, W, S, s, nullptr);
+  if (D == 64) return lse ? xattn_launch<64, true>(q, k, v, out, N, C, heads, H, W, S, s, lse)
+                          : xattn_launch<64, false>(q, k, v, out, N, C, heads, H, W, S, s, nullptr);
+  return cudaErrorInvalidValue;
+}
+
 }  // namespace b200ad

@@ -122,6 +122,16 @@ cudaError_t launch_cross_attn_vec(const float* enc, const float* wv, const float
 // lse (optional, training): row log-sum-exp fp32 [N][heads][H*W] for the backward (log2 domain of the scaled scores)
 cudaError_t launch_mha_flash(const __nv_bfloat16* qkv, __nv_bfloat16* out, int N, int C, int heads, int H, int W, cudaStream_t s,
                              float* lse = nullptr);
+// cross-attention against an encoding of S > 1 tokens (1 <= S <= XATTN_MAX_S).  K / V: bf16 [N][S][C] (token-major).
+constexpr int XATTN_MAX_S = 256;
+// enc fp32 [N][S][X] -> K = enc Wk^T, V = enc Wv^T (wk, wv fp32 [C][X])
+cudaError_t launch_xattn_kv(const float* enc, const float* wk, const float* wv, __nv_bfloat16* k, __nv_bfloat16* v, int N, int S,
+                            int C, int X, cudaStream_t s);
+// fp32 -> bf16, n elements (the parity entry point's K / V)
+cudaError_t launch_f32_to_bf16(const float* src, __nv_bfloat16* dst, long long n, cudaStream_t s);
+// q, out: PF8 with C channels; 8 heads of dim C / heads in {16, 32, 64}; lse (optional, training) as launch_mha_flash's
+cudaError_t launch_xattn(const __nv_bfloat16* q, const __nv_bfloat16* k, const __nv_bfloat16* v, __nv_bfloat16* out, int N,
+                         int C, int heads, int H, int W, int S, cudaStream_t s, float* lse = nullptr);
 
 // generic single-head attention over the fused qkv tensor (AutoencoderKL mid block); scores: N * seq * seq floats of scratch
 cudaError_t launch_attention_1head(const __nv_bfloat16* qkv, __nv_bfloat16* out, float* scores, int N, int C, int H, int W,
@@ -130,5 +140,26 @@ cudaError_t launch_attention_1head(const __nv_bfloat16* qkv, __nv_bfloat16* out,
 cudaError_t launch_vae_sample(const __nv_bfloat16* enc, const float* wq, const float* bq, const float* noise, float* z,
                               float* moments, int N, int C, int L, int H, int W, cudaStream_t s);
 cudaError_t launch_mix1x1(const float* x, const float* w, const float* b, float* y, int N, int L, int HW, cudaStream_t s);
+
+// Stages the K and V of one (sample, head) in shared memory as [plane][key] rows of 8 channels, keys S..SP-1 zero
+// (the layout mha_flash_kernel streams its key tiles in).  The forward (cond_ops.cu) and the
+// backward (cond_bwd.cu) kernels of the cross-attention share it.
+template <int D>
+__device__ __forceinline__ void xattn_stage_kv(uint4* ks, uint4* vs, const __nv_bfloat16* k, const __nv_bfloat16* v, int n,
+                                               int head, int C, int S, int SP) {
+  constexpr int DP = D / 8;
+  const __nv_bfloat16* kg = k + (long long)n * S * C + head * D;
+  const __nv_bfloat16* vg = v + (long long)n * S * C + head * D;
+  for (int i = threadIdx.x; i < DP * SP; i += blockDim.x) {
+    const int key = i / DP, pl = i - key * DP;
+    uint4 a = make_uint4(0, 0, 0, 0), b = make_uint4(0, 0, 0, 0);
+    if (key < S) {
+      a = *reinterpret_cast<const uint4*>(kg + (long long)key * C + pl * 8);
+      b = *reinterpret_cast<const uint4*>(vg + (long long)key * C + pl * 8);
+    }
+    ks[pl * SP + key] = a;
+    vs[pl * SP + key] = b;
+  }
+}
 
 }  // namespace b200ad

@@ -45,14 +45,17 @@ enum OpKind { OP_TEMB = 0, OP_CONV_IN = 1, OP_GN = 2, OP_CONV = 3, OP_PARITY = 5
               OP_PACK_T /* transposed weight packs of a backward plan */, OP_DGRAD, OP_WGRAD, OP_GN_BWD, OP_CHANSUM,
               OP_REDUCE_N, OP_SCATTER, OP_PF8ADD, OP_ATTN_BWD, OP_UNFOLD, OP_SCALAR_WGRAD, OP_CONV_IN_BWD, OP_FLIP, OP_SUMADD,
               OP_LIN_IN, OP_LIN_W, OP_SILU_BWD, OP_SILU_FWD, OP_MEMSET, OP_LN_BWD, OP_GEGLU_BWD, OP_XVEC_BWD, OP_MHA_BWD,
-              OP_ATTN1_BWD, OP_QUANT_BWD, OP_LATENT_IN_BWD, OP_NKINDS };
+              OP_ATTN1_BWD, OP_QUANT_BWD, OP_LATENT_IN_BWD,
+              OP_XKV /* cross-attention K / V projections of an S > 1 encoding */, OP_XATTN /* cross-attention, S > 1 */,
+              OP_XATTN_BWD, OP_XKV_BWD, OP_NKINDS };
 // by OpKind: error messages and the backward profile's keys (tools/cond_train_bench.py matches "mha_bwd x<count>")
 static const char* const op_names[] = {
     "temb", "conv_in", "gn_finalize", "conv_tc", "", "parity_split", "attention", "conv_out", "attention_1head", "vae_sample",
     "mix1x1", "layernorm", "geglu", "mha", "cross_attn_vec", "gn_apply", "pack_transposed", "conv_tc(dgrad)", "wgrad_tc",
     "gn_bwd", "chan_sum", "reduce_n", "scatter", "pf8_add", "attention_bwd", "unfold_up2", "scalar_wgrad", "conv_in(dgrad)",
     "flip", "sum_add", "lin_in", "lin_w", "silu_bwd", "silu_fwd", "memset", "layernorm_bwd", "geglu_bwd",
-    "cross_attn_vec_bwd", "mha_bwd", "attention_1head_bwd", "quant_conv_bwd", "latent_in_bwd"};
+    "cross_attn_vec_bwd", "mha_bwd", "attention_1head_bwd", "quant_conv_bwd", "latent_in_bwd", "cross_attn_kv", "cross_attn",
+    "cross_attn_bwd", "cross_attn_kv_wgrad"};
 static_assert(sizeof(op_names) / sizeof(op_names[0]) == OP_NKINDS, "one name per OpKind");
 
 struct RunArgs {                        // the per-call inputs of a plan
@@ -148,6 +151,7 @@ struct Block {
   // byte offsets in the packed arena, assigned by the layout pass
   size_t conv1[2] = {}, conv2 = 0, shortcut[2] = {};    // resnet K-segments: conv1 over (input, skip), conv2, 1x1 shortcut
   size_t qkv = 0, out = 0;                              // attention / attn1: q | k | v projection, to_out
+  size_t q2 = 0, out2 = 0;                              // transformer attn2 (encodings of S > 1 tokens): to_q, to_out
   size_t proj_in = 0, ff1 = 0, ff2 = 0, proj_out = 0;   // transformer
   size_t seg[4] = {};                                   // down / up: one K-segment per parity; latent out: conv_out
   size_t ident = 0;                                     // identity block of the residual K-segment
@@ -178,6 +182,8 @@ struct Plan {    // everything a plan builder derives from the workspace and (N,
   float* temb_u2 = nullptr;          // training: [N][4 dim0] linear_2 output before SiLU
   float* zq = nullptr;               // autoencoder: post_quant_conv(z), [N][L][h][w]
   std::map<std::string, float*> lse; // training, conditional U-Net: attn1's row log-sum-exp [N][heads][H*W] by block name
+                                     // (attn2's, S > 1: by block name + ".attn2")
+  std::map<std::string, __nv_bfloat16*> xkv; // training, S > 1: attn2's K | V, bf16 [N][S][C] each, by block name
   std::map<std::string, float*> probs; // training, autoencoder: the single-head attention's softmax P [N][HW][HW] by block name
   float* z_in = nullptr;             // training, autoencoder: the decoder's input latents [N][L][h][w] (post_quant_conv wgrad)
   size_t ws_bytes = 0;
@@ -210,8 +216,13 @@ struct NetBase {
   int num_sms = 132;
   const float* enc = nullptr;       // conditional U-Net: encoder_hidden_states [N][enc_S][X] of the next forward
   int enc_S = 0;
+  int enc_len = 1;                  // conditional U-Net: the encoder sequence length the next workspace plan is built for
+  int plan_enc_len = 1;             // ... and the one the bound plan was built for
   int last_launches = 0;
   PackBatch pack_batch;             // device job table of the weight packing (one launch for all K-segments)
+  std::vector<PackJob> xjobs;       // conditional U-Net: the K-segments only S > 1 plans read (layout_attn2)
+  PackBatch xpack_batch;
+  bool xpacked = false;             // xjobs packed from the current parameters
   // backward: one plan per part (U-Net: the whole model; autoencoder: encoder, decoder), built by bind_backward
   int nparts = 1;
   Backward* bwd[2] = {};
@@ -340,14 +351,14 @@ static void p_block(NetBase* h, const Block& k) {
 
 // ================================================================================= packed-weight arena layout
 static size_t add_job(NetBase* h, Bump& b, const std::string& wname, int cout, int cin_total, int K, int cin_off,
-                      int cin_cnt, const TapSet& taps, int cout_real = -1) {
+                      int cin_cnt, const TapSet& taps, int cout_real = -1, std::vector<PackJob>* list = nullptr) {
   PackJob j;
   j.w_param = h->pidx.at(wname);
   j.cout = cout; j.cin_total = cin_total; j.KH = K; j.KW = K; j.cin_off = cin_off; j.ksteps = cin_cnt / 16;
   j.taps = taps.pack;
   j.cout_real = cout_real;
   j.off = take_off(b, (size_t)(cout / 128) * j.ksteps * taps.pack.ntaps * CONV_B_TAP);
-  h->jobs.push_back(j);
+  (list ? *list : h->jobs).push_back(j);
   return j.off;
 }
 static size_t add_ident(NetBase* h, Bump& b, int ch) {  // identity weight blocks for residual-as-K-segment
@@ -413,6 +424,15 @@ static void layout_transformer(NetBase* h, Bump& b, Block& k) {
   k.proj_out = add_job(h, b, n + ".proj_out.weight", c, c, 1, 0, c, taps_conv(1));
   k.ident = add_ident(h, b, c);
 }
+// attn2's to_q and to_out of a transformer block, read only by plans for encodings of S > 1 tokens: their own job list
+// at the end of the arena, packed only while such a plan is bound (pack_xattn), so a one-token model packs what it did
+// before this path existed.
+static void layout_attn2(NetBase* h, Bump& b, Block& k) {
+  const std::string t = k.name + ".transformer_blocks.0";
+  const int c = k.cout;
+  k.q2 = add_job(h, b, t + ".attn2.to_q.weight", c, c, 1, 0, c, taps_conv(1), -1, &h->xjobs);
+  k.out2 = add_job(h, b, t + ".attn2.to_out.0.weight", c, c, 1, 0, c, taps_conv(1), -1, &h->xjobs);
+}
 static void layout_block(NetBase* h, Bump& b, Block& k) {
   switch (k.kind) {
     case BK_RESNET: layout_resnet(h, b, k); break;
@@ -471,6 +491,18 @@ static int pack_common(NetBase* h, cudaStream_t st) {
   return 0;
 }
 
+// Packs the K-segments only plans for S > 1 encoder tokens read (after pptr / packed are set).
+static int pack_xattn(NetBase* h, cudaStream_t st) {
+  if (!h->xjobs.empty()) {
+    std::vector<PackItem> items;
+    items.reserve(h->xjobs.size());
+    for (const PackJob& j : h->xjobs) items.push_back(make_pack_item(h, j, h->packed));
+    CK(launch_pack_batch(h->xpack_batch, items, st));
+  }
+  h->xpacked = true;
+  return 0;
+}
+
 // ================================================================================= launch plan
 // a conv writing `out` (its work decomposition, tiles per item and item count, is filled in by launch_conv_tc)
 static ConvParams conv_geom(int N, const Act& out) {
@@ -505,6 +537,7 @@ struct Builder {
   int heads = 8;                    // transformer: attention heads
   bool nopool = false;  // B200AD_DEBUG_NOPOOL=1: every activation gets its own buffer (per-layer parity taps)
   bool single_head = false;  // attention with one head of dim C (AutoencoderKL mid block) instead of head_dim 8
+  std::map<size_t, size_t> kv_pool;  // the workspace offsets of attn2's K | V buffers (S > 1) by size: shared unless nopool
 
   Act alloc(int C, int H, int W, bool stats) {
     Act a = take_act(ws, N, C, H, W);
@@ -686,29 +719,68 @@ struct Builder {
     conv(p);
   }
 
-  // Transformer2DModel with one BasicTransformerBlock (conditional U-Net), encoder sequence length 1:
-  //   h0 = proj_in(GroupNorm(x));  h2 = h0 + attn1(LN1(h0)) + attn2(enc);  h3 = h2 + ff(LN3(h2));  out = proj_out(h3) + x
-  // attn2 with ONE key is the per-sample vector to_out(to_v(enc)) (softmax over a single key is 1): it rides on the
-  // per-sample additive term of the attn1 output projection.
+  // LayerNorm over channels (eps 1e-5) of src into dst
+  void layer_norm(const Act& src, const Act& dst, const std::string& nm) {
+    emit(OP_LN, [x = src.p, y = dst.p, g = P(nm + ".weight"), b = P(nm + ".bias"), N = N, C = src.C, H = src.H,
+                 W = src.W](const RunArgs&, cudaStream_t s) { return launch_layernorm_pf8(x, y, g, b, N, C, H, W, 1e-5f, s); });
+  }
+
+  // attn2 of a transformer block against an encoding of S > 1 tokens, on h1 = h0 + attn1(LN1(h0)):
+  //   h2 = h1 + to_out(xattn(to_q(LN2(h1)), enc Wk^T, enc Wv^T))
+  Act cross_attention(const Block& k, const Act& h1, int S) {
+    const std::string& n = k.name;
+    const std::string t = n + ".transformer_blocks.0";
+    const int C = h1.C, H = h1.H, W = h1.W;
+    Act n2 = pooled("tf_ln", C, H, W, false);
+    layer_norm(h1, n2, t + ".norm2");
+    Act q2 = pooled("tf_q2", C, H, W, false);
+    linear(q2, n2, k.q2, nullptr);
+    const size_t kv_bytes = (size_t)2 * N * S * C * sizeof(__nv_bfloat16);
+    auto it = kv_pool.find(kv_bytes);
+    if (nopool || it == kv_pool.end()) it = kv_pool.insert_or_assign(kv_bytes, take_off(ws, kv_bytes)).first;
+    __nv_bfloat16* kv = ws.base ? (__nv_bfloat16*)(ws.base + it->second) : nullptr;
+    if (h->training) built->xkv[n] = kv;
+    emit(OP_XKV, [h = h, wk = P(t + ".attn2.to_k.weight"), wv = P(t + ".attn2.to_v.weight"), kv, N = N, S, C,
+                  X = k.cross](const RunArgs&, cudaStream_t s) {
+      return launch_xattn_kv(h->enc, wk, wv, kv, kv + (size_t)N * S * C, N, S, C, X, s);
+    });
+    Act ao2 = pooled("tf_ao", C, H, W, false);    // attn1's output is dead after h1
+    float* lse = h->training ? built->lse[n + ".attn2"] = (float*)ws.take((size_t)N * heads * H * W * sizeof(float)) : nullptr;
+    emit(OP_XATTN, [q = q2.p, kv, o = ao2.p, N = N, C, heads = heads, H, W, S, lse](const RunArgs&, cudaStream_t s) {
+      return launch_xattn(q, kv, kv + (size_t)N * S * C, o, N, C, heads, H, W, S, s, lse);
+    });
+    Act h2 = pooled("tf_h2", C, H, W, false);
+    linear(h2, ao2, k.out2, P(t + ".attn2.to_out.0.bias"), nullptr, &h1, k.ident);
+    if (h->training) {
+      built->taps[n + ".n2"] = n2;
+      built->taps[n + ".q2"] = q2;
+      built->taps[n + ".ao2"] = ao2;
+    }
+    return h2;
+  }
+
+  // Transformer2DModel with one BasicTransformerBlock (conditional U-Net):
+  //   h0 = proj_in(GroupNorm(x));  h1 = h0 + attn1(LN1(h0));  h2 = h1 + attn2(LN2(h1), enc);  h3 = h2 + ff(LN3(h2));
+  //   out = proj_out(h3) + x
+  // Encoder sequence length S = 1: attn2 with ONE key is the per-sample vector to_out(to_v(enc)) (softmax over a single
+  // key is 1): it rides on the per-sample additive term of the attn1 output projection, and h1 is never formed.
+  // S > 1: cross_attention.
   Act transformer(const Block& k, const Act& x) {
     const std::string& n = k.name;
-    const int C = x.C, H = x.H, W = x.W;
+    const int C = x.C, H = x.H, W = x.W, S = h->enc_len;
     const std::string t = n + ".transformer_blocks.0";
     const float2* ssx = gn_finalize(x, nullptr, n + ".norm", 1e-6f);
-    float* vec = (float*)ws.take((size_t)N * C * sizeof(float));
-    emit(OP_XVEC, [h = h, wv = P(t + ".attn2.to_v.weight"), wo = P(t + ".attn2.to_out.0.weight"),
-                   bo = P(t + ".attn2.to_out.0.bias"), vec, N = N, C, X = k.cross](const RunArgs&, cudaStream_t s) {
-      return launch_cross_attn_vec(h->enc, wv, wo, bo, vec, N, C, X, s);
-    });
+    float* vec = nullptr;
+    if (S == 1) {
+      vec = (float*)ws.take((size_t)N * C * sizeof(float));
+      emit(OP_XVEC, [h = h, wv = P(t + ".attn2.to_v.weight"), wo = P(t + ".attn2.to_out.0.weight"),
+                     bo = P(t + ".attn2.to_out.0.bias"), vec, N = N, C, X = k.cross](const RunArgs&, cudaStream_t s) {
+        return launch_cross_attn_vec(h->enc, wv, wo, bo, vec, N, C, X, s);
+      });
+    }
     Act h0 = pooled("tf_h0", C, H, W, false);
     linear(h0, x, k.proj_in, P(n + ".proj_in.bias"), ssx);
     Act n1 = pooled("tf_ln", C, H, W, false);
-    auto layer_norm = [&](const Act& src, const Act& dst, const std::string& nm) {
-      emit(OP_LN, [x = src.p, y = dst.p, g = P(nm + ".weight"), b = P(nm + ".bias"), N = N, C, H, W](const RunArgs&,
-                                                                                                      cudaStream_t s) {
-        return launch_layernorm_pf8(x, y, g, b, N, C, H, W, 1e-5f, s);
-      });
-    };
     layer_norm(h0, n1, t + ".norm1");
     Act qkv = pooled("tf_qkv", 3 * C, H, W, false);
     linear(qkv, n1, k.qkv, nullptr);
@@ -717,8 +789,16 @@ struct Builder {
     emit(OP_MHA, [q = qkv.p, o = ao.p, N = N, C, heads = heads, H, W, lse](const RunArgs&, cudaStream_t s) {
       return launch_mha_flash(q, o, N, C, heads, H, W, s, lse);
     });
-    Act h2 = pooled("tf_h2", C, H, W, false);
-    linear(h2, ao, k.out, P(t + ".attn1.to_out.0.bias"), nullptr, &h0, k.ident, vec, C);
+    Act h2;
+    if (S == 1) {
+      h2 = pooled("tf_h2", C, H, W, false);
+      linear(h2, ao, k.out, P(t + ".attn1.to_out.0.bias"), nullptr, &h0, k.ident, vec, C);
+    } else {
+      Act h1 = pooled("tf_h1", C, H, W, false);
+      linear(h1, ao, k.out, P(t + ".attn1.to_out.0.bias"), nullptr, &h0, k.ident);
+      built->taps[n + ".attn1"] = h1;
+      h2 = cross_attention(k, h1, S);
+    }
     Act n3 = pooled("tf_ln", C, H, W, false);     // the same buffer as n1 unless training
     layer_norm(h2, n3, t + ".norm3");
     Act ff1 = pooled("tf_ff1", 8 * C, H, W, false);
@@ -727,7 +807,7 @@ struct Builder {
     emit(OP_GEGLU, [x = ff1.p, y = gg.p, N = N, C, H, W](const RunArgs&, cudaStream_t s) {
       return launch_geglu_pf8(x, y, N, 4 * C, H, W, s);
     });
-    Act h3 = pooled("tf_h0", C, H, W, false);     // h0 is dead after h2
+    Act h3 = pooled("tf_h0", C, H, W, false);     // h0 is dead after h2 (S > 1: after h1)
     linear(h3, gg, k.ff2, P(t + ".ff.net.2.bias"), nullptr, &h2, k.ident);
     Act out = output(k, C, H, W);
     linear(out, h3, k.proj_out, P(n + ".proj_out.bias"), nullptr, &x, k.ident);

@@ -97,6 +97,8 @@ extern "C" int b200ad_unet_create(const b200ad_unet_config* cfg, b200ad_unet** o
   const int D = cfg->block_out_channels[0] * 4;
   h->off_wcat = take_off(b, (size_t)h->temb_rows * D * 4);
   h->off_bcat = take_off(b, (size_t)h->temb_rows * 4);
+  for (Block& k : h->blocks)
+    if (k.kind == BK_TRANSFORMER) layout_attn2(h, b, k);
   h->packed_bytes = (b.off + 255) & ~(size_t)255;
   h->pptr.assign(h->params.size(), nullptr);
   *out = h;
@@ -119,6 +121,8 @@ extern "C" int b200ad_unet_set_params(b200ad_unet* h, const float* const* params
   for (size_t i = 0; i < h->params.size(); ++i) h->pptr[i] = params[i];
   h->packed = (uint8_t*)packed;
   if (pack_common(h, st)) return -1;
+  h->xpacked = false;
+  if ((h->plan_enc_len > 1 || h->enc_len > 1) && pack_xattn(h, st)) return -1;   // else packed when such a plan is bound
   // concatenated time_emb_proj weights / biases
   const int D = h->cfg.block_out_channels[0] * 4;
   for (const Block& k : h->blocks) {
@@ -149,6 +153,7 @@ static Plan build_plan(const b200ad_unet* h, uint8_t* ws_base, int N, int H, int
   for (int pass = 0; pass < 2; ++pass) {
     l.ops.clear();
     B.pool.clear();
+    B.kv_pool.clear();
     pl.taps.clear();
     B.st.base = pass == 0 ? nullptr : ws_base;
     B.st.off = 0;
@@ -168,15 +173,34 @@ extern "C" size_t b200ad_unet_workspace_bytes(const b200ad_unet* h, int N, int H
 }
 
 extern "C" int b200ad_unet_bind_workspace(b200ad_unet* h, void* workspace, size_t bytes, int N, int H, int W, void* stream) {
-  return bind_workspace(h, build_plan, workspace, bytes, N, H, W, (cudaStream_t)stream);
+  if (bind_workspace(h, build_plan, workspace, bytes, N, H, W, (cudaStream_t)stream)) return -1;
+  h->plan_enc_len = h->enc_len;
+  if (h->plan_enc_len > 1 && !h->xpacked && pack_xattn(h, (cudaStream_t)stream)) return -1;
+  return 0;
+}
+
+extern "C" int b200ad_unet_set_encoder_len(b200ad_unet* h, int S) {
+  if (!h) return set_err("null handle");
+  if (!h->cfg.cross_attention_dim) return set_err("set_encoder_len: this U-Net is unconditional");
+  if (S < 1 || S > XATTN_MAX_S) return set_err("set_encoder_len: encoder sequence length %d outside [1, %d]", S, XATTN_MAX_S);
+  h->enc_len = S;
+  return 0;
+}
+
+// The bound encoding must have the token count the bound plan was built for (its K / V buffers, its op list).
+static int check_encoding(const b200ad_unet* h, const char* what) {
+  if (!h->cfg.cross_attention_dim) return 0;
+  if (!h->enc) return set_err("conditional U-Net: call b200ad_unet_set_encoding before %s", what);
+  if (h->plan_enc_len > 1 && !h->xpacked) return set_err("conditional U-Net: weights not packed for the bound plan");
+  if (h->enc_S != h->plan_enc_len)
+    return set_err("conditional U-Net: the encoding has %d tokens but the workspace is planned for %d (call "
+                   "b200ad_unet_set_encoder_len(%d) and bind the workspace again)", h->enc_S, h->plan_enc_len, h->enc_S);
+  return 0;
 }
 
 static int run_plan(b200ad_unet* h, const RunArgs& a, cudaStream_t st, OpEvents* timing = nullptr) {
   if (h->plan.lists.empty()) return set_err("bind_workspace must be called before forward");
-  if (h->cfg.cross_attention_dim) {   // the transformer blocks read the encoding
-    if (!h->enc) return set_err("conditional U-Net: call b200ad_unet_set_encoding before forward");
-    if (h->enc_S != 1) return set_err("conditional U-Net: encoder sequence length %d (only 1 is implemented)", h->enc_S);
-  }
+  if (check_encoding(h, "forward")) return -1;   // the transformer blocks read the encoding
   return run_ops(h, h->plan.lists[0], a, st, &h->last_launches, timing);
 }
 

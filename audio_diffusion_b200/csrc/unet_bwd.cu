@@ -35,6 +35,7 @@ struct Backward {
   float* grads = nullptr;
   int launches = 0;
   PackBatch pack_batch;              // one launch for all transposed packs
+  int enc_len = 1;                   // conditional U-Net: the encoder sequence length the plan was built for
   // the builder's gradient tensors by forward tap name (arena tensors of their own, final once the plan has run):
   // the whole gradient, and the share of it a skip connection brought (debug_grad)
   std::map<std::string, Act> grad, skipgrad;
@@ -323,10 +324,11 @@ struct BwdBuilder {
 
   // Transformer2DModel with one BasicTransformerBlock (Builder::transformer) in reverse, from G(out) to G(x):
   //   h0 = proj_in(GN(x));  h2 = h0 + attn1(LN1(h0)) + vec;  h3 = h2 + ff2(GEGLU(ff1(LN3(h2))));  out = proj_out(h3) + x
-  // attn2 over ONE key is the per-sample vector vec = Wo (Wv enc) + bo: its gradient is the per-sample channel sum of G(h2)
-  // (the sums the attn1.to_out bias gradient makes).  attn2.to_q, attn2.to_k and norm2 do not reach the output (softmax
-  // over one key is 1), so their gradients stay exactly zero: nothing is launched for them.
-  void transformer_bwd(const Block& k, const std::string& xn) {
+  // Encoder sequence length S = 1: attn2 over ONE key is the per-sample vector vec = Wo (Wv enc) + bo: its gradient is the
+  // per-sample channel sum of G(h2) (the sums the attn1.to_out bias gradient makes).  attn2.to_q, attn2.to_k and norm2 do
+  // not reach the output (softmax over one key is 1), so their gradients stay exactly zero: nothing is launched for them.
+  // S > 1: h1 = h0 + attn1(LN1(h0)), h2 = h1 + attn2(LN2(h1), enc), walked back by cross_attention_bwd.
+  void transformer_bwd(const Block& k, const std::string& xn, int S) {
     const std::string& n = k.name;
     const std::string t = n + ".transformer_blocks.0";
     const Act x = fwd(xn), h0 = fwd(n + ".h0"), n1 = fwd(n + ".n1"), qkv = fwd(n + ".qkv"), ao = fwd(n + ".ao"),
@@ -356,18 +358,26 @@ struct BwdBuilder {
     // norm3 (+ residual) -> G(h2)
     Act Gh2 = tmp("tf_Gh2", C, H, W);
     layer_norm_bwd(Gn, h2, t + ".norm3", Gh2, Gh3);
-    // attn1.to_out and attn2.to_out both add their bias to every pixel of h2: one channel sum gives both bias gradients
     Act Gao = tmp("tf_Gao", C, H, W);
-    dgrad(t + ".attn1.to_out.0.weight", whole(Gh2), Gao, 1);
-    wgrad_conv(whole(Gh2), whole(ao), t + ".attn1.to_out.0.weight", 1);
-    bias_grad(whole(Gh2), t + ".attn1.to_out.0.bias", t + ".attn2.to_out.0.bias");
-    // dvec[n] = per-sample channel sums of G(h2) (last_cs, made just above)
-    emit(OP_XVEC_BWD, [h = h, dvec = last_cs, wv = P(t + ".attn2.to_v.weight"), wo = P(t + ".attn2.to_out.0.weight"),
-                       dwo = PG(t + ".attn2.to_out.0.weight"), dwv = PG(t + ".attn2.to_v.weight"),
-                       scratch = (float*)mem.take((size_t)2 * N * C * sizeof(float)), N = N, C,
-                       X = k.cross](const RunArgs&, cudaStream_t s) {
-      return launch_cross_attn_vec_bwd(h->enc, dvec, wv, wo, dwo, dwv, scratch, N, C, X, s);
-    }, 2);
+    Act Gh1 = Gh2;   // the gradient of attn1's output projection, with its residual h0
+    if (S == 1) {
+      // attn1.to_out and attn2.to_out both add their bias to every pixel of h2: one channel sum gives both bias gradients
+      dgrad(t + ".attn1.to_out.0.weight", whole(Gh2), Gao, 1);
+      wgrad_conv(whole(Gh2), whole(ao), t + ".attn1.to_out.0.weight", 1);
+      bias_grad(whole(Gh2), t + ".attn1.to_out.0.bias", t + ".attn2.to_out.0.bias");
+      // dvec[n] = per-sample channel sums of G(h2) (last_cs, made just above)
+      emit(OP_XVEC_BWD, [h = h, dvec = last_cs, wv = P(t + ".attn2.to_v.weight"), wo = P(t + ".attn2.to_out.0.weight"),
+                         dwo = PG(t + ".attn2.to_out.0.weight"), dwv = PG(t + ".attn2.to_v.weight"),
+                         scratch = (float*)mem.take((size_t)2 * N * C * sizeof(float)), N = N, C,
+                         X = k.cross](const RunArgs&, cudaStream_t s) {
+        return launch_cross_attn_vec_bwd(h->enc, dvec, wv, wo, dwo, dwv, scratch, N, C, X, s);
+      }, 2);
+    } else {
+      Gh1 = cross_attention_bwd(k, Gh2, Gao, Gn, S);
+      dgrad(t + ".attn1.to_out.0.weight", whole(Gh1), Gao, 1);
+      wgrad_conv(whole(Gh1), whole(ao), t + ".attn1.to_out.0.weight", 1);
+      bias_grad(whole(Gh1), t + ".attn1.to_out.0.bias");
+    }
     // attention core (P recomputed from the forward's row log-sum-exp)
     Act Gqkv = tmp("tf_Gqkv", 3 * C, H, W);
     emit(OP_MHA_BWD, [q = qkv.p, o = ao.p, go = Gao.p, lse = h->plan.lse.at(n),
@@ -388,7 +398,7 @@ struct BwdBuilder {
     }
     // norm1 (+ residual) -> G(h0)
     Act Gh0 = tmp("tf_Gh0", C, H, W);
-    layer_norm_bwd(Gn, h0, t + ".norm1", Gh0, Gh2);
+    layer_norm_bwd(Gn, h0, t + ".norm1", Gh0, Gh1);
     // proj_in over GroupNorm(x) (eps 1e-6, no SiLU), then the GroupNorm backward with the outer residual G(out)
     Act T = tmp("tf_T", C, H, W);
     dgrad(n + ".proj_in.weight", whole(Gh0), T, 1);
@@ -396,6 +406,41 @@ struct BwdBuilder {
     wgrad_conv(whole(Gh0), whole(XN), n + ".proj_in.weight", 1);
     bias_grad(whole(Gh0), n + ".proj_in.bias");
     gn_bwd(T, x, nullptr, n + ".norm", false, G(xn), nullptr, Gout.p, skip_of(xn), 1e-6f);
+  }
+
+  // attn2 against S > 1 encoder tokens (Builder::cross_attention) in reverse, from G(h2) to G(h1) (returned):
+  //   h2 = h1 + to_out(ao2),  ao2 = xattn(q2, K, V),  q2 = to_q(n2),  n2 = LN2(h1),  K = enc Wk^T,  V = enc Wv^T
+  // Gao2 and Gn are scratch tensors of C channels (the caller's, free at this point of the walk).
+  Act cross_attention_bwd(const Block& k, const Act& Gh2, const Act& Gao2, const Act& Gn, int S) {
+    const std::string& n = k.name;
+    const std::string t = n + ".transformer_blocks.0";
+    const Act h1 = fwd(n + ".attn1"), n2 = fwd(n + ".n2"), q2 = fwd(n + ".q2"), ao2 = fwd(n + ".ao2");
+    const int C = h1.C, H = h1.H, W = h1.W;
+    // to_out (its residual is h1: G(h1) += G(h2) in the LayerNorm backward below)
+    dgrad(t + ".attn2.to_out.0.weight", whole(Gh2), Gao2, 1);
+    wgrad_conv(whole(Gh2), whole(ao2), t + ".attn2.to_out.0.weight", 1);
+    bias_grad(whole(Gh2), t + ".attn2.to_out.0.bias");
+    // attention core -> G(q2) and dK, dV (fp32 [N][S][C]), then the K / V projections' weight gradients
+    Act Gq2 = tmp("tf_Gq2", C, H, W);
+    const size_t kv = (size_t)N * S * C;
+    float* dkv = (float*)mem.take(2 * kv * sizeof(float));
+    emit(OP_XATTN_BWD, [q = q2.p, kvp = h->plan.xkv.at(n), o = ao2.p, go = Gao2.p, lse = h->plan.lse.at(n + ".attn2"),
+                        dsum = (float*)mem.take((size_t)N * heads * H * W * sizeof(float)),
+                        part = (float*)mem.take(xattn_part_floats(N, C, heads, H, W, S) * sizeof(float)), gq = Gq2.p, dkv,
+                        kv, N = N, C, heads = heads, H, W, S](const RunArgs&, cudaStream_t s) {
+      return launch_xattn_bwd(q, kvp, kvp + kv, o, go, lse, dsum, part, gq, dkv, dkv + kv, N, C, heads, H, W, S, s);
+    }, 4);
+    emit(OP_XKV_BWD, [h = h, dkv, kv, dwk = PG(t + ".attn2.to_k.weight"), dwv = PG(t + ".attn2.to_v.weight"), M = N * S, C,
+                      X = k.cross](const RunArgs&, cudaStream_t s) {
+      return launch_xattn_kv_wgrad(dkv, dkv + kv, h->enc, dwk, dwv, M, C, X, s);
+    });
+    // to_q (no bias)
+    wgrad_conv(whole(Gq2), whole(n2), t + ".attn2.to_q.weight", 1);
+    dgrad(t + ".attn2.to_q.weight", whole(Gq2), Gn, 1);
+    // norm2 (+ residual) -> G(h1)
+    Act Gh1 = tmp("tf_Gh1", C, H, W);
+    layer_norm_bwd(Gn, h1, t + ".norm2", Gh1, Gh2);
+    return Gh1;
   }
 
   // Downsample2D (BK_DOWN: padding 1; BK_DOWN_ASYM: padding (0, 1, 0, 1)): stride-2 3x3 conv on the raw tensor xn -> y
@@ -484,7 +529,11 @@ struct BwdBuilder {
 static int build_unet_backward(b200ad_unet* h, Backward* const* bws, uint8_t* arena, float* grads, size_t* bytes_out) {
   const b200ad_unet_config& c = h->cfg;
   if (!h->training || h->plan.lists.empty()) return set_err("backward needs set_training(1) before bind_workspace");
+  if (h->enc_len != h->plan_enc_len)
+    return set_err("backward: the encoder sequence length is set to %d but the workspace is planned for %d (bind the "
+                   "workspace again)", h->enc_len, h->plan_enc_len);
   Backward* bw = bws[0];
+  bw->enc_len = h->plan_enc_len;
   bw->list.ops.clear();
   bw->jobs.clear();
   bw->arena = arena;
@@ -541,7 +590,7 @@ static int build_unet_backward(b200ad_unet* h, Backward* const* bws, uint8_t* ar
         break;
       case BK_RESNET: B.resnet_bwd(k, in, tap(k.skip)); break;
       case BK_ATTN: B.attention_bwd(k.name, in); break;
-      case BK_TRANSFORMER: B.transformer_bwd(k, in); break;
+      case BK_TRANSFORMER: B.transformer_bwd(k, in, h->plan_enc_len); break;
       case BK_DOWN: B.downsample_bwd(k, in); break;
       case BK_UP: B.upsample_bwd(k.name, in); break;
       case BK_UNET_HEAD: {   // conv_in, then the timestep embedding MLP and the per-resnet projections
@@ -846,8 +895,15 @@ extern "C" int b200ad_vae_encoder_backward(b200ad_vae* h, const float* x, const 
 
 extern "C" int b200ad_unet_backward(b200ad_unet* h, const float* x, const float* g_eps, int accumulate, void* stream) {
   if (!x || !g_eps) return set_err("backward: x and g_eps are required");
-  if (h && h->cfg.cross_attention_dim && (!h->enc || h->enc_S != 1))
-    return set_err("backward: the conditional U-Net needs the forward's encoding (S = 1) bound");
+  if (h && h->cfg.cross_attention_dim && !h->enc) return set_err("backward: the conditional U-Net needs the forward's encoding bound");
+  if (h && h->cfg.cross_attention_dim && h->bwd[0] && !h->bwd[0]->list.ops.empty()) {
+    const int planned = h->bwd[0]->enc_len;
+    if (planned != h->plan_enc_len)
+      return set_err("backward: the backward plan was built for %d encoder tokens but the workspace is planned for %d "
+                     "(call bind_backward again)", planned, h->plan_enc_len);
+    if (h->enc_S != planned)
+      return set_err("backward: the bound encoding has %d tokens but the plan was built for %d", h->enc_S, planned);
+  }
   RunArgs a;
   a.in = x; a.g_eps = g_eps;
   return run_backward(h, 0, a, accumulate, (cudaStream_t)stream);

@@ -111,8 +111,9 @@ class EngineModel(nn.Module):
     def _needs_grad(self) -> bool:
         return torch.is_grad_enabled() and self.training and any(p.requires_grad for p in self.parameters())
 
-    def _ensure_bound(self, n: int, hh: int, ww: int) -> None:
-        """Packs the weights when a parameter's pointer or version changed, and binds the workspace for (n, hh, ww)."""
+    def _ensure_bound(self, n: int, hh: int, ww: int, seq: Optional[int] = None) -> None:
+        """Packs the weights when a parameter's pointer or version changed, and binds the workspace for (n, hh, ww) and,
+        for a conditional U-Net, the encoder sequence length `seq` (None: a model without an encoding)."""
         _lib.require_cuda()
         params = self._plist
         dev = params[0].device
@@ -132,9 +133,11 @@ class EngineModel(nn.Module):
                                               _lib.stream_ptr()))
             self._packed_key = key
             self._ws_key = None  # the plan holds parameter pointers
-        wkey = (n, hh, ww, dev)
+        wkey = (n, hh, ww, dev) if seq is None else (n, hh, ww, dev, seq)
         if wkey != self._ws_key:
             self._fwd_gen = [g + 1 for g in self._fwd_gen]     # the activations of every part are gone
+            if seq is not None:
+                _lib.check(self._fn("set_encoder_len")(self._h, seq))
             need = self._fn("workspace_bytes")(self._h, n, hh, ww)
             if self._ws is None or self._ws.numel() < need or self._ws.device != dev:
                 self._ws = None
@@ -167,10 +170,11 @@ class EngineModel(nn.Module):
                                              self._grad_flat.data_ptr(), _lib.stream_ptr()))
         self._bwd_key = self._ws_key
 
-    def _bind(self, n: int, hh: int, ww: int, train: bool, dev: torch.device) -> None:
-        """Everything a forward of (n, hh, ww) needs bound: mode, weights, workspace and, when training, the backward."""
+    def _bind(self, n: int, hh: int, ww: int, train: bool, dev: torch.device, seq: Optional[int] = None) -> None:
+        """Everything a forward of (n, hh, ww) (and `seq` encoder tokens) needs bound: mode, weights, workspace and, when
+        training, the backward."""
         self._set_training_mode(train)
-        self._ensure_bound(n, hh, ww)
+        self._ensure_bound(n, hh, ww, seq)
         if train:
             self._bind_backward(dev)
 

@@ -169,6 +169,11 @@ class UNet2DModel(EngineModel):
         """The conditional model's validated encoding; None here."""
         return None
 
+    @staticmethod
+    def _seq(enc: Optional[torch.Tensor]) -> Optional[int]:
+        """The encoder sequence length the workspace is planned for (None: no encoding)."""
+        return None if enc is None else int(enc.shape[1])
+
     def _set_encoding(self, enc: Optional[torch.Tensor]) -> None:
         if enc is not None:
             _lib.check(self._fn("set_encoding")(self._h, enc.data_ptr(), enc.shape[1]))
@@ -196,9 +201,9 @@ class UNet2DModel(EngineModel):
         n, _, hh, ww = x.shape
         with torch.cuda.device(x.device):
             self._fwd_gen[0] += 1
-            self._bind(n, hh, ww, train, x.device)
-            t = self._timesteps(timestep, n, x.device)
             e = self._encoding(enc, n, x.device)
+            self._bind(n, hh, ww, train, x.device, self._seq(e))
+            t = self._timesteps(timestep, n, x.device)
             out = torch.empty((n, self.out_channels, hh, ww), dtype=torch.float32, device=x.device)
             self._set_encoding(e)
             _lib.check(self._fn("forward")(self._h, x.data_ptr(), t.data_ptr(), out.data_ptr(), _lib.stream_ptr()))
@@ -242,9 +247,9 @@ class UNet2DModel(EngineModel):
         n, _, hh, ww = x.shape
         with torch.cuda.device(x.device):
             self._fwd_gen[0] += 1
-            self._bind(n, hh, ww, False, x.device)
-            t = self._timesteps(timestep, n, x.device)
             e = self._encoding(enc, n, x.device)
+            self._bind(n, hh, ww, False, x.device, self._seq(e))
+            t = self._timesteps(timestep, n, x.device)
             if out is None:
                 out = torch.empty_like(x)
             eps = torch.empty_like(x) if want_eps else None

@@ -6,13 +6,17 @@ cross-attention reads the 100-d audio encodings of `audiodiffusion/audio_encoder
 Same constructor kwargs and diffusers state-dict keys (`down_blocks.i.attentions.j.transformer_blocks.0.attn1.to_q.weight`, ...).
 Inference and training run in libb200ad.so: every projection / linear of the transformer blocks on the wgmma conv kernel
 (and, in the backward, its data- and weight-gradient forms), self-attention (8 heads, head_dim = channels / 8) on flash-style
-tensor-core kernels (the backward recomputes the attention matrix from the forward's row log-sum-exp), cross-attention
-against the ONE encoder token as a per-sample vector folded into the attn1 output projection.
+tensor-core kernels (the backward recomputes the attention matrix from the forward's row log-sum-exp).  Cross-attention:
+an encoding of ONE token (the pooled AudioEncoder output, (B, 1, 100)) is a per-sample vector folded into the attn1 output
+projection (softmax over one key is 1); an encoding of S > 1 tokens (e.g. `AudioEncoder.encode(files, pool=None)`: one token
+per 5-second slice) runs the cross-attention kernels: the K / V projections of the encoding, flash-style attention of the
+pixels against the S tokens and, in training, its backward down to the to_q / to_k / to_v weight gradients.
 
 Training (`scripts/train_unet.py --encodings`: `model(noisy, t, enc)["sample"]`, MSE, `loss.backward()`) goes through the
 same autograd node as `UNet2DModel`: parameter gradients only, as `p.grad` views of one flat buffer.  Limits: encoder
-sequence length 1 (what the reference's AudioEncoder produces: (B, 1, 100)); no gradient w.r.t. the encoding (the
-reference's encodings are precomputed data), so an encoding with `requires_grad` is refused in training.
+sequence length 1 <= S <= 256 (256 slices of 5 seconds: about 21 minutes of audio; a change of S re-plans the workspace);
+no gradient w.r.t. the encoding (the reference's encodings are precomputed data), so an encoding with `requires_grad` is
+refused in training.
 """
 from __future__ import annotations
 
@@ -23,6 +27,8 @@ import torch
 from ._lib import MAX_BLOCKS, StepCoefC
 from .engine import _Cfg
 from .unet import UNet2DModel, _unet_config
+
+MAX_ENCODER_LEN = 256   # tokens of an encoding (the cross-attention kernels stage all of them in shared memory)
 
 
 class UNet2DConditionModel(UNet2DModel):
@@ -97,8 +103,8 @@ class UNet2DConditionModel(UNet2DModel):
             e = e[:, None, :]
         if e.ndim != 3 or e.shape[0] != n or e.shape[2] != self.config.cross_attention_dim:
             raise ValueError(f"encoder_hidden_states must be ({n}, seq, {self.config.cross_attention_dim}), got {tuple(enc.shape)}")
-        if e.shape[1] != 1:
-            raise NotImplementedError("UNet2DConditionModel(b200): encoder sequence length 1 only (audio_encoder.py encodings)")
+        if not 1 <= e.shape[1] <= MAX_ENCODER_LEN:
+            raise ValueError(f"UNet2DConditionModel(b200): encoder sequence length {e.shape[1]} outside [1, {MAX_ENCODER_LEN}]")
         return e.contiguous()
 
     def forward(self, sample: torch.Tensor, timestep, encoder_hidden_states: torch.Tensor = None, return_dict: bool = True):

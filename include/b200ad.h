@@ -68,8 +68,15 @@ int b200ad_unet_bind_workspace(b200ad_unet* h, void* workspace, size_t bytes, in
 int b200ad_unet_forward(b200ad_unet* h, const float* x, const float* t, float* eps_out, void* stream);
 
 /* Conditional model only: encoder_hidden_states of the next forward (pipeline_audio_diffusion.py:160-161),
- * fp32 [N][S][cross_attention_dim] on the device; S = 1 (what audiodiffusion/audio_encoder.py produces) is implemented. */
+ * fp32 [N][S][cross_attention_dim] on the device, 1 <= S <= 256.  S must be the token count the bound workspace was
+ * planned for (b200ad_unet_set_encoder_len); a forward or backward with another S fails with an error naming both.
+ * S = 1 (the pooled encodings of audiodiffusion/audio_encoder.py) folds attn2 into a per-sample vector; S > 1 (e.g.
+ * AudioEncoder.encode(..., pool=None): one token per 5-second slice) runs the cross-attention kernels. */
 int b200ad_unet_set_encoding(b200ad_unet* h, const float* enc, int S);
+/* Conditional model only: the encoder sequence length S the next b200ad_unet_workspace_bytes / bind_workspace plan for
+ * (default 1); backward_bytes / bind_backward follow the bound workspace and fail if S was changed since.  Error outside
+ * [1, 256] or on an unconditional model. */
+int b200ad_unet_set_encoder_len(b200ad_unet* h, int S);
 
 /* Scheduler-update coefficients (host scalars, computed exactly as DDPMScheduler.step / DDIMScheduler.step do,
  * pipeline_audio_diffusion.py:165-179):
@@ -127,8 +134,9 @@ int b200ad_unet_conv_plan(const b200ad_unet* h, int N, int H, int W, int num_sms
  * then backward(x, dL/d eps). Parameter gradients land in ONE flat fp32 buffer; parameter i of the
  * table lives at float offset b200ad_unet_grad_offset(h, i) — the Python mirror exposes them as `p.grad` views.
  * Conditional model (scripts/train_unet.py --encodings): set_encoding before forward, and the same encoding must still be
- * bound (and alive) at backward, which reads it for attn2.to_v's gradient.  No gradient w.r.t. the encoding is computed;
- * attn2.to_q, attn2.to_k and norm2 get exactly zero gradients (softmax over one encoder token is constant). */
+ * bound (and alive) at backward, which reads it for the attn2.to_k / to_v gradients.  No gradient w.r.t. the encoding is
+ * computed.  With S = 1 encoder token, attn2.to_q, attn2.to_k and norm2 get exactly zero gradients (softmax over one key is
+ * constant); with S > 1 every parameter gets its gradient. */
 int b200ad_unet_set_training(b200ad_unet* h, int on);
 size_t b200ad_unet_grad_floats(b200ad_unet* h);
 size_t b200ad_unet_grad_offset(b200ad_unet* h, int i);
@@ -257,6 +265,15 @@ size_t b200ad_mha_scratch_bytes(int N, int C, int heads, int H, int W);
 int b200ad_mha_forward_backward(const float* q, const float* k, const float* v, const float* dout, float* out, float* dq,
                                 float* dk, float* dv, int N, int C, int heads, int H, int W, void* scratch,
                                 size_t scratch_bytes, void* stream);
+/* Cross-attention of the conditional U-Net against S > 1 encoder tokens (8 heads of dim C / heads in {16, 32, 64},
+ * 1 <= S <= 256) forward and backward in one call, for parity tests: q, dout fp32 [N, C, H, W] (channel c of head
+ * c / (C / heads)), k, v fp32 [N, S, C] -> out = softmax(q k^T / sqrt(D)) v (fp32 [N, C, H, W]) and dq ([N, C, H, W]),
+ * dk, dv ([N, S, C]) = the gradients of <out, dout>.  Runs the training forward kernel (with its row log-sum-exp) and the
+ * backward kernels the model runs.  scratch >= b200ad_xattn_scratch_bytes. */
+size_t b200ad_xattn_scratch_bytes(int N, int C, int heads, int H, int W, int S);
+int b200ad_xattn_forward_backward(const float* q, const float* k, const float* v, const float* dout, float* out, float* dq,
+                                  float* dk, float* dv, int N, int C, int heads, int H, int W, int S, void* scratch,
+                                  size_t scratch_bytes, void* stream);
 /* GroupNorm(groups, eps) [+ SiLU] on fp32 NCHW through the stats + apply kernels. */
 int b200ad_group_norm(const float* x, const float* gamma, const float* beta, float* y, int N, int C, int H, int W,
                       int groups, float eps, int silu, void* scratch, size_t scratch_bytes, void* stream);
