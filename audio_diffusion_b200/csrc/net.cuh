@@ -8,6 +8,7 @@
 #include <cstring>
 #include <functional>
 #include <map>
+#include <set>
 #include <string>
 #include <vector>
 
@@ -166,10 +167,18 @@ static Block& add_block(std::vector<Block>& bl, BlockKind kind, const std::strin
   return bl.back();
 }
 
+// Gradient checkpointing: the forward ops of one block that rebuild its internals (ops[begin, end) of its list; the op
+// that writes the block's output comes after them and is not re-run), and the GroupNorm statistics those ops accumulate,
+// which must be zeroed before they run again.
+struct Recompute {
+  int begin = 0, end = 0;
+  std::vector<std::pair<stat_t*, size_t>> stats;
+};
 struct OpList {  // one launch sequence and the GroupNorm statistics it accumulates (zeroed before every run)
   std::vector<Op> ops;
   stat_t* stats = nullptr;
   size_t stats_bytes = 0;
+  std::vector<Recompute> recompute;  // by block index
 };
 struct Plan {    // everything a plan builder derives from the workspace and (N, H, W)
   std::vector<OpList> lists;         // U-Net: the forward; autoencoder: encoder, decoder
@@ -187,6 +196,8 @@ struct Plan {    // everything a plan builder derives from the workspace and (N,
   std::map<std::string, float*> probs; // training, autoencoder: the single-head attention's softmax P [N][HW][HW] by block name
   float* z_in = nullptr;             // training, autoencoder: the decoder's input latents [N][L][h][w] (post_quant_conv wgrad)
   size_t ws_bytes = 0;
+  bool checkpoint = false;           // a training plan with gradient checkpointing: the backward re-runs `recompute` ops
+  std::set<std::string> rebuilt;     // ... and the taps they rebuild, which share pooled buffers between blocks
 };
 
 struct Backward;   // a backward plan (unet_bwd.cu)
@@ -212,7 +223,9 @@ struct NetBase {
   uint8_t* ws = nullptr;
   size_t ws_bytes = 0;
   Plan plan;
-  bool training = false;            // keep every activation (no pooling) and the timestep-MLP pre-activations for backward
+  bool training = false;            // keep the activations (all of them unless checkpointing) and the timestep-MLP
+                                    // pre-activations for backward
+  bool checkpointing = false;       // training keeps only the block outputs; the backward recomputes each block's internals
   int num_sms = 132;
   const float* enc = nullptr;       // conditional U-Net: encoder_hidden_states [N][enc_S][X] of the next forward
   int enc_S = 0;
@@ -537,7 +550,18 @@ struct Builder {
   int heads = 8;                    // transformer: attention heads
   bool nopool = false;  // B200AD_DEBUG_NOPOOL=1: every activation gets its own buffer (per-layer parity taps)
   bool single_head = false;  // attention with one head of dim C (AutoencoderKL mid block) instead of head_dim 8
-  std::map<size_t, size_t> kv_pool;  // the workspace offsets of attn2's K | V buffers (S > 1) by size: shared unless nopool
+  // gradient checkpointing (training): block outputs keep their own buffers, the internals are pooled as for inference
+  bool ckpt = false;
+  std::map<std::string, size_t> raw_pool;  // workspace offsets of pooled plain buffers by tag and size (unless nopool)
+  int out_op = -1;                  // the block being planned: index of its first output-writing op (-1: none recomputed)
+  Recompute* rec = nullptr;         // ... and its recompute record (checkpointing)
+
+  void reset() {   // before each pass
+    pool.clear();
+    raw_pool.clear();
+    built->taps.clear();
+    built->rebuilt.clear();
+  }
 
   Act alloc(int C, int H, int W, bool stats) {
     Act a = take_act(ws, N, C, H, W);
@@ -545,16 +569,35 @@ struct Builder {
     return a;
   }
   Act pooled(const std::string& tag, int C, int H, int W, bool stats) {
-    const std::string key = S("%s:%d:%d:%d", tag.c_str(), C, H, W);
-    if (nopool) return alloc(C, H, W, stats);
-    auto it = pool.find(key);
-    if (it == pool.end()) it = pool.emplace(key, alloc(C, H, W, false)).first;
-    Act a = it->second;
-    if (stats) a.stats = (stat_t*)st.take((size_t)N * (C / 4) * 2 * sizeof(stat_t));
+    Act a;
+    if (nopool) {
+      a = alloc(C, H, W, false);
+    } else {
+      const std::string key = S("%s:%d:%d:%d", tag.c_str(), C, H, W);
+      auto it = pool.find(key);
+      if (it == pool.end()) it = pool.emplace(key, alloc(C, H, W, false)).first;
+      a = it->second;
+    }
+    if (stats) {
+      const size_t bytes = (size_t)N * (C / 4) * 2 * sizeof(stat_t);
+      a.stats = (stat_t*)st.take(bytes);
+      if (rec) rec->stats.push_back({a.stats, bytes});   // an internal tensor: its statistics are accumulated again
+    }
     return a;
   }
-  Act output(const Block& k, int C, int H, int W) {  // a block's output (raw + stats)
-    return k.pool.empty() ? alloc(C, H, W, true) : pooled(k.pool, C, H, W, true);
+  void* pooled_raw(const std::string& tag, size_t bytes) {   // a plain buffer, pooled by tag and size like pooled()
+    const std::string key = S("%s:%zu", tag.c_str(), bytes);
+    auto it = raw_pool.find(key);
+    if (nopool || it == raw_pool.end()) it = raw_pool.insert_or_assign(key, take_off(ws, bytes)).first;
+    return ws.base ? ws.base + it->second : nullptr;
+  }
+  Act output(const Block& k, int C, int H, int W) {  // a block's output (raw + stats); training keeps every one
+    return k.pool.empty() || h->training ? alloc(C, H, W, true) : pooled(k.pool, C, H, W, true);
+  }
+  void mark_output() { out_op = (int)ops->size(); }   // the ops emitted from here on write the block's output
+  void inner_tap(const std::string& name, const Act& a) {   // a tap of a block's internals
+    built->taps[name] = a;
+    if (ckpt) built->rebuilt.insert(name);
   }
   const float* P(const std::string& name) const { return h->pptr[h->pidx.at(name)]; }
   template <class T> const T* PK(size_t off) const { return h->packed ? (const T*)(h->packed + off) : nullptr; }
@@ -676,6 +719,7 @@ struct Builder {
       conv(p);
     }
     const float2* ss2 = gn_finalize(h1, nullptr, n + ".norm2");
+    mark_output();
     Act out = output(k, cout, H, W);
     {
       ConvParams p = conv_geom(N, out);
@@ -697,7 +741,7 @@ struct Builder {
       }
       conv(p);
     }
-    built->taps[n + ".h1"] = h1;
+    inner_tap(n + ".h1", h1);
     built->taps[n] = out;
     return out;
   }
@@ -731,30 +775,28 @@ struct Builder {
     const std::string& n = k.name;
     const std::string t = n + ".transformer_blocks.0";
     const int C = h1.C, H = h1.H, W = h1.W;
-    Act n2 = pooled("tf_ln", C, H, W, false);
+    Act n2 = pooled(h->training ? "tf_n2" : "tf_ln", C, H, W, false);
     layer_norm(h1, n2, t + ".norm2");
     Act q2 = pooled("tf_q2", C, H, W, false);
     linear(q2, n2, k.q2, nullptr);
-    const size_t kv_bytes = (size_t)2 * N * S * C * sizeof(__nv_bfloat16);
-    auto it = kv_pool.find(kv_bytes);
-    if (nopool || it == kv_pool.end()) it = kv_pool.insert_or_assign(kv_bytes, take_off(ws, kv_bytes)).first;
-    __nv_bfloat16* kv = ws.base ? (__nv_bfloat16*)(ws.base + it->second) : nullptr;
+    __nv_bfloat16* kv = (__nv_bfloat16*)pooled_raw("xkv", (size_t)2 * N * S * C * sizeof(__nv_bfloat16));
     if (h->training) built->xkv[n] = kv;
     emit(OP_XKV, [h = h, wk = P(t + ".attn2.to_k.weight"), wv = P(t + ".attn2.to_v.weight"), kv, N = N, S, C,
                   X = k.cross](const RunArgs&, cudaStream_t s) {
       return launch_xattn_kv(h->enc, wk, wv, kv, kv + (size_t)N * S * C, N, S, C, X, s);
     });
-    Act ao2 = pooled("tf_ao", C, H, W, false);    // attn1's output is dead after h1
-    float* lse = h->training ? built->lse[n + ".attn2"] = (float*)ws.take((size_t)N * heads * H * W * sizeof(float)) : nullptr;
+    Act ao2 = pooled(h->training ? "tf_ao2" : "tf_ao", C, H, W, false);    // attn1's output is dead after h1
+    float* lse = h->training ? built->lse[n + ".attn2"] = (float*)pooled_raw("lse2", (size_t)N * heads * H * W * sizeof(float))
+                             : nullptr;
     emit(OP_XATTN, [q = q2.p, kv, o = ao2.p, N = N, C, heads = heads, H, W, S, lse](const RunArgs&, cudaStream_t s) {
       return launch_xattn(q, kv, kv + (size_t)N * S * C, o, N, C, heads, H, W, S, s, lse);
     });
     Act h2 = pooled("tf_h2", C, H, W, false);
     linear(h2, ao2, k.out2, P(t + ".attn2.to_out.0.bias"), nullptr, &h1, k.ident);
     if (h->training) {
-      built->taps[n + ".n2"] = n2;
-      built->taps[n + ".q2"] = q2;
-      built->taps[n + ".ao2"] = ao2;
+      inner_tap(n + ".n2", n2);
+      inner_tap(n + ".q2", q2);
+      inner_tap(n + ".ao2", ao2);
     }
     return h2;
   }
@@ -780,12 +822,12 @@ struct Builder {
     }
     Act h0 = pooled("tf_h0", C, H, W, false);
     linear(h0, x, k.proj_in, P(n + ".proj_in.bias"), ssx);
-    Act n1 = pooled("tf_ln", C, H, W, false);
+    Act n1 = pooled("tf_ln", C, H, W, false);     // training: n1, n2 and n3 are each kept for the backward
     layer_norm(h0, n1, t + ".norm1");
     Act qkv = pooled("tf_qkv", 3 * C, H, W, false);
     linear(qkv, n1, k.qkv, nullptr);
     Act ao = pooled("tf_ao", C, H, W, false);
-    float* lse = h->training ? built->lse[n] = (float*)ws.take((size_t)N * heads * H * W * sizeof(float)) : nullptr;
+    float* lse = h->training ? built->lse[n] = (float*)pooled_raw("lse1", (size_t)N * heads * H * W * sizeof(float)) : nullptr;
     emit(OP_MHA, [q = qkv.p, o = ao.p, N = N, C, heads = heads, H, W, lse](const RunArgs&, cudaStream_t s) {
       return launch_mha_flash(q, o, N, C, heads, H, W, s, lse);
     });
@@ -796,10 +838,10 @@ struct Builder {
     } else {
       Act h1 = pooled("tf_h1", C, H, W, false);
       linear(h1, ao, k.out, P(t + ".attn1.to_out.0.bias"), nullptr, &h0, k.ident);
-      built->taps[n + ".attn1"] = h1;
+      inner_tap(n + ".attn1", h1);
       h2 = cross_attention(k, h1, S);
     }
-    Act n3 = pooled("tf_ln", C, H, W, false);     // the same buffer as n1 unless training
+    Act n3 = pooled(h->training ? "tf_n3" : "tf_ln", C, H, W, false);
     layer_norm(h2, n3, t + ".norm3");
     Act ff1 = pooled("tf_ff1", 8 * C, H, W, false);
     linear(ff1, n3, k.ff1, P(t + ".ff.net.0.proj.bias"));
@@ -807,21 +849,22 @@ struct Builder {
     emit(OP_GEGLU, [x = ff1.p, y = gg.p, N = N, C, H, W](const RunArgs&, cudaStream_t s) {
       return launch_geglu_pf8(x, y, N, 4 * C, H, W, s);
     });
-    Act h3 = pooled("tf_h0", C, H, W, false);     // h0 is dead after h2 (S > 1: after h1)
+    Act h3 = pooled(h->training ? "tf_h3" : "tf_h0", C, H, W, false);     // h0 is dead after h2 (S > 1: after h1)
     linear(h3, gg, k.ff2, P(t + ".ff.net.2.bias"), nullptr, &h2, k.ident);
+    mark_output();
     Act out = output(k, C, H, W);
     linear(out, h3, k.proj_out, P(n + ".proj_out.bias"), nullptr, &x, k.ident);
-    built->taps[n + ".attn2"] = h2;
+    inner_tap(n + ".attn2", h2);
     built->taps[n] = out;
-    if (h->training) {   // no pooling: every intermediate has its own buffer, kept for BwdBuilder::transformer_bwd
-      built->taps[n + ".h0"] = h0;
-      built->taps[n + ".n1"] = n1;
-      built->taps[n + ".qkv"] = qkv;
-      built->taps[n + ".ao"] = ao;
-      built->taps[n + ".n3"] = n3;
-      built->taps[n + ".ff1"] = ff1;
-      built->taps[n + ".gg"] = gg;
-      built->taps[n + ".h3"] = h3;
+    if (h->training) {   // every intermediate has a buffer of its own within the block, read by BwdBuilder::transformer_bwd
+      inner_tap(n + ".h0", h0);
+      inner_tap(n + ".n1", n1);
+      inner_tap(n + ".qkv", qkv);
+      inner_tap(n + ".ao", ao);
+      inner_tap(n + ".n3", n3);
+      inner_tap(n + ".ff1", ff1);
+      inner_tap(n + ".gg", gg);
+      inner_tap(n + ".h3", h3);
     }
     return out;
   }
@@ -832,10 +875,11 @@ struct Builder {
     const Geom go = make_geom(N, Ho, Wo);
     const size_t tsz = (size_t)N * (C / 8) * go.PL * 8;  // elements per parity tensor
     Act par = pooled("parity", 4 * C, Ho, Wo, false);     // 4 tensors back to back (same bytes as 4C channels)
-    built->taps[k.name + ".parity"] = par;
+    inner_tap(k.name + ".parity", par);
     emit(OP_PARITY, [x, par = par.p, N = N](const RunArgs&, cudaStream_t s) {
       return launch_parity_split(x.p, par, N, x.C, x.H, x.W, s);
     });
+    mark_output();
     Act y = output(k, C, Ho, Wo);
     ConvParams p = conv_geom(N, y);
     p.nseg = 4;
@@ -880,7 +924,8 @@ struct Builder {
     linear(qkv, xn, k.qkv, PK<float>(k.bias));   // q|k|v blocks are contiguous
     Act ao = pooled("attn_o", C, H, W, false);
     if (single_head) {
-      float* scores = (float*)ws.take((size_t)N * H * W * H * W * sizeof(float));
+      const size_t bytes = (size_t)N * H * W * H * W * sizeof(float);
+      float* scores = (float*)(h->training ? pooled_raw("probs", bytes) : ws.take(bytes));
       if (h->training) built->probs[n] = scores;
       emit(OP_ATTN1, [q = qkv.p, o = ao.p, scores, N = N, C, H, W](const RunArgs&, cudaStream_t s) {
         return launch_attention_1head(q, o, scores, N, C, H, W, s);
@@ -890,10 +935,11 @@ struct Builder {
         return launch_attention(q, o, N, C, H, W, s);
       });
     }
+    mark_output();
     Act out = output(k, C, H, W);
     linear(out, ao, k.out, P(n + ".to_out.0.bias"), nullptr, &x, k.ident);   // + residual
-    built->taps[n + ".qkv"] = qkv;
-    built->taps[n + ".ao"] = ao;
+    inner_tap(n + ".qkv", qkv);
+    inner_tap(n + ".ao", ao);
     built->taps[n] = out;
     return out;
   }
@@ -924,7 +970,7 @@ struct Builder {
   // conv_norm_out + SiLU + conv_out on the tensor cores (output padded to 128 channels), then quant_conv + sampling
   Act latent_out(const Block& k, const Act& x) {
     const std::string& n = k.name;
-    Act eo = pooled("enc_out", 128, x.H, x.W, false);
+    Act eo = h->training ? alloc(128, x.H, x.W, false) : pooled("enc_out", 128, x.H, x.W, false);   // kept for the backward
     {
       const float2* ss = gn_finalize(x, nullptr, n + "conv_norm_out");
       ConvParams p = conv_geom(N, eo);
@@ -942,11 +988,16 @@ struct Builder {
     return eo;
   }
 
-  // Appends the plan of a block list.
-  void run(const std::vector<Block>& blocks) {
+  // Appends the plan of a block list, and (checkpointing) each block's recompute record to `recs`.
+  void run(const std::vector<Block>& blocks, std::vector<Recompute>* recs) {
     std::vector<Act> outs(blocks.size());
+    recs->assign(blocks.size(), Recompute());
     for (size_t i = 0; i < blocks.size(); ++i) {
       const Block& k = blocks[i];
+      Recompute& r = (*recs)[i];
+      r.begin = (int)ops->size();
+      out_op = -1;
+      rec = ckpt ? &r : nullptr;
       const Act* x = k.in >= 0 ? &outs[k.in] : nullptr;
       const Act* skip = k.skip >= 0 ? &outs[k.skip] : nullptr;
       switch (k.kind) {
@@ -961,6 +1012,8 @@ struct Builder {
         case BK_CONV_OUT: outs[i] = conv_out(k, *x); break;
         case BK_LATENT_OUT: outs[i] = latent_out(k, *x); break;
       }
+      r.end = out_op < 0 ? r.begin : out_op;   // heads, tails and upsamplers have nothing to recompute
+      rec = nullptr;
     }
   }
 };
@@ -994,6 +1047,14 @@ static int set_training(NetBase* h, int on) {
   if (h->training != (on != 0)) {
     h->training = on != 0;
     h->plan.lists.clear();    // the workspace layout changes: bind_workspace must be called again
+  }
+  return 0;
+}
+static int set_checkpointing(NetBase* h, int on) {
+  if (!h) return set_err("null handle");
+  if (h->checkpointing != (on != 0)) {
+    h->checkpointing = on != 0;
+    h->plan.lists.clear();    // as set_training: bind_workspace and bind_backward must be called again
   }
   return 0;
 }
@@ -1035,6 +1096,9 @@ static int run_ops(const NetBase* h, const OpList& l, const RunArgs& a, cudaStre
 static int debug_tensor(const NetBase* h, const char* name, float* dst, int* dims, cudaStream_t st) {
   auto it = h->plan.taps.find(name);
   if (it == h->plan.taps.end()) return set_err("unknown tap '%s'", name);
+  if (h->plan.rebuilt.count(name))
+    return set_err("tap '%s' is not kept under gradient checkpointing: it lives in a buffer shared between blocks and is "
+                   "recomputed in the backward pass (read it with checkpointing off)", name);
   const Act& a = it->second;
   if (dims) { dims[0] = a.C; dims[1] = a.H; dims[2] = a.W; }
   if (dst) CK(launch_pf8_to_nchw(a.p, dst, h->N, a.C, a.H, a.W, st));

@@ -140,7 +140,7 @@ extern "C" int b200ad_unet_set_params(b200ad_unet* h, const float* const* params
 namespace b200ad {
 
 // Two passes: the stats arena lives at the start of the workspace; its size is found by a dry run.
-static Plan build_plan(const b200ad_unet* h, uint8_t* ws_base, int N, int H, int W) {
+Plan build_plan(const b200ad_unet* h, uint8_t* ws_base, int N, int H, int W) {
   Plan pl;
   pl.lists.resize(1);
   OpList& l = pl.lists[0];
@@ -148,17 +148,16 @@ static Plan build_plan(const b200ad_unet* h, uint8_t* ws_base, int N, int H, int
   B.h = h; B.built = &pl; B.ops = &l.ops;
   B.N = N; B.H = H; B.W = W;
   B.heads = h->cfg.attention_head_dim;
-  B.nopool = debug_nopool() || h->training;
+  B.ckpt = pl.checkpoint = h->training && h->checkpointing;
+  B.nopool = debug_nopool() || (h->training && !B.ckpt);
   B.ws.base = ws_base;
   for (int pass = 0; pass < 2; ++pass) {
     l.ops.clear();
-    B.pool.clear();
-    B.kv_pool.clear();
-    pl.taps.clear();
+    B.reset();
     B.st.base = pass == 0 ? nullptr : ws_base;
     B.st.off = 0;
     B.ws.off = pass == 0 ? 0 : ((l.stats_bytes + 255) & ~(size_t)255);
-    B.run(h->blocks);
+    B.run(h->blocks, &l.recompute);
     if (pass == 0) l.stats_bytes = B.st.off;
   }
   l.stats = (stat_t*)ws_base;

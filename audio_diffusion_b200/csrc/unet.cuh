@@ -6,3 +6,7 @@ struct b200ad_unet : b200ad::NetBase {
   b200ad_unet_config cfg;
   std::vector<b200ad::Block> blocks;
 };
+
+namespace b200ad {
+Plan build_plan(const b200ad_unet* h, uint8_t* ws_base, int N, int H, int W);   // the forward plan (null: sizes only)
+}

@@ -10,6 +10,8 @@
 //   * GroupNorm(+SiLU), attention core, biases / time embedding, conv_in / conv_out are memory-bound kernels (bwd_kernels.cu).
 // The normalised activations the weight gradients read are materialised (no fusion yet).
 // A backward plan is an OpList of net.cuh, run by the forward's executor (run_ops).
+// With gradient checkpointing the forward kept only the block outputs: before a block's backward ops, the plan re-runs the
+// block's own forward ops (Recompute) that rebuild its internals in the forward's pooled buffers.
 #include "bwd_kernels.cuh"
 #include "unet.cuh"
 #include "vae.cuh"
@@ -95,6 +97,14 @@ struct BwdBuilder {
   void emit(OpKind kind, OpFn run, int launches = 1) { bw->list.ops.push_back(Op{kind, launches, {}, std::move(run)}); }
   void zero(void* p, size_t bytes) {
     emit(OP_MEMSET, [p, bytes](const RunArgs&, cudaStream_t s) { return cudaMemsetAsync(p, 0, bytes, s); });
+  }
+  // checkpointing: block `i` of the forward list `fl` rebuilds its internals (never its output) before its backward
+  void recompute(const OpList& fl, int i) {
+    if (!h->plan.checkpoint) return;
+    const Recompute& r = fl.recompute[i];
+    if (r.begin == r.end) return;
+    for (const auto& z : r.stats) zero(z.first, z.second);
+    bw->list.ops.insert(bw->list.ops.end(), fl.ops.begin() + r.begin, fl.ops.begin() + r.end);
   }
 
   // ---- transposed weight packing jobs ----------------------------------------------------------------------------
@@ -582,6 +592,7 @@ static int build_unet_backward(b200ad_unet* h, Backward* const* bws, uint8_t* ar
   for (int i = (int)bl.size() - 1; i >= 0; --i) {
     const Block& k = bl[i];
     const std::string in = tap(k.in);
+    B.recompute(h->plan.lists[0], i);
     switch (k.kind) {
       case BK_CONV_OUT:      // g_eps -> gradient of the last activation
         if (c.out_channels != 1) return set_err("backward: out_channels != 1 is not implemented");
@@ -669,6 +680,7 @@ static int build_vae_backward(b200ad_vae* h, Backward* const* bws, uint8_t* aren
     for (int i = (int)bl.size() - 1; i >= 0; --i) {
       const Block& k = bl[i];
       const std::string in = tap(k.in);
+      B.recompute(pl.lists[part], i);
       switch (k.kind) {
         case BK_CONV_OUT: B.conv_out_bwd(k, in, wflip, zbias); break;
         case BK_LATENT_OUT: {   // g_moments -> quant_conv -> conv_out (C -> 2L, per output channel) -> conv_norm_out + SiLU
@@ -845,6 +857,28 @@ static int bind_backward(Net* h, BuildBackward<Net> build, void* arena, size_t b
   return 0;
 }
 
+// Device bytes a training step of (N, H, W) binds in the handle's checkpointing mode: the training-mode forward workspace
+// plus the backward arena, planned without a device (no buffer is touched).  The handle's bound plan, mode and shape are
+// restored before returning.  0 on error.
+template <class Net>
+static size_t training_bytes(Net* h, Plan (*build)(const Net*, uint8_t*, int, int, int), BuildBackward<Net> bwd, int N,
+                             int H, int W) {
+  const int down = 1 << (h->cfg.num_blocks - 1);
+  if (N < 1 || H < down || W < down || H % down || W % down)
+    return set_err("training_bytes: N must be positive, H and W positive multiples of %d", down), 0;
+  Plan saved = std::move(h->plan);
+  const bool was_training = h->training;
+  const int n0 = h->N, h0 = h->H, w0 = h->W;
+  h->training = true;
+  h->plan = build(h, nullptr, N, H, W);
+  h->N = N; h->H = H; h->W = W;
+  const size_t ws = h->plan.ws_bytes, arena = backward_bytes(h, bwd);
+  h->plan = std::move(saved);
+  h->training = was_training;
+  h->N = n0; h->H = h0; h->W = w0;
+  return arena ? ws + arena : 0;
+}
+
 static int backward_launch_count(const NetBase* h) {   // the last backward of every part
   int n = 0;
   for (int part = 0; h && part < h->nparts; ++part) n += h->bwd[part] ? h->bwd[part]->launches : 0;
@@ -855,6 +889,17 @@ static int backward_launch_count(const NetBase* h) {   // the last backward of e
 
 // ================================================================================= C ABI: the handle protocol
 extern "C" int b200ad_unet_set_training(b200ad_unet* h, int on) { return set_training(h, on); }
+extern "C" int b200ad_unet_set_checkpointing(b200ad_unet* h, int on) { return set_checkpointing(h, on); }
+extern "C" size_t b200ad_unet_training_bytes(b200ad_unet* h, int N, int H, int W, int S) {
+  if (!h) return set_err("null handle"), 0;
+  if (S != 1 && !h->cfg.cross_attention_dim) return set_err("training_bytes: this U-Net is unconditional (S must be 1)"), 0;
+  if (S < 1 || S > XATTN_MAX_S) return set_err("training_bytes: encoder sequence length %d outside [1, %d]", S, XATTN_MAX_S), 0;
+  const int len = h->enc_len, plan_len = h->plan_enc_len;
+  h->enc_len = h->plan_enc_len = S;
+  const size_t bytes = training_bytes(h, build_plan, build_unet_backward, N, H, W);
+  h->enc_len = len; h->plan_enc_len = plan_len;
+  return bytes;
+}
 extern "C" size_t b200ad_unet_grad_floats(b200ad_unet* h) { ensure_bwd(h); return h->bwd[0]->grad_floats; }
 extern "C" size_t b200ad_unet_grad_offset(b200ad_unet* h, int i) { ensure_bwd(h); return h->bwd[0]->goff[i]; }
 extern "C" size_t b200ad_unet_backward_bytes(b200ad_unet* h) { return backward_bytes(h, build_unet_backward); }
@@ -867,6 +912,11 @@ extern "C" int b200ad_unet_debug_grad(b200ad_unet* h, const char* name, int skip
 }
 
 extern "C" int b200ad_vae_set_training(b200ad_vae* h, int on) { return set_training(h, on); }
+extern "C" int b200ad_vae_set_checkpointing(b200ad_vae* h, int on) { return set_checkpointing(h, on); }
+extern "C" size_t b200ad_vae_training_bytes(b200ad_vae* h, int N, int H, int W) {
+  if (!h) return set_err("null handle"), 0;
+  return training_bytes(h, vae_build_plan, build_vae_backward, N, H, W);
+}
 extern "C" size_t b200ad_vae_grad_floats(b200ad_vae* h) { ensure_bwd(h); return h->bwd[0]->grad_floats; }
 extern "C" size_t b200ad_vae_grad_offset(b200ad_vae* h, int i) { ensure_bwd(h); return h->bwd[0]->goff[i]; }
 extern "C" size_t b200ad_vae_backward_bytes(b200ad_vae* h) { return backward_bytes(h, build_vae_backward); }

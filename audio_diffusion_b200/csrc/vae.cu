@@ -46,7 +46,7 @@ static void vae_blocks(b200ad_vae* h) {
 }
 
 // Builds both plans (encoder, then decoder) into one workspace. Layout: [enc stats | dec stats | activations ...].
-static Plan vae_build_plan(const b200ad_vae* h, uint8_t* ws_base, int N, int H, int W) {
+Plan vae_build_plan(const b200ad_vae* h, uint8_t* ws_base, int N, int H, int W) {
   const int f = 1 << (h->cfg.num_blocks - 1);
   Plan pl;
   pl.lists.resize(2);
@@ -55,22 +55,22 @@ static Plan vae_build_plan(const b200ad_vae* h, uint8_t* ws_base, int N, int H, 
   Builder B;
   B.h = h; B.built = &pl; B.N = N;
   B.single_head = true;
-  B.nopool = debug_nopool() || h->training;
+  B.ckpt = pl.checkpoint = h->training && h->checkpointing;
+  B.nopool = debug_nopool() || (h->training && !B.ckpt);
   B.ws.base = ws_base;
   for (int pass = 0; pass < 2; ++pass) {
     enc.ops.clear(); dec.ops.clear();
-    B.pool.clear();
-    pl.taps.clear();
+    B.reset();
     B.st.off = 0;
     B.st.base = pass == 0 ? nullptr : ws_base;
     B.ws.off = pass == 0 ? 0 : ((enc.stats_bytes + dec.stats_bytes + 511) & ~(size_t)255);
     B.ops = &enc.ops; B.H = H; B.W = W;
-    B.run(h->enc);
+    B.run(h->enc, &enc.recompute);
     if (pass == 0) enc.stats_bytes = (B.st.off + 255) & ~(size_t)255;
     B.st.base = (pass == 1 && ws_base) ? ws_base + enc.stats_bytes : nullptr;
     B.st.off = 0;
     B.ops = &dec.ops; B.H = H / f; B.W = W / f;
-    B.run(h->dec);
+    B.run(h->dec, &dec.recompute);
     if (pass == 0) dec.stats_bytes = (B.st.off + 255) & ~(size_t)255;
   }
   enc.stats = (stat_t*)ws_base;

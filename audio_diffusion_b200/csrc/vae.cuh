@@ -9,4 +9,5 @@ struct b200ad_vae : b200ad::NetBase {
 
 namespace b200ad {
 enum { ENC = 0, DEC = 1 };               // the two plans (forward and backward)
+Plan vae_build_plan(const b200ad_vae* h, uint8_t* ws_base, int N, int H, int W);   // both forward plans (null: sizes only)
 }

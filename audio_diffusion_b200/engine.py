@@ -1,7 +1,7 @@
 """`EngineModel` — the `nn.Module` base of the models whose forward and backward run in libb200ad.so (`UNet2DModel`,
 `AutoencoderKL`).  It drives a library handle `b200ad_<prefix>_*` through the protocol both models share: the parameter
-table and its default initialisation, weight packing, the activation workspace, training mode, the backward arena with one
-flat gradient buffer handed out as `p.grad` views, the one-forward-per-backward guard, debug read-outs and the diffusers
+table and its default initialisation, weight packing, the activation workspace, training mode, gradient checkpointing, the
+backward arena with one flat gradient buffer handed out as `p.grad` views, the one-forward-per-backward guard, debug read-outs and the diffusers
 hub directory layout.  PyTorch owns every tensor: parameters are ordinary fp32 `nn.Parameter`s, the packed bf16 weights,
 the workspace and the backward arena are torch byte tensors.
 """
@@ -44,6 +44,7 @@ class EngineModel(nn.Module):
     # backward parts: (name, parameter-name prefixes); each part's backward fills the gradients of its own parameters
     _parts: Tuple[Tuple[str, Union[str, Tuple[str, ...]]], ...] = (("model", ""),)
     _config_keys: Optional[Sequence[str]] = None    # config.json keys from_pretrained hands to the constructor (None: all)
+    _supports_gradient_checkpointing = True
 
     def _fn(self, name: str):
         return getattr(_lib.lib(), f"b200ad_{self._prefix}_{name}")
@@ -76,6 +77,7 @@ class EngineModel(nn.Module):
         self._packed = self._packed_key = None
         self._ws = self._ws_key = None
         self._train_mode = False
+        self._checkpointing = False
         self._fwd_gen = [0] * len(self._parts)   # forwards per part: a backward must see its own forward's activations
         self._bwd_key = None
         self._grad_flat = self._bwd_arena = None
@@ -151,6 +153,29 @@ class EngineModel(nn.Module):
             _lib.check(self._fn("set_training")(self._h, 1 if on else 0))
             self._train_mode = on
             self._ws_key = None        # the workspace layout differs (no buffer pooling when training)
+            self._bwd_key = None
+
+    # ------------------------------------------------------------------ gradient checkpointing (diffusers ModelMixin API)
+    def enable_gradient_checkpointing(self) -> None:
+        """Train keeping only each block's output: the backward recomputes every resnet's, attention's, transformer's and
+        downsampler's internals from its input right before that block's backward (the same forward kernels, into shared
+        buffers).  Less training memory for more time per iteration; gradients equal those without it up to the run-to-run
+        spread of the backward's reductions.  Inference is unaffected."""
+        self._set_checkpointing(True)
+
+    def disable_gradient_checkpointing(self) -> None:
+        """Keep every activation of the training forward again (the default)."""
+        self._set_checkpointing(False)
+
+    @property
+    def is_gradient_checkpointing(self) -> bool:
+        return self._checkpointing
+
+    def _set_checkpointing(self, on: bool) -> None:
+        if self._checkpointing != on:
+            _lib.check(self._fn("set_checkpointing")(self._h, 1 if on else 0))
+            self._checkpointing = on
+            self._ws_key = None        # the training workspace layout and the backward plan differ
             self._bwd_key = None
 
     def _bind_backward(self, dev: torch.device) -> None:

@@ -138,6 +138,19 @@ int b200ad_unet_conv_plan(const b200ad_unet* h, int N, int H, int W, int num_sms
  * computed.  With S = 1 encoder token, attn2.to_q, attn2.to_k and norm2 get exactly zero gradients (softmax over one key is
  * constant); with S > 1 every parameter gets its gradient. */
 int b200ad_unet_set_training(b200ad_unet* h, int on);
+/* Gradient checkpointing (default off; only training plans change).  On, the training forward keeps in buffers of their
+ * own only each block's output with its GroupNorm statistics (conv_in included), the time-embedding MLP values and the
+ * autoencoder's input latents and pre_out / conv_out.  A block's internals (resnet .h1, attention .qkv / .ao / softmax,
+ * the transformer internals with their row log-sum-exp and K / V, a downsampler's .parity) go to the pooled buffers
+ * inference uses.  Right before a block's backward, the backward re-runs the block's own forward ops that rebuild those
+ * internals (never the op that writes the block output), so backward_launch_count includes them.  debug_tensor of such a
+ * tap fails while a checkpointing plan is bound.  Changing the mode clears the plan, as set_training does: call
+ * bind_workspace and bind_backward again. */
+int b200ad_unet_set_checkpointing(b200ad_unet* h, int on);
+/* Device bytes one training step of (N, H, W) with S encoder tokens (1 for an unconditional model) binds in the current
+ * checkpointing mode: the training workspace plus the backward arena (parameters, packed weights and gradients excluded).
+ * Needs no device and leaves the bound plan alone.  0 on error. */
+size_t b200ad_unet_training_bytes(b200ad_unet* h, int N, int H, int W, int S);
 size_t b200ad_unet_grad_floats(b200ad_unet* h);
 size_t b200ad_unet_grad_offset(b200ad_unet* h, int i);
 size_t b200ad_unet_backward_bytes(b200ad_unet* h);       /* arena for activation gradients, temporaries, transposed weights */
@@ -192,6 +205,9 @@ int b200ad_vae_last_launch_count(const b200ad_vae* h);
  * writes only the slots of its own part: the decoder and post_quant_conv, or the encoder and quant_conv.  Implemented for
  * in_channels = out_channels = latent_channels = 1; no gradient w.r.t. the input image is computed. */
 int b200ad_vae_set_training(b200ad_vae* h, int on);
+/* As b200ad_unet_set_checkpointing / b200ad_unet_training_bytes, over both parts (H, W: image resolution). */
+int b200ad_vae_set_checkpointing(b200ad_vae* h, int on);
+size_t b200ad_vae_training_bytes(b200ad_vae* h, int N, int H, int W);
 size_t b200ad_vae_grad_floats(b200ad_vae* h);
 size_t b200ad_vae_grad_offset(b200ad_vae* h, int i);
 size_t b200ad_vae_backward_bytes(b200ad_vae* h);

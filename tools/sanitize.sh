@@ -13,9 +13,11 @@ for tool in memcheck racecheck synccheck; do
   echo "$tool smoke: exit $?"
   tail -3 gpurun_out/sanitizer_${tool}_smoke_${tag}.log
 done
+# the backward cases: the plain backward, and one with gradient checkpointing (it re-runs forward ops into shared buffers)
 for tool in memcheck racecheck; do
   timeout 900 $CS --tool $tool --print-limit 20 --log-file gpurun_out/sanitizer_${tool}_bwd_${tag}.log \
-    python -m pytest tests/test_gpu_train.py -x -q -m gpu -k "test_unet_backward_matches_autograd" \
+    python -m pytest tests/test_gpu_train.py tests/test_gpu_checkpointing.py -x -q -m gpu \
+    -k "test_unet_backward_matches_autograd or (test_checkpointed_training_matches_plain and published)" \
     > gpurun_out/sanitizer_${tool}_bwd_${tag}.out 2>&1
   echo "$tool backward: exit $?"
   tail -3 gpurun_out/sanitizer_${tool}_bwd_${tag}.log
