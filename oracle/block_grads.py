@@ -9,7 +9,9 @@ error of the blocks after it.
 
 `unet_blocks` / `vae_blocks` restate the engine's block lists (input, skip connection, output tap, parameters);
 `chain` runs the references in reverse over given activations, which is how tests/test_cpu_block_backward.py shows that
-the decomposition reproduces autograd through the whole model.
+the decomposition reproduces autograd through the whole model.  The U-Net's timestep MLP (time_embedding.*) belongs to no
+block: every resnet's reference also returns the gradient of the temb_act it reads (block_backward(temb_grad=True)), and
+`temb_backward` takes their sum through the MLP, so that the blocks and the MLP together claim every parameter.
 
 `bf16_storage()` rounds, inside a reference, every conv / linear operand, weight and output to bf16 and every gradient
 that flows back through those operands and outputs: the points where the engine stores a tensor or a gradient in bf16.
@@ -128,12 +130,25 @@ def vae_blocks(cfg: vo.VAEConfig, part: str) -> List[Block]:
     return bl
 
 
+TEMB_PREFIXES = ("time_embedding.",)   # the timestep MLP's parameters: no block's; temb_backward checks them
+
+
 def temb_act(w, cfg, t: torch.Tensor) -> torch.Tensor:
     """silu(time_embedding(t)): what every resnet's time_emb_proj reads (unet_oracle.unet_forward), in w's dtype."""
     dt = w["time_embedding.linear_1.weight"].dtype
     emb = uo.timestep_embedding(t, cfg.block_out_channels[0]).to(dt)
     emb = F.silu(F.linear(emb, w["time_embedding.linear_1.weight"], w["time_embedding.linear_1.bias"]))
     return F.silu(F.linear(emb, w["time_embedding.linear_2.weight"], w["time_embedding.linear_2.bias"]))
+
+
+def temb_backward(w, cfg, t: torch.Tensor, g_temb: torch.Tensor) -> Dict[str, torch.Tensor]:
+    """fp64 autograd of temb_act(w, cfg, t) from the gradient g_temb of its output (the sum of every resnet's, from
+    block_backward): {parameter name: gradient} of the four time_embedding.* tensors."""
+    dev = g_temb.device
+    pw = {k: w[k].detach().to(device=dev, dtype=torch.float64).requires_grad_(True) for k in w
+          if k.startswith(TEMB_PREFIXES)}
+    out = temb_act(pw, cfg, t.to(dev))
+    return dict(zip(pw.keys(), torch.autograd.grad(out, list(pw.values()), g_temb.to(torch.float64))))
 
 
 def _forward(blk: Block, w, xs: Sequence[torch.Tensor], cfg, temb_act, enc):
@@ -237,25 +252,31 @@ def bf16_storage(forward: bool = False, bf16_probs: bool = False):
 
 
 def block_backward(blk: Block, w: Dict[str, torch.Tensor], xs: Sequence[torch.Tensor], gout: torch.Tensor, cfg,
-                   temb_act: Optional[torch.Tensor] = None, enc: Optional[torch.Tensor] = None, rounded: bool = False):
+                   temb_act: Optional[torch.Tensor] = None, enc: Optional[torch.Tensor] = None, rounded: bool = False,
+                   temb_grad: bool = False):
     """fp64 autograd of one block from its inputs xs and output gradient gout.  Returns (gradients w.r.t. xs, {parameter
-    name: gradient} for the block's own parameters).  rounded: under bf16_storage(), with the input gradients rounded to
-    bf16 as the engine stores them."""
+    name: gradient} for the block's own parameters); temb_grad: also, third, the gradient w.r.t. temb_act, or None for a
+    block that does not read it (only the U-Net's resnets do, through time_emb_proj).  rounded: under bf16_storage(),
+    with the input gradients rounded to bf16 as the engine stores them (the temb_act gradient stays fp32 there: the
+    engine sums it from fp32 channel sums)."""
     dev = gout.device
     d = lambda t: t.detach().to(device=dev, dtype=torch.float64)
     pw = {k: d(v).requires_grad_(True) for k, v in w.items() if k.startswith(blk.prefixes)}
     xl = [d(x).requires_grad_(True) for x in xs]
-    ta = d(temb_act) if temb_act is not None else None
+    reads_temb = (temb_grad and temb_act is not None and blk.kind == "resnet"
+                  and blk.name + ".time_emb_proj.weight" in pw)
+    ta = d(temb_act).requires_grad_(reads_temb) if temb_act is not None else None
     en = d(enc) if enc is not None else None
     with bf16_storage() if rounded else contextlib.nullcontext():
         out = _forward(blk, pw, xl, cfg, ta, en)
-        leaves = xl + list(pw.values())
+        leaves = xl + list(pw.values()) + ([ta] if reads_temb else [])
         gr = torch.autograd.grad(out, leaves, d(gout), allow_unused=True)
     gr = [torch.zeros_like(t) if g is None else g for t, g in zip(leaves, gr)]
     gi = gr[:len(xl)]
     if rounded:
         gi = [bf16(g) for g in gi]
-    return gi, dict(zip(pw.keys(), gr[len(xl):]))
+    gp = dict(zip(pw.keys(), gr[len(xl):len(xl) + len(pw)]))
+    return (gi, gp, gr[-1] if reads_temb else None) if temb_grad else (gi, gp)
 
 
 def _probs_rounded(blk: Block, x: torch.Tensor) -> bool:
@@ -411,24 +432,29 @@ def sub_forward(blk: Block, w: Dict[str, torch.Tensor], xs: Sequence[torch.Tenso
 
 
 def chain(blocks: Sequence[Block], acts: Dict[str, torch.Tensor], model_in: torch.Tensor, g_out: torch.Tensor, w, cfg,
-          temb_act=None, enc=None):
+          temb_act=None, enc=None, t=None):
     """Runs block_backward over `blocks` in reverse from the gradient of the model's output, over the activations `acts`
     (by tap name): the gradient of every tap (skip shares added where the skip connection is consumed), every block
-    parameter's gradient, and the gradient w.r.t. the model's input."""
+    parameter's gradient, and the gradient w.r.t. the model's input.  With the timesteps t (U-Net), the resnets'
+    temb_act gradients summed and taken through the timestep MLP (temb_backward) give its parameters' gradients too."""
     G: Dict[str, torch.Tensor] = {}
     grads: Dict[str, torch.Tensor] = {}
-    g_in = None
+    g_in = g_temb = None
     for blk in reversed(blocks):
         gout = g_out if blk.out is None else G[blk.out]
         xs = [model_in if blk.inp is None else acts[blk.inp]] + ([acts[blk.skip]] if blk.skip else [])
-        gi, gp = block_backward(blk, w, xs, gout, cfg, temb_act, enc)
+        gi, gp, gt = block_backward(blk, w, xs, gout, cfg, temb_act, enc, temb_grad=True)
         grads.update(gp)
+        if gt is not None:
+            g_temb = gt if g_temb is None else g_temb + gt
         if blk.inp is None:
             g_in = gi[0]
         else:
             G[blk.inp] = G[blk.inp] + gi[0] if blk.inp in G else gi[0]
         if blk.skip:
             G[blk.skip] = G[blk.skip] + gi[1] if blk.skip in G else gi[1]
+    if t is not None:
+        grads.update(temb_backward(w, cfg, t, g_temb))
     return G, grads, g_in
 
 

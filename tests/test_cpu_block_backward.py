@@ -1,11 +1,13 @@
 """CPU checks of oracle/block_grads.py, the per-block references of tests/test_gpu_block_backward.py.
 
 * Composition: the block references chained in reverse over the oracle's own fp64 activations, from the gradient of the
-  model's output, reproduce fp64 autograd through the whole model (U-Net, conditional U-Net, both autoencoder parts):
-  the block lists, the skip bookkeeping and each block's decomposition are right before any GPU number is trusted.
+  model's output, reproduce fp64 autograd through the whole model (U-Net, conditional U-Net, both autoencoder parts),
+  the U-Net's timestep MLP included: the block lists, the skip bookkeeping and each block's decomposition are right
+  before any GPU number is trusted.
+* Coverage: the blocks and the timestep MLP claim every parameter exactly once.
 * Floor: each block kind's gradients with bf16 storage (bf16_storage()) against exact, at the GPU test's shapes, over the
-  oracle's activations and upstream gradients rounded to bf16 as the engine stores them.  These are the floors the GPU
-  bars are stated from.
+  oracle's activations and upstream gradients rounded to bf16 as the engine stores them, and the timestep MLP's
+  gradients from the resnets' rounded temb_act gradients.  These are the floors the GPU bars are stated from.
 """
 import pytest
 import torch
@@ -56,8 +58,8 @@ def test_unet_block_chain_reproduces_autograd():
     _, ref, _ = loss_and_grads(w, cfg, clean, noise, t)
     blocks = bg.unet_blocks(cfg)
     assert any(b.skip and taps[b.inp].shape[1] + taps[b.skip].shape[1] == 384 for b in blocks)   # cpg 12 straddles
-    _, grads, _ = bg.chain(blocks, taps, noisy, g_eps, w, cfg, taps["temb_act"])
-    _check_params(grads, ref, [k for k in w if not k.startswith("time_embedding.")])
+    _, grads, _ = bg.chain(blocks, taps, noisy, g_eps, w, cfg, taps["temb_act"], t=t)
+    _check_params(grads, ref, list(w))
 
 
 def _cond_chain(cfg_kw, size, n, transformers):
@@ -79,12 +81,12 @@ def _cond_chain(cfg_kw, size, n, transformers):
     pred = unet_cond_forward(w, cfg, noisy, t, enc, taps)
     blocks = bg.unet_blocks(cfg)
     assert sum(b.kind == "transformer" for b in blocks) == transformers
-    _, grads, _ = bg.chain(blocks, taps, noisy, 2 * (pred - noise) / pred.numel(), w, cfg, bg.temb_act(w, cfg, t), enc)
+    _, grads, _ = bg.chain(blocks, taps, noisy, 2 * (pred - noise) / pred.numel(), w, cfg, bg.temb_act(w, cfg, t), enc, t)
     for k in grads:      # attn2.to_q / to_k and norm2 do not reach the output: exactly zero
         if ref[k] is None:
             ref[k] = torch.zeros_like(w[k])
             assert torch.count_nonzero(grads[k]) == 0, k
-    _check_params(grads, ref, [k for k in w if not k.startswith("time_embedding.")])
+    _check_params(grads, ref, list(w))
 
 
 def test_cond_unet_block_chain_reproduces_autograd():
@@ -104,8 +106,8 @@ def test_published_unet_block_chain_reproduces_autograd():
         ["down_blocks.4.attentions.0", "down_blocks.4.attentions.1", "mid_block.attentions.0"]
         + [f"up_blocks.1.attentions.{j}" for j in range(3)])
     assert sum(b.skip is not None for b in blocks) == 6 * 3
-    _, grads, _ = bg.chain(blocks, taps, noisy, g_eps, w, cfg, taps["temb_act"])
-    _check_params(grads, ref, [k for k in w if not k.startswith("time_embedding.")])
+    _, grads, _ = bg.chain(blocks, taps, noisy, g_eps, w, cfg, taps["temb_act"], t=t)
+    _check_params(grads, ref, list(w))
 
 
 @pytest.mark.timeout(300)
@@ -138,16 +140,57 @@ def test_vae_block_chain_reproduces_autograd():
             assert _rel(g_in, xi.grad) < 1e-10
 
 
-def _floors(blocks, taps, model_in, g_out, w, cfg, temb=None, enc=None):
+def _claims(names, blocks, extra=()):
+    """{parameter name: the blocks (or the timestep MLP, "temb") whose prefixes claim it}."""
+    owners = [(b.name or b.kind, b.prefixes) for b in blocks] + [("temb", p) for p in extra]
+    return {k: [o for o, pre in owners if k.startswith(pre)] for k in names}
+
+
+@pytest.mark.parametrize("model", ["published", "train", "cond_small", "cond_published", "vae"])
+def test_every_parameter_claimed_once(model):
+    """Every parameter of the oracle's init_weights is claimed by exactly one block of the per-block references or by the
+    timestep MLP (temb_backward): a parameter outside them would have no per-tensor fp64 check in the GPU per-block
+    tests, as time_embedding.* had none before the MLP was checked.  The conditional U-Net's parameters and block list
+    do not depend on the encoder's token count, so one case covers S = 1 and S > 1.  The autoencoder: encoder and
+    decoder block lists together."""
+    from oracle import unet_cond_oracle as uco
+    from oracle import unet_oracle as uo
+    from oracle import vae_oracle as vo
+    from test_gpu_cond_train import ARCH
+    from test_gpu_fullconfig import REF_ARCH
+    if model == "vae":
+        cfg = vo.VAEConfig()
+        names = list(vo.init_weights(cfg, seed=0))
+        claims = _claims(names, bg.vae_blocks(cfg, "encoder") + bg.vae_blocks(cfg, "decoder"))
+    else:
+        if model.startswith("cond"):
+            arch = COND_CFG if model == "cond_small" else ARCH
+            cfg = uco.CondUNetConfig(sample_size=(32, 32), **{k: arch[k] for k in ("block_out_channels",
+                                                                                    "down_block_types", "up_block_types")})
+            names = list(uco.init_weights(cfg, seed=0))
+        else:
+            cfg = uo.UNetConfig(sample_size=(32, 32), **(REF_ARCH if model == "published" else TRAIN_CFG))
+            names = list(uo.init_weights(cfg, seed=0))
+        claims = _claims(names, bg.unet_blocks(cfg), bg.TEMB_PREFIXES)
+        assert len([k for k, o in claims.items() if o == ["temb"]]) == 4
+    bad = {k: o for k, o in claims.items() if len(o) != 1}
+    assert names and not bad, bad
+
+
+def _floors(blocks, taps, model_in, g_out, w, cfg, temb=None, enc=None, t=None):
     """bf16 floor of every block (rounded storage against exact, over bf16 inputs and upstream gradients), worst per
-    kind: {kind: (activation (a, b, c), parameter (a, b, c))}."""
+    kind: {kind: (activation (a, b, c), parameter (a, b, c))}.  With the timesteps t (U-Net), also "temb": the timestep
+    MLP's parameter gradients from the sum of the resnets' rounded-storage temb_act gradients against the exact sum."""
     G, _, _ = bg.chain(blocks, taps, model_in, g_out, w, cfg, temb, enc)
     out = {}
+    gt_exact = gt_round = 0.0
     for blk in blocks:
         xs = [model_in if blk.inp is None else bg.bf16(taps[blk.inp])] + ([bg.bf16(taps[blk.skip])] if blk.skip else [])
         gout = g_out if blk.out is None else bg.bf16(G[blk.out])
-        ei, ep = bg.block_backward(blk, w, xs, gout, cfg, temb, enc)
-        ri, rp = bg.block_backward(blk, w, xs, gout, cfg, temb, enc, rounded=True)
+        ei, ep, et = bg.block_backward(blk, w, xs, gout, cfg, temb, enc, temb_grad=True)
+        ri, rp, rt = bg.block_backward(blk, w, xs, gout, cfg, temb, enc, True, temb_grad=True)
+        if et is not None:
+            gt_exact, gt_round = gt_exact + et, gt_round + rt
         acts = {} if blk.inp is None else {"in": (ri[0], ei[0])}
         if blk.skip:
             acts["skip"] = (ri[1], ei[1])
@@ -155,6 +198,10 @@ def _floors(blocks, taps, model_in, g_out, w, cfg, temb=None, enc=None):
         wa, wp = bg.worst(rows, True), bg.worst(rows, False)
         pa, pp = out.get(blk.kind, ((0.0,) * 3, (0.0,) * 3))
         out[blk.kind] = (tuple(map(max, pa, wa)), tuple(map(max, pp, wp)))
+    if t is not None:
+        ep, rp = bg.temb_backward(w, cfg, t, gt_exact), bg.temb_backward(w, cfg, t, gt_round)
+        rows, _ = bg.compare_block({}, {k: (rp[k], ep[k]) for k in ep})
+        out["temb"] = ((0.0,) * 3, bg.worst(rows, False))
     for k, (a, p) in out.items():
         print(f"floor {k:12s} act L2 {a[0]:.4f} max {a[1]:.4f} row {a[2]:.4f} | param L2 {p[0]:.4f} max {p[1]:.4f} "
               f"row {p[2]:.4f}")
@@ -175,7 +222,7 @@ def _assert_floors(fl, bars):
 def test_unet_block_floors():
     from test_gpu_block_backward import UNET_BARS
     cfg, w, clean, noise, t, noisy, taps, g_eps = _unet_case((32, 32), 3, 2)
-    _assert_floors(_floors(bg.unet_blocks(cfg), taps, noisy, g_eps, w, cfg, taps["temb_act"]), UNET_BARS)
+    _assert_floors(_floors(bg.unet_blocks(cfg), taps, noisy, g_eps, w, cfg, taps["temb_act"], t=t), UNET_BARS)
 
 
 @pytest.mark.timeout(600)
@@ -193,8 +240,8 @@ def test_cond_unet_block_floors():
     taps = {}
     pred = unet_cond_forward(w, cfg, noisy, T3, enc, taps)
     blocks = bg.unet_blocks(cfg)
-    _assert_floors(_floors(blocks, taps, noisy, 2 * (pred - noise) / pred.numel(), w, cfg, bg.temb_act(w, cfg, T3), enc),
-                   COND_BARS)
+    _assert_floors(_floors(blocks, taps, noisy, 2 * (pred - noise) / pred.numel(), w, cfg, bg.temb_act(w, cfg, T3), enc,
+                           T3), COND_BARS)
 
 
 @pytest.mark.timeout(900)

@@ -14,6 +14,13 @@ and gradient against exact), and no lower than 0.5 %: the engine forms bias grad
 gradient before it stores that gradient in bf16, while the reference sums the stored values (0.1 - 0.3 % measured), and
 that is the floor of the gradients no bf16 rounding reaches.  The floors are in the comments as (a, b, c).  Parameters
 whose exact gradient is zero (softmax-invariant key biases) are listed, not compared.
+
+The U-Net's timestep MLP (time_embedding.linear_1 / linear_2) belongs to no block: after the walk, the engine's gradients
+of its four tensors are compared with fp64 autograd of the MLP (block_grads.temb_backward) from the sum of every resnet's
+fp64 gradient w.r.t. the temb_act it reads, as the "temb" row.  That checks, past the per-resnet time_emb_proj gradients,
+the engine's gradient w.r.t. temb_act (its per-resnet rows scattered into one [N][rows] array and multiplied by the
+concatenated time_emb_proj weights) and the MLP backward after it.  Its floor is the MLP's gradients from the resnets'
+rounded-storage temb_act gradients against the exact ones (tests/test_cpu_block_backward.py's _floors).
 """
 import pytest
 import torch
@@ -37,6 +44,7 @@ UNET_BARS = {
     "attn": ((0.005, 0.009, 0.005), (0.0123, 0.0153, 0.0906)),   # floor (0.0017, 0.003, 0.0017) | (0.0041, 0.0051, 0.0302)
     "up": ((0.0087, 0.0116, 0.0084), (0.005, 0.005, 0.005)),   # floor (0.0029, 0.0039, 0.0028) | (0.0, 0.0, 0.0)
     "tail": ((0.0072, 0.0134, 0.0069), (0.005, 0.005, 0.005)),   # floor (0.0024, 0.0045, 0.0023) | (0.0002, 0.0003, 0.0002)
+    "temb": ((0.005, 0.005, 0.005), (0.006, 0.0066, 0.0843)),   # floor (0.0, 0.0, 0.0) | (0.002, 0.0022, 0.0281)
 }
 COND_BARS = {
     "head": ((0.005, 0.005, 0.005), (0.005, 0.005, 0.005)),   # floor (0.0, 0.0, 0.0) | (0.0, 0.0, 0.0)
@@ -45,6 +53,7 @@ COND_BARS = {
     "down": ((0.0069, 0.0096, 0.0066), (0.005, 0.005, 0.005)),   # floor (0.0023, 0.0032, 0.0022) | (0.0, 0.0, 0.0)
     "up": ((0.0087, 0.0114, 0.0084), (0.005, 0.005, 0.005)),   # floor (0.0029, 0.0038, 0.0028) | (0.0, 0.0, 0.0)
     "tail": ((0.0072, 0.0141, 0.0072), (0.005, 0.005, 0.005)),   # floor (0.0024, 0.0047, 0.0024) | (0.0002, 0.0003, 0.0002)
+    "temb": ((0.005, 0.005, 0.005), (0.0069, 0.0087, 0.0672)),   # floor (0.0, 0.0, 0.0) | (0.0023, 0.0029, 0.0224)
 }
 VAE_BARS = {
     "decoder:dec_head": ((0.005, 0.005, 0.005), (0.005, 0.005, 0.005)),   # floor (0.0, 0.0, 0.0) | (0.0, 0.0, 0.0)
@@ -60,18 +69,38 @@ VAE_BARS = {
 }
 
 
-def _run_checks(model, blocks, model_in, g_out, w, cfg, bars, prefix="", temb=None, enc=None, g_in=None):
-    """Compares every block; prints one table row per block; returns the blocks over their bars."""
+def _run_checks(model, blocks, model_in, g_out, w, cfg, bars, prefix="", temb=None, enc=None, g_in=None, t=None):
+    """Compares every block; prints one table row per block; returns the blocks over their bars.  A U-Net (temb given)
+    also needs its timesteps t: after the walk, the engine's time_embedding.* gradients against temb_backward of the sum
+    of every resnet's fp64 temb_act gradient, as the "temb" row."""
+    assert (temb is None) == (t is None), "a U-Net's checks need both temb and t"
     named = dict(model.named_parameters())
     skip_taps = {b.skip for b in blocks if b.skip}
     fails, worst_kind = [], {}
+    g_temb = None
     print(f"\n{'block':44s} {'kind':12s} {'act L2':>7s} {'max':>7s} {'row':>7s} | {'par L2':>7s} {'max':>7s} {'row':>7s}")
+
+    def row(name, kind, rows, skipped):
+        wa, wp = bg.worst(rows, True), bg.worst(rows, False)
+        ba, bp = bars[kind]
+        over = [r for r in rows if any(e > b for e, b in zip(r[2:], ba if r[1] else bp))]
+        print(f"{name:44s} {kind:12s} {wa[0]:7.4f} {wa[1]:7.4f} {wa[2]:7.4f} | {wp[0]:7.4f} {wp[1]:7.4f} "
+              f"{wp[2]:7.4f}{'  OVER' if over else ''}{'  (zero ref: ' + ', '.join(skipped) + ')' if skipped else ''}")
+        for r in over:
+            print(f"    {r[0]}: {r[2]:.4f} {r[3]:.4f} {r[4]:.4f}")
+        if over:
+            fails.append((name, [(r[0], round(r[2], 4), round(r[3], 4), round(r[4], 4)) for r in over]))
+        pa, pp = worst_kind.get(kind, ((0.0,) * 3, (0.0,) * 3))
+        worst_kind[kind] = (tuple(map(max, pa, wa)), tuple(map(max, pp, wp)))
+
     for blk in reversed(blocks):
         xs = [model_in if blk.inp is None else model.debug_tensor(blk.inp)]
         if blk.skip:
             xs.append(model.debug_tensor(blk.skip))
         gout = g_out if blk.out is None else model.debug_grad(blk.out)
-        gi, gp = bg.block_backward(blk, w, xs, gout, cfg, temb, enc)
+        gi, gp, gt = bg.block_backward(blk, w, xs, gout, cfg, temb, enc, temb_grad=True)
+        if gt is not None:
+            g_temb = gt if g_temb is None else g_temb + gt
         acts = {}
         if blk.inp is not None:
             ref = gi[0]
@@ -83,18 +112,11 @@ def _run_checks(model, blocks, model_in, g_out, w, cfg, bars, prefix="", temb=No
         if blk.skip:
             acts[f"skip G({blk.skip})"] = (model.debug_grad(blk.skip, skip=True), gi[1])
         rows, skipped = bg.compare_block(acts, {k: (named[k].grad, gp[k]) for k in gp})
-        wa, wp = bg.worst(rows, True), bg.worst(rows, False)
-        kind = prefix + blk.kind
-        ba, bp = bars[kind]
-        over = [r for r in rows if any(e > b for e, b in zip(r[2:], ba if r[1] else bp))]
-        print(f"{blk.name or 'conv_out':44s} {kind:12s} {wa[0]:7.4f} {wa[1]:7.4f} {wa[2]:7.4f} | {wp[0]:7.4f} {wp[1]:7.4f} "
-              f"{wp[2]:7.4f}{'  OVER' if over else ''}{'  (zero ref: ' + ', '.join(skipped) + ')' if skipped else ''}")
-        for r in over:
-            print(f"    {r[0]}: {r[2]:.4f} {r[3]:.4f} {r[4]:.4f}")
-        if over:
-            fails.append((blk.name, [(r[0], round(r[2], 4), round(r[3], 4), round(r[4], 4)) for r in over]))
-        pa, pp = worst_kind.get(kind, ((0.0,) * 3, (0.0,) * 3))
-        worst_kind[kind] = (tuple(map(max, pa, wa)), tuple(map(max, pp, wp)))
+        row(blk.name or "conv_out", prefix + blk.kind, rows, skipped)
+    if t is not None:    # the timestep MLP, from the resnets' temb_act gradients (engine: gproj -> time_emb_proj^T -> MLP)
+        ref = bg.temb_backward(w, cfg, t, g_temb)
+        rows, skipped = bg.compare_block({}, {k: (named[k].grad, ref[k]) for k in ref})
+        row("time_embedding", prefix + "temb", rows, skipped)
     print("worst per kind (activation a, b, c | parameter a, b, c) against the bars:")
     for kind, (a, p) in worst_kind.items():
         print(f"  {kind:20s} {a[0]:.4f} {a[1]:.4f} {a[2]:.4f} | {p[0]:.4f} {p[1]:.4f} {p[2]:.4f}   bars {bars[kind]}")
@@ -130,7 +152,8 @@ def test_unet_backward_per_block(cuda, size):
     g_eps = 2 * (pred.detach() - noise) / pred.numel()
     w64 = _w64(w, cuda)
     blocks = bg.unet_blocks(cfg)
-    fails = _run_checks(model, blocks, noisy, g_eps, w64, cfg, UNET_BARS, temb=bg.temb_act(w64, cfg, t.to(cuda)))
+    fails = _run_checks(model, blocks, noisy, g_eps, w64, cfg, UNET_BARS, temb=bg.temb_act(w64, cfg, t.to(cuda)),
+                        t=t.to(cuda))
     assert not fails, fails
 
 
@@ -162,7 +185,7 @@ def test_cond_unet_backward_per_block(cuda):
     assert len(zero) == 6 * 4 and all(torch.count_nonzero(named[k].grad) == 0 for k in zero)
     w64 = _w64(w, cuda)
     fails = _run_checks(model, bg.unet_blocks(cfg), noisy, g_eps, w64, cfg, COND_BARS,
-                        temb=bg.temb_act(w64, cfg, t.to(cuda)), enc=enc)
+                        temb=bg.temb_act(w64, cfg, t.to(cuda)), enc=enc, t=t.to(cuda))
     assert not fails, fails
 
 

@@ -2,6 +2,8 @@
 100-d token per 5-second slice, (B, S, 100)): the cross-attention kernels against fp32 autograd, the model forward,
 sampling and training against the fp32 oracle (oracle/unet_cond_oracle.py, which attends over any number of tokens), and
 the S = 1 path left as it was.  Bars: those of tests/test_gpu_cond.py and tests/test_gpu_cond_train.py."""
+import time
+
 import numpy as np
 import pytest
 import torch
@@ -410,14 +412,11 @@ def test_cond_seq_forward_per_block(cuda, monkeypatch, s):
     check_against_floors(f"UNet2DConditionModel 32x32 batch 3, {s} tokens", rows, floors, COND_SEQ_FWD_BARS[s], t0)
 
 
-@pytest.mark.timeout(600)
-@pytest.mark.parametrize("s", [3, 77])
-def test_cond_seq_backward_per_block(cuda, s):
-    """After one training forward and backward with an (3, s, 100) encoding: every block's input gradient(s) and parameter
-    gradients against fp64 autograd of that block from the engine's own input activations and output gradient.  The
-    transformers' walk covers attn2.to_out, the cross-attention backward (dQ, the split dK / dV partial sums), the K / V
-    weight gradients, to_q, LN2 with its residual and the two to_out biases; attn2.to_q, attn2.to_k and norm2 get non-zero
-    gradients inside the bars.  The other block kinds keep test_gpu_block_backward.py's COND_BARS."""
+def cond_seq_backward_case(cuda, s, checkpointing=False):
+    """One training forward and backward of the two-level conditional U-Net with an (3, s, 100) encoding, every block and
+    the timestep MLP against fp64 (test_gpu_block_backward._run_checks), and the transformer and MLP bars against the
+    floors at these inputs.  checkpointing: under enable_gradient_checkpointing(), at the same bars (the floors depend on
+    the seeds alone, so they are not measured again)."""
     from audio_diffusion_b200.unet_cond import UNet2DConditionModel
     from oracle import block_grads as bg
     from oracle.schedulers_oracle import OracleDDPM
@@ -430,6 +429,8 @@ def test_cond_seq_backward_per_block(cuda, s):
     model = UNet2DConditionModel(sample_size=(32, 32), **COND_ARCH)
     model.load_state_dict(w)
     model = model.to(cuda).train()
+    if checkpointing:
+        model.enable_gradient_checkpointing()
     g = torch.Generator().manual_seed(4)
     clean = torch.rand(3, 1, 32, 32, generator=g) * 2 - 1
     noise = torch.randn(3, 1, 32, 32, generator=g)
@@ -446,17 +447,39 @@ def test_cond_seq_backward_per_block(cuda, s):
     w64 = _w64(w, cuda)
     bars = dict(COND_BARS, transformer=COND_SEQ_BWD_TRANSFORMER_BARS[s])
     blocks = bg.unet_blocks(cfg)
+    torch.cuda.reset_peak_memory_stats()
+    t0 = time.perf_counter()
     temb = bg.temb_act(w64, cfg, t.to(cuda))
-    fails = _run_checks(model, blocks, noisy, g_eps, w64, cfg, bars, temb=temb, enc=enc)
+    fails = _run_checks(model, blocks, noisy, g_eps, w64, cfg, bars, temb=temb, enc=enc, t=t.to(cuda))
+    torch.cuda.synchronize()
+    print(f"\n{s} tokens{', checkpointed' if checkpointing else ''}: fp64 time {time.perf_counter() - t0:.1f} s, peak "
+          f"device memory {torch.cuda.max_memory_allocated() / 2 ** 30:.1f} GiB")
     assert not fails, fails
-    # the transformer bars against the floor at these inputs (oracle activations, fp64 on the device)
+    if checkpointing:
+        return
+    # the transformer and MLP bars against the floor at these inputs (oracle activations, fp64 on the device; the MLP's,
+    # COND_BARS', measured on the CPU with one token: (0.0022, 0.0036, 0.0261) with 3 tokens, (0.0022, 0.0029, 0.0298)
+    # with 77 on an H100)
     taps = {}
     x64, n64, e64 = noisy.double(), noise.double(), enc.double()
     with torch.no_grad():
         ref = unet_cond_forward(w64, cfg, x64, t.to(cuda), e64, taps)
-    fl = _floors(blocks, taps, x64, 2 * (ref - n64) / ref.numel(), w64, cfg, temb, e64)["transformer"]
-    for f, b in zip(fl[0] + fl[1], bars["transformer"][0] + bars["transformer"][1]):
-        assert f < b <= max(3.3 * round(f, 4), 5e-3) + 1e-9, (fl, bars["transformer"])
+    fl = _floors(blocks, taps, x64, 2 * (ref - n64) / ref.numel(), w64, cfg, temb, e64, t.to(cuda))
+    for kind in ("transformer", "temb"):
+        for f, b in zip(fl[kind][0] + fl[kind][1], bars[kind][0] + bars[kind][1]):
+            assert f < b <= max(3.3 * round(f, 4), 5e-3) + 1e-9, (kind, fl[kind], bars[kind])
+
+
+@pytest.mark.timeout(600)
+@pytest.mark.parametrize("s", [3, 77])
+def test_cond_seq_backward_per_block(cuda, s):
+    """After one training forward and backward with an (3, s, 100) encoding: every block's input gradient(s) and parameter
+    gradients against fp64 autograd of that block from the engine's own input activations and output gradient, and the
+    timestep MLP's gradients from the resnets' temb_act gradients.  The transformers' walk covers attn2.to_out, the
+    cross-attention backward (dQ, the split dK / dV partial sums), the K / V weight gradients, to_q, LN2 with its
+    residual and the two to_out biases; attn2.to_q, attn2.to_k and norm2 get non-zero gradients inside the bars.  The
+    other block kinds keep test_gpu_block_backward.py's COND_BARS."""
+    cond_seq_backward_case(cuda, s)
 
 
 # ---------------------------------------------------------------------------------------------------- errors
