@@ -75,16 +75,19 @@ SYMBOLS = {
     "b200ad_unet_conv_plan": (_I, [_VP, _I, _I, _I, _I, C.POINTER(_I), _I]),
     "b200ad_unet_set_training": (_I, [_VP, _I]),
     "b200ad_unet_set_checkpointing": (_I, [_VP, _I]),
+    "b200ad_unet_set_param_grads": (_I, [_VP, _I]),
     "b200ad_unet_training_bytes": (_SZ, [_VP, _I, _I, _I, _I]),
     "b200ad_unet_grad_floats": (_SZ, [_VP]),
     "b200ad_unet_grad_offset": (_SZ, [_VP, _I]),
     "b200ad_unet_backward_bytes": (_SZ, [_VP]),
     "b200ad_unet_bind_backward": (_I, [_VP, _VP, _SZ, _VP, _VP]),
     "b200ad_unet_backward": (_I, [_VP, _VP, _VP, _I, _VP]),
+    "b200ad_unet_backward_input": (_I, [_VP, _VP, _VP, _VP, _I, _VP]),
     "b200ad_unet_backward_launch_count": (_I, [_VP]),
     "b200ad_unet_debug_grad": (_I, [_VP, C.c_char_p, _I, _VP, C.POINTER(_I), _VP]),
     "b200ad_vae_set_training": (_I, [_VP, _I]),
     "b200ad_vae_set_checkpointing": (_I, [_VP, _I]),
+    "b200ad_vae_set_param_grads": (_I, [_VP, _I]),
     "b200ad_vae_training_bytes": (_SZ, [_VP, _I, _I, _I]),
     "b200ad_vae_grad_floats": (_SZ, [_VP]),
     "b200ad_vae_grad_offset": (_SZ, [_VP, _I]),
@@ -92,6 +95,7 @@ SYMBOLS = {
     "b200ad_vae_bind_backward": (_I, [_VP, _VP, _SZ, _VP, _VP]),
     "b200ad_vae_decoder_backward": (_I, [_VP, _VP, _VP, _I, _VP]),
     "b200ad_vae_encoder_backward": (_I, [_VP, _VP, _VP, _I, _VP]),
+    "b200ad_vae_encoder_backward_input": (_I, [_VP, _VP, _VP, _VP, _I, _VP]),
     "b200ad_vae_backward_launch_count": (_I, [_VP]),
     "b200ad_vae_debug_grad": (_I, [_VP, C.c_char_p, _I, _VP, C.POINTER(_I), _VP]),
     "b200ad_vae_create": (_I, [C.POINTER(VAEConfigC), C.POINTER(_VP)]),

@@ -85,10 +85,12 @@ cudaError_t launch_attention_1head_bwd(const __nv_bfloat16* qkv, const __nv_bflo
 // fp32 [N][L2][H][W] (gh_nc) and [L2][N][H][W] (gh_cn); dwq / dbq accumulated.  L2 <= 8.
 cudaError_t launch_quant_conv_bwd(const float* gm, const __nv_bfloat16* h, const float* wq, float* gh_nc, float* gh_cn,
                                   float* dwq, float* dbq, int N, int L2, int H, int W, cudaStream_t s);
-// conv_in (3x3, L -> C) on post_quant_conv(z) (1x1, L -> L): gy (PF8, C channels) -> gz (fp32 [N][L][H][W]);
-// dwpq / dbpq accumulated (z: the forward's input latents).  L <= 4.
-cudaError_t launch_latent_in_bwd(const __nv_bfloat16* gy, const float* win, const float* wpq, const float* z, float* gz,
-                                 float* dwpq, float* dbpq, int N, int C, int L, int H, int W, cudaStream_t s);
+// Data gradient of conv_in (3x3, 1 -> C) down to its input: gy (PF8, C channels) -> gx (fp32 [N][H][W], overwritten,
+// fixed-order fp32 sums).  Decoder head (wpq given): conv_in reads post_quant_conv(z) (1x1, 1 -> 1), gx is the gradient
+// w.r.t. z, and with dwpq given dwpq / dbpq are accumulated (z: the forward's input latents).
+cudaError_t launch_conv_in_dgrad(const __nv_bfloat16* gy, const float* win, float* gx, int N, int C, int H, int W,
+                                 cudaStream_t s, const float* wpq = nullptr, const float* z = nullptr, float* dwpq = nullptr,
+                                 float* dbpq = nullptr);
 
 // Weight gradient on wgmma (wgrad_tc.cu):  dw[(co * cin_total + ci_off + ci) * ntaps_total + tapidx[t]] +=
 //   sum_{n, p} gy[n][co][p] * act[n][ci][p + shift[t]].   gy / act are channel views: `*_img_planes` planes per image in the

@@ -99,6 +99,7 @@ __global__ void __launch_bounds__(256) layernorm_bwd_pf8_kernel(const __nv_bfloa
       *reinterpret_cast<uint4*>(gx + off + (long long)pl * g.PL * 8) = pack8_f(o);
     }
   }
+  if (!dgamma) return;   // no parameter gradients (uniform over the CTA)
 #pragma unroll
   for (int j = 0; j < 2; ++j) {
     const int pl = lane + 32 * j;

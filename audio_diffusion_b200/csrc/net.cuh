@@ -48,7 +48,9 @@ enum OpKind { OP_TEMB = 0, OP_CONV_IN = 1, OP_GN = 2, OP_CONV = 3, OP_PARITY = 5
               OP_LIN_IN, OP_LIN_W, OP_SILU_BWD, OP_SILU_FWD, OP_MEMSET, OP_LN_BWD, OP_GEGLU_BWD, OP_XVEC_BWD, OP_MHA_BWD,
               OP_ATTN1_BWD, OP_QUANT_BWD, OP_LATENT_IN_BWD,
               OP_XKV /* cross-attention K / V projections of an S > 1 encoding */, OP_XATTN /* cross-attention, S > 1 */,
-              OP_XATTN_BWD, OP_XKV_BWD, OP_NKINDS };
+              OP_XATTN_BWD, OP_XKV_BWD,
+              OP_INPUT_DGRAD /* conv_in's data gradient to the model's input: runs only when the call passes g_x */,
+              OP_NKINDS };
 // by OpKind: error messages and the backward profile's keys (tools/cond_train_bench.py matches "mha_bwd x<count>")
 static const char* const op_names[] = {
     "temb", "conv_in", "gn_finalize", "conv_tc", "", "parity_split", "attention", "conv_out", "attention_1head", "vae_sample",
@@ -56,7 +58,7 @@ static const char* const op_names[] = {
     "gn_bwd", "chan_sum", "reduce_n", "scatter", "pf8_add", "attention_bwd", "unfold_up2", "scalar_wgrad", "conv_in(dgrad)",
     "flip", "sum_add", "lin_in", "lin_w", "silu_bwd", "silu_fwd", "memset", "layernorm_bwd", "geglu_bwd",
     "cross_attn_vec_bwd", "mha_bwd", "attention_1head_bwd", "quant_conv_bwd", "latent_in_bwd", "cross_attn_kv", "cross_attn",
-    "cross_attn_bwd", "cross_attn_kv_wgrad"};
+    "cross_attn_bwd", "cross_attn_kv_wgrad", "input_dgrad"};
 static_assert(sizeof(op_names) / sizeof(op_names[0]) == OP_NKINDS, "one name per OpKind");
 
 struct RunArgs {                        // the per-call inputs of a plan
@@ -72,6 +74,7 @@ struct RunArgs {                        // the per-call inputs of a plan
   const float* g_eps = nullptr;         // the gradient of the model output (U-Net: eps; autoencoder decoder: the image)
   const float* g_mom = nullptr;         // autoencoder encoder: the gradient of the moments
   float* g_z = nullptr;                 // autoencoder decoder: the gradient w.r.t. the latents (written)
+  float* g_x = nullptr;                 // U-Net / autoencoder encoder: the gradient w.r.t. the input (written; null: none)
 };
 
 using OpFn = std::function<cudaError_t(const RunArgs&, cudaStream_t)>;
@@ -226,6 +229,8 @@ struct NetBase {
   bool training = false;            // keep the activations (all of them unless checkpointing) and the timestep-MLP
                                     // pre-activations for backward
   bool checkpointing = false;       // training keeps only the block outputs; the backward recomputes each block's internals
+  bool param_grads = true;          // the backward computes the parameter gradients (off: data gradients only, no flat
+                                    // gradient buffer)
   int num_sms = 132;
   const float* enc = nullptr;       // conditional U-Net: encoder_hidden_states [N][enc_S][X] of the next forward
   int enc_S = 0;
@@ -1058,6 +1063,14 @@ static int set_checkpointing(NetBase* h, int on) {
   }
   return 0;
 }
+static int set_param_grads(NetBase* h, int on) {
+  if (!h) return set_err("null handle");
+  if (h->param_grads != (on != 0)) {
+    h->param_grads = on != 0;
+    h->plan.lists.clear();    // as set_checkpointing: the backward arena differs
+  }
+  return 0;
+}
 
 // ================================================================================= plan executor
 struct OpEvents {   // per-op timing: an event before the first op of a run and one after every op
@@ -1084,10 +1097,11 @@ static int run_ops(const NetBase* h, const OpList& l, const RunArgs& a, cudaStre
   int n = 0;
   for (size_t i = 0; i < l.ops.size(); ++i) {
     const Op& op = l.ops[i];
-    const cudaError_t e = op.run ? op.run(a, st) : launch_conv_tc(op.conv, h->num_sms, st);
+    const bool skip = op.kind == OP_INPUT_DGRAD && !a.g_x;   // the input gradient is computed only when asked for
+    const cudaError_t e = skip ? cudaSuccess : op.run ? op.run(a, st) : launch_conv_tc(op.conv, h->num_sms, st);
     if (e != cudaSuccess) return set_err("%s: %s", op_names[op.kind], cudaGetErrorString(e));
     if (timing) CK(cudaEventRecord(timing->ev[i + 1], st));
-    n += op.launches;
+    n += skip ? 0 : op.launches;
   }
   *launches = n;
   return 0;

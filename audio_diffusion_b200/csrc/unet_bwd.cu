@@ -9,6 +9,10 @@
 //   * weight gradients run on wgrad_tc_kernel (wgmma, pixels as the reduction dimension, MN-major operands);
 //   * GroupNorm(+SiLU), attention core, biases / time embedding, conv_in / conv_out are memory-bound kernels (bwd_kernels.cu).
 // The normalised activations the weight gradients read are materialised (no fusion yet).
+// With parameter gradients off (set_param_grads(0): a frozen model differentiated w.r.t. its input) the plan carries the
+// data gradients only: no weight-gradient, bias, GroupNorm / LayerNorm affine or timestep-MLP work, and no flat buffer.
+// The heads' conv_in data gradient to the model's input (OP_INPUT_DGRAD) is in every plan and runs only when the call
+// passes g_x.
 // A backward plan is an OpList of net.cuh, run by the forward's executor (run_ops).
 // With gradient checkpointing the forward kept only the block outputs: before a block's backward ops, the plan re-runs the
 // block's own forward ops (Recompute) that rebuild its internals in the forward's pooled buffers.
@@ -54,6 +58,7 @@ struct BwdBuilder {
   float* cs = nullptr;                        // [N][maxC] channel sums scratch
   float* gsums = nullptr;                     // GroupNorm backward scratch [N][maxC][2]
   float* gproj = nullptr;                     // U-Net: [N][temb_rows]
+  bool pg = true;                             // parameter gradients: emitters whose only output is one emit nothing
   int heads = 8;                              // conditional U-Net: attention heads of the transformer blocks
   bool single_head = false;                   // attention with one head of dim C (the autoencoder) instead of head_dim 8
   // per-sample channel sums produced by the GroupNorm-backward apply pass for the gradient tensor it writes (keyed by that
@@ -149,6 +154,7 @@ struct BwdBuilder {
   }
   // weight gradient of the forward K-segment with tap set t (of ntaps_total taps of the weight) that read `act`
   void wgrad(const View& gy, const View& act, float* dw, int cin_total, int ci_off, int ntaps_total, const TapSet& t) {
+    if (!pg) return;
     WgradDesc d{};
     d.gy = gy.p; d.act = act.p; d.dw = dw; d.N = N; d.H = gy.H; d.W = gy.W; d.cout = gy.C; d.cin = act.C;
     d.gy_img_planes = gy.img_planes; d.act_img_planes = act.img_planes;
@@ -161,6 +167,7 @@ struct BwdBuilder {
   }
   // per-channel sums of a gradient -> bias gradient(s); last_cs: the [N][C] sums (valid until the next chan_sum)
   void bias_grad(const View& g, const std::string& bname, const std::string& bname2 = "") {
+    if (!pg) return;
     float* db = PG(bname);
     float* db2 = bname2.empty() ? nullptr : PG(bname2);
     auto it = csum_of.find(g.off);
@@ -176,7 +183,9 @@ struct BwdBuilder {
       return launch_chan_sum(g.p, sums, N, g.C, g.img_planes, g.H, g.W, s, db, db2);
     });
   }
+  // the normalised input a weight gradient reads (parameter gradients off: none)
   Act gn_apply(const std::string& tag, const Act& a, const Act* b, const std::string& norm, bool silu, float eps = -1.f) {
+    if (!pg) return Act{};
     Act out = tmp(tag, a.C + (b ? b->C : 0), a.H, a.W);
     const GnApplyParams p = gn_params(h, N, a, b, norm, out.p, silu, eps);
     emit(OP_GNAPPLY, [p](const RunArgs&, cudaStream_t s) { return launch_gn_apply(p, s); });
@@ -195,7 +204,7 @@ struct BwdBuilder {
     p.sums = gsums;
     p.csum0 = nullptr;
     const size_t need = (size_t)N * a.C;
-    if (csum_used + need <= csum_floats) {
+    if (pg && csum_used + need <= csum_floats) {   // the sums only feed bias gradients
       p.csum0 = csum_arena ? csum_arena + csum_used : nullptr;
       csum_of[d0.off] = p.csum0;
       csum_used += need;
@@ -220,11 +229,21 @@ struct BwdBuilder {
   // weight gradient of a 3x3 conv with one fp32 output channel x (null: the gradient passed to backward(); flip: x is
   // that output's gradient, `g` the conv's input) or one fp32 input channel x (the conv's output gradient is `g`)
   void scalar_wgrad(const Act& g, const float* x, bool x_is_input, float* dw, int flip) {
+    if (!pg) return;
     emit(OP_SCALAR_WGRAD, [g, x, x_is_input, dw, flip, N = N](const RunArgs& a, cudaStream_t s) {
       return launch_scalar_conv_wgrad(g.p, x ? x : x_is_input ? a.in : a.g_eps, dw, N, g.C, g.H, g.W, flip, s);
     });
   }
+  // conv_in's (3x3, 1 -> C) data gradient from G(conv_in) to the model's input: RunArgs::g_x (fp32 [N][1][H][W], written);
+  // run_ops skips the op when the call passes no g_x
+  void input_dgrad(const std::string& conv_in, const Act& Gx) {
+    emit(OP_INPUT_DGRAD, [gy = Gx.p, win = P(conv_in + ".weight"), N = N, C = Gx.C, H = Gx.H,
+                          W = Gx.W](const RunArgs& a, cudaStream_t s) {
+      return launch_conv_in_dgrad(gy, win, a.g_x, N, C, H, W, s);
+    });
+  }
   void sum_add(const float* x, long long n, float* dst) {   // x null: the gradient passed to backward()
+    if (!pg) return;
     emit(OP_SUMADD, [x, n, dst](const RunArgs& a, cudaStream_t s) { return launch_sum_add(x ? x : a.g_eps, n, dst, s); });
   }
 
@@ -251,7 +270,7 @@ struct BwdBuilder {
     gn_bwd(T1, h1, nullptr, n + ".norm2", true, Gh1, nullptr, nullptr, nullptr);
     // conv1 bias + time embedding projection rows of this block
     bias_grad(whole(Gh1), n + ".conv1.bias");
-    if (k.temb_row >= 0)
+    if (k.temb_row >= 0 && pg)
       emit(OP_SCATTER, [sums = last_cs, gproj = gproj, N = N, co, rows = h->temb_rows, row = k.temb_row](const RunArgs&,
                                                                                                          cudaStream_t s) {
         return launch_scatter_rows(sums, gproj, N, co, rows, row, s);
@@ -375,13 +394,14 @@ struct BwdBuilder {
       dgrad(t + ".attn1.to_out.0.weight", whole(Gh2), Gao, 1);
       wgrad_conv(whole(Gh2), whole(ao), t + ".attn1.to_out.0.weight", 1);
       bias_grad(whole(Gh2), t + ".attn1.to_out.0.bias", t + ".attn2.to_out.0.bias");
-      // dvec[n] = per-sample channel sums of G(h2) (last_cs, made just above)
-      emit(OP_XVEC_BWD, [h = h, dvec = last_cs, wv = P(t + ".attn2.to_v.weight"), wo = P(t + ".attn2.to_out.0.weight"),
-                         dwo = PG(t + ".attn2.to_out.0.weight"), dwv = PG(t + ".attn2.to_v.weight"),
-                         scratch = (float*)mem.take((size_t)2 * N * C * sizeof(float)), N = N, C,
-                         X = k.cross](const RunArgs&, cudaStream_t s) {
-        return launch_cross_attn_vec_bwd(h->enc, dvec, wv, wo, dwo, dwv, scratch, N, C, X, s);
-      }, 2);
+      // dvec[n] = per-sample channel sums of G(h2) (last_cs, made just above); it reaches parameters only
+      if (pg)
+        emit(OP_XVEC_BWD, [h = h, dvec = last_cs, wv = P(t + ".attn2.to_v.weight"), wo = P(t + ".attn2.to_out.0.weight"),
+                           dwo = PG(t + ".attn2.to_out.0.weight"), dwv = PG(t + ".attn2.to_v.weight"),
+                           scratch = (float*)mem.take((size_t)2 * N * C * sizeof(float)), N = N, C,
+                           X = k.cross](const RunArgs&, cudaStream_t s) {
+          return launch_cross_attn_vec_bwd(h->enc, dvec, wv, wo, dwo, dwv, scratch, N, C, X, s);
+        }, 2);
     } else {
       Gh1 = cross_attention_bwd(k, Gh2, Gao, Gn, S);
       dgrad(t + ".attn1.to_out.0.weight", whole(Gh1), Gao, 1);
@@ -440,10 +460,11 @@ struct BwdBuilder {
                         kv, N = N, C, heads = heads, H, W, S](const RunArgs&, cudaStream_t s) {
       return launch_xattn_bwd(q, kvp, kvp + kv, o, go, lse, dsum, part, gq, dkv, dkv + kv, N, C, heads, H, W, S, s);
     }, 4);
-    emit(OP_XKV_BWD, [h = h, dkv, kv, dwk = PG(t + ".attn2.to_k.weight"), dwv = PG(t + ".attn2.to_v.weight"), M = N * S, C,
-                      X = k.cross](const RunArgs&, cudaStream_t s) {
-      return launch_xattn_kv_wgrad(dkv, dkv + kv, h->enc, dwk, dwv, M, C, X, s);
-    });
+    if (pg)
+      emit(OP_XKV_BWD, [h = h, dkv, kv, dwk = PG(t + ".attn2.to_k.weight"), dwv = PG(t + ".attn2.to_v.weight"),
+                        M = N * S, C, X = k.cross](const RunArgs&, cudaStream_t s) {
+        return launch_xattn_kv_wgrad(dkv, dkv + kv, h->enc, dwk, dwv, M, C, X, s);
+      });
     // to_q (no bias)
     wgrad_conv(whole(Gq2), whole(n2), t + ".attn2.to_q.weight", 1);
     dgrad(t + ".attn2.to_q.weight", whole(Gq2), Gn, 1);
@@ -501,8 +522,8 @@ struct BwdBuilder {
     emit(OP_PARITY, [gy = Gy.p, gpar = gpar.p, N = N, C, H = y.H, W = y.W](const RunArgs&, cudaStream_t s) {
       return launch_parity_split(gy, gpar, N, C, H, W, s);
     });
-    float* dwf = (float*)mem.take((size_t)4 * C * C * 4 * sizeof(float));
-    zero(dwf, (size_t)4 * C * C * 4 * sizeof(float));
+    float* dwf = pg ? (float*)mem.take((size_t)4 * C * C * 4 * sizeof(float)) : nullptr;
+    if (pg) zero(dwf, (size_t)4 * C * C * 4 * sizeof(float));
     Act Gx = G(xn);
     ConvParams dg = conv_geom(N, Gx);
     UnfoldMasks um{};
@@ -518,9 +539,10 @@ struct BwdBuilder {
         seg(dg.seg[pidx], whole(plane), tjob(n + ".weight", C, C, 3, bwd_taps), bwd_taps);
       }
     dg.nseg = 4;
-    emit(OP_UNFOLD, [dwf, dw = PG(n + ".weight"), nco_ci = (long long)C * C, um](const RunArgs&, cudaStream_t s) {
-      return launch_unfold_up2(dwf, dw, nco_ci, um, s);
-    });
+    if (pg)
+      emit(OP_UNFOLD, [dwf, dw = PG(n + ".weight"), nco_ci = (long long)C * C, um](const RunArgs&, cudaStream_t s) {
+        return launch_unfold_up2(dwf, dw, nco_ci, um, s);
+      });
     conv(dg);
   }
 
@@ -547,9 +569,10 @@ static int build_unet_backward(b200ad_unet* h, Backward* const* bws, uint8_t* ar
   bw->list.ops.clear();
   bw->jobs.clear();
   bw->arena = arena;
-  bw->grads = grads;
+  bw->grads = h->param_grads ? grads : nullptr;
   BwdBuilder B;
   B.h = h; B.bw = bw; B.N = h->N;
+  B.pg = h->param_grads;
   B.heads = c.attention_head_dim;
   B.mem.base = arena;
   B.pack_op();
@@ -558,13 +581,16 @@ static int build_unet_backward(b200ad_unet* h, Backward* const* bws, uint8_t* ar
   const int D = c.block_out_channels[0] * 4;
   B.cs = (float*)B.mem.take((size_t)h->N * 3 * maxC * sizeof(float));
   B.gsums = (float*)B.mem.take((size_t)h->N * 3 * maxC * 2 * sizeof(float));
-  B.gproj = (float*)B.mem.take((size_t)h->N * h->temb_rows * sizeof(float));
-  B.csum_floats = (size_t)h->N * 65536;       // all GroupNorm-backward outputs of the reference architecture: 16 K channels
-  B.csum_arena = (float*)B.mem.take(B.csum_floats * sizeof(float));
-  B.zero(B.csum_arena, B.csum_floats * sizeof(float));
-  float* g_act = (float*)B.mem.take((size_t)h->N * D * sizeof(float));   // gradient w.r.t. silu(linear_2)
-  float* g_h1 = (float*)B.mem.take((size_t)h->N * D * sizeof(float));
-  float* h1v = (float*)B.mem.take((size_t)h->N * D * sizeof(float));
+  float *g_act = nullptr, *g_h1 = nullptr, *h1v = nullptr;
+  if (B.pg) {   // bias-gradient sums and the timestep MLP's backward
+    B.gproj = (float*)B.mem.take((size_t)h->N * h->temb_rows * sizeof(float));
+    B.csum_floats = (size_t)h->N * 65536;     // all GroupNorm-backward outputs of the reference architecture: 16 K channels
+    B.csum_arena = (float*)B.mem.take(B.csum_floats * sizeof(float));
+    B.zero(B.csum_arena, B.csum_floats * sizeof(float));
+    g_act = (float*)B.mem.take((size_t)h->N * D * sizeof(float));   // gradient w.r.t. silu(linear_2)
+    g_h1 = (float*)B.mem.take((size_t)h->N * D * sizeof(float));
+    h1v = (float*)B.mem.take((size_t)h->N * D * sizeof(float));
+  }
   float* wflip = (float*)B.mem.take((size_t)c.block_out_channels[0] * 9 * sizeof(float));
   const float* zbias = (const float*)B.mem.take((size_t)c.block_out_channels[0] * sizeof(float));   // never written: zeros
 
@@ -597,7 +623,7 @@ static int build_unet_backward(b200ad_unet* h, Backward* const* bws, uint8_t* ar
       case BK_CONV_OUT:      // g_eps -> gradient of the last activation
         if (c.out_channels != 1) return set_err("backward: out_channels != 1 is not implemented");
         B.conv_out_bwd(k, in, wflip, zbias);
-        B.zero(B.gproj, (size_t)h->N * h->temb_rows * sizeof(float));
+        if (B.pg) B.zero(B.gproj, (size_t)h->N * h->temb_rows * sizeof(float));
         break;
       case BK_RESNET: B.resnet_bwd(k, in, tap(k.skip)); break;
       case BK_ATTN: B.attention_bwd(k.name, in); break;
@@ -610,6 +636,8 @@ static int build_unet_backward(b200ad_unet* h, Backward* const* bws, uint8_t* ar
         const Act Gx = B.G(n);
         if (!B.skipgrad.count(n)) return set_err("backward: conv_in skip gradient missing");
         // (the first resnet's GroupNorm backward already added the skip contribution)
+        B.input_dgrad(n, Gx);
+        if (!B.pg) break;
         B.scalar_wgrad(Gx, nullptr, true, B.PG(n + ".weight"), 0);
         B.bias_grad(BwdBuilder::whole(Gx), n + ".bias");
         const Plan& pl = h->plan;
@@ -656,8 +684,11 @@ static int build_vae_backward(b200ad_vae* h, Backward* const* bws, uint8_t* aren
   for (const auto& kv : h->plan.taps) maxC = kv.second.C > maxC ? kv.second.C : maxC;
   B.cs = (float*)B.mem.take((size_t)h->N * 3 * maxC * sizeof(float));
   B.gsums = (float*)B.mem.take((size_t)h->N * 3 * maxC * 2 * sizeof(float));
-  B.csum_floats = (size_t)h->N * 65536;
-  B.csum_arena = (float*)B.mem.take(B.csum_floats * sizeof(float));
+  B.pg = h->param_grads;
+  if (B.pg) {
+    B.csum_floats = (size_t)h->N * 65536;
+    B.csum_arena = (float*)B.mem.take(B.csum_floats * sizeof(float));
+  }
   float* wflip = (float*)B.mem.take((size_t)Cmax * L2 * 9 * sizeof(float));
   const float* zbias = (const float*)B.mem.take((size_t)Cmax * sizeof(float));   // never written: zeros
   float* gh = (float*)B.mem.take((size_t)2 * h->N * L2 * hl * wl * sizeof(float));  // encoder tail: [N][2L] | [2L][N]
@@ -667,12 +698,12 @@ static int build_vae_backward(b200ad_vae* h, Backward* const* bws, uint8_t* aren
     bw->list.ops.clear();
     bw->jobs.clear();
     bw->arena = arena;
-    bw->grads = grads;
+    bw->grads = h->param_grads ? grads : nullptr;
     B.bw = bw;
     B.grad.clear(); B.skipgrad.clear(); B.csum_of.clear();
     B.csum_used = 0;
     B.pack_op();
-    B.zero(B.csum_arena, B.csum_floats * sizeof(float));
+    if (B.pg) B.zero(B.csum_arena, B.csum_floats * sizeof(float));
     const std::vector<Block>& bl = part == ENC ? h->enc : h->dec;
     auto tap = [&](int i) {
       return i < 0 ? std::string() : (bl[i].kind == BK_CONV_IN || bl[i].kind == BK_LATENT_IN) ? bl[i].name + "conv_in" : bl[i].name;
@@ -709,18 +740,19 @@ static int build_vae_backward(b200ad_vae* h, Backward* const* bws, uint8_t* aren
         case BK_ATTN: B.attention_bwd(k.name, in); break;
         case BK_DOWN_ASYM: B.downsample_bwd(k, in); break;
         case BK_UP: B.upsample_bwd(k.name, in); break;
-        case BK_CONV_IN:        // encoder head: weight gradients only (no gradient w.r.t. the image)
+        case BK_CONV_IN:        // encoder head: weight gradients, and the gradient w.r.t. the image when asked for
         case BK_LATENT_IN: {    // decoder head: conv_in on post_quant_conv(z), then the gradient w.r.t. z
           const std::string n = tap(i);
-          const Act x = B.fwd(n);
           const Act Gx = B.G(n);
           B.scalar_wgrad(Gx, k.kind == BK_CONV_IN ? nullptr : pl.zq, true, B.PG(n + ".weight"), 0);
           B.bias_grad(BwdBuilder::whole(Gx), n + ".bias");
-          if (k.kind == BK_LATENT_IN)
+          if (k.kind == BK_CONV_IN)
+            B.input_dgrad(n, Gx);
+          else
             B.emit(OP_LATENT_IN_BWD, [gy = Gx.p, win = B.P(n + ".weight"), wpq = B.P("post_quant_conv.weight"), z = pl.z_in,
                                       dw = B.PG("post_quant_conv.weight"), db = B.PG("post_quant_conv.bias"), N = h->N,
-                                      C = x.C, L = k.cin, H = x.H, W = x.W](const RunArgs& a, cudaStream_t s) {
-              return launch_latent_in_bwd(gy, win, wpq, z, a.g_z, dw, db, N, C, L, H, W, s);
+                                      C = Gx.C, H = Gx.H, W = Gx.W](const RunArgs& a, cudaStream_t s) {
+              return launch_conv_in_dgrad(gy, win, a.g_z, N, C, H, W, s, wpq, z, dw, db);
             });
           break;
         }
@@ -769,7 +801,8 @@ static int run_backward(NetBase* h, int part, const RunArgs& a, int accumulate, 
   Backward* bw = h->bwd[part];
   // B200AD_BWD_PROFILE=1: CUDA events around every op, per-kind totals printed to stderr (tools/train_bench.py)
   static const bool prof = [] { const char* e = getenv("B200AD_BWD_PROFILE"); return e && e[0] == '1'; }();
-  if (!accumulate) CK(cudaMemsetAsync(bw->grads + bw->zero_off, 0, bw->zero_floats * sizeof(float), st));   // every kernel below ADDS
+  if (bw->grads && !accumulate)   // every kernel below ADDS
+    CK(cudaMemsetAsync(bw->grads + bw->zero_off, 0, bw->zero_floats * sizeof(float), st));
   OpEvents ev;
   if (run_ops(h, bw->list, a, st, &bw->launches, prof ? &ev : nullptr)) return -1;
   if (prof) {
@@ -844,6 +877,7 @@ template <class Net> static size_t backward_bytes(Net* h, BuildBackward<Net> bui
 
 template <class Net>
 static int bind_backward(Net* h, BuildBackward<Net> build, void* arena, size_t bytes, float* grads, cudaStream_t st) {
+  if (h->param_grads && !grads) return set_err("bind_backward: the gradient buffer is required unless parameter gradients are off");
   Backward sized[2];
   const size_t need = backward_size(h, build, sized);
   if (!need) return -1;
@@ -890,6 +924,7 @@ static int backward_launch_count(const NetBase* h) {   // the last backward of e
 // ================================================================================= C ABI: the handle protocol
 extern "C" int b200ad_unet_set_training(b200ad_unet* h, int on) { return set_training(h, on); }
 extern "C" int b200ad_unet_set_checkpointing(b200ad_unet* h, int on) { return set_checkpointing(h, on); }
+extern "C" int b200ad_unet_set_param_grads(b200ad_unet* h, int on) { return set_param_grads(h, on); }
 extern "C" size_t b200ad_unet_training_bytes(b200ad_unet* h, int N, int H, int W, int S) {
   if (!h) return set_err("null handle"), 0;
   if (S != 1 && !h->cfg.cross_attention_dim) return set_err("training_bytes: this U-Net is unconditional (S must be 1)"), 0;
@@ -913,6 +948,7 @@ extern "C" int b200ad_unet_debug_grad(b200ad_unet* h, const char* name, int skip
 
 extern "C" int b200ad_vae_set_training(b200ad_vae* h, int on) { return set_training(h, on); }
 extern "C" int b200ad_vae_set_checkpointing(b200ad_vae* h, int on) { return set_checkpointing(h, on); }
+extern "C" int b200ad_vae_set_param_grads(b200ad_vae* h, int on) { return set_param_grads(h, on); }
 extern "C" size_t b200ad_vae_training_bytes(b200ad_vae* h, int N, int H, int W) {
   if (!h) return set_err("null handle"), 0;
   return training_bytes(h, vae_build_plan, build_vae_backward, N, H, W);
@@ -935,15 +971,20 @@ extern "C" int b200ad_vae_decoder_backward(b200ad_vae* h, const float* g_x, floa
   return run_backward(h, DEC, a, accumulate, (cudaStream_t)stream);
 }
 
-extern "C" int b200ad_vae_encoder_backward(b200ad_vae* h, const float* x, const float* g_moments, int accumulate,
-                                           void* stream) {
+extern "C" int b200ad_vae_encoder_backward_input(b200ad_vae* h, const float* x, const float* g_moments, float* g_x,
+                                                 int accumulate, void* stream) {
   if (!x || !g_moments) return set_err("encoder_backward: x and g_moments are required");
   RunArgs a;
-  a.in = x; a.g_mom = g_moments;
+  a.in = x; a.g_mom = g_moments; a.g_x = g_x;
   return run_backward(h, ENC, a, accumulate, (cudaStream_t)stream);
 }
+extern "C" int b200ad_vae_encoder_backward(b200ad_vae* h, const float* x, const float* g_moments, int accumulate,
+                                           void* stream) {
+  return b200ad_vae_encoder_backward_input(h, x, g_moments, nullptr, accumulate, stream);
+}
 
-extern "C" int b200ad_unet_backward(b200ad_unet* h, const float* x, const float* g_eps, int accumulate, void* stream) {
+extern "C" int b200ad_unet_backward_input(b200ad_unet* h, const float* x, const float* g_eps, float* g_x, int accumulate,
+                                          void* stream) {
   if (!x || !g_eps) return set_err("backward: x and g_eps are required");
   if (h && h->cfg.cross_attention_dim && !h->enc) return set_err("backward: the conditional U-Net needs the forward's encoding bound");
   if (h && h->cfg.cross_attention_dim && h->bwd[0] && !h->bwd[0]->list.ops.empty()) {
@@ -955,6 +996,9 @@ extern "C" int b200ad_unet_backward(b200ad_unet* h, const float* x, const float*
       return set_err("backward: the bound encoding has %d tokens but the plan was built for %d", h->enc_S, planned);
   }
   RunArgs a;
-  a.in = x; a.g_eps = g_eps;
+  a.in = x; a.g_eps = g_eps; a.g_x = g_x;
   return run_backward(h, 0, a, accumulate, (cudaStream_t)stream);
+}
+extern "C" int b200ad_unet_backward(b200ad_unet* h, const float* x, const float* g_eps, int accumulate, void* stream) {
+  return b200ad_unet_backward_input(h, x, g_eps, nullptr, accumulate, stream);
 }

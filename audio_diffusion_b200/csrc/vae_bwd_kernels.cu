@@ -1,6 +1,7 @@
 // Backward kernels of the autoencoder's own layers (AutoencoderKL training, scripts/train_vae.py): the single-head
-// attention of the mid blocks on the tensor cores, the encoder tail (quant_conv on the moments) and the decoder head
-// (conv_in to the latents, post_quant_conv).  Everything else of the autoencoder backward reuses the U-Net's kernels.
+// attention of the mid blocks on the tensor cores, the encoder tail (quant_conv on the moments) and conv_in's data gradient
+// (the decoder head's, through post_quant_conv to the latents; the U-Net's and the encoder's, to their inputs).  Everything
+// else of the autoencoder backward reuses the U-Net's kernels.
 // Oracle: torch autograd over oracle/vae_oracle.py.
 #include "bwd_kernels.cuh"
 
@@ -235,6 +236,7 @@ __global__ void __launch_bounds__(256) quant_conv_bwd_kernel(const float* __rest
       gh_cn[((long long)i * N + n) * HW + p] = s;
     }
   }
+  if (!dwq) return;   // no parameter gradients (uniform over the CTA)
   for (int o = 0; o < L2; ++o) {
     float b = warp_sum_v(gv[o]);
     if ((threadIdx.x & 31) == 0) atomicAdd(dbq + o, b);
@@ -251,51 +253,86 @@ cudaError_t launch_quant_conv_bwd(const float* gm, const __nv_bfloat16* h, const
   return cudaGetLastError();
 }
 
-// Decoder head: zq = post_quant_conv(z) (1x1, L -> L, fp32), y = conv_in(zq) (3x3, L -> C).  From g_y (PF8, C channels):
-//   g_zq[l][p] = sum_c sum_t Win[c][l][t] g_y[c][p - shift(t)]     (one warp per pixel, lanes over 8-channel planes)
-//   g_z = Wpq^T g_zq;  dWpq += g_zq z^T;  dbpq += sum g_zq.
-__global__ void __launch_bounds__(256) latent_in_bwd_kernel(const __nv_bfloat16* __restrict__ gy, const float* __restrict__ win,
-                                                            const float* __restrict__ wpq, const float* __restrict__ z,
-                                                            float* __restrict__ gz, float* __restrict__ dwpq,
-                                                            float* __restrict__ dbpq, int N, int C, int L, int H, int W) {
+// conv_in's data gradient down to its one input channel (the U-Net's sample, the encoder's image, the decoder's
+// post_quant_conv(z)).  From g_y (PF8, C channels, the gradient of conv_in's output):
+//   g[n][p] = sum_c sum_t Win[c][t] g_y[n][c][p - shift(t)]
+// One thread per pixel: the 32 threads of a warp read 32 neighbouring pixels of one 8-channel plane per tap, so g_y is
+// read from DRAM once and the taps' re-reads hit L1; the weights sit in shared memory as [plane][tap][8].  The sum is
+// fixed-order fp32: plane pl goes into partial pl % 32 (its planes, taps and channels in order), and the 32 partials
+// are added pairwise at distances 16, 8, 4, 2, 1 (as a binary tree: partial i + partial i + 16 first).  That is the order of the earlier one-warp-per-pixel decoder kernel
+// (lanes over planes, then an xor-shuffle sum), so the decoder's g_z is bitwise what it was.
+// wpq null: gx = g (fp32 [N][H][W], overwritten, no atomics).  Otherwise the decoder head, zq = post_quant_conv(z) (1x1,
+// 1 -> 1): gx = Wpq g, and with dwpq given, dWpq += sum g z, dbpq += sum g.
+constexpr int CIN_DG_THREADS = 256;
+__global__ void __launch_bounds__(CIN_DG_THREADS) conv_in_dgrad_kernel(const __nv_bfloat16* __restrict__ gy,
+                                                                       const float* __restrict__ win,
+                                                                       const float* __restrict__ wpq,
+                                                                       const float* __restrict__ z, float* __restrict__ gx,
+                                                                       float* __restrict__ dwpq, float* __restrict__ dbpq,
+                                                                       int N, int C, int H, int W) {
+  extern __shared__ float4 sw4[];   // [C/8][9][8] floats
+  float* sw = reinterpret_cast<float*>(sw4);
+  for (int i = threadIdx.x; i < C * 9; i += blockDim.x) {
+    const int c = i / 9, t = i - c * 9;
+    sw[((c >> 3) * 9 + t) * 8 + (c & 7)] = win[i];
+  }
+  __syncthreads();
   const Geom g = make_geom(N, H, W);
-  const int HW = H * W, lane = threadIdx.x & 31;
-  const int tok = blockIdx.x * 8 + (threadIdx.x >> 5);
+  const int HW = H * W, np = C / 8;
+  const int tok = blockIdx.x * CIN_DG_THREADS + threadIdx.x;
   if (tok >= N * HW) return;
   const int n = tok / HW, p = tok - n * HW, y = p / W, x = p - y * W;
-  float gzq[4] = {};
-  for (int pl = lane; pl < C / 8; pl += 32) {
-    const __nv_bfloat16* plane = gy + ((long long)n * (C / 8) + pl) * g.PL * 8;
+  const __nv_bfloat16* img = gy + (long long)n * np * g.PL * 8;
+  // the partials in bit-reversed order j(k), so that each pairwise sum is made as soon as both halves exist: after leaf
+  // k, the subtrees of levels 0 .. (trailing ones of k) are complete; stk[l] holds the pending left half of level l
+  float stk[5], gs = 0.f;
 #pragma unroll
-    for (int t = 0; t < 9; ++t) {
-      const int yy = y - (t / 3 - 1), xx = x - (t % 3 - 1);
-      if (yy < 0 || yy >= H || xx < 0 || xx >= W) continue;
-      float gv[8];
-      const uint4 u = *reinterpret_cast<const uint4*>(plane + (long long)(g.lead + yy * g.Wp + xx) * 8);
-      const uint32_t uu[4] = {u.x, u.y, u.z, u.w};
+  for (int k = 0; k < 32; ++k) {
+    const int j = ((k & 1) << 4) | ((k & 2) << 2) | (k & 4) | ((k & 8) >> 2) | ((k & 16) >> 4);
+    float acc = 0.f;
+    for (int pl = j; pl < np; pl += 32) {
+      const __nv_bfloat16* plane = img + (long long)pl * g.PL * 8;
 #pragma unroll
-      for (int e = 0; e < 4; ++e) { const float2 f = unpack_bf16x2(uu[e]); gv[2 * e] = f.x; gv[2 * e + 1] = f.y; }
-      for (int l = 0; l < L; ++l)
+      for (int t = 0; t < 9; ++t) {
+        const int yy = y - (t / 3 - 1), xx = x - (t % 3 - 1);
+        if (yy < 0 || yy >= H || xx < 0 || xx >= W) continue;
+        const uint4 u = __ldg(reinterpret_cast<const uint4*>(plane + (long long)(g.lead + yy * g.Wp + xx) * 8));
+        const uint32_t uu[4] = {u.x, u.y, u.z, u.w};
+        const float4 w0 = sw4[(pl * 9 + t) * 2], w1 = sw4[(pl * 9 + t) * 2 + 1];
+        const float wv[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
 #pragma unroll
-        for (int e = 0; e < 8; ++e) gzq[l] = fmaf(__ldg(win + ((long long)(pl * 8 + e) * L + l) * 9 + t), gv[e], gzq[l]);
+        for (int e = 0; e < 4; ++e) {
+          const float2 f = unpack_bf16x2(uu[e]);
+          acc = fmaf(wv[2 * e], f.x, acc);
+          acc = fmaf(wv[2 * e + 1], f.y, acc);
+        }
+      }
     }
+    bool open = true;
+#pragma unroll
+    for (int l = 0; l < 5; ++l)
+      if (open) {
+        if (k & (1 << l)) acc = stk[l] + acc;
+        else { stk[l] = acc; open = false; }
+      }
+    if (open) gs = acc;   // k = 31: the whole tree
   }
-  for (int l = 0; l < L; ++l) gzq[l] = warp_sum_v(gzq[l]);
-  if (lane != 0) return;
-  for (int i = 0; i < L; ++i) {
-    float s = 0.f;
-    for (int o = 0; o < L; ++o) s = fmaf(wpq[o * L + i], gzq[o], s);
-    gz[((long long)n * L + i) * HW + p] = s;
+  const long long at = (long long)n * HW + p;
+  if (!wpq) {
+    gx[at] = gs;
+    return;
   }
-  for (int o = 0; o < L; ++o) {
-    atomicAdd(dbpq + o, gzq[o]);
-    for (int i = 0; i < L; ++i) atomicAdd(dwpq + o * L + i, gzq[o] * z[((long long)n * L + i) * HW + p]);
+  gx[at] = fmaf(wpq[0], gs, 0.f);
+  if (dwpq) {
+    atomicAdd(dbpq, gs);
+    atomicAdd(dwpq, gs * z[at]);
   }
 }
-cudaError_t launch_latent_in_bwd(const __nv_bfloat16* gy, const float* win, const float* wpq, const float* z, float* gz,
-                                 float* dwpq, float* dbpq, int N, int C, int L, int H, int W, cudaStream_t s) {
-  if (L > 4) return cudaErrorInvalidValue;
-  latent_in_bwd_kernel<<<(N * H * W + 7) / 8, 256, 0, s>>>(gy, win, wpq, z, gz, dwpq, dbpq, N, C, L, H, W);
+cudaError_t launch_conv_in_dgrad(const __nv_bfloat16* gy, const float* win, float* gx, int N, int C, int H, int W,
+                                 cudaStream_t s, const float* wpq, const float* z, float* dwpq, float* dbpq) {
+  if (C % 8 || C > 1024) return cudaErrorInvalidValue;
+  conv_in_dgrad_kernel<<<(N * H * W + CIN_DG_THREADS - 1) / CIN_DG_THREADS, CIN_DG_THREADS, (size_t)C * 9 * sizeof(float), s>>>(
+      gy, win, wpq, z, gx, dwpq, dbpq, N, C, H, W);
   return cudaGetLastError();
 }
 

@@ -4,6 +4,14 @@ table and its default initialisation, weight packing, the activation workspace, 
 backward arena with one flat gradient buffer handed out as `p.grad` views, the one-forward-per-backward guard, debug read-outs and the diffusers
 hub directory layout.  PyTorch owns every tensor: parameters are ordinary fp32 `nn.Parameter`s, the packed bf16 weights,
 the workspace and the backward arena are torch byte tensors.
+
+Gradients: parameter gradients are produced in train() mode with grad enabled and some parameter requiring grad, as
+diffusers models train.  A gradient w.r.t. the model's input (the U-Nets' sample, the autoencoder's image or latents) is
+produced whenever grad is enabled and that input requires grad, in train() or eval().  When only the input gradient is
+wanted (a frozen or eval() model: guidance, latent optimisation, saliency), the backward runs in data-gradient-only mode:
+no weight-gradient work, no flat gradient buffer, no `p.grad`, no all-reduce.  Moving between that mode and parameter
+training re-plans the workspace, as switching between training and inference does, so alternate them per phase rather
+than per step.
 """
 from __future__ import annotations
 
@@ -78,6 +86,7 @@ class EngineModel(nn.Module):
         self._ws = self._ws_key = None
         self._train_mode = False
         self._checkpointing = False
+        self._param_grads = True                 # the library's mode: the backward computes parameter gradients
         self._fwd_gen = [0] * len(self._parts)   # forwards per part: a backward must see its own forward's activations
         self._bwd_key = None
         self._grad_flat = self._bwd_arena = None
@@ -111,7 +120,13 @@ class EngineModel(nn.Module):
         return _lib.B200ADError(f"{type(self).__name__}(b200): {msg}")
 
     def _needs_grad(self) -> bool:
+        """Whether a call produces parameter gradients."""
         return torch.is_grad_enabled() and self.training and any(p.requires_grad for p in self.parameters())
+
+    @staticmethod
+    def _input_grad(x: torch.Tensor) -> bool:
+        """Whether a call produces the gradient w.r.t. its input x (in train() or eval())."""
+        return torch.is_grad_enabled() and x.requires_grad
 
     def _ensure_bound(self, n: int, hh: int, ww: int, seq: Optional[int] = None) -> None:
         """Packs the weights when a parameter's pointer or version changed, and binds the workspace for (n, hh, ww) and,
@@ -178,13 +193,23 @@ class EngineModel(nn.Module):
             self._ws_key = None        # the training workspace layout and the backward plan differ
             self._bwd_key = None
 
+    def _set_param_grads(self, on: bool) -> None:
+        """The backward's mode: parameter gradients too (training), or data gradients only (a frozen model's input
+        gradient).  A change re-plans the workspace and the backward, as _set_training_mode does."""
+        if self._param_grads != on:
+            _lib.check(self._fn("set_param_grads")(self._h, 1 if on else 0))
+            self._param_grads = on
+            self._ws_key = None
+            self._bwd_key = None
+
     def _bind_backward(self, dev: torch.device) -> None:
-        """The backward arena and the flat gradient buffer, (re)bound whenever the workspace was."""
+        """The backward arena and (parameter gradients on) the flat gradient buffer, (re)bound whenever the workspace was."""
         if self._bwd_key == self._ws_key:
             return
-        nfl = self._fn("grad_floats")(self._h)
-        if self._grad_flat is None or self._grad_flat.numel() != nfl or self._grad_flat.device != dev:
-            self._grad_flat = torch.zeros(nfl, dtype=torch.float32, device=dev)
+        if self._param_grads:
+            nfl = self._fn("grad_floats")(self._h)
+            if self._grad_flat is None or self._grad_flat.numel() != nfl or self._grad_flat.device != dev:
+                self._grad_flat = torch.zeros(nfl, dtype=torch.float32, device=dev)
         need = self._fn("backward_bytes")(self._h)
         if need == 0:
             _lib.check(-1)
@@ -192,13 +217,17 @@ class EngineModel(nn.Module):
             self._bwd_arena = None
             self._bwd_arena = torch.empty(need, dtype=torch.uint8, device=dev)
         _lib.check(self._fn("bind_backward")(self._h, self._bwd_arena.data_ptr(), self._bwd_arena.numel(),
-                                             self._grad_flat.data_ptr(), _lib.stream_ptr()))
+                                             self._grad_flat.data_ptr() if self._param_grads else None,
+                                             _lib.stream_ptr()))
         self._bwd_key = self._ws_key
 
-    def _bind(self, n: int, hh: int, ww: int, train: bool, dev: torch.device, seq: Optional[int] = None) -> None:
+    def _bind(self, n: int, hh: int, ww: int, train: bool, dev: torch.device, seq: Optional[int] = None,
+              param_grads: bool = True) -> None:
         """Everything a forward of (n, hh, ww) (and `seq` encoder tokens) needs bound: mode, weights, workspace and, when
-        training, the backward."""
+        training (a forward with a backward), the backward with or without parameter gradients."""
         self._set_training_mode(train)
+        if train:
+            self._set_param_grads(param_grads)
         self._ensure_bound(n, hh, ww, seq)
         if train:
             self._bind_backward(dev)

@@ -4,7 +4,9 @@
 Same constructor kwargs, same state-dict key layout (SURVEY §8b) and the same call convention
 `unet(sample, timestep)["sample"]`; the forward runs entirely in libb200ad.so (wgmma implicit-GEMM convs, fused GroupNorm
 statistics, fused scheduler step).  Training: with grad enabled and the module in train() mode, the forward is an autograd
-node whose backward runs in libb200ad.so too (unet_bwd.cu).  The engine plumbing is `EngineModel`'s (engine.py).
+node whose backward runs in libb200ad.so too (unet_bwd.cu).  A `sample` that requires grad gets its gradient in train()
+or eval() (guidance, saliency); a frozen or eval() model then runs a backward without parameter gradients, and moving
+between that and parameter training re-plans the workspace.  The engine plumbing is `EngineModel`'s (engine.py).
 """
 from __future__ import annotations
 
@@ -12,6 +14,7 @@ import ctypes as C
 from typing import Optional, Sequence, Tuple, Union
 
 import torch
+from torch.autograd.function import once_differentiable
 
 from . import _lib
 from ._lib import MAX_BLOCKS, StepCoefC, UNetConfigC
@@ -45,33 +48,43 @@ def _unet_config(in_channels: int, out_channels: int, layers_per_block: int, blo
 
 
 class _UNetFunction(torch.autograd.Function):
-    """Autograd node of the training forward: the backward pass is `b200ad_unet_backward` (all parameter gradients in one
-    call); the gradient w.r.t. the input sample is not produced (the reference never needs it).  `enc` is the conditional
-    model's encoding (None for UNet2DModel): the node keeps it alive and the backward binds it again, since the library
-    reads it for the cross-attention weight gradients; no gradient w.r.t. it is produced."""
+    """Autograd node of the forward with a backward: `b200ad_unet_backward_input`, which writes the gradient w.r.t. the
+    sample when x requires grad.  param_grads: all parameter gradients in the same call (the params are the node's
+    inputs); otherwise the data-gradient-only backward (no params, no flat buffer, no all-reduce).  `enc` is the
+    conditional model's encoding (None for UNet2DModel): the node keeps it alive and the backward binds it again, since
+    the library reads it for the cross-attention weight gradients; no gradient w.r.t. it is produced."""
 
     @staticmethod
-    def forward(ctx, model, x, t, enc, *params):
-        out = model._run(x, t, enc, train=True)
+    def forward(ctx, model, param_grads, x, t, enc, *params):
+        out = model._run(x, t, enc, train=True, param_grads=param_grads)
         ctx.model = model
+        ctx.param_grads = param_grads
+        ctx.nparams = len(params)
         ctx.gen = model._fwd_gen[0]     # the activations live in the model's single workspace: backward must see THIS forward
         ctx.save_for_backward(x, enc)
         return out
 
     @staticmethod
+    @once_differentiable
     def backward(ctx, g):
         x, enc = ctx.saved_tensors
         m = ctx.model
         m._check_gen(0, ctx.gen)
         g = g.to(torch.float32).contiguous()
+        gx = torch.empty_like(x) if ctx.needs_input_grad[2] else None
 
         def launch(accumulate):
             m._set_encoding(enc)      # another call may have bound a different encoding since the forward
-            _lib.check(m._fn("backward")(m._h, x.data_ptr(), g.data_ptr(), accumulate, _lib.stream_ptr()))
-            if not m._no_sync:
+            _lib.check(m._fn("backward_input")(m._h, x.data_ptr(), g.data_ptr(), gx.data_ptr() if gx is not None else None,
+                                               accumulate, _lib.stream_ptr()))
+            if ctx.param_grads and not m._no_sync:
                 m._allreduce_gradients()
-        m._backward_part(0, launch)     # fills p.grad (views of the flat gradient buffer)
-        return (None, None, None, None) + (None,) * len(m._pnames)
+        if ctx.param_grads:
+            m._backward_part(0, launch)     # fills p.grad (views of the flat gradient buffer)
+        else:
+            with torch.cuda.device(x.device):
+                launch(0)
+        return (None, None, gx, None, None) + (None,) * ctx.nparams
 
 
 class UNet2DModel(EngineModel):
@@ -180,29 +193,29 @@ class UNet2DModel(EngineModel):
 
     # ------------------------------------------------------------------ public call
     def forward(self, sample: torch.Tensor, timestep, return_dict: bool = True):
-        """ε = unet(sample, timestep)["sample"] — pipeline_audio_diffusion.py:163."""
-        if sample.requires_grad:
-            raise NotImplementedError(f"{type(self).__name__}(b200): gradients w.r.t. the input sample are not computed")
+        """ε = unet(sample, timestep)["sample"] — pipeline_audio_diffusion.py:163.  Differentiable w.r.t. the parameters
+        (train() mode) and w.r.t. a `sample` that requires grad (train() or eval())."""
         return self._forward(sample, timestep, None, return_dict)
 
     def _forward(self, sample: torch.Tensor, timestep, enc, return_dict: bool):
         x = self._check_input(sample)
-        if self._needs_grad():    # training step (scripts/train_unet.py:257-259): forward keeps every activation
-            n = x.shape[0]
+        param_grads = self._needs_grad()
+        if param_grads or self._input_grad(x):    # a training step (scripts/train_unet.py:257-259) and / or a sample
+            n = x.shape[0]                          # gradient: the forward keeps every activation
             t, e = self._timesteps(timestep, n, x.device), self._encoding(enc, n, x.device)
-            out = _UNetFunction.apply(self, x, t, e, *self._plist)
+            out = _UNetFunction.apply(self, param_grads, x, t, e, *(self._plist if param_grads else ()))
         else:
             out = self._run(x, timestep, enc, train=False)
         return UNet2DOutput(out) if return_dict else (out,)
 
-    def _run(self, x: torch.Tensor, timestep, enc, train: bool) -> torch.Tensor:
+    def _run(self, x: torch.Tensor, timestep, enc, train: bool, param_grads: bool = True) -> torch.Tensor:
         """One forward into a new output tensor; timestep and encoding are converted after binding (already converted
         ones, as the training node passes them, are left as they are)."""
         n, _, hh, ww = x.shape
         with torch.cuda.device(x.device):
             self._fwd_gen[0] += 1
             e = self._encoding(enc, n, x.device)
-            self._bind(n, hh, ww, train, x.device, self._seq(e))
+            self._bind(n, hh, ww, train, x.device, self._seq(e), param_grads)
             t = self._timesteps(timestep, n, x.device)
             out = torch.empty((n, self.out_channels, hh, ww), dtype=torch.float32, device=x.device)
             self._set_encoding(e)

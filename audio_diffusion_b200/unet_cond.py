@@ -13,10 +13,12 @@ per 5-second slice) runs the cross-attention kernels: the K / V projections of t
 pixels against the S tokens and, in training, its backward down to the to_q / to_k / to_v weight gradients.
 
 Training (`scripts/train_unet.py --encodings`: `model(noisy, t, enc)["sample"]`, MSE, `loss.backward()`) goes through the
-same autograd node as `UNet2DModel`: parameter gradients only, as `p.grad` views of one flat buffer.  Limits: encoder
-sequence length 1 <= S <= 256 (256 slices of 5 seconds: about 21 minutes of audio; a change of S re-plans the workspace);
-no gradient w.r.t. the encoding (the reference's encodings are precomputed data), so an encoding with `requires_grad` is
-refused in training.
+same autograd node as `UNet2DModel`: parameter gradients as `p.grad` views of one flat buffer, and the gradient w.r.t. a
+`sample` that requires grad (in train() or eval(); a frozen or eval() model runs the backward without parameter
+gradients, and moving between that and parameter training re-plans the workspace).  Limits: encoder sequence length
+1 <= S <= 256 (256 slices of 5 seconds: about 21 minutes of audio; a change of S re-plans the workspace); no gradient
+w.r.t. the encoding (the reference's encodings are precomputed data), so an encoding with `requires_grad` is refused
+whenever the call has a backward (parameter or sample gradients).
 """
 from __future__ import annotations
 
@@ -109,10 +111,9 @@ class UNet2DConditionModel(UNet2DModel):
 
     def forward(self, sample: torch.Tensor, timestep, encoder_hidden_states: torch.Tensor = None, return_dict: bool = True):
         """ε = unet(sample, timestep, encoding)["sample"] — pipeline_audio_diffusion.py:161 (inference) and
-        scripts/train_unet.py:255 (training: in train mode with grad enabled, backward() fills the parameter gradients)."""
-        if self._needs_grad():
-            if sample.requires_grad:
-                raise NotImplementedError("UNet2DConditionModel(b200): gradients w.r.t. the input sample are not computed")
+        scripts/train_unet.py:255 (training: in train mode with grad enabled, backward() fills the parameter gradients).
+        A `sample` that requires grad gets its gradient in train() or eval()."""
+        if self._needs_grad() or self._input_grad(sample):
             if torch.is_tensor(encoder_hidden_states) and encoder_hidden_states.requires_grad:
                 raise NotImplementedError("UNet2DConditionModel(b200): gradients w.r.t. encoder_hidden_states are not computed "
                                           "(pass precomputed encodings, e.g. .detach())")

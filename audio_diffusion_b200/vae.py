@@ -10,12 +10,16 @@ parameters (fp32 `nn.Parameter`s), the packed bf16 weights and the activation wo
 Training (scripts/train_vae.py): with grad enabled, the module in train() mode and a parameter requiring grad, `encode`
 and `decode` are autograd nodes whose backward passes run in libb200ad.so (unet_bwd.cu); the posterior is then a torch
 expression on the differentiable moments, so autograd carries the reparameterisation, the logvar clamp and `kl()`.
+An image (encode) or latents (decode) that require grad get their gradient in train() or eval(): a frozen or eval()
+autoencoder runs the backward without parameter gradients (a loss in pixel space behind a frozen decoder, latents
+optimised against a target), and moving between that and parameter training re-plans the workspace.
 """
 from __future__ import annotations
 
 from typing import Optional, Sequence, Tuple
 
 import torch
+from torch.autograd.function import once_differentiable
 
 from . import _lib
 from ._lib import MAX_BLOCKS, VAEConfigC
@@ -29,50 +33,69 @@ class DecoderOutput(dict):
         self.sample = sample
 
 
+def _run_part(vae, part: int, param_grads: bool, launch) -> None:
+    """A part's backward: with parameter gradients through _backward_part (p.grad views), otherwise launch(0) alone."""
+    if param_grads:
+        vae._backward_part(part, launch)
+    else:
+        with torch.cuda.device(vae._bwd_arena.device):
+            launch(0)
+
+
 class _VAEEncodeFunction(torch.autograd.Function):
-    """Autograd node of the training encoder: x -> moments; the backward pass is `b200ad_vae_encoder_backward` (the
-    encoder's and quant_conv's parameter gradients).  No gradient w.r.t. the image is produced."""
+    """Autograd node of the encoder with a backward: x -> moments; the backward pass is
+    `b200ad_vae_encoder_backward_input`: the encoder's and quant_conv's parameter gradients (param_grads; the params are
+    the node's inputs) and, when x requires grad, the gradient w.r.t. the image."""
 
     @staticmethod
-    def forward(ctx, vae, x, *params):
-        m = vae._encode_train(x)
+    def forward(ctx, vae, param_grads, x, *params):
+        m = vae._encode_train(x, param_grads)
         ctx.vae = vae
+        ctx.param_grads = param_grads
+        ctx.nparams = len(params)
         ctx.gen = vae._fwd_gen[0]
         ctx.save_for_backward(x)
         return m
 
     @staticmethod
+    @once_differentiable
     def backward(ctx, g):
         (x,) = ctx.saved_tensors
         vae = ctx.vae
         vae._check_gen(0, ctx.gen)
         g = g.to(torch.float32).contiguous()
-        vae._backward_part(0, lambda accumulate: _lib.check(vae._fn("encoder_backward")(
-            vae._h, x.data_ptr(), g.data_ptr(), accumulate, _lib.stream_ptr())))
-        return (None, None) + (None,) * len(vae._pnames)
+        gx = torch.empty_like(x) if ctx.needs_input_grad[2] else None
+        _run_part(vae, 0, ctx.param_grads, lambda accumulate: _lib.check(vae._fn("encoder_backward_input")(
+            vae._h, x.data_ptr(), g.data_ptr(), gx.data_ptr() if gx is not None else None, accumulate,
+            _lib.stream_ptr())))
+        return (None, None, gx) + (None,) * ctx.nparams
 
 
 class _VAEDecodeFunction(torch.autograd.Function):
-    """Autograd node of the training decoder: z -> image; the backward pass is `b200ad_vae_decoder_backward` (the
-    decoder's and post_quant_conv's parameter gradients, and the gradient w.r.t. z)."""
+    """Autograd node of the decoder with a backward: z -> image; the backward pass is `b200ad_vae_decoder_backward`:
+    the gradient w.r.t. z and (param_grads; the params are the node's inputs) the decoder's and post_quant_conv's
+    parameter gradients."""
 
     @staticmethod
-    def forward(ctx, vae, z, *params):
-        out = vae._decode_train(z)
+    def forward(ctx, vae, param_grads, z, *params):
+        out = vae._decode_train(z, param_grads)
         ctx.vae = vae
+        ctx.param_grads = param_grads
+        ctx.nparams = len(params)
         ctx.gen = vae._fwd_gen[1]
         ctx.zshape = z.shape
         return out
 
     @staticmethod
+    @once_differentiable
     def backward(ctx, g):
         vae = ctx.vae
         vae._check_gen(1, ctx.gen)
         g = g.to(torch.float32).contiguous()
         gz = torch.empty(ctx.zshape, dtype=torch.float32, device=g.device)
-        vae._backward_part(1, lambda accumulate: _lib.check(vae._fn("decoder_backward")(
+        _run_part(vae, 1, ctx.param_grads, lambda accumulate: _lib.check(vae._fn("decoder_backward")(
             vae._h, g.data_ptr(), gz.data_ptr(), accumulate, _lib.stream_ptr())))
-        return (None, gz) + (None,) * len(vae._pnames)
+        return (None, None, gz) + (None,) * ctx.nparams
 
 
 class _NoBackward(torch.autograd.Function):
@@ -98,17 +121,19 @@ class DiagonalGaussianDistribution:
     Training: the moments are the encoder node's differentiable output and every method is a torch expression on them.
     """
 
-    def __init__(self, vae: "AutoencoderKL", x: torch.Tensor, train: bool = False, refuse: Optional[str] = None):
+    def __init__(self, vae: "AutoencoderKL", x: torch.Tensor, train: bool = False, refuse: Optional[str] = None,
+                 param_grads: bool = True):
         self._vae = vae
         self._x = x
         self._train = train
+        self._param_grads = param_grads
         self._refuse = refuse
         self._moments: Optional[torch.Tensor] = None
 
     def _run(self, noise: Optional[torch.Tensor]) -> torch.Tensor:
         z, m = self._vae._encode(self._x, noise)
         if self._refuse:
-            z, m = self._vae._no_backward(self._refuse, z), self._vae._no_backward(self._refuse, m)
+            z, m = self._vae._no_backward(self._refuse, z, self._x), self._vae._no_backward(self._refuse, m, self._x)
         self._moments = m
         return z
 
@@ -116,7 +141,8 @@ class DiagonalGaussianDistribution:
     def parameters(self) -> torch.Tensor:
         if self._moments is None:
             if self._train:
-                self._moments = _VAEEncodeFunction.apply(self._vae, self._x, *self._vae._plist)
+                pg = self._param_grads
+                self._moments = _VAEEncodeFunction.apply(self._vae, pg, self._x, *(self._vae._plist if pg else ()))
             else:
                 self._run(None)
         return self._moments
@@ -266,28 +292,29 @@ class AutoencoderKL(EngineModel):
                     "activations; raise max_batch)")
         return None
 
-    def _no_backward(self, reason: str, t: torch.Tensor) -> torch.Tensor:
-        return _NoBackward.apply(reason, t, *self._plist)
+    def _no_backward(self, reason: str, t: torch.Tensor, inp: torch.Tensor) -> torch.Tensor:
+        """t, marked as having no backward: it requires grad when the call's input `inp` or a parameter does."""
+        return _NoBackward.apply(reason, t, inp, *self._plist)
 
-    def _encode_train(self, x: torch.Tensor) -> torch.Tensor:
+    def _encode_train(self, x: torch.Tensor, param_grads: bool) -> torch.Tensor:
         n, _, hh, ww = x.shape
         if hh % self._factor or ww % self._factor:
             raise ValueError(f"AutoencoderKL(b200): H and W must be multiples of {self._factor}")
         lshape = self.latent_shape(x.shape)
         with torch.cuda.device(x.device):
-            self._bind(n, hh, ww, True, x.device)
+            self._bind(n, hh, ww, True, x.device, param_grads=param_grads)
             self._fwd_gen[0] += 1
             z = torch.empty(lshape, dtype=torch.float32, device=x.device)
             m = torch.empty((n, 2 * lshape[1], lshape[2], lshape[3]), dtype=torch.float32, device=x.device)
             _lib.check(self._fn("encode")(self._h, x.data_ptr(), None, z.data_ptr(), m.data_ptr(), _lib.stream_ptr()))
         return m
 
-    def _decode_train(self, z: torch.Tensor) -> torch.Tensor:
+    def _decode_train(self, z: torch.Tensor, param_grads: bool) -> torch.Tensor:
         z = z.detach().to(torch.float32).contiguous()
         n, _, lh, lw = z.shape
         hh, ww = lh * self._factor, lw * self._factor
         with torch.cuda.device(z.device):
-            self._bind(n, hh, ww, True, z.device)
+            self._bind(n, hh, ww, True, z.device, param_grads=param_grads)
             self._fwd_gen[1] += 1
             out = torch.empty((n, self.config.out_channels, hh, ww), dtype=torch.float32, device=z.device)
             _lib.check(self._fn("decode")(self._h, z.data_ptr(), out.data_ptr(), _lib.stream_ptr()))
@@ -300,27 +327,31 @@ class AutoencoderKL(EngineModel):
 
     # ------------------------------------------------------------------ public calls
     def encode(self, x: torch.Tensor, return_dict: bool = True):
-        """`vqvae.encode(x).latent_dist` — the encoder runs when the distribution is sampled / inspected."""
+        """`vqvae.encode(x).latent_dist` — the encoder runs when the distribution is sampled / inspected.  Differentiable
+        w.r.t. the parameters (train() mode) and w.r.t. an image that requires grad (train() or eval())."""
         x = self._check(x, self.config.in_channels, "encode input")
-        grad = self._needs_grad()
+        param_grads = self._needs_grad()
+        grad = param_grads or self._input_grad(x)
         refuse = self._train_refusal(x.shape[0]) if grad else None
-        dist = DiagonalGaussianDistribution(self, x, train=grad and not refuse, refuse=refuse)
+        dist = DiagonalGaussianDistribution(self, x, train=grad and not refuse, refuse=refuse, param_grads=param_grads)
         if not return_dict:
             return (dist,)
         return AutoencoderKLOutput(dist)
 
     def decode(self, z: torch.Tensor, return_dict: bool = True):
-        """`vqvae.decode(z)["sample"]` (pipeline_audio_diffusion.py:190)."""
-        grad = self._needs_grad()
+        """`vqvae.decode(z)["sample"]` (pipeline_audio_diffusion.py:190).  Differentiable w.r.t. the parameters (train()
+        mode) and w.r.t. latents that require grad (train() or eval())."""
+        param_grads = self._needs_grad()
+        grad = param_grads or self._input_grad(z)
         refuse = self._train_refusal(z.shape[0]) if grad else None
         if grad and not refuse:
             self._check(z, self.config.latent_channels, "latents")
-            out = _VAEDecodeFunction.apply(self, z, *self._plist)
+            out = _VAEDecodeFunction.apply(self, param_grads, z, *(self._plist if param_grads else ()))
             return (out,) if not return_dict else DecoderOutput(out)
         with torch.no_grad():
             res = self._decode_infer(z, return_dict)
         if refuse:
-            out = self._no_backward(refuse, res[0] if not return_dict else res.sample)
+            out = self._no_backward(refuse, res[0] if not return_dict else res.sample, z)
             return (out,) if not return_dict else DecoderOutput(out)
         return res
 

@@ -147,8 +147,14 @@ int b200ad_unet_set_training(b200ad_unet* h, int on);
  * tap fails while a checkpointing plan is bound.  Changing the mode clears the plan, as set_training does: call
  * bind_workspace and bind_backward again. */
 int b200ad_unet_set_checkpointing(b200ad_unet* h, int on);
+/* Parameter gradients (default on: the backward fills the flat gradient buffer).  Off, the backward plan computes data
+ * gradients only (the gradient w.r.t. the input, for a frozen model): no weight, bias, GroupNorm / LayerNorm affine or
+ * timestep-MLP gradients, a smaller arena (backward_bytes, training_bytes), and bind_backward takes grads = NULL.  Changing
+ * the mode clears the plan, as set_checkpointing does: call bind_workspace and bind_backward again. */
+int b200ad_unet_set_param_grads(b200ad_unet* h, int on);
 /* Device bytes one training step of (N, H, W) with S encoder tokens (1 for an unconditional model) binds in the current
- * checkpointing mode: the training workspace plus the backward arena (parameters, packed weights and gradients excluded).
+ * checkpointing and parameter-gradient modes: the training workspace plus the backward arena (parameters, packed weights
+ * and gradients excluded).
  * Needs no device and leaves the bound plan alone.  0 on error. */
 size_t b200ad_unet_training_bytes(b200ad_unet* h, int N, int H, int W, int S);
 size_t b200ad_unet_grad_floats(b200ad_unet* h);
@@ -158,6 +164,10 @@ int b200ad_unet_bind_backward(b200ad_unet* h, void* arena, size_t bytes, float* 
 /* x: the forward input [N, 1, H, W]; g_eps: gradient of the loss w.r.t. the forward output, fp32 [N, 1, H, W].
  * accumulate = 0 zeroes the gradient buffer first; != 0 adds to it (gradient accumulation, `accelerator.accumulate`). */
 int b200ad_unet_backward(b200ad_unet* h, const float* x, const float* g_eps, int accumulate, void* stream);
+/* b200ad_unet_backward that also writes the gradient w.r.t. the input sample, fp32 [N, 1, H, W] (overwritten, never
+ * accumulated), into g_x; in either parameter-gradient mode.  g_x = NULL: exactly b200ad_unet_backward. */
+int b200ad_unet_backward_input(b200ad_unet* h, const float* x, const float* g_eps, float* g_x, int accumulate,
+                               void* stream);
 int b200ad_unet_backward_launch_count(const b200ad_unet* h);
 /* Debug / parity, after a backward: copy the gradient of the loss w.r.t. the forward tap `name` to fp32 NCHW (skip = 0),
  * or the share of it that a skip connection brought (skip = 1).  Returns the number of channels, or negative (unknown
@@ -203,10 +213,12 @@ int b200ad_vae_last_launch_count(const b200ad_vae* h);
  * blocks' softmax) -> bind_backward -> per step: encode(x) -> decode(z) -> decoder_backward -> encoder_backward.
  * Parameter i's gradient lives at float offset b200ad_vae_grad_offset(h, i) of one flat fp32 buffer.  Each backward
  * writes only the slots of its own part: the decoder and post_quant_conv, or the encoder and quant_conv.  Implemented for
- * in_channels = out_channels = latent_channels = 1; no gradient w.r.t. the input image is computed. */
+ * in_channels = out_channels = latent_channels = 1. */
 int b200ad_vae_set_training(b200ad_vae* h, int on);
 /* As b200ad_unet_set_checkpointing / b200ad_unet_training_bytes, over both parts (H, W: image resolution). */
 int b200ad_vae_set_checkpointing(b200ad_vae* h, int on);
+/* As b200ad_unet_set_param_grads, over both parts. */
+int b200ad_vae_set_param_grads(b200ad_vae* h, int on);
 size_t b200ad_vae_training_bytes(b200ad_vae* h, int N, int H, int W);
 size_t b200ad_vae_grad_floats(b200ad_vae* h);
 size_t b200ad_vae_grad_offset(b200ad_vae* h, int i);
@@ -217,6 +229,10 @@ int b200ad_vae_bind_backward(b200ad_vae* h, void* arena, size_t bytes, float* gr
 int b200ad_vae_decoder_backward(b200ad_vae* h, const float* g_x, float* g_z_out, int accumulate, void* stream);
 /* x: the encoded image [N, in, H, W]; g_moments: gradient w.r.t. the moments (quant_conv's output) [N, 2L, H/f, W/f]. */
 int b200ad_vae_encoder_backward(b200ad_vae* h, const float* x, const float* g_moments, int accumulate, void* stream);
+/* b200ad_vae_encoder_backward that also writes the gradient w.r.t. the image, fp32 [N, 1, H, W] (overwritten), into g_x.
+ * g_x = NULL: exactly b200ad_vae_encoder_backward. */
+int b200ad_vae_encoder_backward_input(b200ad_vae* h, const float* x, const float* g_moments, float* g_x, int accumulate,
+                                      void* stream);
 /* Kernel launches of the last decoder_backward plus those of the last encoder_backward. */
 int b200ad_vae_backward_launch_count(const b200ad_vae* h);
 /* As b200ad_unet_debug_grad, over the last decoder and encoder backward. */
