@@ -15,14 +15,15 @@ block: every resnet's reference also returns the gradient of the temb_act it rea
 
 `bf16_storage()` rounds, inside a reference, every conv / linear operand, weight and output to bf16 and every gradient
 that flows back through those operands and outputs: the points where the engine stores a tensor or a gradient in bf16.
-Comparing a reference run under it with the exact one gives the bf16 floor of a block's gradients.
+Comparing a reference run under it with the exact one gives the bf16 floor of a block's gradients: `backward_floors`,
+worst per block kind over a model's blocks.
 
 The forward: `block_forward` is the same `_forward` evaluated in fp64 without autograd; `sub_forward` splits a resnet, an
 attention block and a transformer into the steps whose outputs the engine keeps as taps (`.h1`; `.qkv`, `.ao`; `.h0` ..
 `.h3`), each step computed from the given values of the steps before it, so that a per-step comparison on the engine's
 own taps pins an error to one step.  tests/test_cpu_block_forward.py shows that both restate the model.  Their rounded
 forms add the bf16 points only the forward has (bf16_storage(forward=True), the stored outputs), which give the forward
-floors; the backward floors do not use them.
+floors (`forward_floors`); the backward floors do not use them.
 """
 from __future__ import annotations
 
@@ -499,3 +500,66 @@ def worst(rows, is_act: bool):
     """Largest (a), (b), (c) over the rows of one class (activation or parameter gradients)."""
     sel = [r[2:] for r in rows if r[1] == is_act]
     return tuple(max((s[i] for s in sel), default=0.0) for i in range(3))
+
+
+def backward_floors(blocks, taps, model_in, g_out, w, cfg, temb=None, enc=None, t=None):
+    """bf16 floor of every block (rounded storage against exact, over bf16 inputs and upstream gradients), worst per
+    kind: {kind: (activation (a, b, c), parameter (a, b, c))}.  With the timesteps t (U-Net), also "temb": the timestep
+    MLP's parameter gradients from the sum of the resnets' rounded-storage temb_act gradients against the exact sum."""
+    G, _, _ = chain(blocks, taps, model_in, g_out, w, cfg, temb, enc)
+    out = {}
+    gt_exact = gt_round = 0.0
+    for blk in blocks:
+        xs = [model_in if blk.inp is None else bf16(taps[blk.inp])] + ([bf16(taps[blk.skip])] if blk.skip else [])
+        gout = g_out if blk.out is None else bf16(G[blk.out])
+        ei, ep, et = block_backward(blk, w, xs, gout, cfg, temb, enc, temb_grad=True)
+        ri, rp, rt = block_backward(blk, w, xs, gout, cfg, temb, enc, True, temb_grad=True)
+        if et is not None:
+            gt_exact, gt_round = gt_exact + et, gt_round + rt
+        acts = {} if blk.inp is None else {"in": (ri[0], ei[0])}
+        if blk.skip:
+            acts["skip"] = (ri[1], ei[1])
+        rows, _ = compare_block(acts, {k: (rp[k], ep[k]) for k in ep})
+        wa, wp = worst(rows, True), worst(rows, False)
+        pa, pp = out.get(blk.kind, ((0.0,) * 3, (0.0,) * 3))
+        out[blk.kind] = (tuple(map(max, pa, wa)), tuple(map(max, pp, wp)))
+    if t is not None:
+        ep, rp = temb_backward(w, cfg, t, gt_exact), temb_backward(w, cfg, t, gt_round)
+        rows, _ = compare_block({}, {k: (rp[k], ep[k]) for k in ep})
+        out["temb"] = ((0.0,) * 3, worst(rows, False))
+    for k, (a, p) in out.items():
+        print(f"floor {k:12s} act L2 {a[0]:.4f} max {a[1]:.4f} row {a[2]:.4f} | param L2 {p[0]:.4f} max {p[1]:.4f} "
+              f"row {p[2]:.4f}")
+    return out
+
+
+def mean_offset(got, ref):
+    """Largest |mean over the pixels of the error| of one (sample, channel), over the RMS of the reference: what a wrong
+    per-sample time-embedding row or bias adds to a resnet's h1 is constant over the pixels, while rounding errors
+    average out there."""
+    err = (got.double() - ref.double()).mean(dim=(2, 3))
+    return (err.abs().max() / ref.double().pow(2).mean().sqrt()).item()
+
+
+def forward_floors(blocks, otaps, model_in, w, cfg, temb=None, enc=None, prefix="", taps=None):
+    """bf16 floor of every block and step, worst per key: {key: (a, b, c)}."""
+    fl = {}
+
+    def put(key, got, ref):
+        e = errors(got, ref, act=True)
+        fl[key] = tuple(map(max, fl.get(key, (0.0,) * 3), e))
+        if key.endswith(".h1"):
+            fl[key + ":mean"] = tuple(map(max, fl.get(key + ":mean", (0.0,) * 3), (mean_offset(got, ref),) * 3))
+
+    for blk in blocks:
+        xs = [model_in if blk.inp is None else bf16(otaps[blk.inp])] + ([bf16(otaps[blk.skip])] if blk.skip else [])
+        put(prefix + blk.kind, block_forward(blk, w, xs, cfg, temb, enc, rounded=True),
+            block_forward(blk, w, xs, cfg, temb, enc))
+        if blk.kind in EVAL_SUBTAPS:
+            exact = sub_forward(blk, w, xs, cfg, temb, enc, taps=taps)
+            get = lambda s: bf16(exact[s])
+            ex = sub_forward(blk, w, xs, cfg, temb, enc, get=get, taps=taps)
+            rd = sub_forward(blk, w, xs, cfg, temb, enc, get=get, taps=taps, rounded=True)
+            for s in ex:
+                put(prefix + blk.kind + (".out" if s == "out" else s), rd[s], ex[s])
+    return fl

@@ -21,6 +21,7 @@ from typing import Dict, Optional
 import torch
 
 from .schedulers_oracle import OracleDDPM
+from .unet_cond_oracle import CondUNetConfig, unet_cond_forward
 from .unet_oracle import UNetConfig, unet_forward
 
 
@@ -79,6 +80,18 @@ def loss_and_grads(w: Dict[str, torch.Tensor], cfg: UNetConfig, clean: torch.Ten
     loss = torch.mean((pred - noise) ** 2)
     grads = torch.autograd.grad(loss, list(wl.values()))
     return loss.detach(), dict(zip(wl.keys(), grads)), pred.detach()
+
+
+def cond_loss_and_grads(w: Dict[str, torch.Tensor], cfg: CondUNetConfig, clean: torch.Tensor, noise: torch.Tensor,
+                        t: torch.Tensor, enc: torch.Tensor):
+    """MSE(ε̂, ε) of one conditional training step (scripts/train_unet.py:250-258) and its parameter gradients, by
+    autograd over the conditional oracle forward."""
+    noisy = OracleDDPM().add_noise(clean, noise, t)
+    wl = {k: v.detach().clone().requires_grad_(True) for k, v in w.items()}
+    pred = unet_cond_forward(wl, cfg, noisy, t, enc)
+    loss = torch.mean((pred - noise) ** 2)
+    grads = torch.autograd.grad(loss, list(wl.values()))
+    return loss.detach(), dict(zip(wl.keys(), grads))
 
 
 def train_step(w: Dict[str, torch.Tensor], cfg: UNetConfig, state: TrainState, clean: torch.Tensor, noise: torch.Tensor,

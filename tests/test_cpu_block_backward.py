@@ -5,20 +5,18 @@
   the U-Net's timestep MLP included: the block lists, the skip bookkeeping and each block's decomposition are right
   before any GPU number is trusted.
 * Coverage: the blocks and the timestep MLP claim every parameter exactly once.
-* Floor: each block kind's gradients with bf16 storage (bf16_storage()) against exact, at the GPU test's shapes, over the
-  oracle's activations and upstream gradients rounded to bf16 as the engine stores them, and the timestep MLP's
-  gradients from the resnets' rounded temb_act gradients.  These are the floors the GPU bars are stated from.
+* Floor (block_grads.backward_floors): each block kind's gradients with bf16 storage (bf16_storage()) against exact, at
+  the GPU test's shapes, over the oracle's activations and upstream gradients rounded to bf16 as the engine stores
+  them, and the timestep MLP's gradients from the resnets' rounded temb_act gradients.  These are the floors the GPU
+  bars (tests/cases.py) are stated from.
 """
 import pytest
 import torch
 
+from blockcheck import bar_in_range
+from cases import (COND_BARS, LDM, PUBLISHED, PUBLISHED_ATTN, PUBLISHED_COND, T3, TWO_LEVEL, TWO_LEVEL_COND, UNET_BARS,
+                   VAE_BARS, draw, oracle_config)
 from oracle import block_grads as bg
-
-TRAIN_CFG = dict(in_channels=1, out_channels=1, layers_per_block=2, block_out_channels=(128, 256),
-                 down_block_types=("DownBlock2D", "AttnDownBlock2D"), up_block_types=("AttnUpBlock2D", "UpBlock2D"))
-COND_CFG = dict(block_out_channels=(128, 256), down_block_types=("CrossAttnDownBlock2D", "DownBlock2D"),
-                up_block_types=("UpBlock2D", "CrossAttnUpBlock2D"))
-T3 = torch.tensor([37, 412, 903])
 
 
 def _d(w):
@@ -37,15 +35,14 @@ def _check_params(grads, ref, expect):
     assert worst[0] < 1e-9      # fp64 rounding; a wrong decomposition or skip share is off by O(1)
 
 
-def _unet_case(size, n, seed, arch=TRAIN_CFG):
+def _unet_case(size, n, seed, arch=TWO_LEVEL):
     from oracle.schedulers_oracle import OracleDDPM
-    from oracle.unet_oracle import UNetConfig, init_weights, unet_forward
-    cfg = UNetConfig(sample_size=size, **arch)
+    from oracle.unet_oracle import init_weights, unet_forward
+    cfg = oracle_config(arch, size)
     w = _d(init_weights(cfg, seed=seed))
-    g = torch.Generator().manual_seed(seed + 1)
-    clean = (torch.rand(n, 1, *size, generator=g) * 2 - 1).double()
-    noise = torch.randn(n, 1, *size, generator=g).double()
-    t = T3[:n]
+    clean, noise, _ = draw(n, size, seed)
+    clean, noise = clean.double(), noise.double()
+    t = torch.tensor(T3[:n])
     noisy = OracleDDPM().add_noise(clean, noise, t)
     taps = {}
     pred = unet_forward(w, cfg, noisy, t, taps)
@@ -62,17 +59,14 @@ def test_unet_block_chain_reproduces_autograd():
     _check_params(grads, ref, list(w))
 
 
-def _cond_chain(cfg_kw, size, n, transformers):
+def _cond_chain(arch, size, n, transformers):
     """The conditional U-Net's block references chained over the oracle's activations against whole-model autograd."""
     from oracle.schedulers_oracle import OracleDDPM
-    from oracle.unet_cond_oracle import CondUNetConfig, init_weights, unet_cond_forward
-    cfg = CondUNetConfig(sample_size=size, **cfg_kw)
+    from oracle.unet_cond_oracle import init_weights, unet_cond_forward
+    cfg = oracle_config(arch, size)
     w = _d(init_weights(cfg, seed=3))
-    g = torch.Generator().manual_seed(4)
-    clean = (torch.rand(n, 1, *size, generator=g) * 2 - 1).double()
-    noise = torch.randn(n, 1, *size, generator=g).double()
-    enc = torch.randn(n, 1, 100, generator=g).double()
-    t = T3[:n]
+    clean, noise, enc = (v.double() for v in draw(n, size, 3, 1))
+    t = torch.tensor(T3[:n])
     noisy = OracleDDPM().add_noise(clean, noise, t)
     wl = {k: v.clone().requires_grad_(True) for k, v in w.items()}
     pred = unet_cond_forward(wl, cfg, noisy, t, enc)
@@ -90,7 +84,7 @@ def _cond_chain(cfg_kw, size, n, transformers):
 
 
 def test_cond_unet_block_chain_reproduces_autograd():
-    _cond_chain(COND_CFG, (16, 16), 3, 6)
+    _cond_chain(TWO_LEVEL_COND, (16, 16), 3, 6)
 
 
 @pytest.mark.timeout(300)
@@ -98,13 +92,10 @@ def test_published_unet_block_chain_reproduces_autograd():
     """The six-level UNet2DModel the GPU tests train at 64x64 and 256x256: attention at down block 4 and up block 1, skip
     connections across six levels, at 64x64 so that the last level is 2x2."""
     from oracle.train_oracle import loss_and_grads
-    from test_gpu_fullconfig import REF_ARCH
-    cfg, w, clean, noise, t, noisy, taps, g_eps = _unet_case((64, 64), 2, 2, REF_ARCH)
+    cfg, w, clean, noise, t, noisy, taps, g_eps = _unet_case((64, 64), 2, 2, PUBLISHED)
     _, ref, _ = loss_and_grads(w, cfg, clean, noise, t)
     blocks = bg.unet_blocks(cfg)
-    assert [b.name for b in blocks if b.kind == "attn"] == (
-        ["down_blocks.4.attentions.0", "down_blocks.4.attentions.1", "mid_block.attentions.0"]
-        + [f"up_blocks.1.attentions.{j}" for j in range(3)])
+    assert [b.name for b in blocks if b.kind == "attn"] == PUBLISHED_ATTN
     assert sum(b.skip is not None for b in blocks) == 6 * 3
     _, grads, _ = bg.chain(blocks, taps, noisy, g_eps, w, cfg, taps["temb_act"], t=t)
     _check_params(grads, ref, list(w))
@@ -114,8 +105,7 @@ def test_published_unet_block_chain_reproduces_autograd():
 def test_published_cond_unet_block_chain_reproduces_autograd():
     """The four-level UNet2DConditionModel the GPU tests train at 64x64 (transformers in three down and three up blocks
     and the mid block), at 32x32."""
-    from test_gpu_cond_train import ARCH
-    _cond_chain({k: ARCH[k] for k in ("block_out_channels", "down_block_types", "up_block_types")}, (32, 32), 2, 16)
+    _cond_chain(PUBLISHED_COND, (32, 32), 2, 16)
 
 
 def test_vae_block_chain_reproduces_autograd():
@@ -156,56 +146,18 @@ def test_every_parameter_claimed_once(model):
     from oracle import unet_cond_oracle as uco
     from oracle import unet_oracle as uo
     from oracle import vae_oracle as vo
-    from test_gpu_cond_train import ARCH
-    from test_gpu_fullconfig import REF_ARCH
     if model == "vae":
-        cfg = vo.VAEConfig()
+        cfg = oracle_config(LDM)
         names = list(vo.init_weights(cfg, seed=0))
         claims = _claims(names, bg.vae_blocks(cfg, "encoder") + bg.vae_blocks(cfg, "decoder"))
     else:
-        if model.startswith("cond"):
-            arch = COND_CFG if model == "cond_small" else ARCH
-            cfg = uco.CondUNetConfig(sample_size=(32, 32), **{k: arch[k] for k in ("block_out_channels",
-                                                                                    "down_block_types", "up_block_types")})
-            names = list(uco.init_weights(cfg, seed=0))
-        else:
-            cfg = uo.UNetConfig(sample_size=(32, 32), **(REF_ARCH if model == "published" else TRAIN_CFG))
-            names = list(uo.init_weights(cfg, seed=0))
+        arch = {"published": PUBLISHED, "train": TWO_LEVEL, "cond_small": TWO_LEVEL_COND, "cond_published": PUBLISHED_COND}
+        cfg = oracle_config(arch[model], (32, 32))
+        names = list((uco if model.startswith("cond") else uo).init_weights(cfg, seed=0))
         claims = _claims(names, bg.unet_blocks(cfg), bg.TEMB_PREFIXES)
         assert len([k for k, o in claims.items() if o == ["temb"]]) == 4
     bad = {k: o for k, o in claims.items() if len(o) != 1}
     assert names and not bad, bad
-
-
-def _floors(blocks, taps, model_in, g_out, w, cfg, temb=None, enc=None, t=None):
-    """bf16 floor of every block (rounded storage against exact, over bf16 inputs and upstream gradients), worst per
-    kind: {kind: (activation (a, b, c), parameter (a, b, c))}.  With the timesteps t (U-Net), also "temb": the timestep
-    MLP's parameter gradients from the sum of the resnets' rounded-storage temb_act gradients against the exact sum."""
-    G, _, _ = bg.chain(blocks, taps, model_in, g_out, w, cfg, temb, enc)
-    out = {}
-    gt_exact = gt_round = 0.0
-    for blk in blocks:
-        xs = [model_in if blk.inp is None else bg.bf16(taps[blk.inp])] + ([bg.bf16(taps[blk.skip])] if blk.skip else [])
-        gout = g_out if blk.out is None else bg.bf16(G[blk.out])
-        ei, ep, et = bg.block_backward(blk, w, xs, gout, cfg, temb, enc, temb_grad=True)
-        ri, rp, rt = bg.block_backward(blk, w, xs, gout, cfg, temb, enc, True, temb_grad=True)
-        if et is not None:
-            gt_exact, gt_round = gt_exact + et, gt_round + rt
-        acts = {} if blk.inp is None else {"in": (ri[0], ei[0])}
-        if blk.skip:
-            acts["skip"] = (ri[1], ei[1])
-        rows, _ = bg.compare_block(acts, {k: (rp[k], ep[k]) for k in ep})
-        wa, wp = bg.worst(rows, True), bg.worst(rows, False)
-        pa, pp = out.get(blk.kind, ((0.0,) * 3, (0.0,) * 3))
-        out[blk.kind] = (tuple(map(max, pa, wa)), tuple(map(max, pp, wp)))
-    if t is not None:
-        ep, rp = bg.temb_backward(w, cfg, t, gt_exact), bg.temb_backward(w, cfg, t, gt_round)
-        rows, _ = bg.compare_block({}, {k: (rp[k], ep[k]) for k in ep})
-        out["temb"] = ((0.0,) * 3, bg.worst(rows, False))
-    for k, (a, p) in out.items():
-        print(f"floor {k:12s} act L2 {a[0]:.4f} max {a[1]:.4f} row {a[2]:.4f} | param L2 {p[0]:.4f} max {p[1]:.4f} "
-              f"row {p[2]:.4f}")
-    return out
 
 
 def _assert_floors(fl, bars):
@@ -215,39 +167,34 @@ def _assert_floors(fl, bars):
     rounding reaches (downsample / upsample weights, the scalar-kernel heads and tails)."""
     for kind, (a, p) in fl.items():
         for f, b in zip(a + p, bars[kind][0] + bars[kind][1]):
-            assert f < b <= max(3 * round(f, 4), 5e-3) + 1e-9, (kind, a, p, bars[kind])   # floors as printed
+            assert bar_in_range(f, b, 3, 4, 5e-3), (kind, a, p, bars[kind])   # floors as printed
 
 
 @pytest.mark.timeout(600)
 def test_unet_block_floors():
-    from test_gpu_block_backward import UNET_BARS
     cfg, w, clean, noise, t, noisy, taps, g_eps = _unet_case((32, 32), 3, 2)
-    _assert_floors(_floors(bg.unet_blocks(cfg), taps, noisy, g_eps, w, cfg, taps["temb_act"], t=t), UNET_BARS)
+    _assert_floors(bg.backward_floors(bg.unet_blocks(cfg), taps, noisy, g_eps, w, cfg, taps["temb_act"], t=t), UNET_BARS)
 
 
 @pytest.mark.timeout(600)
 def test_cond_unet_block_floors():
     from oracle.schedulers_oracle import OracleDDPM
-    from oracle.unet_cond_oracle import CondUNetConfig, init_weights, unet_cond_forward
-    from test_gpu_block_backward import COND_BARS
-    cfg = CondUNetConfig(sample_size=(32, 32), **COND_CFG)
+    from oracle.unet_cond_oracle import init_weights, unet_cond_forward
+    cfg = oracle_config(TWO_LEVEL_COND, (32, 32))
     w = _d(init_weights(cfg, seed=3))
-    g = torch.Generator().manual_seed(4)
-    clean = (torch.rand(3, 1, 32, 32, generator=g) * 2 - 1).double()
-    noise = torch.randn(3, 1, 32, 32, generator=g).double()
-    enc = torch.randn(3, 1, 100, generator=g).double()
-    noisy = OracleDDPM().add_noise(clean, noise, T3)
+    clean, noise, enc = (v.double() for v in draw(3, (32, 32), 3, 1))
+    t = torch.tensor(T3)
+    noisy = OracleDDPM().add_noise(clean, noise, t)
     taps = {}
-    pred = unet_cond_forward(w, cfg, noisy, T3, enc, taps)
+    pred = unet_cond_forward(w, cfg, noisy, t, enc, taps)
     blocks = bg.unet_blocks(cfg)
-    _assert_floors(_floors(blocks, taps, noisy, 2 * (pred - noise) / pred.numel(), w, cfg, bg.temb_act(w, cfg, T3), enc,
-                           T3), COND_BARS)
+    _assert_floors(bg.backward_floors(blocks, taps, noisy, 2 * (pred - noise) / pred.numel(), w, cfg,
+                                      bg.temb_act(w, cfg, t), enc, t), COND_BARS)
 
 
 @pytest.mark.timeout(900)
 def test_vae_block_floors():
     from oracle import vae_oracle as vo
-    from test_gpu_block_backward import VAE_BARS
     cfg = vo.VAEConfig()
     w = _d(vo.init_weights(cfg, seed=0))
     g = torch.Generator().manual_seed(1)
@@ -259,6 +206,6 @@ def test_vae_block_floors():
     for part, inp, gout, fwd in (("decoder", z, gx, vo.decode), ("encoder", x, gm, vo.encode_moments)):
         taps = {}
         fwd(w, cfg, inp, taps)
-        for k, v in _floors(bg.vae_blocks(cfg, part), taps, inp, gout, w, cfg).items():
+        for k, v in bg.backward_floors(bg.vae_blocks(cfg, part), taps, inp, gout, w, cfg).items():
             fl[part + ":" + k] = v
     _assert_floors(fl, VAE_BARS)

@@ -12,9 +12,8 @@ tests/test_gpu_block_forward.py.
 import pytest
 import torch
 
+from cases import PUBLISHED, PUBLISHED_COND, T3, oracle_config
 from oracle import block_grads as bg
-
-T3 = torch.tensor([37, 412, 903])
 
 
 def _d(w):
@@ -52,15 +51,15 @@ def _chain(blocks, model_in, w, cfg, taps, model_out, temb=None, enc=None):
 def test_published_unet_block_forward_chain():
     """The six-level UNet2DModel at 64x64 (the last level 2x2), per-sample timesteps."""
     from oracle.schedulers_oracle import OracleDDPM
-    from oracle.unet_oracle import UNetConfig, init_weights, unet_forward
-    from test_gpu_fullconfig import REF_ARCH
-    cfg = UNetConfig(sample_size=(64, 64), **REF_ARCH)
+    from oracle.unet_oracle import init_weights, unet_forward
+    cfg = oracle_config(PUBLISHED, (64, 64))
     w = _d(init_weights(cfg, seed=2))
     g = torch.Generator().manual_seed(3)
+    t = torch.tensor(T3[:2])
     x = OracleDDPM().add_noise((torch.rand(2, 1, 64, 64, generator=g) * 2 - 1).double(),
-                               torch.randn(2, 1, 64, 64, generator=g).double(), T3[:2])
+                               torch.randn(2, 1, 64, 64, generator=g).double(), t)
     taps = {}
-    eps = unet_forward(w, cfg, x, T3[:2], taps)
+    eps = unet_forward(w, cfg, x, t, taps)
     blocks = bg.unet_blocks(cfg)
     assert sum(blk.kind == "attn" for blk in blocks) == 6
     _chain(blocks, x, w, cfg, taps, eps, taps["temb_act"])
@@ -69,19 +68,18 @@ def test_published_unet_block_forward_chain():
 @pytest.mark.timeout(300)
 def test_published_cond_unet_block_forward_chain():
     """The four-level UNet2DConditionModel at 32x32: sixteen transformers, distinct encodings."""
-    from oracle.unet_cond_oracle import CondUNetConfig, init_weights, unet_cond_forward
-    from test_gpu_cond_train import ARCH
-    cfg = CondUNetConfig(sample_size=(32, 32), **{k: ARCH[k] for k in ("block_out_channels", "down_block_types",
-                                                                         "up_block_types")})
+    from oracle.unet_cond_oracle import init_weights, unet_cond_forward
+    cfg = oracle_config(PUBLISHED_COND, (32, 32))
     w = _d(init_weights(cfg, seed=3))
     g = torch.Generator().manual_seed(4)
     x = torch.randn(2, 1, 32, 32, generator=g).double()
     enc = torch.randn(2, 1, 100, generator=g).double()
+    t = torch.tensor(T3[:2])
     taps = {}
-    eps = unet_cond_forward(w, cfg, x, T3[:2], enc, taps)
+    eps = unet_cond_forward(w, cfg, x, t, enc, taps)
     blocks = bg.unet_blocks(cfg)
     assert sum(blk.kind == "transformer" for blk in blocks) == 16
-    _chain(blocks, x, w, cfg, taps, eps, bg.temb_act(w, cfg, T3[:2]), enc)
+    _chain(blocks, x, w, cfg, taps, eps, bg.temb_act(w, cfg, t), enc)
 
 
 @pytest.mark.timeout(300)
@@ -103,14 +101,13 @@ def test_forward_rounding_model():
     """The probabilities are rounded where the engine packs them to bf16 (attention_mma_kernel: seq % 16 == 0 and
     seq <= 1536; mha_flash_kernel: always) and nowhere else (attention_kernel, the single-head attention).  A rounded
     reference differs from the exact one by a bf16 floor: more than 1e-4, less than 2 % relative L2."""
-    from oracle.unet_oracle import UNetConfig, init_weights
-    from test_gpu_fullconfig import REF_ARCH
+    from oracle.unet_oracle import init_weights
     blk = bg.Block("attn", "mid_block.attentions.0", "x", None, "y", ("mid_block.attentions.0.",))
     for hw, rounds in (((6, 10), False), ((4, 4), True), ((16, 16), True), ((40, 40), False)):
         assert bg._probs_rounded(blk, torch.zeros(1, 8, *hw)) == rounds, hw
     assert bg._probs_rounded(bg.Block("transformer", "t", "x", None, "y", ()), torch.zeros(1, 8, 6, 10))
     assert not bg._probs_rounded(bg.Block("attn1", "a", "x", None, "y", ()), torch.zeros(1, 8, 32, 32))
-    cfg = UNetConfig(sample_size=(64, 64), **REF_ARCH)
+    cfg = oracle_config(PUBLISHED, (64, 64))
     w = _d(init_weights(cfg, seed=2))
     g = torch.Generator().manual_seed(7)
     for hw in ((4, 4), (6, 10)):

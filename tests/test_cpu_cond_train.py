@@ -3,21 +3,11 @@ the cross-attention's softmax is constant, so attn2.to_q, attn2.to_k and norm2 g
 and attn2.to_out (the per-sample vector Wo (Wv enc) + bo) get real ones.  The engine launches nothing for the former."""
 import torch
 
-from oracle.schedulers_oracle import OracleDDPM
-from oracle.unet_cond_oracle import CondUNetConfig, init_weights, unet_cond_forward
+from oracle.train_oracle import cond_loss_and_grads
+from oracle.unet_cond_oracle import CondUNetConfig, init_weights
 
 SMALL = dict(sample_size=(8, 8), block_out_channels=(32, 64), down_block_types=("CrossAttnDownBlock2D", "DownBlock2D"),
              up_block_types=("UpBlock2D", "CrossAttnUpBlock2D"))
-
-
-def cond_loss_and_grads(w, cfg, clean, noise, t, enc):
-    """MSE(ε̂, ε) of one conditional training step (scripts/train_unet.py:250-258) and its parameter gradients."""
-    noisy = OracleDDPM().add_noise(clean, noise, t)
-    wl = {k: v.detach().clone().requires_grad_(True) for k, v in w.items()}
-    pred = unet_cond_forward(wl, cfg, noisy, t, enc)
-    loss = torch.mean((pred - noise) ** 2)
-    grads = torch.autograd.grad(loss, list(wl.values()))
-    return loss.detach(), dict(zip(wl.keys(), grads))
 
 
 def test_cond_cross_attention_gradients():

@@ -10,15 +10,8 @@
 import pytest
 import torch
 
+from cases import PLAIN_BYTES, T3, TWO_LEVEL, TWO_LEVEL_COND, draw, model_256, oracle_config, training_bytes
 from oracle import block_grads as bg
-
-from test_cpu_checkpointing import PLAIN_BYTES, _model, _training_bytes
-
-TRAIN_CFG = dict(in_channels=1, out_channels=1, layers_per_block=2, block_out_channels=(128, 256),
-                 down_block_types=("DownBlock2D", "AttnDownBlock2D"), up_block_types=("AttnUpBlock2D", "UpBlock2D"))
-COND_CFG = dict(block_out_channels=(128, 256), down_block_types=("CrossAttnDownBlock2D", "DownBlock2D"),
-                up_block_types=("UpBlock2D", "CrossAttnUpBlock2D"))
-T3 = torch.tensor([37, 412, 903])
 
 
 def test_symbols_exported():
@@ -32,16 +25,16 @@ def test_symbols_exported():
 @pytest.mark.parametrize("which", ["published", "ldm"])
 def test_training_bytes_data_only_smaller(which):
     from audio_diffusion_b200 import _lib
-    m = _model(which)
+    m = model_256(which)
     set_pg = getattr(_lib.lib(), f"b200ad_{'vae' if which == 'ldm' else 'unet'}_set_param_grads")
-    full = _training_bytes(m, which)
+    full = training_bytes(m, which)
     assert full == PLAIN_BYTES[which]
     assert set_pg(m._h, 0) == 0
-    data = _training_bytes(m, which)
+    data = training_bytes(m, which)
     print(f"{which}: {full / 2**30:.2f} GiB -> {data / 2**30:.2f} GiB without parameter gradients")
     assert 0 < data < full
     assert set_pg(m._h, 1) == 0
-    assert _training_bytes(m, which) == full
+    assert training_bytes(m, which) == full
 
 
 def _floor(f, x, g_out):
@@ -57,36 +50,34 @@ def _floor(f, x, g_out):
 
 
 def test_unet_sample_grad_floor():
-    """UNet2DModel TRAIN_CFG, 32x32, batch 3, T3: the MSE loss of tests/test_gpu_input_grad.py."""
+    """UNet2DModel TWO_LEVEL, 32x32, batch 3, T3: the MSE loss of tests/test_gpu_input_grad.py."""
     from oracle.schedulers_oracle import OracleDDPM
-    from oracle.unet_oracle import UNetConfig, init_weights, unet_forward
-    cfg = UNetConfig(sample_size=(32, 32), **TRAIN_CFG)
+    from oracle.unet_oracle import init_weights, unet_forward
+    cfg = oracle_config(TWO_LEVEL, (32, 32))
     w = {k: v.double() for k, v in init_weights(cfg, seed=2).items()}
-    g = torch.Generator().manual_seed(3)
-    clean = torch.rand(3, 1, 32, 32, generator=g) * 2 - 1
-    noise = torch.randn(3, 1, 32, 32, generator=g)
-    noisy = OracleDDPM().add_noise(clean, noise, T3).double()
-    pred = unet_forward(w, cfg, noisy, T3)
+    clean, noise, _ = draw(3, (32, 32), 2)
+    t = torch.tensor(T3)
+    noisy = OracleDDPM().add_noise(clean, noise, t).double()
+    pred = unet_forward(w, cfg, noisy, t)
     g_eps = 2 * (pred - noise.double()) / pred.numel()
-    a, b, c = _floor(lambda x: unet_forward(w, cfg, x, T3), noisy, g_eps)
+    a, b, c = _floor(lambda x: unet_forward(w, cfg, x, t), noisy, g_eps)
     assert max(a, b, c) < 0.05
 
 
 @pytest.mark.parametrize("seq", [1, 8])
 def test_cond_unet_sample_grad_floor(seq):
-    """UNet2DConditionModel COND_CFG, 32x32, batch 3, T3, an encoding of `seq` tokens."""
+    """UNet2DConditionModel TWO_LEVEL_COND, 32x32, batch 3, T3, an encoding of `seq` tokens."""
     from oracle.schedulers_oracle import OracleDDPM
-    from oracle.unet_cond_oracle import CondUNetConfig, init_weights, unet_cond_forward
-    cfg = CondUNetConfig(sample_size=(32, 32), **COND_CFG)
+    from oracle.unet_cond_oracle import init_weights, unet_cond_forward
+    cfg = oracle_config(TWO_LEVEL_COND, (32, 32))
     w = {k: v.double() for k, v in init_weights(cfg, seed=3).items()}
-    g = torch.Generator().manual_seed(4)
-    clean = torch.rand(3, 1, 32, 32, generator=g) * 2 - 1
-    noise = torch.randn(3, 1, 32, 32, generator=g)
-    enc = torch.randn(3, seq, 100, generator=g).double()
-    noisy = OracleDDPM().add_noise(clean, noise, T3).double()
-    pred = unet_cond_forward(w, cfg, noisy, T3, enc)
+    clean, noise, enc = draw(3, (32, 32), 3, seq)
+    enc = enc.double()
+    t = torch.tensor(T3)
+    noisy = OracleDDPM().add_noise(clean, noise, t).double()
+    pred = unet_cond_forward(w, cfg, noisy, t, enc)
     g_eps = 2 * (pred - noise.double()) / pred.numel()
-    a, b, c = _floor(lambda x: unet_cond_forward(w, cfg, x, T3, enc), noisy, g_eps)
+    a, b, c = _floor(lambda x: unet_cond_forward(w, cfg, x, t, enc), noisy, g_eps)
     assert max(a, b, c) < 0.05
 
 

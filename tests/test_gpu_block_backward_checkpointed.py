@@ -16,8 +16,9 @@ limit measured.
 """
 import pytest
 
-from test_gpu_block_backward_trained import UNET64_BARS, UNET64_FWD_BARS, _cond_64_case, _unet_case, _vae_256_case
-from test_gpu_cond_seq import cond_seq_backward_case
+from blockcheck import unet_backward_case, vae_backward_case
+from cases import (COND64_BARS, COND_BARS, COND_SEQ_BWD_TRANSFORMER_BARS, PUBLISHED, PUBLISHED_ATTN, PUBLISHED_COND, T3, T5,
+                   TWO_LEVEL_COND, UNET64_BARS, VAE256_BARS)
 
 pytestmark = pytest.mark.gpu
 
@@ -26,7 +27,8 @@ pytestmark = pytest.mark.gpu
 def test_unet_64_packed_backward_per_block_checkpointed(cuda):
     """The published UNet2DModel at 64x64, batch 5 (packed 8x8 / 4x4 / 2x2 levels, a one-image last item), checkpointed:
     the bars of test_unet_64_packed_backward_per_block.  fp64 work: 0.5 s, 3.4 GiB peak."""
-    _unet_case(cuda, (64, 64), 5, 9, UNET64_BARS, UNET64_FWD_BARS, checkpointing=True)
+    _, blocks = unet_backward_case(cuda, PUBLISHED, (64, 64), 5, 9, T5, UNET64_BARS, checkpointing=True)
+    assert [b.name for b in blocks if b.kind == "attn"] == PUBLISHED_ATTN
 
 
 @pytest.mark.timeout(600)
@@ -34,7 +36,8 @@ def test_cond_unet_64_backward_per_block_checkpointed(cuda):
     """The published UNet2DConditionModel at 64x64, batch 2, one-token encodings, checkpointed: the transformers' recompute
     of their flash-attention log-sum-exp at seq 4096 / 1024 / 256 / 64.  The bars of test_cond_unet_64_backward_per_block.
     fp64 work: 0.7 s, 11.4 GiB peak."""
-    _cond_64_case(cuda, checkpointing=True)
+    _, blocks = unet_backward_case(cuda, PUBLISHED_COND, (64, 64), 2, 6, [211, 650], COND64_BARS, s=1, checkpointing=True)
+    assert sum(b.kind == "transformer" for b in blocks) == 16
 
 
 @pytest.mark.timeout(600)
@@ -42,7 +45,8 @@ def test_cond_seq_77_backward_per_block_checkpointed(cuda):
     """The two-level UNet2DConditionModel at 32x32, batch 3, with a 77-token encoding, checkpointed: the recompute of the
     cross-attention's K / V projections and log-sum-exp as well.  The bars of test_cond_seq_backward_per_block[77].
     fp64 work: 0.3 s, 1.5 GiB peak."""
-    cond_seq_backward_case(cuda, 77, checkpointing=True)
+    bars = dict(COND_BARS, transformer=COND_SEQ_BWD_TRANSFORMER_BARS[77])
+    unet_backward_case(cuda, TWO_LEVEL_COND, (32, 32), 3, 3, T3, bars, s=77, checkpointing=True, one_token_grads=True)
 
 
 @pytest.mark.timeout(600)
@@ -50,4 +54,4 @@ def test_vae_256_backward_per_block_checkpointed(cuda):
     """The ldm autoencoder at 256x256, batch 2, checkpointed: the single-head attention's probabilities over 1024 tokens
     and the asymmetric downsampler's parity planes recomputed.  The bars of test_vae_256_backward_per_block.
     fp64 work: 0.8 s, 5.7 GiB peak."""
-    _vae_256_case(cuda, checkpointing=True)
+    vae_backward_case(cuda, (256, 256), 4, VAE256_BARS, checkpointing=True)

@@ -9,13 +9,14 @@ packed 8x8 / 4x4 / 2x2 levels with a partly filled last item (batch 5), per-samp
 autoencoder's single-head attention backward over S = 1024 tokens (16x16 tiles, 32 k-steps), the conditional model's
 multi-head flash attention backward at seq 4096 (head_dim 16) and at the 16x16 / 8x8 levels (head_dim 64), and a
 non-square image (96x160: odd 3x5 / 6x10 levels, the SIMT attention backward over 60 tokens).  Every U-Net case also
-checks the timestep MLP's gradients (the "temb" row, tests/test_gpu_block_backward.py).  The helpers run the same cases
-with gradient checkpointing for tests/test_gpu_block_backward_checkpointed.py.
+checks the timestep MLP's gradients (the "temb" row, tests/test_gpu_block_backward.py).  The same cases run with
+gradient checkpointing in tests/test_gpu_block_backward_checkpointed.py, at the bars tests/cases.py keeps for both.
 
 Bars.  The fp64 oracle of the whole model at these shapes is too slow for the CPU, so each block's bf16 floor is measured
-here, in the same run, as tests/test_cpu_block_backward.py measures it at small shapes (`_floors`): the fp64 oracle's own
-forward on the GPU gives every block's input activations, block_grads.chain every block's output gradient, and each
-block's reference under bf16_storage() on those rounded to bf16 is compared with the exact one, worst per block kind.
+here, in the same run, as tests/test_cpu_block_backward.py measures it at small shapes (block_grads.backward_floors):
+the fp64 oracle's own forward on the GPU gives every block's input activations, block_grads.chain every block's output
+gradient, and each block's reference under bf16_storage() on those rounded to bf16 is compared with the exact one, worst
+per block kind.
 The oracle's activations make the floor a function of the seeds alone.  The engine's own inputs would not: they move
 between runs with the order of its fp32 atomics, and that moves the max and worst-row floors of some parameter gradients
 by up to 2x, because each is one extreme of a different rounding pattern.  The bars below are three times the floor and
@@ -27,22 +28,14 @@ The fp64 work (the oracle forward, and the exact and rounded reference of every 
 prints its time and the peak device memory, and its docstring gives what an H100 (80 GB SXM) measured.
 """
 import contextlib
-import time
 
 import pytest
 import torch
 
-from oracle import block_grads as bg
-from test_cpu_block_backward import _floors
-from test_gpu_block_backward import _run_checks, _w64
-from test_gpu_block_forward import _floors as _fwd_floors
-from test_gpu_block_forward import check_against_floors, forward_checks
-from test_gpu_cond_train import ARCH as COND_ARCH
-from test_gpu_fullconfig import REF_ARCH
+from blockcheck import unet_backward_case, vae_backward_case
+from cases import COND64_BARS, PUBLISHED, PUBLISHED_ATTN, PUBLISHED_COND, T5, UNET64_BARS, VAE256_BARS
 
 pytestmark = pytest.mark.gpu
-
-T5 = [37, 211, 412, 650, 903]    # five distinct timesteps: per-sample sums over an odd batch with a one-image last item
 
 # kind -> ((activation a, b, c), (parameter a, b, c))
 UNET256_BARS = {
@@ -54,15 +47,6 @@ UNET256_BARS = {
     "tail": ((0.0072, 0.0186, 0.0066), (0.005, 0.005, 0.005)),   # floor (0.0024, 0.0062, 0.0022) | (0.0001, 0.0002, 0.0001)
     "temb": ((0.005, 0.005, 0.005), (0.0057, 0.0066, 0.0717)),   # floor (0.0, 0.0, 0.0) | (0.0019, 0.0022, 0.0239)
 }
-UNET64_BARS = {
-    "head": ((0.005, 0.005, 0.005), (0.005, 0.005, 0.005)),   # floor (0.0, 0.0, 0.0) | (0.0, 0.0, 0.0)
-    "resnet": ((0.0132, 0.0204, 0.0171), (0.015, 0.0201, 0.0651)),   # floor (0.0044, 0.0068, 0.0057) | (0.005, 0.0067, 0.0217)
-    "down": ((0.0072, 0.009, 0.0072), (0.005, 0.005, 0.005)),   # floor (0.0024, 0.003, 0.0024) | (0.0, 0.0, 0.0)
-    "attn": ((0.0066, 0.0093, 0.0078), (0.0174, 0.0201, 0.0615)),   # floor (0.0022, 0.0031, 0.0026) | (0.0058, 0.0067, 0.0205)
-    "up": ((0.0087, 0.0132, 0.0096), (0.005, 0.005, 0.005)),   # floor (0.0029, 0.0044, 0.0032) | (0.0, 0.0, 0.0)
-    "tail": ((0.0069, 0.0123, 0.0069), (0.005, 0.005, 0.005)),   # floor (0.0023, 0.0041, 0.0023) | (0.0001, 0.0002, 0.0001)
-    "temb": ((0.005, 0.005, 0.005), (0.006, 0.0063, 0.0618)),   # floor (0.0, 0.0, 0.0) | (0.002, 0.0021, 0.0206)
-}
 UNET96x160_BARS = {
     "head": ((0.005, 0.005, 0.005), (0.005, 0.005, 0.005)),   # floor (0.0, 0.0, 0.0) | (0.0, 0.0, 0.0)
     "resnet": ((0.0129, 0.0222, 0.0135), (0.0144, 0.0195, 0.105)),   # floor (0.0043, 0.0074, 0.0045) | (0.0048, 0.0065, 0.035)
@@ -71,27 +55,6 @@ UNET96x160_BARS = {
     "up": ((0.0087, 0.015, 0.0093), (0.005, 0.005, 0.005)),   # floor (0.0029, 0.005, 0.0031) | (0.0, 0.0, 0.0)
     "tail": ((0.0072, 0.0123, 0.0066), (0.005, 0.005, 0.005)),   # floor (0.0024, 0.0041, 0.0022) | (0.0001, 0.0002, 0.0001)
     "temb": ((0.005, 0.005, 0.005), (0.0057, 0.0081, 0.0873)),   # floor (0.0, 0.0, 0.0) | (0.0019, 0.0027, 0.0291)
-}
-VAE256_BARS = {
-    "decoder:dec_head": ((0.005, 0.005, 0.005), (0.005, 0.005, 0.005)),   # floor (0.0, 0.0, 0.0) | (0.0, 0.0, 0.0)
-    "decoder:resnet_vae": ((0.0123, 0.0156, 0.0117), (0.0159, 0.0243, 0.0372)),   # floor (0.0041, 0.0052, 0.0039) | (0.0053, 0.0081, 0.0124)
-    "decoder:attn1": ((0.0051, 0.0084, 0.005), (0.012, 0.0159, 0.0939)),   # floor (0.0017, 0.0028, 0.0015) | (0.004, 0.0053, 0.0313)
-    "decoder:up": ((0.0087, 0.015, 0.0081), (0.005, 0.005, 0.005)),   # floor (0.0029, 0.005, 0.0027) | (0.0, 0.0, 0.0)
-    "decoder:tail": ((0.0069, 0.0183, 0.0066), (0.0066, 0.0072, 0.0066)),   # floor (0.0023, 0.0061, 0.0022) | (0.0022, 0.0024, 0.0022)
-    "encoder:head": ((0.005, 0.005, 0.005), (0.005, 0.005, 0.005)),   # floor (0.0, 0.0, 0.0) | (0.0, 0.0, 0.0)
-    "encoder:resnet_vae": ((0.0123, 0.0183, 0.0117), (0.0147, 0.0192, 0.0336)),   # floor (0.0041, 0.0061, 0.0039) | (0.0049, 0.0064, 0.0112)
-    "encoder:down_asym": ((0.0072, 0.0105, 0.0066), (0.005, 0.005, 0.005)),   # floor (0.0024, 0.0035, 0.0022) | (0.0, 0.0, 0.0)
-    "encoder:attn1": ((0.0051, 0.0066, 0.005), (0.0198, 0.0168, 0.0903)),   # floor (0.0017, 0.0022, 0.0016) | (0.0066, 0.0056, 0.0301)
-    "encoder:enc_tail": ((0.0069, 0.0135, 0.0066), (0.0066, 0.0078, 0.0066)),   # floor (0.0023, 0.0045, 0.0022) | (0.0022, 0.0026, 0.0022)
-}
-COND64_BARS = {
-    "head": ((0.005, 0.005, 0.005), (0.005, 0.005, 0.005)),   # floor (0.0, 0.0, 0.0) | (0.0, 0.0, 0.0)
-    "resnet": ((0.0126, 0.0183, 0.0123), (0.0135, 0.0192, 0.132)),   # floor (0.0042, 0.0061, 0.0041) | (0.0045, 0.0064, 0.044)
-    "transformer": ((0.009, 0.0141, 0.0096), (0.0237, 0.0279, 0.1374)),   # floor (0.003, 0.0047, 0.0032) | (0.0079, 0.0093, 0.0458)
-    "down": ((0.0072, 0.0108, 0.0069), (0.005, 0.005, 0.005)),   # floor (0.0024, 0.0036, 0.0023) | (0.0, 0.0, 0.0)
-    "up": ((0.009, 0.015, 0.0084), (0.005, 0.005, 0.005)),   # floor (0.003, 0.005, 0.0028) | (0.0, 0.0, 0.0)
-    "tail": ((0.0072, 0.0117, 0.0066), (0.005, 0.005, 0.005)),   # floor (0.0024, 0.0039, 0.0022) | (0.0002, 0.0003, 0.0002)
-    "temb": ((0.005, 0.005, 0.005), (0.006, 0.006, 0.0765)),   # floor (0.0, 0.0, 0.0) | (0.002, 0.002, 0.0255)
 }
 
 # the training forward (no timestep dedupe; every transformer tap kept: .h0, .n1, .qkv, .ao, .attn2, .n3, .ff1, .gg, .h3),
@@ -187,84 +150,12 @@ COND64_FWD_BARS = {
 }
 
 
-def _report_time(name, t0):
-    torch.cuda.synchronize()
-    print(f"\n{name}: fp64 time {time.perf_counter() - t0:.1f} s, peak device memory "
-          f"{torch.cuda.max_memory_allocated() / 2 ** 30:.1f} GiB on {torch.cuda.get_device_properties(0).name}")
-
-
-def _report(name, floors, bars, t0):
-    """Prints the floors as a bar table (three times the floor, no lower than 0.5 %), the time and the peak memory of the
-    reference work; returns the bars outside (floor, max(3.3 x floor, 0.5 %)]."""
-    _report_time(name, t0)
-    print("floors as bars (3 x floor, >= 0.005):")
-    bad = []
-    for kind, (a, p) in floors.items():
-        fl = tuple(round(f, 4) for f in a + p)
-        sug = tuple(round(max(3 * f, 0.005), 4) for f in fl)
-        print(f'    "{kind}": ({sug[:3]}, {sug[3:]}),   # floor {fl[:3]} | {fl[3:]}')
-        for f, b in zip(a + p, bars[kind][0] + bars[kind][1]):
-            if not f < b <= max(3.3 * round(f, 4), 5e-3) + 1e-9:
-                bad.append((kind, round(f, 4), b))
-    return bad
-
-
-def _unet_case(cuda, size, n, seed, bars, fwd_bars, checkpointing=False, levels=None):
+def _unet_case(cuda, size, n, seed, bars, fwd_bars):
     """The published UNet2DModel at `size`, batch n: one training forward and backward, every block and the timestep MLP
-    against fp64 (_run_checks), the floors of the bars measured in the same run, and the training forward block by block.
-    checkpointing: the same with enable_gradient_checkpointing(), whose backward recomputes each block's internals; the
-    block outputs and their gradients, all the per-block comparison reads, are kept, so it is held to the same bars (the
-    floors depend on the seeds alone) and skips the training-forward checks (the internal taps are not kept).  levels:
-    the expected (H, W) of every level, read from the engine's down-block outputs."""
-    from audio_diffusion_b200.unet import UNet2DModel
-    from oracle.schedulers_oracle import OracleDDPM
-    from oracle.unet_oracle import UNetConfig, init_weights, unet_forward
-    cfg = UNetConfig(sample_size=size, **REF_ARCH)
-    w = init_weights(cfg, seed=seed)
-    model = UNet2DModel(sample_size=size, **REF_ARCH)
-    model.load_state_dict(w)
-    model = model.to(cuda).train()
-    if checkpointing:
-        model.enable_gradient_checkpointing()
-    g = torch.Generator().manual_seed(seed + 1)
-    clean = torch.rand(n, 1, *size, generator=g) * 2 - 1
-    noise = torch.randn(n, 1, *size, generator=g)
-    t = torch.tensor(T5[:n])
-    noisy = OracleDDPM().add_noise(clean, noise, t).to(cuda)
-    pred = model(noisy, t.to(cuda))["sample"]
-    noise = noise.to(cuda)
-    torch.nn.functional.mse_loss(pred, noise).backward()
-    g_eps = 2 * (pred.detach() - noise) / pred.numel()
-    eps = pred.detach()
-    del pred
-    blocks = bg.unet_blocks(cfg)
-    assert [b.name for b in blocks if b.kind == "attn"] == (
-        ["down_blocks.4.attentions.0", "down_blocks.4.attentions.1", "mid_block.attentions.0"]
-        + [f"up_blocks.1.attentions.{j}" for j in range(3)])
-    if levels is not None:
-        got = [tuple(model.debug_tensor(f"down_blocks.{i}.resnets.0").shape[2:]) for i in range(len(levels))]
-        assert got == list(levels), got
-    w64 = _w64(w, cuda)
-    torch.cuda.reset_peak_memory_stats()
-    t0 = time.perf_counter()
-    temb = bg.temb_act(w64, cfg, t.to(cuda))
-    fails = _run_checks(model, blocks, noisy, g_eps, w64, cfg, bars, temb=temb, t=t.to(cuda))
-    name = f"UNet2DModel {size[0]}x{size[1]} batch {n}"
-    if checkpointing:
-        _report_time(name + ", checkpointed", t0)
-        assert not fails, fails
-        return
-    taps = {}
-    with torch.no_grad():
-        pred = unet_forward(w64, cfg, noisy.double(), t.to(cuda), taps)
-    floors = _floors(blocks, taps, noisy.double(), 2 * (pred - noise.double()) / pred.numel(), w64, cfg, taps["temb_act"],
-                     t=t.to(cuda))
-    bad = _report(name, floors, bars, t0)
-    frows = forward_checks(model.debug_tensor, blocks, noisy, eps, w64, cfg, temb, taps="all")
-    ffl = _fwd_floors(blocks, taps, noisy.double(), w64, cfg, temb, taps="all")
-    assert not fails, fails
-    assert not bad, bad
-    check_against_floors(name + ", training forward", frows, ffl, fwd_bars, t0)
+    against fp64, the floors of the bars measured in the same run, and the training forward block by block."""
+    model, blocks = unet_backward_case(cuda, PUBLISHED, size, n, seed, T5[:n], bars, floors=True, fwd_bars=fwd_bars)
+    assert [b.name for b in blocks if b.kind == "attn"] == PUBLISHED_ATTN
+    return model
 
 
 @pytest.mark.timeout(900)
@@ -294,58 +185,9 @@ def test_unet_96x160_backward_per_block(cuda):
     non-square images.  fp64 work: 2.3 s, 6.3 GiB peak."""
     levels = [(96 >> i, 160 >> i) for i in range(6)]
     assert levels[4] == (6, 10) and 6 * 10 % 16 != 0
-    _unet_case(cuda, (96, 160), 3, 15, UNET96x160_BARS, UNET96x160_FWD_BARS, levels=levels)
-
-
-def _vae_256_case(cuda, checkpointing=False):
-    """The ldm autoencoder at 256x256, batch 2: decoder and encoder backward block by block, the floors and the training
-    forward as _unet_case (checkpointing: the block comparison only, at the same bars)."""
-    from audio_diffusion_b200.vae import AutoencoderKL
-    from oracle import vae_oracle as vo
-    cfg = vo.VAEConfig()
-    w = vo.init_weights(cfg, seed=4)
-    nb = len(cfg.block_out_channels)
-    model = AutoencoderKL(in_channels=1, out_channels=1, down_block_types=("DownEncoderBlock2D",) * nb,
-                          up_block_types=("UpDecoderBlock2D",) * nb, block_out_channels=cfg.block_out_channels,
-                          layers_per_block=cfg.layers_per_block, latent_channels=1, max_batch=2)
-    model.load_state_dict(w)
-    model = model.to(cuda).train()
-    if checkpointing:
-        model.enable_gradient_checkpointing()
-    g = torch.Generator().manual_seed(5)
-    x = torch.randn(2, 1, 256, 256, generator=g).clamp(-1, 1).to(cuda)
-    z = torch.randn(2, 1, 32, 32, generator=g).to(cuda)
-    gx = torch.randn(2, 1, 256, 256, generator=g).to(cuda)
-    gm = torch.randn(2, 2, 32, 32, generator=g).to(cuda)
-    mom = model.encode(x).latent_dist.parameters
-    mom.backward(gm)
-    zz = z.clone().requires_grad_(True)
-    img = model.decode(zz).sample
-    img.backward(gx)
-    w64 = _w64(w, cuda)
-    torch.cuda.reset_peak_memory_stats()
-    t0 = time.perf_counter()
-    fails = _run_checks(model, bg.vae_blocks(cfg, "decoder"), z, gx, w64, cfg, VAE256_BARS, "decoder:", g_in=zz.grad)
-    fails += _run_checks(model, bg.vae_blocks(cfg, "encoder"), x, gm, w64, cfg, VAE256_BARS, "encoder:")
-    if checkpointing:
-        _report_time("AutoencoderKL 256x256 batch 2, checkpointed", t0)
-        assert not fails, fails
-        return
-    floors, frows, ffl = {}, [], {}
-    for part, inp, gout, fwd, out in (("decoder", z, gx, vo.decode, img.detach()),
-                                      ("encoder", x, gm, vo.encode_moments, mom.detach())):
-        taps = {}
-        with torch.no_grad():
-            fwd(w64, cfg, inp.double(), taps)
-        blocks = bg.vae_blocks(cfg, part)
-        for k, v in _floors(blocks, taps, inp.double(), gout.double(), w64, cfg).items():
-            floors[part + ":" + k] = v
-        frows += forward_checks(model.debug_tensor, blocks, inp.double(), out, w64, cfg, prefix=part + ":", taps="all")
-        ffl.update(_fwd_floors(blocks, taps, inp.double(), w64, cfg, prefix=part + ":", taps="all"))
-    bad = _report("AutoencoderKL 256x256 batch 2", floors, VAE256_BARS, t0)
-    assert not fails, fails
-    assert not bad, bad
-    check_against_floors("AutoencoderKL 256x256 batch 2, training forward", frows, ffl, VAE256_FWD_BARS, t0)
+    model = _unet_case(cuda, (96, 160), 3, 15, UNET96x160_BARS, UNET96x160_FWD_BARS)
+    got = [tuple(model.debug_tensor(f"down_blocks.{i}.resnets.0").shape[2:]) for i in range(len(levels))]
+    assert got == levels, got
 
 
 @pytest.mark.timeout(600)
@@ -354,56 +196,7 @@ def test_vae_256_backward_per_block(cuda):
     backward over S = 1024 tokens, the asymmetric (0, 1, 0, 1)-padded downsampler's data gradient from 256 to 128, and
     every 256x256 / 128x128 resnet; decoder backward from a seeded image gradient, encoder backward from seeded moment
     gradients.  fp64 work: 2.9 s, 12.0 GiB peak."""
-    _vae_256_case(cuda)
-
-
-def _cond_64_case(cuda, checkpointing=False):
-    """The published UNet2DConditionModel at 64x64, batch 2, one-token encodings: as _unet_case."""
-    from audio_diffusion_b200.unet_cond import UNet2DConditionModel
-    from oracle.schedulers_oracle import OracleDDPM
-    from oracle.unet_cond_oracle import CondUNetConfig, init_weights, unet_cond_forward
-    cfg = CondUNetConfig(sample_size=(64, 64), block_out_channels=COND_ARCH["block_out_channels"],
-                         down_block_types=COND_ARCH["down_block_types"], up_block_types=COND_ARCH["up_block_types"])
-    w = init_weights(cfg, seed=6)
-    model = UNet2DConditionModel(sample_size=(64, 64), **COND_ARCH)
-    model.load_state_dict(w)
-    model = model.to(cuda).train()
-    if checkpointing:
-        model.enable_gradient_checkpointing()
-    g = torch.Generator().manual_seed(7)
-    clean = torch.rand(2, 1, 64, 64, generator=g) * 2 - 1
-    noise = torch.randn(2, 1, 64, 64, generator=g)
-    enc = torch.randn(2, 1, 100, generator=g).to(cuda)
-    t = torch.tensor([211, 650])
-    noisy = OracleDDPM().add_noise(clean, noise, t).to(cuda)
-    pred = model(noisy, t.to(cuda), enc)["sample"]
-    noise = noise.to(cuda)
-    torch.nn.functional.mse_loss(pred, noise).backward()
-    g_eps = 2 * (pred.detach() - noise) / pred.numel()
-    eps = pred.detach()
-    del pred
-    blocks = bg.unet_blocks(cfg)
-    assert sum(b.kind == "transformer" for b in blocks) == 16
-    w64 = _w64(w, cuda)
-    torch.cuda.reset_peak_memory_stats()
-    t0 = time.perf_counter()
-    temb = bg.temb_act(w64, cfg, t.to(cuda))
-    fails = _run_checks(model, blocks, noisy, g_eps, w64, cfg, COND64_BARS, temb=temb, enc=enc, t=t.to(cuda))
-    if checkpointing:
-        _report_time("UNet2DConditionModel 64x64 batch 2, checkpointed", t0)
-        assert not fails, fails
-        return
-    taps = {}
-    with torch.no_grad():
-        pred = unet_cond_forward(w64, cfg, noisy.double(), t.to(cuda), enc.double(), taps)
-    floors = _floors(blocks, taps, noisy.double(), 2 * (pred - noise.double()) / pred.numel(), w64, cfg, temb,
-                     enc.double(), t.to(cuda))
-    bad = _report("UNet2DConditionModel 64x64 batch 2", floors, COND64_BARS, t0)
-    frows = forward_checks(model.debug_tensor, blocks, noisy, eps, w64, cfg, temb, enc.double(), taps="all")
-    ffl = _fwd_floors(blocks, taps, noisy.double(), w64, cfg, temb, enc.double(), taps="all")
-    assert not fails, fails
-    assert not bad, bad
-    check_against_floors("UNet2DConditionModel 64x64 batch 2, training forward", frows, ffl, COND64_FWD_BARS, t0)
+    vae_backward_case(cuda, (256, 256), 4, VAE256_BARS, floors=True, fwd_bars=VAE256_FWD_BARS)
 
 
 @pytest.mark.timeout(600)
@@ -412,7 +205,9 @@ def test_cond_unet_64_backward_per_block(cuda):
     mid block at 8x8) at its 64x64 latent, batch 2 with distinct encodings: the flash attention backward inside the model
     at seq 4096 (head_dim 16) and at 16x16 / 8x8 (head_dim 64), on real activations.  fp64 work: 1.8 s, 18.0 GiB
     peak."""
-    _cond_64_case(cuda)
+    _, blocks = unet_backward_case(cuda, PUBLISHED_COND, (64, 64), 2, 6, [211, 650], COND64_BARS, s=1, floors=True,
+                                   fwd_bars=COND64_FWD_BARS)
+    assert sum(b.kind == "transformer" for b in blocks) == 16
 
 
 @pytest.mark.timeout(600)
@@ -428,7 +223,7 @@ def test_batch16_gradient_equals_four_accumulated_micro_batches(cuda):
     gradient norm is 1e-3 of the largest) differ by 1.5 % between the accumulated and the full batch and by the same
     1.5 % between two runs of the full batch, from fp32 summation order alone."""
     from audio_diffusion_b200.unet import UNet2DModel
-    model = UNet2DModel(sample_size=(256, 256), seed=3, **REF_ARCH).to(cuda).train()
+    model = UNet2DModel(sample_size=(256, 256), seed=3, **PUBLISHED).to(cuda).train()
     g = torch.Generator().manual_seed(8)
     x = torch.randn(16, 1, 256, 256, generator=g).to(cuda)
     tgt = torch.randn(16, 1, 256, 256, generator=g).to(cuda)

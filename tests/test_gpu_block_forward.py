@@ -16,22 +16,19 @@ max |err| / max |ref|, worst (sample, channel group) row; for `.h1` also `.h1:me
 of one (sample, channel) over the reference's RMS, which sees a wrong time-embedding row that the row metric, diluted
 by the rounding noise of the whole row, does not.
 
-Bars.  The floor is measured in the same run (`_floors`): the fp64 oracle's forward on the compared samples gives every
+Bars.  The floor is measured in the same run (block_grads.forward_floors): the fp64 oracle's forward on the compared samples gives every
 block's inputs; each block's reference and each step's reference under the forward rounding model
 (bf16_storage(forward=True): bf16 conv / linear operands, weights and outputs, the bf16 probability numerators of the
 tensor-core attention kernels, conv_out's bf16 weights, every tap stored in bf16) on those inputs rounded to bf16,
 against the exact one; worst per key.  Each bar is 3x its floor; every run asserts that the engine is within its bars
 and that each bar lies in (floor, 3.3 x floor].
 """
-import time
-
 import pytest
 import torch
 
+from blockcheck import forward_case
+from cases import LDM, PUBLISHED, PUBLISHED_COND
 from oracle import block_grads as bg
-from test_gpu_block_backward import _w64
-from test_gpu_cond_train import ARCH as COND_ARCH
-from test_gpu_fullconfig import REF_ARCH
 
 pytestmark = pytest.mark.gpu
 
@@ -117,150 +114,10 @@ VAE256_BARS = {
 }
 
 
-def _keyed_errors(rows, key, got, ref):
-    rows.append((key,) + bg.errors(got, ref, act=True))
-    if key.endswith(".h1"):
-        rows.append((key + ":mean",) + (_mean_offset(got, ref),) * 3)
-
-
-def _mean_offset(got, ref):
-    """Largest |mean over the pixels of the error| of one (sample, channel), over the RMS of the reference: what a wrong
-    per-sample time-embedding row or bias adds to a resnet's h1 is constant over the pixels, while rounding errors
-    average out there."""
-    err = (got.double() - ref.double()).mean(dim=(2, 3))
-    return (err.abs().max() / ref.double().pow(2).mean().sqrt()).item()
-
-
-def forward_checks(read, blocks, model_in, model_out, w, cfg, temb=None, enc=None, prefix="", taps=None, sel=None):
-    """Compares every block and sub-block tap of the engine's forward with its fp64 reference on the engine's own inputs;
-    read(name) reads an engine activation (debug_tensor), sel: the compared samples (None: all), model_in / model_out are
-    the model's input and output on them; taps: the sub-taps to read (None: those kept in eval mode, "all": every one).
-    Returns [(block, key, a, b, c)] and prints one table row per block and key."""
-    si = None if sel is None else torch.tensor(sel, device=model_out.device)
-    tap = lambda name: (read(name) if si is None else read(name).index_select(0, si)).double()
-    out = []
-    print(f"\n{'block':44s} {'key':22s} {'L2':>8s} {'max':>8s} {'row':>8s}")
-    for blk in blocks:
-        xs = [model_in if blk.inp is None else tap(blk.inp)] + ([tap(blk.skip)] if blk.skip else [])
-        got = model_out if blk.out is None else tap(blk.out)
-        rows = []
-        _keyed_errors(rows, prefix + blk.kind, got, bg.block_forward(blk, w, xs, cfg, temb, enc))
-        if blk.kind in bg.EVAL_SUBTAPS:
-            subs = bg.sub_forward(blk, w, xs, cfg, temb, enc, get=lambda s: tap(blk.name + s), taps=taps)
-            for s, ref in subs.items():
-                _keyed_errors(rows, prefix + blk.kind + (".out" if s == "out" else s),
-                              got if s == "out" else tap(blk.name + s), ref)
-        if blk.kind in ("down", "down_asym"):
-            par = read(blk.name + ".parity")        # the batch's four parity tensors viewed as one of 4C channels
-            n, c4, hh, ww = par.shape
-            par = par.reshape(n, c4 // 8, 8, hh, ww).reshape(4, n, c4 // 4, hh, ww)   # four tensors back to back
-            x = read(blk.inp)
-            split = torch.stack([x[:, :, a::2, b::2] for a in (0, 1) for b in (0, 1)]).to(par.dtype)
-            same = torch.equal(par, split)
-            rows.append((prefix + blk.kind + ".parity", 0.0 if same else 1.0, 0.0 if same else 1.0, 0.0 if same else 1.0))
-        for key, a, b, c in rows:
-            print(f"{blk.name or 'conv_out':44s} {key:22s} {a:8.5f} {b:8.5f} {c:8.5f}")
-            out.append((blk.name, key, a, b, c))
-    return out
-
-
-def _floors(blocks, otaps, model_in, w, cfg, temb=None, enc=None, prefix="", taps=None):
-    """bf16 floor of every block and step, worst per key: {key: (a, b, c)}."""
-    fl = {}
-
-    def put(key, got, ref):
-        e = bg.errors(got, ref, act=True)
-        fl[key] = tuple(map(max, fl.get(key, (0.0,) * 3), e))
-        if key.endswith(".h1"):
-            fl[key + ":mean"] = tuple(map(max, fl.get(key + ":mean", (0.0,) * 3), (_mean_offset(got, ref),) * 3))
-
-    for blk in blocks:
-        xs = [model_in if blk.inp is None else bg.bf16(otaps[blk.inp])] + ([bg.bf16(otaps[blk.skip])] if blk.skip else [])
-        put(prefix + blk.kind, bg.block_forward(blk, w, xs, cfg, temb, enc, rounded=True),
-            bg.block_forward(blk, w, xs, cfg, temb, enc))
-        if blk.kind in bg.EVAL_SUBTAPS:
-            exact = bg.sub_forward(blk, w, xs, cfg, temb, enc, taps=taps)
-            get = lambda s: bg.bf16(exact[s])
-            ex = bg.sub_forward(blk, w, xs, cfg, temb, enc, get=get, taps=taps)
-            rd = bg.sub_forward(blk, w, xs, cfg, temb, enc, get=get, taps=taps, rounded=True)
-            for s in ex:
-                put(prefix + blk.kind + (".out" if s == "out" else s), rd[s], ex[s])
-    return fl
-
-
-def check_against_floors(name, rows, floors, bars, t0):
-    """Prints the floors as a bar table and the fp64 time and peak memory; asserts the engine within its bars and every
-    bar in (floor, 3.3 x floor]."""
-    torch.cuda.synchronize()
-    props = torch.cuda.get_device_properties(0)
-    print(f"\n{name}: fp64 time {time.perf_counter() - t0:.1f} s, peak device memory "
-          f"{torch.cuda.max_memory_allocated() / 2 ** 30:.1f} GiB on {props.name}")
-    print("floors as bars (3 x floor):")
-    for key, f in sorted(floors.items()):
-        f = tuple(round(v, 5) for v in f)
-        print(f'    "{key}": ({round(3 * f[0], 5)}, {round(3 * f[1], 5)}, {round(3 * f[2], 5)}),   # floor {f}')
-    use = bars or {k: tuple(3 * round(v, 5) for v in f) for k, f in floors.items()}
-    over = [r for r in rows if r[1].endswith(".parity") and r[2] != 0.0]
-    over += [r for r in rows if not r[1].endswith(".parity") and any(e > b for e, b in zip(r[2:], use[r[1]]))]
-    for r in over:
-        print("OVER", r, use.get(r[1]))
-    assert bars, f"{name}: no bars stated"
-    bad = [(k, f, bars.get(k)) for k, f in floors.items()
-           if k not in bars or not all(v < b <= 3.3 * round(v, 5) + 1e-9 for v, b in zip(f, bars[k]))]
-    assert not over, over
-    assert not bad, bad
-
-
-def _power_limit():
-    import subprocess
-    try:
-        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
-                              capture_output=True, text=True, timeout=30).stdout.strip()
-    except Exception as e:   # the card name is printed by check_against_floors in any case
-        return f"power limit not read: {e}"
-
-
-def _unet_case(cuda, monkeypatch, size, n, sel, t, seed, bars):
-    """UNet2DModel (the published six-level architecture) in eval mode at `size`, batch n, timesteps t; samples sel
-    compared.  Returns the input, timesteps, weights and eps of the whole batch for the caller's further checks."""
-    from audio_diffusion_b200.unet import UNet2DModel
-    from oracle.unet_oracle import UNetConfig, init_weights, unet_forward
-    monkeypatch.setenv("B200AD_DEBUG_NOPOOL", "1")
-    cfg = UNetConfig(sample_size=size, **REF_ARCH)
-    w = init_weights(cfg, seed=seed)
-    model = UNet2DModel(sample_size=size, **REF_ARCH)
-    model.load_state_dict(w)
-    model = model.to(cuda).eval()
-    g = torch.Generator().manual_seed(seed + 1)
-    x = torch.randn(n, 1, *size, generator=g).to(cuda)
-    t = torch.tensor(t, dtype=torch.float32, device=cuda)
-    with torch.no_grad():
-        eps = model(x, t)["sample"]
-    print(f"\n{_power_limit()}")
-    si = torch.tensor(sel, device=cuda)
-    w64 = _w64(w, cuda)
-    blocks = bg.unet_blocks(cfg)
-    torch.cuda.reset_peak_memory_stats()
-    t0 = time.perf_counter()
-    ts = t.long().index_select(0, si)
-    temb = bg.temb_act(w64, cfg, ts)
-    xin = x.index_select(0, si).double()
-    rows = forward_checks(model.debug_tensor, blocks, xin, eps.index_select(0, si), w64, cfg, temb, sel=sel)
-    del model
-    torch.cuda.empty_cache()
-    otaps = {}
-    with torch.no_grad():
-        unet_forward(w64, cfg, xin, ts, otaps)
-    floors = _floors(blocks, otaps, xin, w64, cfg, temb)
-    del otaps
-    check_against_floors(f"UNet2DModel {size[0]}x{size[1]} batch {n}, samples {sel}", rows, floors, bars, t0)
-    return x, t, w, eps
-
-
 def _pooled_eps(cuda, w, size, x, t):
     """eps of the same input through a model with pooled activation buffers (the default), twice."""
     from audio_diffusion_b200.unet import UNet2DModel
-    model = UNet2DModel(sample_size=size, **REF_ARCH)
+    model = UNet2DModel(sample_size=size, **PUBLISHED)
     model.load_state_dict(w)
     model = model.to(cuda).eval()
     with torch.no_grad():
@@ -279,7 +136,7 @@ def test_unet_256_batch64_forward_per_block(cuda, monkeypatch):
     power limit, fp64 work 3 s, 32.1 GiB peak device memory."""
     sel = [0, 1, 13, 27, 62, 63]
     t = [999 - 7 * (i % 13) for i in range(64)]
-    x, tt, w, eps = _unet_case(cuda, monkeypatch, (256, 256), 64, sel, t, 11, UNET256_BARS)
+    x, tt, w, eps = forward_case(cuda, monkeypatch, PUBLISHED, (256, 256), 64, 11, UNET256_BARS, t=t, sel=sel)
     monkeypatch.delenv("B200AD_DEBUG_NOPOOL")
     torch.cuda.empty_cache()
     e1, e2 = _pooled_eps(cuda, w, (256, 256), x, tt)
@@ -294,7 +151,8 @@ def test_unet_64_batch5_forward_per_block(cuda, monkeypatch):
     """The published UNet2DModel at 64x64, batch 5: the 8x8, 4x4 and 2x2 levels are packed, the last item holds one
     image (sample 4).  Attention at 4x4 (16 tokens: attention_mma_kernel) and, in the mid block, 2x2 (attention_kernel).
     All samples compared.  H100 80GB HBM3, 700 W: fp64 work 0.8 s, 2.1 GiB peak."""
-    _unet_case(cuda, monkeypatch, (64, 64), 5, list(range(5)), [37, 211, 412, 650, 903], 13, UNET64_BARS)
+    forward_case(cuda, monkeypatch, PUBLISHED, (64, 64), 5, 13, UNET64_BARS, t=[37, 211, 412, 650, 903],
+                 sel=list(range(5)))
 
 
 @pytest.mark.timeout(600)
@@ -303,10 +161,10 @@ def test_unet_96x160_forward_per_block(cuda, monkeypatch):
     launch_attention runs the SIMT attention_kernel (its `.ao` rows in the table); the levels 3x5, 6x10, 12x20 ... 96x160
     are odd and non-square.  H100 80GB HBM3, 700 W: fp64 work 0.9 s, 2.9 GiB peak."""
     from oracle.unet_oracle import UNetConfig
-    blocks = bg.unet_blocks(UNetConfig(sample_size=(96, 160), **REF_ARCH))
+    blocks = bg.unet_blocks(UNetConfig(sample_size=(96, 160), **PUBLISHED))
     assert [b.name for b in blocks if b.kind == "attn"][0] == "down_blocks.4.attentions.0"   # 96 / 16 x 160 / 16
     assert (96 // 16) * (160 // 16) % 16 != 0
-    _unet_case(cuda, monkeypatch, (96, 160), 3, [0, 1, 2], [999, 500, 999], 15, UNET96x160_BARS)
+    forward_case(cuda, monkeypatch, PUBLISHED, (96, 160), 3, 15, UNET96x160_BARS, t=[999, 500, 999], sel=[0, 1, 2])
 
 
 @pytest.mark.timeout(600)
@@ -314,34 +172,7 @@ def test_cond_unet_64_forward_per_block(cuda, monkeypatch):
     """The published UNet2DConditionModel at its 64x64 latent, batch 3, distinct encodings: every transformer's eval path
     (mha_flash_kernel at seq 4096 / 1024 / 256 / 64 and the one-key cross attention folded into a per-sample vector).
     H100 80GB HBM3, 700 W: fp64 work 1.4 s, 15.8 GiB peak."""
-    from audio_diffusion_b200.unet_cond import UNet2DConditionModel
-    from oracle.unet_cond_oracle import CondUNetConfig, init_weights, unet_cond_forward
-    monkeypatch.setenv("B200AD_DEBUG_NOPOOL", "1")
-    cfg = CondUNetConfig(sample_size=(64, 64), **{k: COND_ARCH[k] for k in ("block_out_channels", "down_block_types",
-                                                                              "up_block_types")})
-    w = init_weights(cfg, seed=17)
-    model = UNet2DConditionModel(sample_size=(64, 64), **COND_ARCH)
-    model.load_state_dict(w)
-    model = model.to(cuda).eval()
-    g = torch.Generator().manual_seed(18)
-    x = torch.randn(3, 1, 64, 64, generator=g).to(cuda)
-    enc = torch.randn(3, 1, 100, generator=g).to(cuda)
-    t = torch.tensor([37, 412, 903], device=cuda)
-    with torch.no_grad():
-        eps = model(x, t, enc)["sample"]
-    print(f"\n{_power_limit()}")
-    w64 = _w64(w, cuda)
-    blocks = bg.unet_blocks(cfg)
-    torch.cuda.reset_peak_memory_stats()
-    t0 = time.perf_counter()
-    temb = bg.temb_act(w64, cfg, t)
-    e64 = enc.double()
-    rows = forward_checks(model.debug_tensor, blocks, x.double(), eps, w64, cfg, temb, e64)
-    otaps = {}
-    with torch.no_grad():
-        unet_cond_forward(w64, cfg, x.double(), t, e64, otaps)
-    floors = _floors(blocks, otaps, x.double(), w64, cfg, temb, e64)
-    check_against_floors("UNet2DConditionModel 64x64 batch 3", rows, floors, COND64_BARS, t0)
+    forward_case(cuda, monkeypatch, PUBLISHED_COND, (64, 64), 3, 17, COND64_BARS, t=[37, 412, 903], s=1)
 
 
 @pytest.mark.timeout(600)
@@ -350,35 +181,7 @@ def test_vae_256_forward_per_block(cuda, monkeypatch):
     over S = 1024 tokens, the asymmetric 256 -> 128 downsampler; compared output: the moments), decode from seeded
     latents (teacher-forced: the decoder's blocks read the engine's own activations).  H100 80GB HBM3, 700 W: fp64 work
     1.8 s, 6.6 GiB peak."""
-    from audio_diffusion_b200.vae import AutoencoderKL
-    from oracle import vae_oracle as vo
-    monkeypatch.setenv("B200AD_DEBUG_NOPOOL", "1")
-    cfg = vo.VAEConfig()
-    w = vo.init_weights(cfg, seed=19)
-    nb = len(cfg.block_out_channels)
-    model = AutoencoderKL(in_channels=1, out_channels=1, down_block_types=("DownEncoderBlock2D",) * nb,
-                          up_block_types=("UpDecoderBlock2D",) * nb, block_out_channels=cfg.block_out_channels,
-                          layers_per_block=cfg.layers_per_block, latent_channels=1, max_batch=3)
-    model.load_state_dict(w)
-    model = model.to(cuda).eval()
-    g = torch.Generator().manual_seed(20)
-    x = torch.randn(3, 1, 256, 256, generator=g).clamp(-1, 1).to(cuda)
-    z = torch.randn(3, 1, 32, 32, generator=g).to(cuda)
-    print(f"\n{_power_limit()}")
-    w64 = _w64(w, cuda)
-    torch.cuda.reset_peak_memory_stats()
-    t0 = time.perf_counter()
-    rows, floors = [], {}
-    for part, inp, fwd in (("encoder", x, vo.encode_moments), ("decoder", z, vo.decode)):
-        with torch.no_grad():
-            out = model.encode(inp).latent_dist.parameters if part == "encoder" else model.decode(inp).sample
-        blocks = bg.vae_blocks(cfg, part)
-        rows += forward_checks(model.debug_tensor, blocks, inp.double(), out, w64, cfg, prefix=part + ":")
-        otaps = {}
-        with torch.no_grad():
-            fwd(w64, cfg, inp.double(), otaps)
-        floors.update(_floors(blocks, otaps, inp.double(), w64, cfg, prefix=part + ":"))
-    check_against_floors("AutoencoderKL 256x256 batch 3", rows, floors, VAE256_BARS, t0)
+    forward_case(cuda, monkeypatch, LDM, (256, 256), 3, 19, VAE256_BARS)
 
 
 @pytest.mark.timeout(600)
@@ -394,7 +197,7 @@ def test_fused_step_256_batch64(cuda, kind):
     model(x, t), and two model(x, t) calls bit-identical."""
     from audio_diffusion_b200.schedulers import DDIMScheduler, DDPMScheduler
     from audio_diffusion_b200.unet import UNet2DModel
-    model = UNet2DModel(sample_size=(256, 256), seed=21, **REF_ARCH).to(cuda).eval()
+    model = UNet2DModel(sample_size=(256, 256), seed=21, **PUBLISHED).to(cuda).eval()
     g = torch.Generator().manual_seed(22)
     x = torch.randn(64, 1, 256, 256, generator=g).to(cuda)
     z = torch.randn(64, 1, 256, 256, generator=g).to(cuda) if kind == "ddpm" else None

@@ -9,16 +9,10 @@ import gc
 import pytest
 import torch
 
+from cases import LDM, PUBLISHED, PUBLISHED_COND
+
 pytestmark = pytest.mark.gpu
 
-PUBLISHED = dict(in_channels=1, out_channels=1, layers_per_block=2, block_out_channels=(128, 128, 256, 256, 512, 512),
-                 down_block_types=("DownBlock2D",) * 4 + ("AttnDownBlock2D", "DownBlock2D"),
-                 up_block_types=("UpBlock2D", "AttnUpBlock2D", "UpBlock2D", "UpBlock2D", "UpBlock2D", "UpBlock2D"))
-COND = dict(in_channels=1, out_channels=1, layers_per_block=2, block_out_channels=(128, 256, 512, 512),
-            down_block_types=("CrossAttnDownBlock2D",) * 3 + ("DownBlock2D",),
-            up_block_types=("UpBlock2D",) + ("CrossAttnUpBlock2D",) * 3, cross_attention_dim=100)
-LDM = dict(in_channels=1, out_channels=1, latent_channels=1, layers_per_block=2, block_out_channels=(128, 256, 512, 512),
-           down_block_types=("DownEncoderBlock2D",) * 4, up_block_types=("UpDecoderBlock2D",) * 4)
 K_SPREAD = 4.0     # checkpointed gradient error allowed, in units of the plain backward's run-to-run difference
 
 
@@ -27,7 +21,7 @@ def _unet(cuda, s, seed=0):
     from audio_diffusion_b200.unet_cond import UNet2DConditionModel
     if s is None:
         return UNet2DModel(sample_size=(64, 64), seed=seed, **PUBLISHED).to(cuda).train()
-    return UNet2DConditionModel(sample_size=(64, 64), seed=seed, **COND).to(cuda).train()
+    return UNet2DConditionModel(sample_size=(64, 64), seed=seed, **PUBLISHED_COND).to(cuda).train()
 
 
 def _inputs(cuda, s, n=4, size=64, seed=1):

@@ -6,11 +6,9 @@ import numpy as np
 import pytest
 import torch
 
-pytestmark = pytest.mark.gpu
+from cases import PUBLISHED_COND
 
-ARCH = dict(in_channels=1, out_channels=1, layers_per_block=2, block_out_channels=(128, 256, 512, 512),
-            down_block_types=("CrossAttnDownBlock2D",) * 3 + ("DownBlock2D",),
-            up_block_types=("UpBlock2D",) + ("CrossAttnUpBlock2D",) * 3, cross_attention_dim=100)
+pytestmark = pytest.mark.gpu
 
 
 def _build(cuda, size, seed=0):
@@ -18,7 +16,7 @@ def _build(cuda, size, seed=0):
     from oracle.unet_cond_oracle import CondUNetConfig, init_weights
     ocfg = CondUNetConfig(sample_size=size)
     w = init_weights(ocfg, seed=seed)
-    model = UNet2DConditionModel(sample_size=size, **ARCH)
+    model = UNet2DConditionModel(sample_size=size, **PUBLISHED_COND)
     assert set(model.state_dict().keys()) == set(w.keys())
     model.load_state_dict(w)
     return model.to(cuda).eval(), ocfg, w

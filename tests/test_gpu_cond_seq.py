@@ -2,33 +2,16 @@
 100-d token per 5-second slice, (B, S, 100)): the cross-attention kernels against fp32 autograd, the model forward,
 sampling and training against the fp32 oracle (oracle/unet_cond_oracle.py, which attends over any number of tokens), and
 the S = 1 path left as it was.  Bars: those of tests/test_gpu_cond.py and tests/test_gpu_cond_train.py."""
-import time
-
 import numpy as np
 import pytest
 import torch
 
+from blockcheck import forward_case, unet_backward_case
+from cases import COND_BARS, COND_SEQ_BWD_TRANSFORMER_BARS, ONE_TOKEN_ZERO, PUBLISHED_COND, T3, TWO_LEVEL_COND, build
+from oracle.train_oracle import cond_loss_and_grads
+
 pytestmark = pytest.mark.gpu
 
-ARCH = dict(in_channels=1, out_channels=1, layers_per_block=2, block_out_channels=(128, 256, 512, 512),
-            down_block_types=("CrossAttnDownBlock2D",) * 3 + ("DownBlock2D",),
-            up_block_types=("UpBlock2D",) + ("CrossAttnUpBlock2D",) * 3, cross_attention_dim=100)
-# two levels, transformers at head_dim 16 in the down and the up block (tests/test_gpu_cond_train.py's SMALL)
-SMALL = dict(ARCH, block_out_channels=(128, 256), down_block_types=("CrossAttnDownBlock2D", "DownBlock2D"),
-             up_block_types=("UpBlock2D", "CrossAttnUpBlock2D"))
-ONE_TOKEN_ZERO = ("attn2.to_q.weight", "attn2.to_k.weight", "norm2.weight", "norm2.bias")
-
-
-def _build(cuda, size, seed, arch=ARCH, train=False):
-    from audio_diffusion_b200.unet_cond import UNet2DConditionModel
-    from oracle.unet_cond_oracle import CondUNetConfig, init_weights
-    ocfg = CondUNetConfig(sample_size=size, block_out_channels=arch["block_out_channels"],
-                          down_block_types=arch["down_block_types"], up_block_types=arch["up_block_types"])
-    w = init_weights(ocfg, seed=seed)
-    model = UNet2DConditionModel(sample_size=size, **arch)
-    model.load_state_dict(w)
-    model = model.to(cuda)
-    return (model.train() if train else model.eval()), ocfg, w
 
 
 def _rel(got, ref):
@@ -83,7 +66,7 @@ def test_cond_seq_layers_and_eps(cuda, monkeypatch, size, s):
     block) and epsilon against unet_cond_forward, with test_gpu_cond.py's bars."""
     from oracle.unet_cond_oracle import unet_cond_forward
     monkeypatch.setenv("B200AD_DEBUG_NOPOOL", "1")
-    model, ocfg, w = _build(cuda, size, seed=s)
+    model, ocfg, w = build(PUBLISHED_COND, s, cuda, size, train=False)
     g = torch.Generator().manual_seed(42 + s)
     x = torch.randn(2, 1, *size, generator=g)
     enc = torch.randn(2, s, 100, generator=g)
@@ -112,8 +95,8 @@ def test_cond_seq_layers_and_eps(cuda, monkeypatch, size, s):
 def test_one_token_path_unchanged_after_longer_encoding(cuda):
     """S = 1 keeps its own plan: after a model has run with S = 2, its S = 1 output equals a fresh model's bit for bit, and
     the S = 1 launch count is the fresh model's."""
-    a, _, _ = _build(cuda, (32, 32), seed=7)
-    b, _, _ = _build(cuda, (32, 32), seed=7)
+    a, _, _ = build(PUBLISHED_COND, 7, cuda, (32, 32), train=False)
+    b, _, _ = build(PUBLISHED_COND, 7, cuda, (32, 32), train=False)
     g = torch.Generator().manual_seed(8)
     x = torch.randn(2, 1, 32, 32, generator=g).to(cuda)
     e2 = torch.randn(2, 2, 100, generator=g).to(cuda)
@@ -130,7 +113,7 @@ def test_one_token_path_unchanged_after_longer_encoding(cuda):
 def test_identical_tokens_match_one_token(cuda):
     """Two identical tokens attend exactly like one (softmax splits evenly over equal keys): the S = 2 path (K / V
     projections, cross-attention kernel) and the S = 1 path (per-sample vector) differ only by bf16 rounding."""
-    model, _, _ = _build(cuda, (32, 32), seed=9)
+    model, _, _ = build(PUBLISHED_COND, 9, cuda, (32, 32), train=False)
     g = torch.Generator().manual_seed(10)
     x = torch.randn(2, 1, 32, 32, generator=g).to(cuda)
     e1 = torch.randn(2, 1, 100, generator=g).to(cuda)
@@ -151,7 +134,7 @@ def test_cond_seq_pipeline_matches_oracle_loop(cuda, s):
     from audio_diffusion_b200.schedulers import DDPMScheduler
     from oracle.schedulers_oracle import OracleDDPM
     from oracle.unet_cond_oracle import unet_cond_forward
-    model, ocfg, w = _build(cuda, (32, 32), seed=2)
+    model, ocfg, w = build(PUBLISHED_COND, 2, cuda, (32, 32), train=False)
     pipe = AudioDiffusionPipeline(vqvae=None, unet=model, mel=Mel(x_res=32, y_res=32, hop_length=512), scheduler=DDPMScheduler())
     pipe.set_progress_bar_config(disable=True)
     g = torch.Generator().manual_seed(9)
@@ -174,17 +157,6 @@ def test_cond_seq_pipeline_matches_oracle_loop(cuda, s):
 
 
 # ---------------------------------------------------------------------------------------------------- training
-def cond_loss_and_grads(w, cfg, clean, noise, t, enc):
-    from oracle.schedulers_oracle import OracleDDPM
-    from oracle.unet_cond_oracle import unet_cond_forward
-    noisy = OracleDDPM().add_noise(clean, noise, t)
-    wl = {k: v.detach().clone().requires_grad_(True) for k, v in w.items()}
-    pred = unet_cond_forward(wl, cfg, noisy, t, enc)
-    loss = torch.mean((pred - noise) ** 2)
-    grads = torch.autograd.grad(loss, list(wl.values()))
-    return loss.detach(), dict(zip(wl.keys(), grads))
-
-
 @pytest.mark.timeout(900)
 @pytest.mark.parametrize("s", [2, 77])
 @pytest.mark.parametrize("arch,size", [("full", (32, 32)), ("small", (64, 64))])
@@ -194,7 +166,7 @@ def test_cond_seq_backward_matches_autograd(cuda, arch, size, s):
     parameters that get exactly zero gradients with one token (attn2.to_q, attn2.to_k, norm2) are non-zero and inside
     those bars."""
     from oracle.schedulers_oracle import OracleDDPM
-    model, ocfg, w = _build(cuda, size, seed=20 + s, arch=ARCH if arch == "full" else SMALL, train=True)
+    model, ocfg, w = build(PUBLISHED_COND if arch == "full" else TWO_LEVEL_COND, 20 + s, cuda, size)
     g = torch.Generator().manual_seed(s)
     clean = torch.rand(2, 1, *size, generator=g) * 2 - 1
     noise = torch.randn(2, 1, *size, generator=g)
@@ -259,7 +231,7 @@ def test_xattn_backward_deterministic(cuda, d, s, hh):
 
 def test_cond_seq_gradient_accumulation_equals_full_batch(cuda):
     """Two half-batches (loss / 2 each, the first under no_sync) give the full batch's gradient, with 9 tokens."""
-    model, _, _ = _build(cuda, (32, 32), seed=3, train=True)
+    model, _, _ = build(PUBLISHED_COND, 3, cuda, (32, 32))
     g = torch.Generator().manual_seed(6)
     x = torch.randn(2, 1, 32, 32, generator=g).to(cuda)
     tgt = torch.randn(2, 1, 32, 32, generator=g).to(cuda)
@@ -289,7 +261,7 @@ def test_cond_seq_two_training_steps_match_oracle(cuda):
         from diffusers.optimization import get_scheduler
     finally:
         sys.path.pop(0)
-    model, ocfg, w = _build(cuda, (32, 32), seed=4, arch=SMALL, train=True)
+    model, ocfg, w = build(TWO_LEVEL_COND, 4, cuda, (32, 32))
     w0 = {k: v.clone() for k, v in w.items()}
     opt = FusedAdamW(model.parameters(), lr=1e-4, betas=(0.95, 0.999), weight_decay=1e-6, eps=1e-8, max_grad_norm=1.0)
     ema = EMAModel(model.parameters(), inv_gamma=1.0, power=0.75, max_value=0.9999)
@@ -339,7 +311,7 @@ def test_cond_seq_two_training_steps_match_oracle(cuda):
 # the mid block), batch 3, against fp64 on the engine's own activations (oracle/block_grads.py) with the bars of
 # tests/test_gpu_block_forward.py / tests/test_gpu_block_backward.py: 3 x the bf16 floor of each block kind, measured at
 # these shapes, seeds and token counts; each test recomputes the floors and asserts every bar within (floor, 3.3 x floor].
-# S -> key -> (a, b, c): 3 x the bf16 floor of tests/test_gpu_block_forward.py's _floors at this test's shapes and seeds
+# S -> key -> (a, b, c): 3 x the bf16 floor of block_grads.forward_floors at this test's shapes and seeds
 COND_SEQ_FWD_BARS = {
     3: {
         "down": (0.00681, 0.00885, 0.00696),   # floor (0.00227, 0.00295, 0.00232)
@@ -368,11 +340,6 @@ COND_SEQ_FWD_BARS = {
         "up": (0.00732, 0.01071, 0.00762),   # floor (0.00244, 0.00357, 0.00254)
     },
 }
-# S -> the transformer's (activation a, b, c), (parameter a, b, c): 3 x the bf16 floor (at least 0.5 %)
-COND_SEQ_BWD_TRANSFORMER_BARS = {
-    3: ((0.009, 0.0147, 0.0096), (0.0225, 0.0282, 0.0855)),   # floor (0.003, 0.0049, 0.0032) | (0.0075, 0.0094, 0.0285)
-    77: ((0.009, 0.0111, 0.0093), (0.0216, 0.0204, 0.0948)),   # floor (0.003, 0.0037, 0.0031) | (0.0072, 0.0068, 0.0316)
-}
 
 
 @pytest.mark.timeout(600)
@@ -380,94 +347,7 @@ COND_SEQ_BWD_TRANSFORMER_BARS = {
 def test_cond_seq_forward_per_block(cuda, monkeypatch, s):
     """Every block, and every transformer's h2 (.attn2, after the LN2 / to_q / K-V / cross-attention / to_out steps), of
     the eval forward with an (3, s, 100) encoding, from the engine's own inputs."""
-    import time
-    from audio_diffusion_b200.unet_cond import UNet2DConditionModel
-    from oracle import block_grads as bg
-    from oracle.unet_cond_oracle import CondUNetConfig, init_weights, unet_cond_forward
-    from test_gpu_block_backward import COND_ARCH, _w64
-    from test_gpu_block_forward import _floors, check_against_floors, forward_checks
-    monkeypatch.setenv("B200AD_DEBUG_NOPOOL", "1")
-    cfg = CondUNetConfig(sample_size=(32, 32), **{k: COND_ARCH[k] for k in ("block_out_channels", "down_block_types",
-                                                                              "up_block_types")})
-    w = init_weights(cfg, seed=17)
-    model = UNet2DConditionModel(sample_size=(32, 32), **COND_ARCH)
-    model.load_state_dict(w)
-    model = model.to(cuda).eval()
-    g = torch.Generator().manual_seed(18)
-    x = torch.randn(3, 1, 32, 32, generator=g).to(cuda)
-    enc = torch.randn(3, s, 100, generator=g).to(cuda)
-    t = torch.tensor([37, 412, 903], device=cuda)
-    with torch.no_grad():
-        eps = model(x, t, enc)["sample"]
-    w64 = _w64(w, cuda)
-    blocks = bg.unet_blocks(cfg)
-    t0 = time.perf_counter()
-    temb = bg.temb_act(w64, cfg, t)
-    e64 = enc.double()
-    rows = forward_checks(model.debug_tensor, blocks, x.double(), eps, w64, cfg, temb, e64)
-    otaps = {}
-    with torch.no_grad():
-        unet_cond_forward(w64, cfg, x.double(), t, e64, otaps)
-    floors = _floors(blocks, otaps, x.double(), w64, cfg, temb, e64)
-    check_against_floors(f"UNet2DConditionModel 32x32 batch 3, {s} tokens", rows, floors, COND_SEQ_FWD_BARS[s], t0)
-
-
-def cond_seq_backward_case(cuda, s, checkpointing=False):
-    """One training forward and backward of the two-level conditional U-Net with an (3, s, 100) encoding, every block and
-    the timestep MLP against fp64 (test_gpu_block_backward._run_checks), and the transformer and MLP bars against the
-    floors at these inputs.  checkpointing: under enable_gradient_checkpointing(), at the same bars (the floors depend on
-    the seeds alone, so they are not measured again)."""
-    from audio_diffusion_b200.unet_cond import UNet2DConditionModel
-    from oracle import block_grads as bg
-    from oracle.schedulers_oracle import OracleDDPM
-    from oracle.unet_cond_oracle import CondUNetConfig, init_weights, unet_cond_forward
-    from test_cpu_block_backward import _floors
-    from test_gpu_block_backward import COND_ARCH, COND_BARS, T3, _run_checks, _w64
-    cfg = CondUNetConfig(sample_size=(32, 32), block_out_channels=COND_ARCH["block_out_channels"],
-                         down_block_types=COND_ARCH["down_block_types"], up_block_types=COND_ARCH["up_block_types"])
-    w = init_weights(cfg, seed=3)
-    model = UNet2DConditionModel(sample_size=(32, 32), **COND_ARCH)
-    model.load_state_dict(w)
-    model = model.to(cuda).train()
-    if checkpointing:
-        model.enable_gradient_checkpointing()
-    g = torch.Generator().manual_seed(4)
-    clean = torch.rand(3, 1, 32, 32, generator=g) * 2 - 1
-    noise = torch.randn(3, 1, 32, 32, generator=g)
-    enc = torch.randn(3, s, 100, generator=g).to(cuda)
-    t = torch.tensor(T3)
-    noisy = OracleDDPM().add_noise(clean, noise, t).to(cuda)
-    pred = model(noisy, t.to(cuda), enc)["sample"]
-    noise = noise.to(cuda)
-    torch.nn.functional.mse_loss(pred, noise).backward()
-    g_eps = 2 * (pred.detach() - noise) / pred.numel()
-    named = dict(model.named_parameters())
-    once = [k for k in named if k.endswith(ONE_TOKEN_ZERO) and ".transformer_blocks." in k]
-    assert len(once) == 6 * 4 and all(torch.count_nonzero(named[k].grad) > 0 for k in once)
-    w64 = _w64(w, cuda)
-    bars = dict(COND_BARS, transformer=COND_SEQ_BWD_TRANSFORMER_BARS[s])
-    blocks = bg.unet_blocks(cfg)
-    torch.cuda.reset_peak_memory_stats()
-    t0 = time.perf_counter()
-    temb = bg.temb_act(w64, cfg, t.to(cuda))
-    fails = _run_checks(model, blocks, noisy, g_eps, w64, cfg, bars, temb=temb, enc=enc, t=t.to(cuda))
-    torch.cuda.synchronize()
-    print(f"\n{s} tokens{', checkpointed' if checkpointing else ''}: fp64 time {time.perf_counter() - t0:.1f} s, peak "
-          f"device memory {torch.cuda.max_memory_allocated() / 2 ** 30:.1f} GiB")
-    assert not fails, fails
-    if checkpointing:
-        return
-    # the transformer and MLP bars against the floor at these inputs (oracle activations, fp64 on the device; the MLP's,
-    # COND_BARS', measured on the CPU with one token: (0.0022, 0.0036, 0.0261) with 3 tokens, (0.0022, 0.0029, 0.0298)
-    # with 77 on an H100)
-    taps = {}
-    x64, n64, e64 = noisy.double(), noise.double(), enc.double()
-    with torch.no_grad():
-        ref = unet_cond_forward(w64, cfg, x64, t.to(cuda), e64, taps)
-    fl = _floors(blocks, taps, x64, 2 * (ref - n64) / ref.numel(), w64, cfg, temb, e64, t.to(cuda))
-    for kind in ("transformer", "temb"):
-        for f, b in zip(fl[kind][0] + fl[kind][1], bars[kind][0] + bars[kind][1]):
-            assert f < b <= max(3.3 * round(f, 4), 5e-3) + 1e-9, (kind, fl[kind], bars[kind])
+    forward_case(cuda, monkeypatch, TWO_LEVEL_COND, (32, 32), 3, 17, COND_SEQ_FWD_BARS[s], t=T3, s=s)
 
 
 @pytest.mark.timeout(600)
@@ -478,8 +358,13 @@ def test_cond_seq_backward_per_block(cuda, s):
     timestep MLP's gradients from the resnets' temb_act gradients.  The transformers' walk covers attn2.to_out, the
     cross-attention backward (dQ, the split dK / dV partial sums), the K / V weight gradients, to_q, LN2 with its
     residual and the two to_out biases; attn2.to_q, attn2.to_k and norm2 get non-zero gradients inside the bars.  The
-    other block kinds keep test_gpu_block_backward.py's COND_BARS."""
-    cond_seq_backward_case(cuda, s)
+    other block kinds keep test_gpu_block_backward.py's COND_BARS.
+    The transformer and MLP bars are checked against the floors at these inputs (oracle activations, fp64 on the device;
+    the MLP's, COND_BARS', measured on the CPU with one token: (0.0022, 0.0036, 0.0261) with 3 tokens, (0.0022, 0.0029,
+    0.0298) with 77 on an H100)."""
+    bars = dict(COND_BARS, transformer=COND_SEQ_BWD_TRANSFORMER_BARS[s])
+    unet_backward_case(cuda, TWO_LEVEL_COND, (32, 32), 3, 3, T3, bars, s=s, one_token_grads=True, floors=True,
+                       floor_kinds=("transformer", "temb"))
 
 
 # ---------------------------------------------------------------------------------------------------- errors
@@ -488,7 +373,7 @@ def test_cond_seq_errors(cuda):
     and the backward return an error status naming both counts; so does a backward whose plan predates a workspace
     re-planned for another count.  Training with an encoding that requires grad: refused."""
     from audio_diffusion_b200 import _lib
-    model, _, _ = _build(cuda, (32, 32), seed=1)
+    model, _, _ = build(PUBLISHED_COND, 1, cuda, (32, 32), train=False)
     x = torch.randn(2, 1, 32, 32).to(cuda)
     t = torch.tensor([10, 500]).to(cuda)
     with pytest.raises(ValueError, match="256"):
@@ -510,7 +395,7 @@ def test_cond_seq_errors(cuda):
     torch.cuda.synchronize()
     with torch.no_grad():
         assert torch.isfinite(model(x, t, e2)["sample"]).all()    # the handle is still usable
-    tm, _, _ = _build(cuda, (32, 32), seed=1, train=True)
+    tm, _, _ = build(PUBLISHED_COND, 1, cuda, (32, 32))
     tm(x, t, e2)["sample"].sum().backward()
     assert tm._fn("set_encoding")(tm._h, e3.data_ptr(), 3) == 0
     g = torch.ones_like(x)

@@ -8,25 +8,10 @@ import math
 import pytest
 import torch
 
+from cases import ONE_TOKEN_ZERO, PUBLISHED_COND, TWO_LEVEL_COND
+from oracle.train_oracle import cond_loss_and_grads
+
 pytestmark = pytest.mark.gpu
-
-ARCH = dict(in_channels=1, out_channels=1, layers_per_block=2, block_out_channels=(128, 256, 512, 512),
-            down_block_types=("CrossAttnDownBlock2D",) * 3 + ("DownBlock2D",),
-            up_block_types=("UpBlock2D",) + ("CrossAttnUpBlock2D",) * 3, cross_attention_dim=100)
-ZERO_GRAD = ("attn2.to_q.weight", "attn2.to_k.weight", "norm2.weight", "norm2.bias")
-
-
-def cond_loss_and_grads(w, cfg, clean, noise, t, enc):
-    """MSE(ε̂, ε) of one conditional training step (scripts/train_unet.py:250-258) and its parameter gradients, by fp32
-    autograd over the oracle."""
-    from oracle.schedulers_oracle import OracleDDPM
-    from oracle.unet_cond_oracle import unet_cond_forward
-    noisy = OracleDDPM().add_noise(clean, noise, t)
-    wl = {k: v.detach().clone().requires_grad_(True) for k, v in w.items()}
-    pred = unet_cond_forward(wl, cfg, noisy, t, enc)
-    loss = torch.mean((pred - noise) ** 2)
-    grads = torch.autograd.grad(loss, list(wl.values()))
-    return loss.detach(), dict(zip(wl.keys(), grads))
 
 
 def _rel_l2(got, ref):
@@ -63,12 +48,7 @@ def test_mha_forward_backward_matches_autograd(cuda, d, hh, ww):
     assert all(e <= 2e-2 for e in errs.values()), errs
 
 
-# two levels, transformers at 32x32 (head_dim 16) in the down and the up block: the scale of test_gpu_train.py's TRAIN_CFG
-SMALL = dict(ARCH, block_out_channels=(128, 256), down_block_types=("CrossAttnDownBlock2D", "DownBlock2D"),
-             up_block_types=("UpBlock2D", "CrossAttnUpBlock2D"))
-
-
-def _build(cuda, size, seed, arch=ARCH):
+def _build(cuda, size, seed, arch=PUBLISHED_COND):
     from audio_diffusion_b200.unet_cond import UNet2DConditionModel
     from oracle.unet_cond_oracle import CondUNetConfig, init_weights
     ocfg = CondUNetConfig(sample_size=size, block_out_channels=arch["block_out_channels"],
@@ -116,7 +96,7 @@ def _check_grads(cuda, size, n, seed):
     bad = [(e, k) for e, k, s, _ in rows if e > 0.10 and s > 1e-3 * gmax]
     assert total <= 3e-2 and not bad, (total, bad[:10])
     named = dict(model.named_parameters())
-    zero = [k for k in named if any(k.endswith(".transformer_blocks.0." + z) for z in ZERO_GRAD)]
+    zero = [k for k in named if any(k.endswith(".transformer_blocks.0." + z) for z in ONE_TOKEN_ZERO)]
     assert len(zero) == 16 * 4
     assert all(torch.count_nonzero(named[k].grad) == 0 for k in zero)
     return model, noisy, t, enc, pred
@@ -175,7 +155,7 @@ def test_cond_two_training_steps_match_oracle(cuda):
         from diffusers.optimization import get_scheduler
     finally:
         sys.path.pop(0)
-    model, ocfg, w = _build(cuda, (32, 32), seed=4, arch=SMALL)
+    model, ocfg, w = _build(cuda, (32, 32), seed=4, arch=TWO_LEVEL_COND)
     w0 = {k: v.clone() for k, v in w.items()}
     opt = FusedAdamW(model.parameters(), lr=1e-4, betas=(0.95, 0.999), weight_decay=1e-6, eps=1e-8, max_grad_norm=1.0)
     ema = EMAModel(model.parameters(), inv_gamma=1.0, power=0.75, max_value=0.9999)

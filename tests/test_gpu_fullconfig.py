@@ -23,15 +23,9 @@ import numpy as np
 import pytest
 import torch
 
-pytestmark = pytest.mark.gpu
+from cases import PUBLISHED, TWO_LEVEL
 
-REF_ARCH = dict(
-    in_channels=1, out_channels=1, layers_per_block=2, block_out_channels=(128, 128, 256, 256, 512, 512),
-    down_block_types=("DownBlock2D",) * 4 + ("AttnDownBlock2D", "DownBlock2D"),
-    up_block_types=("UpBlock2D", "AttnUpBlock2D", "UpBlock2D", "UpBlock2D", "UpBlock2D", "UpBlock2D"))
-SMALL = dict(
-    in_channels=1, out_channels=1, layers_per_block=2, block_out_channels=(128, 256),
-    down_block_types=("DownBlock2D", "AttnDownBlock2D"), up_block_types=("AttnUpBlock2D", "UpBlock2D"))
+pytestmark = pytest.mark.gpu
 
 
 def _build(cuda, arch, size, seed=0):
@@ -60,7 +54,7 @@ def test_unet_reference_arch_256_per_layer(cuda, monkeypatch):
     are 77 % of the FLOPs and the only ones on the W = 256 tiling with the full channel mix), batch 2, vs the fp32 oracle."""
     from oracle.unet_oracle import unet_forward
     monkeypatch.setenv("B200AD_DEBUG_NOPOOL", "1")
-    model, ocfg, w = _build(cuda, REF_ARCH, (256, 256))
+    model, ocfg, w = _build(cuda, PUBLISHED, (256, 256))
     g = torch.Generator().manual_seed(42)
     x = torch.randn(2, 1, 256, 256, generator=g)
     t = torch.tensor([37, 911])
@@ -116,7 +110,7 @@ def test_full_trajectory_reference_arch_64(cuda, kind, steps):
     from audio_diffusion_b200.pipeline import AudioDiffusionPipeline
     from audio_diffusion_b200.schedulers import DDIMScheduler, DDPMScheduler
     from oracle.schedulers_oracle import OracleDDIM, OracleDDPM
-    model, ocfg, w = _build(cuda, REF_ARCH, (64, 64))
+    model, ocfg, w = _build(cuda, PUBLISHED, (64, 64))
     sch, osch = (DDIMScheduler(), OracleDDIM()) if kind == "ddim" else (DDPMScheduler(), OracleDDPM())
     pipe = AudioDiffusionPipeline(vqvae=None, unet=model, mel=Mel(x_res=64, y_res=64, hop_length=1024), scheduler=sch)
     pipe.set_progress_bar_config(disable=True)
@@ -182,7 +176,7 @@ def test_audio_conditioned_inpainting_matches_oracle_loop(cuda, kind):
     from audio_diffusion_b200.mel import Mel
     from audio_diffusion_b200.pipeline import AudioDiffusionPipeline
     from audio_diffusion_b200.schedulers import DDIMScheduler, DDPMScheduler
-    model, ocfg, w = _build(cuda, SMALL, (32, 32), seed=3)
+    model, ocfg, w = _build(cuda, TWO_LEVEL, (32, 32), seed=3)
     mel = Mel(x_res=32, y_res=32, hop_length=512)
     rng = np.random.default_rng(1)
     n = mel.x_res * mel.hop_length * 2

@@ -17,16 +17,11 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from cases import LDM, T3, TWO_LEVEL, TWO_LEVEL_COND, build, draw, w64
 from oracle import block_grads as bg
 
 pytestmark = pytest.mark.gpu
 
-TRAIN_CFG = dict(in_channels=1, out_channels=1, layers_per_block=2, block_out_channels=(128, 256),
-                 down_block_types=("DownBlock2D", "AttnDownBlock2D"), up_block_types=("AttnUpBlock2D", "UpBlock2D"))
-COND_ARCH = dict(in_channels=1, out_channels=1, layers_per_block=2, block_out_channels=(128, 256),
-                 down_block_types=("CrossAttnDownBlock2D", "DownBlock2D"),
-                 up_block_types=("UpBlock2D", "CrossAttnUpBlock2D"), cross_attention_dim=100)
-T3 = [37, 412, 903]
 HEAD_BAR = 1e-4
 K_SPREAD = 4.0
 # end to end, (a, b, c)
@@ -40,37 +35,20 @@ def _unet_case(cuda, seq=None, size=(32, 32)):
     """(model in train(), fp64 weights on the device, oracle forward f(x), noisy sample, timesteps, encoding, noise) with
     the seeds of tests/test_cpu_input_grad.py."""
     from oracle.schedulers_oracle import OracleDDPM
+    from oracle.unet_cond_oracle import unet_cond_forward
+    from oracle.unet_oracle import unet_forward
+    arch, seed = (TWO_LEVEL, 2) if seq is None else (TWO_LEVEL_COND, 3)
+    model, cfg, w = build(arch, seed, cuda, size)
+    clean, noise, enc = draw(3, size, seed, seq)
     t = torch.tensor(T3)
-    if seq is None:
-        from audio_diffusion_b200.unet import UNet2DModel
-        from oracle.unet_oracle import UNetConfig, init_weights, unet_forward
-        cfg = UNetConfig(sample_size=size, **TRAIN_CFG)
-        w = init_weights(cfg, seed=2)
-        model = UNet2DModel(sample_size=size, **TRAIN_CFG)
-        g = torch.Generator().manual_seed(3)
-        enc = None
-    else:
-        from audio_diffusion_b200.unet_cond import UNet2DConditionModel
-        from oracle.unet_cond_oracle import CondUNetConfig, init_weights, unet_cond_forward
-        cfg = CondUNetConfig(sample_size=size, block_out_channels=COND_ARCH["block_out_channels"],
-                             down_block_types=COND_ARCH["down_block_types"], up_block_types=COND_ARCH["up_block_types"])
-        w = init_weights(cfg, seed=3)
-        model = UNet2DConditionModel(sample_size=size, **COND_ARCH)
-        g = torch.Generator().manual_seed(4)
-    clean = torch.rand(3, 1, *size, generator=g) * 2 - 1
-    noise = torch.randn(3, 1, *size, generator=g)
-    if seq is not None:
-        enc = torch.randn(3, seq, 100, generator=g).to(cuda)
     noisy = OracleDDPM().add_noise(clean, noise, t).to(cuda)
-    model.load_state_dict(w)
-    model = model.to(cuda).train()
-    w64 = {k: v.to(device=cuda, dtype=torch.float64) for k, v in w.items()}
-    tc = t.to(cuda)
+    wd, tc = w64(w, cuda), t.to(cuda)
     if seq is None:
-        f = lambda x: unet_forward(w64, cfg, x, tc)
+        f = lambda x: unet_forward(wd, cfg, x, tc)
     else:
-        f = lambda x: unet_cond_forward(w64, cfg, x, tc, enc.double())
-    return model, w64, f, noisy, tc, enc, noise.to(cuda)
+        enc = enc.to(cuda)
+        f = lambda x: unet_cond_forward(wd, cfg, x, tc, enc.double())
+    return model, wd, f, noisy, tc, enc, noise.to(cuda)
 
 
 def _call(model, x, t, enc):
@@ -89,20 +67,11 @@ def _sample_grad(model, x, t, enc, noise):
 
 
 def _vae(cuda, max_batch=2):
-    from audio_diffusion_b200.vae import AutoencoderKL
-    from oracle import vae_oracle as vo
-    cfg = vo.VAEConfig()
-    w = vo.init_weights(cfg, seed=0)
-    nb = len(cfg.block_out_channels)
-    model = AutoencoderKL(in_channels=1, out_channels=1, down_block_types=("DownEncoderBlock2D",) * nb,
-                          up_block_types=("UpDecoderBlock2D",) * nb, block_out_channels=cfg.block_out_channels,
-                          layers_per_block=cfg.layers_per_block, latent_channels=1, max_batch=max_batch)
-    model.load_state_dict(w)
+    model, cfg, w = build(LDM, 0, cuda, max_batch=max_batch)
     g = torch.Generator().manual_seed(1)
     x = torch.randn(2, 1, 64, 64, generator=g).clamp(-1, 1).to(cuda)
     gm = torch.randn(2, 2, 8, 8, generator=g).to(cuda)
-    w64 = {k: v.to(device=cuda, dtype=torch.float64) for k, v in w.items()}
-    return model.to(cuda).train(), w64, cfg, x, gm
+    return model, w64(w, cuda), cfg, x, gm
 
 
 def _image_grad(vae, x, gm):

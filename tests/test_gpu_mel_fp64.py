@@ -53,8 +53,8 @@ import pytest
 import scipy.fft
 import torch
 
+from blockcheck import power_limit
 from oracle import mel_oracle as mo
-from test_gpu_block_forward import _power_limit
 
 pytestmark = pytest.mark.gpu
 
@@ -171,7 +171,7 @@ def _decode(cfg, images, dev, n_iter):
 
 
 def _header(name):
-    print(f"\n{name} on {torch.cuda.get_device_properties(0).name} ({_power_limit()})")
+    print(f"\n{name} on {torch.cuda.get_device_properties(0).name} ({power_limit()})")
 
 
 @pytest.mark.parametrize("cfg", CONFIGS, ids=CFG_IDS)

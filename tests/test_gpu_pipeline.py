@@ -7,19 +7,17 @@ import numpy as np
 import pytest
 import torch
 
-pytestmark = pytest.mark.gpu
+from cases import TWO_LEVEL
 
-SMALL = dict(
-    in_channels=1, out_channels=1, layers_per_block=2, block_out_channels=(128, 256),
-    down_block_types=("DownBlock2D", "AttnDownBlock2D"), up_block_types=("AttnUpBlock2D", "UpBlock2D"))
+pytestmark = pytest.mark.gpu
 
 
 def _models(cuda, seed=0):
     from audio_diffusion_b200.unet import UNet2DModel
     from oracle.unet_oracle import UNetConfig, init_weights
-    ocfg = UNetConfig(sample_size=(32, 32), **SMALL)
+    ocfg = UNetConfig(sample_size=(32, 32), **TWO_LEVEL)
     w = init_weights(ocfg, seed=seed)
-    m = UNet2DModel(sample_size=(32, 32), **SMALL)
+    m = UNet2DModel(sample_size=(32, 32), **TWO_LEVEL)
     m.load_state_dict(w)
     return m.to(cuda), ocfg, w
 
@@ -161,9 +159,9 @@ def _latent_pipe(cuda, sch):
     from oracle.unet_oracle import UNetConfig, init_weights
     from oracle.vae_oracle import VAEConfig
     from oracle.vae_oracle import init_weights as vae_init
-    ocfg = UNetConfig(sample_size=(8, 8), **SMALL)
+    ocfg = UNetConfig(sample_size=(8, 8), **TWO_LEVEL)
     w = init_weights(ocfg, seed=5)
-    unet = UNet2DModel(sample_size=(8, 8), **SMALL)
+    unet = UNet2DModel(sample_size=(8, 8), **TWO_LEVEL)
     unet.load_state_dict(w)
     vcfg = VAEConfig()
     vw = vae_init(vcfg, seed=6)
@@ -229,8 +227,8 @@ def test_golden_reference_driven_images(cuda):
     from audio_diffusion_b200.unet import UNet2DModel
     from oracle.unet_oracle import UNetConfig, init_weights
     z = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "pipeline_ddpm_small.npz"))
-    w = init_weights(UNetConfig(sample_size=(32, 32), **SMALL), seed=int(z["weight_seed"]))
-    m = UNet2DModel(sample_size=(32, 32), **SMALL)
+    w = init_weights(UNetConfig(sample_size=(32, 32), **TWO_LEVEL), seed=int(z["weight_seed"]))
+    m = UNet2DModel(sample_size=(32, 32), **TWO_LEVEL)
     m.load_state_dict(w)
     pipe = AudioDiffusionPipeline(vqvae=None, unet=m.to(cuda), mel=Mel(x_res=32, y_res=32, hop_length=512, n_iter=2),
                                   scheduler=DDPMScheduler())

@@ -4,6 +4,8 @@ relative (fused multiply-adds and the order of the gradient-norm reduction diffe
 import pytest
 import torch
 
+from cases import TWO_LEVEL
+
 pytestmark = pytest.mark.gpu
 
 
@@ -57,10 +59,6 @@ def test_mse_loss_grad(cuda):
     assert torch.allclose(grad.cpu(), p.grad, rtol=1e-6, atol=1e-9)
 
 
-TRAIN_CFG = dict(in_channels=1, out_channels=1, layers_per_block=2, block_out_channels=(128, 256),
-                 down_block_types=("DownBlock2D", "AttnDownBlock2D"), up_block_types=("AttnUpBlock2D", "UpBlock2D"))
-
-
 def _grad_report(model, grads_ref):
     rows = []
     num = den = 0.0
@@ -85,9 +83,9 @@ def test_unet_backward_matches_autograd(cuda):
     from oracle.schedulers_oracle import OracleDDPM
     from oracle.train_oracle import loss_and_grads
     from oracle.unet_oracle import UNetConfig, init_weights
-    ocfg = UNetConfig(sample_size=(32, 32), **TRAIN_CFG)
+    ocfg = UNetConfig(sample_size=(32, 32), **TWO_LEVEL)
     w = init_weights(ocfg, seed=2)
-    model = UNet2DModel(sample_size=(32, 32), **TRAIN_CFG)
+    model = UNet2DModel(sample_size=(32, 32), **TWO_LEVEL)
     model.load_state_dict(w)
     model = model.to(cuda).train()
     g = torch.Generator().manual_seed(3)
@@ -131,10 +129,10 @@ def test_two_training_steps_match_oracle(cuda):
         from diffusers.optimization import get_scheduler
     finally:
         sys.path.pop(0)
-    ocfg = UNetConfig(sample_size=(32, 32), **TRAIN_CFG)
+    ocfg = UNetConfig(sample_size=(32, 32), **TWO_LEVEL)
     w = init_weights(ocfg, seed=4)
     w0 = {k: v.clone() for k, v in w.items()}
-    model = UNet2DModel(sample_size=(32, 32), **TRAIN_CFG)
+    model = UNet2DModel(sample_size=(32, 32), **TWO_LEVEL)
     model.load_state_dict(w)
     model = model.to(cuda).train()
     opt = FusedAdamW(model.parameters(), lr=1e-4, betas=(0.95, 0.999), weight_decay=1e-6, eps=1e-8, max_grad_norm=1.0)
@@ -214,7 +212,7 @@ def test_ema_copy_to_refreshes_packed_weights(cuda):
     that the parameters changed (its bf16-packed copy is keyed on parameter versions)."""
     from audio_diffusion_b200.training import EMAModel
     from audio_diffusion_b200.unet import UNet2DModel
-    m = UNet2DModel(sample_size=(32, 32), seed=1, **TRAIN_CFG).to(cuda)
+    m = UNet2DModel(sample_size=(32, 32), seed=1, **TWO_LEVEL).to(cuda)
     x = torch.randn(1, 1, 32, 32, generator=torch.Generator().manual_seed(0)).to(cuda)
     with torch.no_grad():
         a = m(x, 10)["sample"].clone()
@@ -230,7 +228,7 @@ def test_gradient_accumulation_equals_full_batch(cuda):
     """`accelerator.accumulate(model)` (scripts/train_unet.py:252): two micro-batches with loss / 2 each, gradients left in
     place between the backward calls, give the gradient of the full batch (GroupNorm is per sample)."""
     from audio_diffusion_b200.unet import UNet2DModel
-    model = UNet2DModel(sample_size=(32, 32), seed=3, **TRAIN_CFG).to(cuda).train()
+    model = UNet2DModel(sample_size=(32, 32), seed=3, **TWO_LEVEL).to(cuda).train()
     g = torch.Generator().manual_seed(6)
     x = torch.randn(2, 1, 32, 32, generator=g).to(cuda)
     tgt = torch.randn(2, 1, 32, 32, generator=g).to(cuda)
@@ -252,7 +250,7 @@ def test_backward_after_second_forward_is_refused(cuda):
     would silently give wrong gradients, so the engine refuses (ADVICE r1)."""
     from audio_diffusion_b200._lib import B200ADError
     from audio_diffusion_b200.unet import UNet2DModel
-    model = UNet2DModel(sample_size=(32, 32), seed=3, **TRAIN_CFG).to(cuda).train()
+    model = UNet2DModel(sample_size=(32, 32), seed=3, **TWO_LEVEL).to(cuda).train()
     x = torch.randn(2, 1, 32, 32, generator=torch.Generator().manual_seed(1)).to(cuda)
     t = torch.tensor([10, 500]).to(cuda)
     first = model(x, t)["sample"]

@@ -9,11 +9,9 @@ import os
 import pytest
 import torch
 
-pytestmark = pytest.mark.gpu
+from cases import TWO_LEVEL
 
-SMALL = dict(
-    in_channels=1, out_channels=1, layers_per_block=2, block_out_channels=(128, 256),
-    down_block_types=("DownBlock2D", "AttnDownBlock2D"), up_block_types=("AttnUpBlock2D", "UpBlock2D"))
+pytestmark = pytest.mark.gpu
 
 
 def _build(cuda, cfg_kwargs, sample_size, seed=0):
@@ -40,7 +38,7 @@ def test_unet_small_layers(cuda):
     from oracle.unet_oracle import unet_forward
     os.environ["B200AD_DEBUG_NOPOOL"] = "1"
     try:
-        model, ocfg, w = _build(cuda, SMALL, (32, 32))
+        model, ocfg, w = _build(cuda, TWO_LEVEL, (32, 32))
         g = torch.Generator().manual_seed(42)
         x = torch.randn(2, 1, 32, 32, generator=g)
         t = torch.tensor([17, 801])
@@ -67,7 +65,7 @@ def test_unet_small_layers(cuda):
 def test_unet_small_pooled_matches(cuda):
     """Buffer pooling must not change results; scalar timestep broadcast (pipeline_audio_diffusion.py:163)."""
     from oracle.unet_oracle import unet_forward
-    model, ocfg, w = _build(cuda, SMALL, (32, 32), seed=1)
+    model, ocfg, w = _build(cuda, TWO_LEVEL, (32, 32), seed=1)
     g = torch.Generator().manual_seed(7)
     x = torch.randn(3, 1, 32, 32, generator=g)
     ref = unet_forward(w, ocfg, x, torch.tensor(999))
