@@ -173,10 +173,27 @@ class UNet2DModel(EngineModel):
         return t.contiguous()
 
     def _check_input(self, sample: torch.Tensor) -> torch.Tensor:
+        """The sample as the library reads it; refuses one that is not (N, in_channels, H, W), whose planes conv_in
+        would read past."""
         _lib.require_cuda()
         if sample.device.type != "cuda":
             raise self._err("input must be a CUDA tensor (no CPU fallback)")
+        if sample.dim() != 4 or sample.shape[1] != self.in_channels:
+            raise ValueError(f"{type(self).__name__}(b200): sample must be (N, {self.in_channels}, H, W), "
+                             f"got {tuple(sample.shape)}")
         return sample.to(torch.float32).contiguous()
+
+    def _check_step(self, x: torch.Tensor, name: str, t: Optional[torch.Tensor]) -> None:
+        """Refuses a fused step the scheduler update cannot write in place of the sample: eps with other planes than the
+        sample, or a noise / output tensor `t` (None: not given) of another shape, dtype, layout or device than x."""
+        if self.out_channels != self.in_channels:
+            raise ValueError(f"{type(self).__name__}(b200): a fused scheduler step needs out_channels == in_channels, "
+                             f"got {self.out_channels} and {self.in_channels}")
+        if t is not None and (t.shape != x.shape or t.device != x.device
+                              or (name == "out" and (t.dtype != torch.float32 or not t.is_contiguous()))):
+            raise ValueError(f"{type(self).__name__}(b200): {name} must be a {'contiguous fp32 ' if name == 'out' else ''}"
+                             f"tensor of the sample's shape {tuple(x.shape)} on {x.device}, got {tuple(t.shape)} "
+                             f"{t.dtype} on {t.device}")
 
     def _encoding(self, enc, n: int, dev) -> Optional[torch.Tensor]:
         """The conditional model's validated encoding; None here."""
@@ -257,6 +274,8 @@ class UNet2DModel(EngineModel):
     def _forward_step(self, sample: torch.Tensor, timestep, coef: StepCoefC, enc, noise: Optional[torch.Tensor],
                       out: Optional[torch.Tensor], want_eps: bool):
         x = self._check_input(sample)
+        self._check_step(x, "noise", noise)
+        self._check_step(x, "out", out)
         n, _, hh, ww = x.shape
         with torch.cuda.device(x.device):
             self._fwd_gen[0] += 1
@@ -278,6 +297,7 @@ class UNet2DModel(EngineModel):
         from `sample`) and is cached per shape, so repeated pipeline calls re-use one captured graph as long as the model
         stays bound the same way (weights, batch, mode)."""
         x = self._check_input(sample)
+        self._check_step(x, "sample", None)
         n, _, hh, ww = x.shape
         cache = self.__dict__.setdefault("_steppers", {})
         key = (tuple(x.shape), x.device)
@@ -339,6 +359,9 @@ class GraphStepper:
         m = self.model
         if (m._packed_key, m._ws_key) != self._bound:
             raise _lib.B200ADError("GraphStepper: the model was re-bound (weights, batch or mode changed) after the capture")
+        if noise is not None and noise.shape != self.x.shape:     # copy_ would broadcast it
+            raise ValueError(f"GraphStepper: noise must have the sample's shape {tuple(self.x.shape)}, "
+                             f"got {tuple(noise.shape)}")
         c = StepCoefC(coef.sqrt_1m_at, coef.inv_sqrt_at, coef.clip, coef.c_x0, coef.c_xt, coef.c_eps,
                       coef.c_z if noise is not None else 0.0, coef.do_clip)
         with torch.cuda.device(self.x.device):

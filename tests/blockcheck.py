@@ -1,8 +1,9 @@
 """How the per-block fp64 checks compare: every block of the engine's forward or backward against the fp64 reference of
 that one block (oracle/block_grads.py) on the engine's own inputs, one table row per block, the bars against the bf16
 floors measured from the oracle's activations, and the fp64 time and peak device memory of the comparison.  The drivers
-run one case of tests/test_gpu_block_backward*.py, tests/test_gpu_block_forward.py and tests/test_gpu_cond_seq.py each,
-with the architectures, builders and seeded inputs of tests/cases.py."""
+run one case of tests/test_gpu_block_backward*.py, tests/test_gpu_block_forward.py, tests/test_gpu_latent_unet.py and
+tests/test_gpu_cond_seq.py each, with the architectures, builders and seeded inputs of tests/cases.py; check_fused_step
+is the fused scheduler update's fp64 check."""
 import time
 
 import torch
@@ -292,7 +293,7 @@ def forward_case(cuda, monkeypatch, arch, size, n, seed, bars, t=None, s=None, s
             floors.update(bg.forward_floors(blocks, otaps, inp.double(), w64, cfg, prefix=part + ":"))
         check_against_floors(f"AutoencoderKL {size[0]}x{size[1]} batch {n}", rows, floors, bars, t0)
         return None
-    x = torch.randn(n, 1, *size, generator=g).to(cuda)
+    x = torch.randn(n, arch.get("in_channels", 1), *size, generator=g).to(cuda)
     enc = None if s is None else torch.randn(n, s, 100, generator=g).to(cuda)
     t = torch.tensor(t, dtype=torch.float32, device=cuda)
     with torch.no_grad():
@@ -322,3 +323,34 @@ def forward_case(cuda, monkeypatch, arch, size, n, seed, bars, t=None, s=None, s
             + (f", {s} tokens" if s and s > 1 else "") + ("" if sel is None else f", samples {sel}"))
     check_against_floors(name, rows, floors, bars, t0)
     return x, t, w, eps
+
+
+def pooled_eps(cuda, arch, w, size, x, t):
+    """eps of the same input through a UNet2DModel of `arch` with pooled activation buffers (the default), twice."""
+    from audio_diffusion_b200.unet import UNet2DModel
+    model = UNet2DModel(sample_size=size, **arch)
+    model.load_state_dict(w)
+    model = model.to(cuda).eval()
+    with torch.no_grad():
+        return model(x, t)["sample"], model(x, t)["sample"]
+
+
+# ---------------------------------------------------------------------------------------------------- fused step
+def check_fused_step(c, x, eps, x_out, z=None):
+    """x_out of a fused scheduler step against the fp64 update of b200ad_step_coef's formula (include/b200ad.h) on the
+    engine's own eps and the same noise z: the kernel evaluates it in six fp32 operations, so each element may differ by
+    at most 8 fp32 roundings (8 * 2^-24) of the sum of its terms' magnitudes.  Asserts that bar on every channel plane;
+    returns (the largest error over its bar per plane, the fraction of elements whose x0 the clip reaches)."""
+    xd, ed = x.double(), eps.double()
+    x0 = (xd - c.sqrt_1m_at * ed) * c.inv_sqrt_at
+    clipped = (x0.abs() > c.clip).double().mean().item()
+    if c.do_clip:
+        x0 = x0.clamp(-c.clip, c.clip)
+    ref = c.c_x0 * x0 + c.c_xt * xd + c.c_eps * ed
+    mag = abs(c.c_x0) * c.inv_sqrt_at * (xd.abs() + c.sqrt_1m_at * ed.abs()) + abs(c.c_xt) * xd.abs() + abs(c.c_eps) * ed.abs()
+    if z is not None:
+        ref = ref + c.c_z * z.double()
+        mag = mag + abs(c.c_z) * z.double().abs()
+    ratio = ((x_out.double() - ref).abs() / (8 * 2.0 ** -24 * mag + 1e-30)).amax(dim=(0, 2, 3)).tolist()
+    assert max(ratio) <= 1.0, ratio
+    return ratio, clipped

@@ -7,6 +7,8 @@ import torch
 PUBLISHED = dict(in_channels=1, out_channels=1, layers_per_block=2, block_out_channels=(128, 128, 256, 256, 512, 512),
                  down_block_types=("DownBlock2D",) * 4 + ("AttnDownBlock2D", "DownBlock2D"),
                  up_block_types=("UpBlock2D", "AttnUpBlock2D", "UpBlock2D", "UpBlock2D", "UpBlock2D", "UpBlock2D"))
+# the same U-Net over a hub VAE's four latent channels (scripts/train_unet.py --vae: in = out = latent_channels)
+PUBLISHED4 = dict(PUBLISHED, in_channels=4, out_channels=4)
 # scripts/train_unet.py's UNet2DConditionModel (--encodings): transformers in three down and three up blocks
 PUBLISHED_COND = dict(in_channels=1, out_channels=1, layers_per_block=2, block_out_channels=(128, 256, 512, 512),
                       down_block_types=("CrossAttnDownBlock2D",) * 3 + ("DownBlock2D",),
@@ -71,12 +73,12 @@ def w64(w, dev):
     return {k: v.to(device=dev, dtype=torch.float64) for k, v in w.items()}
 
 
-def draw(n, size, seed, s=None):
-    """The seeded inputs of a training step on weights of `seed`: clean images in [-1, 1), the noise and (s tokens) an
-    encoding, drawn in that order from Generator(seed + 1)."""
+def draw(n, size, seed, s=None, c=1):
+    """The seeded inputs of a training step on weights of `seed`: clean c-channel images in [-1, 1), the noise and (s
+    tokens) an encoding, drawn in that order from Generator(seed + 1)."""
     g = torch.Generator().manual_seed(seed + 1)
-    clean = torch.rand(n, 1, *size, generator=g) * 2 - 1
-    noise = torch.randn(n, 1, *size, generator=g)
+    clean = torch.rand(n, c, *size, generator=g) * 2 - 1
+    noise = torch.randn(n, c, *size, generator=g)
     enc = None if s is None else torch.randn(n, s, 100, generator=g)
     return clean, noise, enc
 

@@ -14,8 +14,8 @@ import pytest
 import torch
 
 from blockcheck import bar_in_range
-from cases import (COND_BARS, LDM, PUBLISHED, PUBLISHED_ATTN, PUBLISHED_COND, T3, TWO_LEVEL, TWO_LEVEL_COND, UNET_BARS,
-                   VAE_BARS, draw, oracle_config)
+from cases import (COND_BARS, LDM, PUBLISHED, PUBLISHED4, PUBLISHED_ATTN, PUBLISHED_COND, T3, TWO_LEVEL, TWO_LEVEL_COND,
+                   UNET_BARS, VAE_BARS, draw, oracle_config)
 from oracle import block_grads as bg
 
 
@@ -40,7 +40,7 @@ def _unet_case(size, n, seed, arch=TWO_LEVEL):
     from oracle.unet_oracle import init_weights, unet_forward
     cfg = oracle_config(arch, size)
     w = _d(init_weights(cfg, seed=seed))
-    clean, noise, _ = draw(n, size, seed)
+    clean, noise, _ = draw(n, size, seed, c=arch["in_channels"])
     clean, noise = clean.double(), noise.double()
     t = torch.tensor(T3[:n])
     noisy = OracleDDPM().add_noise(clean, noise, t)
@@ -99,6 +99,33 @@ def test_published_unet_block_chain_reproduces_autograd():
     assert sum(b.skip is not None for b in blocks) == 6 * 3
     _, grads, _ = bg.chain(blocks, taps, noisy, g_eps, w, cfg, taps["temb_act"], t=t)
     _check_params(grads, ref, list(w))
+
+
+# the attention parameters whose gradients are exactly zero over one token: the softmax over one key is 1 whatever the
+# scores, so no gradient reaches q or k (to_k.bias never gets one: the softmax is invariant to it)
+ONE_TOKEN_ATTN_ZERO = ("to_q.weight", "to_q.bias", "to_k.weight")
+
+
+@pytest.mark.timeout(300)
+@pytest.mark.parametrize("arch", [PUBLISHED, PUBLISHED4], ids=["1ch", "4ch"])
+def test_published_unet_32_block_chain_reproduces_autograd(arch):
+    """The six-level UNet2DModel at its 32x32 latent, with 1 and with 4 latent channels: the 1x1 bottom level (down block
+    5, the mid block, up block 0), the stride-2 conv from 2x2 to 1x1 and the upsample from 1x1 to 2x2.  The mid block
+    attends over one token, so its q and k gradients are exactly zero in fp64, in autograd and in the block chain; the
+    2x2 attention blocks' are not."""
+    from oracle.train_oracle import loss_and_grads
+    cfg, w, clean, noise, t, noisy, taps, g_eps = _unet_case((32, 32), 2, 2, arch)
+    _, ref, _ = loss_and_grads(w, cfg, clean, noise, t)
+    blocks = bg.unet_blocks(cfg)
+    assert [b.name for b in blocks if b.kind == "attn"] == PUBLISHED_ATTN
+    assert taps["mid_block.attentions.0"].shape[2:] == (1, 1)
+    _, grads, _ = bg.chain(blocks, taps, noisy, g_eps, w, cfg, taps["temb_act"], t=t)
+    _check_params(grads, ref, list(w))
+    for blk in PUBLISHED_ATTN:
+        for k in ONE_TOKEN_ATTN_ZERO:
+            zero = blk == "mid_block.attentions.0"
+            for g in (ref[f"{blk}.{k}"], grads[f"{blk}.{k}"]):
+                assert (torch.count_nonzero(g) == 0) == zero, (blk, k)
 
 
 @pytest.mark.timeout(300)

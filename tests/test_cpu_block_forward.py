@@ -12,7 +12,7 @@ tests/test_gpu_block_forward.py.
 import pytest
 import torch
 
-from cases import PUBLISHED, PUBLISHED_COND, T3, oracle_config
+from cases import PUBLISHED, PUBLISHED4, PUBLISHED_COND, T3, oracle_config
 from oracle import block_grads as bg
 
 
@@ -62,6 +62,35 @@ def test_published_unet_block_forward_chain():
     eps = unet_forward(w, cfg, x, t, taps)
     blocks = bg.unet_blocks(cfg)
     assert sum(blk.kind == "attn" for blk in blocks) == 6
+    _chain(blocks, x, w, cfg, taps, eps, taps["temb_act"])
+
+
+@pytest.mark.timeout(300)
+@pytest.mark.parametrize("arch", [PUBLISHED, PUBLISHED4], ids=["1ch", "4ch"])
+def test_published_unet_32_block_forward_chain(arch):
+    """The six-level UNet2DModel at its 32x32 latent (scripts/train_unet.py --vae), with 1 and with 4 latent channels:
+    the levels run 32, 16, 8, 4, 2, 1, the attention blocks sit at 2x2 (down block 4, up block 1) and at 1x1 (the mid
+    block), and the chain reaches the 1x1 bottom level, its one-token attention and the 4-plane head and tail."""
+    from oracle.unet_oracle import init_weights, unet_forward
+    cfg = oracle_config(arch, (32, 32))
+    w = _d(init_weights(cfg, seed=2))
+    c = arch["in_channels"]
+    x = torch.randn(2, c, 32, 32, generator=torch.Generator().manual_seed(3)).double()
+    t = torch.tensor(T3[:2])
+    taps = {}
+    eps = unet_forward(w, cfg, x, t, taps)
+    assert eps.shape == x.shape
+    blocks = bg.unet_blocks(cfg)
+    hw = {b.name: taps[b.out].shape[2] for b in blocks if b.out is not None}
+    assert sorted(set(hw.values()), reverse=True) == [32, 16, 8, 4, 2, 1]
+    assert all(taps[b.out].shape[2:] == (h, h) for b in blocks if b.out is not None for h in [hw[b.name]])
+    attn = {b.name: hw[b.name] for b in blocks if b.kind == "attn"}
+    assert attn == {"down_blocks.4.attentions.0": 2, "down_blocks.4.attentions.1": 2, "mid_block.attentions.0": 1,
+                    **{f"up_blocks.1.attentions.{j}": 2 for j in range(3)}}, attn
+    assert {b.name for b in blocks if hw.get(b.name) == 1} == {
+        "down_blocks.4.downsamplers.0.conv", "down_blocks.5.resnets.0", "down_blocks.5.resnets.1",
+        "mid_block.resnets.0", "mid_block.attentions.0", "mid_block.resnets.1",
+        "up_blocks.0.resnets.0", "up_blocks.0.resnets.1", "up_blocks.0.resnets.2"}
     _chain(blocks, x, w, cfg, taps, eps, taps["temb_act"])
 
 

@@ -26,7 +26,7 @@ and that each bar lies in (floor, 3.3 x floor].
 import pytest
 import torch
 
-from blockcheck import forward_case
+from blockcheck import check_fused_step, forward_case, pooled_eps
 from cases import LDM, PUBLISHED, PUBLISHED_COND
 from oracle import block_grads as bg
 
@@ -114,16 +114,6 @@ VAE256_BARS = {
 }
 
 
-def _pooled_eps(cuda, w, size, x, t):
-    """eps of the same input through a model with pooled activation buffers (the default), twice."""
-    from audio_diffusion_b200.unet import UNet2DModel
-    model = UNet2DModel(sample_size=size, **PUBLISHED)
-    model.load_state_dict(w)
-    model = model.to(cuda).eval()
-    with torch.no_grad():
-        return model(x, t)["sample"], model(x, t)["sample"]
-
-
 @pytest.mark.timeout(1200)
 def test_unet_256_batch64_forward_per_block(cuda, monkeypatch):
     """The published UNet2DModel at 256x256, batch 64 (the benchmarked shape: the conv planner's 8x32 and 16x16 tiles and
@@ -139,7 +129,7 @@ def test_unet_256_batch64_forward_per_block(cuda, monkeypatch):
     x, tt, w, eps = forward_case(cuda, monkeypatch, PUBLISHED, (256, 256), 64, 11, UNET256_BARS, t=t, sel=sel)
     monkeypatch.delenv("B200AD_DEBUG_NOPOOL")
     torch.cuda.empty_cache()
-    e1, e2 = _pooled_eps(cuda, w, (256, 256), x, tt)
+    e1, e2 = pooled_eps(cuda, PUBLISHED, w, (256, 256), x, tt)
     spread = (e1 - e2).abs().max().item()
     diff = (e1 - eps).abs().max().item()
     print(f"pooled vs unpooled eps: max |diff| {diff:.3e}; two pooled runs: {spread:.3e}")
@@ -189,9 +179,8 @@ def test_vae_256_forward_per_block(cuda, monkeypatch):
 def test_fused_step_256_batch64(cuda, kind):
     """The fused scheduler update of conv_out at the benchmarked shape (256x256, batch 64, pooled buffers): one DDPM step
     with noise at t = 999, where the x0 clip is active, and one DDIM step (eta = 0, 50 steps, t = 980).
-    x_out against the fp64 update of b200ad_step_coef's formula (include/b200ad.h) on the engine's own eps and the same z:
-    the kernel evaluates it in six fp32 operations, so each element may differ by at most 8 fp32 roundings
-    (8 * 2^-24) of the sum of its terms' magnitudes.  eps of the fused step against model(x, t) on the same input: equal,
+    x_out against the fp64 update on the engine's own eps and the same z, within 8 fp32 roundings of the sum of its
+    terms' magnitudes (blockcheck.check_fused_step).  eps of the fused step against model(x, t) on the same input: equal,
     or within what two identical model(x, t) calls differ by.  Measured on an H100 80GB HBM3 at 700 W: x0 clipped for
     99.6 % (DDPM) and 99.5 % (DDIM) of the elements; the largest error 0.24 and 0.16 of its bar; eps bit-identical to
     model(x, t), and two model(x, t) calls bit-identical."""
@@ -209,22 +198,11 @@ def test_fused_step_256_batch64(cuda, kind):
     with torch.no_grad():
         x_out, eps = model.forward_step(x, t, c, noise=z, want_eps=True)
         e1, e2 = model(x, t)["sample"], model(x, t)["sample"]
-    xd, ed = x.double(), eps.double()
-    x0 = (xd - c.sqrt_1m_at * ed) * c.inv_sqrt_at
-    clipped = (x0.abs() > c.clip).double().mean().item()
-    if c.do_clip:
-        x0 = x0.clamp(-c.clip, c.clip)
-    ref = c.c_x0 * x0 + c.c_xt * xd + c.c_eps * ed
-    mag = abs(c.c_x0) * c.inv_sqrt_at * (xd.abs() + c.sqrt_1m_at * ed.abs()) + abs(c.c_xt) * xd.abs() + abs(c.c_eps) * ed.abs()
-    if z is not None:
-        ref = ref + c.c_z * z.double()
-        mag = mag + abs(c.c_z) * z.double().abs()
-    ratio = ((x_out.double() - ref).abs() / (8 * 2.0 ** -24 * mag + 1e-30)).max().item()
+    ratio, clipped = check_fused_step(c, x, eps, x_out, z)
     spread = (e1 - e2).abs().max().item()
     diff = (eps - e1).abs().max().item()
-    print(f"\n{kind} t={t}: x0 clipped for {clipped:.1%} of the elements; max |x_out - ref| / bar {ratio:.3f}; "
+    print(f"\n{kind} t={t}: x0 clipped for {clipped:.1%} of the elements; max |x_out - ref| / bar {ratio[0]:.3f}; "
           f"eps vs model(x, t) {diff:.3e}, two model(x, t) calls {spread:.3e}")
     if kind == "ddpm":
         assert clipped > 0.05
-    assert ratio <= 1.0, ratio
     assert diff <= spread, (diff, spread)

@@ -1,4 +1,5 @@
-"""GPU parity of single kernels (through the C ABI) against plain PyTorch fp32 on the CPU.
+"""GPU parity of single kernels (through the C ABI) against plain PyTorch on the CPU (fp64 for the conv, folded-upsample
+and GroupNorm kernels, fp32 for the others).
 
 Tolerances: operands are rounded to bf16 on both sides, accumulation is fp32, the kernel stores bf16
 (relative rounding 2^-9), so |err| <= 1.5e-2 * max|ref| is the stated per-op bound.
@@ -26,11 +27,11 @@ def _conv(cuda, N, cin, cout, H, W, K, stride, temb=False, res=False, seed=0):
     te = torch.randn(N, cout, generator=g) if temb else None
     Ho, Wo = H // stride, W // stride
     r = _bf(torch.randn(N, cout, Ho, Wo, generator=g)) if res else None
-    ref = F.conv2d(x, w, b, stride=stride, padding=K // 2)
+    ref = F.conv2d(x.double(), w.double(), b.double(), stride=stride, padding=K // 2)
     if temb:
-        ref = ref + te[:, :, None, None]
+        ref = ref + te[:, :, None, None].double()
     if res:
-        ref = ref + r
+        ref = ref + r.double()
     d = lambda t: t.to(cuda).contiguous() if t is not None else None
     xd, wd, bd, ted, rd = d(x), d(w), d(b), d(te), d(r)
     y = torch.empty(N, cout, Ho, Wo, device=cuda)
@@ -71,6 +72,12 @@ def test_conv3x3_stride2_to_small_images(cuda):
     _conv(cuda, 6, 128, 128, 8, 8, 3, 2, seed=10)
 
 
+@pytest.mark.parametrize("N", [128, 5])
+def test_conv3x3_stride2_2x2_to_1x1(cuda, N):
+    """The latent U-Net's last downsampler (32x32 latent: 2x2 -> 1x1, 512 channels): one real tap per output pixel."""
+    _conv(cuda, N, 512, 512, 2, 2, 3, 2, seed=N)
+
+
 def test_conv3x3_wide(cuda):
     _conv(cuda, 2, 128, 128, 8, 128, 3, 1)
     _conv(cuda, 1, 64, 128, 12, 256, 3, 1, seed=3)
@@ -92,19 +99,28 @@ def test_conv3x3_stride2(cuda):
 
 @pytest.mark.parametrize("silu", [0, 1])
 def test_group_norm(cuda, silu):
+    _group_norm(cuda, 2, 384, 16, 16, silu)
+
+
+@pytest.mark.parametrize("N", [128, 5])
+def test_group_norm_1x1(cuda, N):
+    """The latent U-Net's 1x1 bottom level: each group is 16 channels of one pixel."""
+    _group_norm(cuda, N, 512, 1, 1, 1)
+
+
+def _group_norm(cuda, N, Cc, H, W, silu):
     from audio_diffusion_b200 import _lib
     L = _lib.lib()
     g = torch.Generator().manual_seed(1)
-    N, Cc, H, W = 2, 384, 16, 16
     x = _bf(torch.randn(N, Cc, H, W, generator=g) * 2 + 0.5)
     gamma = torch.randn(Cc, generator=g)
     beta = torch.randn(Cc, generator=g)
-    ref = F.group_norm(x, 32, gamma, beta, 1e-5)
+    ref = F.group_norm(x.double(), 32, gamma.double(), beta.double(), 1e-5)
     if silu:
         ref = F.silu(ref)
     xd, gd, bd = x.to(cuda), gamma.to(cuda), beta.to(cuda)
     y = torch.empty_like(xd)
-    nb = 1 << 26
+    nb = 1 << 28     # the padded planes of 128 1x1 images need 134 MiB
     scratch = torch.empty(nb, dtype=torch.uint8, device=cuda)
     _lib.check(L.b200ad_group_norm(xd.data_ptr(), gd.data_ptr(), bd.data_ptr(), y.data_ptr(), N, Cc, H, W, 32, 1e-5,
                                    silu, scratch.data_ptr(), nb, _lib.stream_ptr()))
@@ -162,17 +178,18 @@ def test_fused_groupnorm_conv(cuda, silu, N, cin, cout, H, W, K):
 
 
 @pytest.mark.parametrize("N,C,cout,H,W", [(2, 128, 128, 16, 16), (1, 128, 256, 8, 64), (1, 256, 128, 4, 128),
-                                          (5, 128, 128, 8, 8), (6, 256, 128, 4, 4)])
+                                          (5, 128, 128, 8, 8), (6, 256, 128, 4, 4), (128, 512, 512, 1, 1),
+                                          (5, 512, 512, 1, 1), (128, 512, 512, 2, 2), (5, 512, 512, 2, 2)])
 def test_upsample_conv_folded(cuda, N, C, cout, H, W):
     """conv3x3(nearest_2x(x)) computed as four 2x2 convs with pre-summed weights on the low-res tensor (b200ad_conv2d with
-    stride = -2). The weight sums are rounded to bf16 once, so compare against the fp32 reference with 2e-2 * max|ref|."""
+    stride = -2). The weight sums are rounded to bf16 once, so compare against the fp64 reference with 2e-2 * max|ref|."""
     from audio_diffusion_b200 import _lib
     L = _lib.lib()
     g = torch.Generator().manual_seed(21)
     x = _bf(torch.randn(N, C, H, W, generator=g))
     w = _bf(torch.randn(cout, C, 3, 3, generator=g) / (C * 9) ** 0.5)
     b = torch.randn(cout, generator=g)
-    ref = F.conv2d(F.interpolate(x, scale_factor=2.0, mode="nearest"), w, b, padding=1)
+    ref = F.conv2d(F.interpolate(x.double(), scale_factor=2.0, mode="nearest"), w.double(), b.double(), padding=1)
     xd, wd, bd = x.to(cuda), w.to(cuda), b.to(cuda)
     y = torch.empty(N, cout, 2 * H, 2 * W, device=cuda)
     stats = torch.empty(N, cout // 4, 2, device=cuda)
