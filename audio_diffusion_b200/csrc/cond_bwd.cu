@@ -1,5 +1,5 @@
 // Backward kernels of the conditional U-Net's transformer blocks (the forward is cond_ops.cu; the walk is
-// BwdBuilder::transformer_bwd in unet_bwd.cu): LayerNorm and GEGLU backward, the cross-attention vector's weight
+// BwdBuilder::transformer_bwd in backward.cu): LayerNorm and GEGLU backward, the cross-attention vector's weight
 // gradients, and the multi-head self-attention backward on tensor cores (FlashAttention-2 style: P is recomputed from Q, K
 // and the row log-sum-exp the training forward saved, never materialised).
 // Oracle: torch autograd over oracle/unet_cond_oracle.py.

@@ -169,6 +169,10 @@ static Block& add_block(std::vector<Block>& bl, BlockKind kind, const std::strin
   bl.push_back(b);
   return bl.back();
 }
+// The forward tap that holds a block's output (heads: their conv_in's).
+static std::string block_tap(const Block& k) {
+  return k.kind == BK_UNET_HEAD || k.kind == BK_CONV_IN || k.kind == BK_LATENT_IN ? k.name + "conv_in" : k.name;
+}
 
 // Gradient checkpointing: the forward ops of one block that rebuild its internals (ops[begin, end) of its list; the op
 // that writes the block's output comes after them and is not re-run), and the GroupNorm statistics those ops accumulate,
@@ -203,13 +207,17 @@ struct Plan {    // everything a plan builder derives from the workspace and (N,
   std::set<std::string> rebuilt;     // ... and the taps they rebuild, which share pooled buffers between blocks
 };
 
-struct Backward;   // a backward plan (unet_bwd.cu)
+struct Backward;   // a backward plan (backward.cu)
 
-// State shared by the model handles (U-Net, VAE): parameter table, packed-weight arena layout, workspace plan, backward
-// plans.
+// State shared by the model handles (U-Net, VAE): the block lists, parameter table, packed-weight arena layout, workspace
+// plan, backward plans.
 struct NetBase {
+  std::vector<Block> parts[2];      // the architecture, one block list per model part (U-Net: the whole model;
+                                    // autoencoder: encoder, decoder)
   int norm_groups = 32;
   float norm_eps = 1e-5f;
+  int heads = 8;                    // conditional U-Net: attention heads of the transformer blocks
+  bool single_head = false;         // attention with one head of dim C (the autoencoder) instead of head_dim 8
   std::vector<Param> params;
   std::map<std::string, int> pidx;
   std::vector<const float*> pptr;
@@ -245,7 +253,7 @@ struct NetBase {
   int nparts = 1;
   Backward* bwd[2] = {};
 };
-void release_backward(NetBase* h);   // frees h->bwd (unet_bwd.cu)
+void release_backward(NetBase* h);   // frees h->bwd (backward.cu)
 
 static PackItem make_pack_item(const NetBase* h, const PackJob& j, uint8_t* arena) {
   PackItem it;
@@ -552,9 +560,7 @@ struct Builder {
   std::vector<Op>* ops;
   std::map<std::string, Act> pool;  // reusable transient buffers keyed by tag
   int N, H = 0, W = 0;              // H, W: input size of the block list being planned
-  int heads = 8;                    // transformer: attention heads
   bool nopool = false;  // B200AD_DEBUG_NOPOOL=1: every activation gets its own buffer (per-layer parity taps)
-  bool single_head = false;  // attention with one head of dim C (AutoencoderKL mid block) instead of head_dim 8
   // gradient checkpointing (training): block outputs keep their own buffers, the internals are pooled as for inference
   bool ckpt = false;
   std::map<std::string, size_t> raw_pool;  // workspace offsets of pooled plain buffers by tag and size (unless nopool)
@@ -658,7 +664,7 @@ struct Builder {
                       W = W, x](const RunArgs& a, cudaStream_t s) {
       return launch_conv_in(src ? src : a.in, w, b, N, cin, H, W, x.C, x.p, x.stats, s);
     });
-    built->taps[k.name + "conv_in"] = x;
+    built->taps[block_tap(k)] = x;
     return x;
   }
 
@@ -791,9 +797,10 @@ struct Builder {
       return launch_xattn_kv(h->enc, wk, wv, kv, kv + (size_t)N * S * C, N, S, C, X, s);
     });
     Act ao2 = pooled(h->training ? "tf_ao2" : "tf_ao", C, H, W, false);    // attn1's output is dead after h1
-    float* lse = h->training ? built->lse[n + ".attn2"] = (float*)pooled_raw("lse2", (size_t)N * heads * H * W * sizeof(float))
-                             : nullptr;
-    emit(OP_XATTN, [q = q2.p, kv, o = ao2.p, N = N, C, heads = heads, H, W, S, lse](const RunArgs&, cudaStream_t s) {
+    float* lse = h->training
+                     ? built->lse[n + ".attn2"] = (float*)pooled_raw("lse2", (size_t)N * h->heads * H * W * sizeof(float))
+                     : nullptr;
+    emit(OP_XATTN, [q = q2.p, kv, o = ao2.p, N = N, C, heads = h->heads, H, W, S, lse](const RunArgs&, cudaStream_t s) {
       return launch_xattn(q, kv, kv + (size_t)N * S * C, o, N, C, heads, H, W, S, s, lse);
     });
     Act h2 = pooled("tf_h2", C, H, W, false);
@@ -832,8 +839,9 @@ struct Builder {
     Act qkv = pooled("tf_qkv", 3 * C, H, W, false);
     linear(qkv, n1, k.qkv, nullptr);
     Act ao = pooled("tf_ao", C, H, W, false);
-    float* lse = h->training ? built->lse[n] = (float*)pooled_raw("lse1", (size_t)N * heads * H * W * sizeof(float)) : nullptr;
-    emit(OP_MHA, [q = qkv.p, o = ao.p, N = N, C, heads = heads, H, W, lse](const RunArgs&, cudaStream_t s) {
+    float* lse = h->training ? built->lse[n] = (float*)pooled_raw("lse1", (size_t)N * h->heads * H * W * sizeof(float))
+                             : nullptr;
+    emit(OP_MHA, [q = qkv.p, o = ao.p, N = N, C, heads = h->heads, H, W, lse](const RunArgs&, cudaStream_t s) {
       return launch_mha_flash(q, o, N, C, heads, H, W, s, lse);
     });
     Act h2;
@@ -928,7 +936,7 @@ struct Builder {
     Act qkv = pooled("qkv", 3 * C, H, W, false);
     linear(qkv, xn, k.qkv, PK<float>(k.bias));   // q|k|v blocks are contiguous
     Act ao = pooled("attn_o", C, H, W, false);
-    if (single_head) {
+    if (h->single_head) {
       const size_t bytes = (size_t)N * H * W * H * W * sizeof(float);
       float* scores = (float*)(h->training ? pooled_raw("probs", bytes) : ws.take(bytes));
       if (h->training) built->probs[n] = scores;

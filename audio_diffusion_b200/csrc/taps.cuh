@@ -1,6 +1,6 @@
 // Tap sets of the implicit-GEMM convolution: for every way a conv K-segment reads its source, the weight taps to pack, the
 // window offset (dh, dw) of each tap relative to the output pixel, and the weight-gradient slot each tap accumulates into.
-// The model plans (net.cuh, unet_bwd.cu) and the op-level entry points (api.cu) build their segments from these. Host only.
+// The model plans (net.cuh, backward.cu) and the op-level entry points (api.cu) build their segments from these. Host only.
 #pragma once
 #include "conv_tc.cuh"
 #include "kernels.cuh"

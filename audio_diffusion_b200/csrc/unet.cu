@@ -90,14 +90,15 @@ extern "C" int b200ad_unet_create(const b200ad_unet_config* cfg, b200ad_unet** o
   h->cfg = *cfg;
   h->norm_groups = cfg->norm_num_groups;
   h->norm_eps = cfg->norm_eps;
-  h->blocks = unet_blocks(*cfg);
-  for (const Block& k : h->blocks) p_block(h, k);
+  h->heads = cfg->attention_head_dim;
+  std::vector<Block>& bl = h->parts[0] = unet_blocks(*cfg);
+  for (const Block& k : bl) p_block(h, k);
   Bump b;
-  for (Block& k : h->blocks) layout_block(h, b, k);
+  for (Block& k : bl) layout_block(h, b, k);
   const int D = cfg->block_out_channels[0] * 4;
   h->off_wcat = take_off(b, (size_t)h->temb_rows * D * 4);
   h->off_bcat = take_off(b, (size_t)h->temb_rows * 4);
-  for (Block& k : h->blocks)
+  for (Block& k : bl)
     if (k.kind == BK_TRANSFORMER) layout_attn2(h, b, k);
   h->packed_bytes = (b.off + 255) & ~(size_t)255;
   h->pptr.assign(h->params.size(), nullptr);
@@ -125,7 +126,7 @@ extern "C" int b200ad_unet_set_params(b200ad_unet* h, const float* const* params
   if ((h->plan_enc_len > 1 || h->enc_len > 1) && pack_xattn(h, st)) return -1;   // else packed when such a plan is bound
   // concatenated time_emb_proj weights / biases
   const int D = h->cfg.block_out_channels[0] * 4;
-  for (const Block& k : h->blocks) {
+  for (const Block& k : h->parts[0]) {
     if (k.temb_row < 0) continue;
     CK(cudaMemcpyAsync(h->packed + h->off_wcat + (size_t)k.temb_row * D * 4,
                        h->pptr[h->pidx.at(k.name + ".time_emb_proj.weight")], (size_t)k.cout * D * 4,
@@ -147,7 +148,6 @@ Plan build_plan(const b200ad_unet* h, uint8_t* ws_base, int N, int H, int W) {
   Builder B;
   B.h = h; B.built = &pl; B.ops = &l.ops;
   B.N = N; B.H = H; B.W = W;
-  B.heads = h->cfg.attention_head_dim;
   B.ckpt = pl.checkpoint = h->training && h->checkpointing;
   B.nopool = debug_nopool() || (h->training && !B.ckpt);
   B.ws.base = ws_base;
@@ -157,7 +157,7 @@ Plan build_plan(const b200ad_unet* h, uint8_t* ws_base, int N, int H, int W) {
     B.st.base = pass == 0 ? nullptr : ws_base;
     B.st.off = 0;
     B.ws.off = pass == 0 ? 0 : ((l.stats_bytes + 255) & ~(size_t)255);
-    B.run(h->blocks, &l.recompute);
+    B.run(h->parts[0], &l.recompute);
     if (pass == 0) l.stats_bytes = B.st.off;
   }
   l.stats = (stat_t*)ws_base;

@@ -1,10 +1,9 @@
-// The U-Net handle (shared by the forward plan, unet.cu, and the backward plan, unet_bwd.cu).
+// The U-Net handle (shared by the forward plan, unet.cu, and the backward plan, backward.cu).
 #pragma once
 #include "net.cuh"
 
-struct b200ad_unet : b200ad::NetBase {
+struct b200ad_unet : b200ad::NetBase {   // one model part: parts[0]
   b200ad_unet_config cfg;
-  std::vector<b200ad::Block> blocks;
 };
 
 namespace b200ad {

@@ -10,9 +10,9 @@ using namespace b200ad;
 
 namespace b200ad {
 
-// AutoencoderKL as two block lists.  Transient activations ping-pong between two pooled buffers per (C, H, W): every block
-// reads its input from one and writes its output to the other (the shortcut K-segment re-reads the input while the output
-// is being written).
+// AutoencoderKL as two block lists, h->parts[ENC] and h->parts[DEC].  Transient activations ping-pong between two pooled
+// buffers per (C, H, W): every block reads its input from one and writes its output to the other (the shortcut K-segment
+// re-reads the input while the output is being written).
 static void vae_blocks(b200ad_vae* h) {
   const b200ad_vae_config& c = h->cfg;
   const int nb = c.num_blocks;
@@ -25,7 +25,7 @@ static void vae_blocks(b200ad_vae* h) {
     add_block(bl, BK_ATTN, n + ".attentions.0", ch, ch, pp());
     add_block(bl, BK_RESNET, n + ".resnets.1", ch, ch, pp());
   };
-  std::vector<Block>& e = h->enc;
+  std::vector<Block>& e = h->parts[ENC];
   add_block(e, BK_CONV_IN, "encoder.", c.in_channels, boc[0], pp());
   for (int i = 0; i < nb; ++i) {
     for (int j = 0; j < c.layers_per_block; ++j)
@@ -34,7 +34,7 @@ static void vae_blocks(b200ad_vae* h) {
   }
   mid(e, "encoder.mid_block");
   add_block(e, BK_LATENT_OUT, "encoder.", boc[nb - 1], 2 * c.latent_channels, "");
-  std::vector<Block>& d = h->dec;
+  std::vector<Block>& d = h->parts[DEC];
   add_block(d, BK_LATENT_IN, "decoder.", c.latent_channels, boc[nb - 1], pp());
   mid(d, "decoder.mid_block");
   for (int i = 0; i < nb; ++i) {
@@ -54,7 +54,6 @@ Plan vae_build_plan(const b200ad_vae* h, uint8_t* ws_base, int N, int H, int W) 
   OpList& dec = pl.lists[DEC];
   Builder B;
   B.h = h; B.built = &pl; B.N = N;
-  B.single_head = true;
   B.ckpt = pl.checkpoint = h->training && h->checkpointing;
   B.nopool = debug_nopool() || (h->training && !B.ckpt);
   B.ws.base = ws_base;
@@ -65,12 +64,12 @@ Plan vae_build_plan(const b200ad_vae* h, uint8_t* ws_base, int N, int H, int W) 
     B.st.base = pass == 0 ? nullptr : ws_base;
     B.ws.off = pass == 0 ? 0 : ((enc.stats_bytes + dec.stats_bytes + 511) & ~(size_t)255);
     B.ops = &enc.ops; B.H = H; B.W = W;
-    B.run(h->enc, &enc.recompute);
+    B.run(h->parts[ENC], &enc.recompute);
     if (pass == 0) enc.stats_bytes = (B.st.off + 255) & ~(size_t)255;
     B.st.base = (pass == 1 && ws_base) ? ws_base + enc.stats_bytes : nullptr;
     B.st.off = 0;
     B.ops = &dec.ops; B.H = H / f; B.W = W / f;
-    B.run(h->dec, &dec.recompute);
+    B.run(h->parts[DEC], &dec.recompute);
     if (pass == 0) dec.stats_bytes = (B.st.off + 255) & ~(size_t)255;
   }
   enc.stats = (stat_t*)ws_base;
@@ -91,12 +90,13 @@ extern "C" int b200ad_vae_create(const b200ad_vae_config* cfg, b200ad_vae** out)
   h->nparts = 2;
   h->norm_groups = cfg->norm_num_groups;
   h->norm_eps = cfg->norm_eps;
+  h->single_head = true;
   vae_blocks(h);
   Bump b;
-  for (const Block& k : h->enc) p_block(h, k);
-  for (const Block& k : h->dec) p_block(h, k);
-  for (Block& k : h->enc) layout_block(h, b, k);
-  for (Block& k : h->dec) layout_block(h, b, k);
+  for (const std::vector<Block>& bl : h->parts)
+    for (const Block& k : bl) p_block(h, k);
+  for (std::vector<Block>& bl : h->parts)
+    for (Block& k : bl) layout_block(h, b, k);
   h->packed_bytes = (b.off + 255) & ~(size_t)255;
   h->pptr.assign(h->params.size(), nullptr);
   *out = h;

@@ -4,7 +4,7 @@
 Same constructor kwargs, same state-dict key layout (SURVEY §8b) and the same call convention
 `unet(sample, timestep)["sample"]`; the forward runs entirely in libb200ad.so (wgmma implicit-GEMM convs, fused GroupNorm
 statistics, fused scheduler step).  Training: with grad enabled and the module in train() mode, the forward is an autograd
-node whose backward runs in libb200ad.so too (unet_bwd.cu).  A `sample` that requires grad gets its gradient in train()
+node whose backward runs in libb200ad.so too (backward.cu).  A `sample` that requires grad gets its gradient in train()
 or eval() (guidance, saliency); a frozen or eval() model then runs a backward without parameter gradients, and moving
 between that and parameter training re-plans the workspace.  The engine plumbing is `EngineModel`'s (engine.py).
 """

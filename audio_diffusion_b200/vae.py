@@ -8,7 +8,7 @@ Encoder, decoder, quant/post-quant convs and the posterior sampling run in libb2
 parameters (fp32 `nn.Parameter`s), the packed bf16 weights and the activation workspace (engine.py).  No CPU fallback.
 
 Training (scripts/train_vae.py): with grad enabled, the module in train() mode and a parameter requiring grad, `encode`
-and `decode` are autograd nodes whose backward passes run in libb200ad.so (unet_bwd.cu); the posterior is then a torch
+and `decode` are autograd nodes whose backward passes run in libb200ad.so (backward.cu); the posterior is then a torch
 expression on the differentiable moments, so autograd carries the reparameterisation, the logvar clamp and `kl()`.
 An image (encode) or latents (decode) that require grad get their gradient in train() or eval(): a frozen or eval()
 autoencoder runs the backward without parameter gradients (a loss in pixel space behind a frozen decoder, latents

@@ -1,6 +1,6 @@
 """Per-block fp64 references of the U-Net and autoencoder backward (TEST INFRASTRUCTURE, see oracle/__init__.py).
 
-The engine's backward walks the forward's block list in reverse (csrc/unet_bwd.cu).  Each block there turns the gradient
+The engine's backward walks the forward's block list in reverse (csrc/backward.cu).  Each block there turns the gradient
 of its output into the gradients of its input(s) and of its own parameters.  `block_backward` does the same for one block
 by fp64 autograd over the oracle's pieces (`unet_oracle._resnet` / `_attention`, `unet_cond_oracle._transformer`,
 `vae_oracle._resnet` / `_attn`, and the oracles' inline down- / upsample, head and tail code), from whatever input

@@ -86,12 +86,13 @@ def unet_forward(dev):
     return rec, {"sample": out}
 
 
-def _unet_train(model, dev, n, hw, enc=None):
+def _unet_train(model, dev, n, hw, enc=None, sample_grad=False):
+    """One step of forward + MSE + backward; sample_grad: the sample requires grad (its gradient is saved too)."""
     sch = DDPMScheduler()
     clean = seeded(3, n, 1, hw, hw, dev=dev).clamp(-1, 1)
     noise = seeded(4, n, 1, hw, hw, dev=dev)
     t = torch.tensor([37, 712][:n], device=dev)
-    noisy = sch.add_noise(clean, noise, t)
+    noisy = sch.add_noise(clean, noise, t).requires_grad_(sample_grad)
 
     def step():
         pred = model(noisy, t)["sample"] if enc is None else model(noisy, t, enc)["sample"]
@@ -103,18 +104,51 @@ def _unet_train(model, dev, n, hw, enc=None):
            "last_backward_launch_count": model.last_backward_launch_count,
            "workspace_bytes": L.b200ad_unet_workspace_bytes(model._h, n, hw, hw),
            "backward_bytes": L.b200ad_unet_backward_bytes(model._h)}
-    return rec, {"sample": pred, "grad_flat": model._grad_flat.clone()}
+    tensors = {"sample": pred}
+    if model._grad_flat is not None:
+        tensors["grad_flat"] = model._grad_flat.clone()
+    if sample_grad:
+        tensors["sample_grad"] = noisy.grad
+    return rec, tensors
+
+
+def _unet(dev, checkpointing=False):
+    model = UNet2DModel(sample_size=(256, 256), seed=0, **UNET_ARCH).to(dev)
+    if checkpointing:
+        model.enable_gradient_checkpointing()
+    return model
 
 
 def unet_train(dev):
     """One training step (forward + MSE + backward) of the published U-Net, batch 2, 256 x 256."""
-    return _unet_train(UNet2DModel(sample_size=(256, 256), seed=0, **UNET_ARCH).to(dev).train(), dev, 2, 256)
+    return _unet_train(_unet(dev).train(), dev, 2, 256)
+
+
+def unet_train_ckpt(dev):
+    """unet_train with gradient checkpointing: the backward recomputes each block's internals."""
+    return _unet_train(_unet(dev, checkpointing=True).train(), dev, 2, 256)
+
+
+def unet_train_sample_grad(dev):
+    """unet_train with a sample that requires grad: the parameter gradients and the sample gradient."""
+    return _unet_train(_unet(dev).train(), dev, 2, 256, sample_grad=True)
+
+
+def unet_frozen_sample_grad(dev):
+    """A frozen eval() U-Net differentiated with respect to its sample: the data-gradient-only backward."""
+    return _unet_train(_unet(dev).eval().requires_grad_(False), dev, 2, 256, sample_grad=True)
 
 
 def cond_train(dev):
     """One training step of the conditional U-Net at its 64 x 64 latent, batch 1, encoder sequence length 1."""
     model = UNet2DConditionModel(sample_size=(64, 64), seed=0, **COND_ARCH).to(dev).train()
     return _unet_train(model, dev, 1, 64, enc=seeded(5, 1, 1, 100, dev=dev))
+
+
+def cond_train_s77(dev):
+    """cond_train with an encoder sequence of 77 tokens (cross-attention over a key sequence), batch 2."""
+    model = UNet2DConditionModel(sample_size=(64, 64), seed=0, **COND_ARCH).to(dev).train()
+    return _unet_train(model, dev, 2, 64, enc=seeded(5, 2, 77, 100, dev=dev))
 
 
 def vae_infer(dev):
@@ -132,9 +166,14 @@ def vae_infer(dev):
     return rec, {"z": z, "image": y}
 
 
-def vae_train(dev):
-    """One training step of the autoencoder (encode, sample, decode, L1 + KL, backward), batch 2, 64 x 64."""
-    vae = AutoencoderKL(seed=0, max_batch=2, **VAE_ARCH).to(dev).train()
+def _vae(dev, checkpointing=False):
+    vae = AutoencoderKL(seed=0, max_batch=2, **VAE_ARCH).to(dev)
+    if checkpointing:
+        vae.enable_gradient_checkpointing()
+    return vae
+
+
+def _vae_train(vae, dev):
     x = seeded(8, 2, 1, 64, 64, dev=dev).clamp(-1, 1)
     noise = torch.Generator().manual_seed(9)
 
@@ -149,8 +188,42 @@ def vae_train(dev):
     return rec, {"image": y, "grad_flat": vae._grad_flat.clone()}
 
 
-WORKLOADS = {"unet_forward": unet_forward, "unet_train": unet_train, "cond_train": cond_train, "vae_infer": vae_infer,
-             "vae_train": vae_train}
+def vae_train(dev):
+    """One training step of the autoencoder (encode, sample, decode, L1 + KL, backward), batch 2, 64 x 64."""
+    return _vae_train(_vae(dev).train(), dev)
+
+
+def vae_train_ckpt(dev):
+    """vae_train with gradient checkpointing."""
+    return _vae_train(_vae(dev, checkpointing=True).train(), dev)
+
+
+def vae_frozen_input_grad(dev):
+    """A frozen eval() autoencoder differentiated with respect to its inputs (data-gradient-only backward): the decoder's
+    latent gradient, then the encoder's image gradient, batch 2, 64 x 64."""
+    vae = _vae(dev).eval().requires_grad_(False)
+    z = seeded(10, 2, 1, 8, 8, dev=dev).requires_grad_(True)
+    g_img = seeded(11, 2, 1, 64, 64, dev=dev)
+    x = seeded(12, 2, 1, 64, 64, dev=dev).clamp(-1, 1).requires_grad_(True)
+    g_mom = seeded(13, 2, 2, 8, 8, dev=dev)
+
+    def step():
+        y = vae.decode(z).sample
+        y.backward(g_img)
+        dec_launches = vae.last_backward_launch_count
+        vae.encode(x).latent_dist.parameters.backward(g_mom)
+        return y.detach(), dec_launches
+    (y, dec_launches), seq = traced(step)
+    rec = {"launches": seq, "decoder_backward_launch_count": dec_launches,
+           "encoder_backward_launch_count": vae.last_backward_launch_count,
+           "backward_bytes": _lib.lib().b200ad_vae_backward_bytes(vae._h)}
+    return rec, {"image": y, "latent_grad": z.grad, "image_grad": x.grad}
+
+
+WORKLOADS = {"unet_forward": unet_forward, "unet_train": unet_train, "unet_train_ckpt": unet_train_ckpt,
+             "unet_train_sample_grad": unet_train_sample_grad, "unet_frozen_sample_grad": unet_frozen_sample_grad,
+             "cond_train": cond_train, "cond_train_s77": cond_train_s77, "vae_infer": vae_infer, "vae_train": vae_train,
+             "vae_train_ckpt": vae_train_ckpt, "vae_frozen_input_grad": vae_frozen_input_grad}
 
 
 def main():

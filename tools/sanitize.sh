@@ -1,8 +1,8 @@
 #!/bin/bash
 # compute-sanitizer evidence (SURVEY §5): memcheck + racecheck + synccheck over the smoke invocation (forward + fused
 # scheduler step: conv_tc / conv_in / conv_out / attention / temb kernels) and memcheck + racecheck over one small backward
-# (unet_bwd / wgrad_tc / bwd kernels) and the Mel codec.  Logs go to gpurun_out/sanitizer_<tool>_<what>_<tag>.log; the
-# summaries are copied to profiles/.
+# (backward / wgrad_tc / bwd kernels) and the Mel codec.  Each run logs to sanitizer_<tool>_<what>_<tag>.log in the
+# output directory below; the summaries are copied to profiles/.
 # usage (on the GPU box): tools/sanitize.sh [tag]
 tag=${1:-r02}
 mkdir -p gpurun_out
