@@ -1,7 +1,8 @@
 """audio_diffusion_b200 — H100-native (sm_90a) engine for the teticio/audio-diffusion hot path.
 
 Public surface mirrors the reference objects the unchanged `AudioDiffusionPipeline` drives:
-`UNet2DModel`, `AutoencoderKL`, `DDPMScheduler`, `DDIMScheduler`, `Mel`, `AudioDiffusionPipeline`.
+`UNet2DModel`, `AutoencoderKL`, `DDPMScheduler`, `DDIMScheduler`, `DPMSolverMultistepScheduler`, `Mel`,
+`AudioDiffusionPipeline`.
 """
 __version__ = "0.1.0"
 
@@ -16,7 +17,7 @@ def __getattr__(name):
     if name == "AutoencoderKL":
         from .vae import AutoencoderKL
         return AutoencoderKL
-    if name in ("DDPMScheduler", "DDIMScheduler"):
+    if name in ("DDPMScheduler", "DDIMScheduler", "DPMSolverMultistepScheduler"):
         from . import schedulers
         return getattr(schedulers, name)
     if name == "Mel":

@@ -43,6 +43,11 @@ class StepCoefC(C.Structure):
                 ("c_xt", C.c_float), ("c_eps", C.c_float), ("c_z", C.c_float), ("do_clip", C.c_int)]
 
 
+class MultistepCoefC(C.Structure):
+    """b200ad_multistep_coef: a step's coefficients plus those of the two earlier data predictions (history buffers)."""
+    _fields_ = [("step", StepCoefC), ("c_h1", C.c_float), ("c_h2", C.c_float)]
+
+
 class MelConfigC(C.Structure):
     _fields_ = [("x_res", C.c_int), ("y_res", C.c_int), ("sample_rate", C.c_int), ("n_fft", C.c_int),
                 ("hop_length", C.c_int), ("top_db", C.c_int), ("n_iter", C.c_int)]
@@ -68,6 +73,9 @@ SYMBOLS = {
     "b200ad_unet_forward_step": (_I, [_VP, _VP, _VP, _VP, C.POINTER(StepCoefC), _VP, _VP, _VP]),
     "b200ad_unet_forward_step_dev": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _VP]),
     "b200ad_step_scalars_upload": (_I, [C.POINTER(StepCoefC), C.c_float, _VP, _VP, C.c_int, _VP]),
+    "b200ad_unet_forward_multistep": (_I, [_VP, _VP, _VP, _VP, C.POINTER(MultistepCoefC), _VP, _VP, _VP, _VP, _VP]),
+    "b200ad_unet_forward_multistep_dev": (_I, [_VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),
+    "b200ad_multistep_scalars_upload": (_I, [C.POINTER(MultistepCoefC), C.c_float, _VP, _VP, C.c_int, _VP]),
     "b200ad_unet_profile_step": (_I, [_VP, _VP, _VP, _VP, C.POINTER(StepCoefC), _VP, C.POINTER(C.c_float),
                                       C.POINTER(_I), C.POINTER(C.c_double), _I, _VP]),
     "b200ad_unet_debug_tensor": (_I, [_VP, C.c_char_p, _VP, C.POINTER(_I), _VP]),

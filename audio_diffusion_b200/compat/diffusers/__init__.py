@@ -7,7 +7,7 @@ import torch
 from audio_diffusion_b200.hub_io import model_from_dir, save_model
 from audio_diffusion_b200.mel import Mel
 from audio_diffusion_b200.pipeline import (AudioPipelineOutput, BaseOutput, DiffusionPipeline, ImagePipelineOutput)
-from audio_diffusion_b200.schedulers import DDIMScheduler, DDPMScheduler
+from audio_diffusion_b200.schedulers import DDIMScheduler, DDPMScheduler, DPMSolverMultistepScheduler
 from audio_diffusion_b200.unet import UNet2DModel
 from audio_diffusion_b200.unet_cond import UNet2DConditionModel
 from audio_diffusion_b200.vae import AutoencoderKL

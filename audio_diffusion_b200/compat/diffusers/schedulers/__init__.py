@@ -1,1 +1,1 @@
-from audio_diffusion_b200.schedulers import DDIMScheduler, DDPMScheduler  # noqa: F401
+from audio_diffusion_b200.schedulers import DDIMScheduler, DDPMScheduler, DPMSolverMultistepScheduler  # noqa: F401

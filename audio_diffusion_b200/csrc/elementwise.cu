@@ -554,11 +554,20 @@ __global__ void __launch_bounds__(256, CO_CTAS_PER_SM) conv_out_kernel(const Con
           const long long idx = (((long long)n * p.cout + co) * p.H + h) * p.W + w;
           if (p.eps_out) p.eps_out[idx] = e;
           if (p.x_out) {
-            const StepCoef cf = p.coef_dev ? *p.coef_dev : p.coef;
+            const StepCoef cf = p.coef_dev ? p.coef_dev->s : p.coef.s;
             const float xv = p.x[idx];
             float x0 = (xv - cf.sqrt_1m_at * e) * cf.inv_sqrt_at;
             if (cf.do_clip) x0 = fminf(fmaxf(x0, -cf.clip), cf.clip);
             float rr = cf.c_x0 * x0 + cf.c_xt * xv + cf.c_eps * e;
+            if (p.hist1) {                 // multistep: this thread alone reads and rewrites element idx of the history
+              const float h1 = p.hist1[idx];
+              rr += (p.coef_dev ? p.coef_dev->c_h1 : p.coef.c_h1) * h1;
+              if (p.hist2) {
+                rr += (p.coef_dev ? p.coef_dev->c_h2 : p.coef.c_h2) * p.hist2[idx];
+                p.hist2[idx] = h1;
+              }
+              p.hist1[idx] = x0;
+            }
             if (p.z) rr += cf.c_z * p.z[idx];
             p.x_out[idx] = rr;
           }

@@ -67,10 +67,15 @@ cudaError_t launch_conv_in(const float* x, const float* w, const float* b, int N
 // conv_norm_out + SiLU + conv_out (3x3, C -> cout small) fused with the scheduler update.
 // eps_out (optional): model output, fp32 NCHW.  If x_out != null:
 //   x0 = clamp((x - sqrt_1m_at * eps) * inv_sqrt_at, -clip, clip);  x_out = c_x0 * x0 + c_xt * x + c_eps * eps + c_z * z
-// which covers DDPM (c_eps = 0) and DDIM (c_xt = 0).
+// which covers DDPM (c_eps = 0) and DDIM (c_xt = 0).  Multistep (DPM-Solver++, hist1 != null): x_out also gets
+// c_h1 * hist1 + c_h2 * hist2 (the x0 of the previous two steps), then hist2 <- hist1 (if hist2) and hist1 <- x0.
 struct StepCoef {
   float sqrt_1m_at, inv_sqrt_at, clip, c_x0, c_xt, c_eps, c_z;
   int do_clip;
+};
+struct MultistepCoef {
+  StepCoef s;
+  float c_h1, c_h2;
 };
 struct ConvOutParams {
   const __nv_bfloat16* src;   // raw PF8, C channels
@@ -86,9 +91,12 @@ struct ConvOutParams {
   const float* x;             // fp32 NCHW current sample (scheduler input) or null
   const float* z;             // fp32 NCHW noise or null
   float* x_out;               // fp32 NCHW or null
-  StepCoef coef;
-  const StepCoef* coef_dev;   // optional: the coefficients live on the device (CUDA-graph replay: nothing per-step is baked
-                              // into the launch); overrides `coef`
+  MultistepCoef coef;
+  const MultistepCoef* coef_dev;  // optional: the coefficients live on the device (CUDA-graph replay: nothing per-step is
+                                  // baked into the launch); overrides `coef`.  Without history only its `s` is read, so
+                                  // it may point at a plain StepCoef.
+  float* hist1;               // fp32 NCHW x0 of the previous step, or null (then c_h1 / c_h2 and hist2 are unused)
+  float* hist2;               // fp32 NCHW x0 of the step before that, or null
 };
 cudaError_t launch_conv_out(const ConvOutParams& p, cudaStream_t s);
 

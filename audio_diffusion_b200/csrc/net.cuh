@@ -68,8 +68,10 @@ struct RunArgs {                        // the per-call inputs of a plan
   float* out = nullptr;                 // U-Net: eps (optional); autoencoder: z (encode) or the image (decode)
   float* moments = nullptr;             // autoencoder encode (optional)
   float* x_out = nullptr;               // U-Net: the scheduler update (optional), with coef or coef_dev
-  const b200ad_step_coef* coef = nullptr;
-  const b200ad_step_coef* coef_dev = nullptr;
+  const b200ad_multistep_coef* coef = nullptr;
+  const b200ad_multistep_coef* coef_dev = nullptr;   // without history only its `step` is read
+  float* hist1 = nullptr;               // U-Net multistep update: x0 of the previous two steps (optional)
+  float* hist2 = nullptr;
   // backward (`in`: the forward's input)
   const float* g_eps = nullptr;         // the gradient of the model output (U-Net: eps; autoencoder decoder: the image)
   const float* g_mom = nullptr;         // autoencoder encoder: the gradient of the moments
@@ -971,9 +973,11 @@ struct Builder {
       ConvOutParams q = p;
       q.eps_out = a.out;
       q.x = a.in; q.z = a.noise; q.x_out = a.x_out;
+      q.hist1 = a.hist1; q.hist2 = a.hist2;
       static_assert(sizeof(b200ad_step_coef) == sizeof(StepCoef), "step-coefficient layouts differ");
-      q.coef_dev = reinterpret_cast<const StepCoef*>(a.coef_dev);
-      if (a.coef) memcpy(&q.coef, a.coef, sizeof(StepCoef));
+      static_assert(sizeof(b200ad_multistep_coef) == sizeof(MultistepCoef), "multistep-coefficient layouts differ");
+      q.coef_dev = reinterpret_cast<const MultistepCoef*>(a.coef_dev);
+      if (a.coef) memcpy(&q.coef, a.coef, sizeof(MultistepCoef));
       return launch_conv_out(q, s);
     });
     built->taps[n + "pre_out"] = x;

@@ -212,8 +212,9 @@ extern "C" int b200ad_unet_profile_step(b200ad_unet* h, const float* x, const fl
   const std::vector<Op>& ops = h->plan.lists[0].ops;
   const int nops = (int)ops.size();
   if (nops > max_ops) return set_err("profile_step: %d ops > max_ops %d", nops, max_ops);
+  const b200ad_multistep_coef mc = {*coef, 0.f, 0.f};
   RunArgs a;
-  a.in = x; a.t = t; a.noise = z; a.coef = coef; a.x_out = x_out;
+  a.in = x; a.t = t; a.noise = z; a.coef = &mc; a.x_out = x_out;
   OpEvents ev;
   if (run_plan(h, a, st, &ev)) return -1;
   CK(cudaStreamSynchronize(st));
@@ -270,32 +271,58 @@ extern "C" int b200ad_unet_forward(b200ad_unet* h, const float* x, const float* 
   a.in = x; a.t = t; a.out = eps_out;
   return run_plan(h, a, (cudaStream_t)stream);
 }
-extern "C" int b200ad_unet_forward_step(b200ad_unet* h, const float* x, const float* t, const float* z,
-                                        const b200ad_step_coef* coef, float* x_out, float* eps_out, void* stream) {
+// The DDPM / DDIM step is the multistep step without history.
+extern "C" int b200ad_unet_forward_multistep(b200ad_unet* h, const float* x, const float* t, const float* z,
+                                             const b200ad_multistep_coef* coef, float* hist1, float* hist2, float* x_out,
+                                             float* eps_out, void* stream) {
   if (!coef || !x_out) return set_err("coef and x_out are required");
+  if (hist2 && !hist1) return set_err("forward_multistep: hist2 needs hist1");
   RunArgs a;
-  a.in = x; a.t = t; a.noise = z; a.coef = coef; a.x_out = x_out; a.out = eps_out;
+  a.in = x; a.t = t; a.noise = z; a.coef = coef; a.x_out = x_out; a.out = eps_out; a.hist1 = hist1; a.hist2 = hist2;
   return run_plan(h, a, (cudaStream_t)stream);
 }
+extern "C" int b200ad_unet_forward_step(b200ad_unet* h, const float* x, const float* t, const float* z,
+                                        const b200ad_step_coef* coef, float* x_out, float* eps_out, void* stream) {
+  if (!coef) return set_err("coef and x_out are required");
+  const b200ad_multistep_coef mc = {*coef, 0.f, 0.f};
+  return b200ad_unet_forward_multistep(h, x, t, z, &mc, nullptr, nullptr, x_out, eps_out, stream);
+}
 // per-step scalars -> device (kernel ARGUMENTS are copied at launch time, so the host may run any number of steps ahead)
-__global__ void step_scalars_kernel(b200ad_step_coef coef, float t, b200ad_step_coef* coef_dev, float* t_dev, int n) {
+template <typename Coef>
+__global__ void step_scalars_kernel(Coef coef, float t, Coef* coef_dev, float* t_dev, int n) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i == 0) *coef_dev = coef;
   if (i < n) t_dev[i] = t;
 }
-extern "C" int b200ad_step_scalars_upload(const b200ad_step_coef* coef, float t, b200ad_step_coef* coef_dev, float* t_dev, int n,
-                                          void* stream) {
+template <typename Coef>
+static int step_scalars_upload(const Coef* coef, float t, Coef* coef_dev, float* t_dev, int n, void* stream) {
   if (!coef || !coef_dev || !t_dev || n < 1) return set_err("step_scalars_upload: bad arguments");
   step_scalars_kernel<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream>>>(*coef, t, coef_dev, t_dev, n);
   CK(cudaGetLastError());
   return 0;
 }
+extern "C" int b200ad_step_scalars_upload(const b200ad_step_coef* coef, float t, b200ad_step_coef* coef_dev, float* t_dev, int n,
+                                          void* stream) {
+  return step_scalars_upload(coef, t, coef_dev, t_dev, n, stream);
+}
+extern "C" int b200ad_multistep_scalars_upload(const b200ad_multistep_coef* coef, float t, b200ad_multistep_coef* coef_dev,
+                                               float* t_dev, int n, void* stream) {
+  return step_scalars_upload(coef, t, coef_dev, t_dev, n, stream);
+}
+extern "C" int b200ad_unet_forward_multistep_dev(b200ad_unet* h, const float* x, const float* t, const float* z,
+                                                 const b200ad_multistep_coef* coef_dev, float* hist1, float* hist2,
+                                                 float* x_out, void* stream) {
+  if (!coef_dev || !x_out) return set_err("coef_dev and x_out are required");
+  if (hist2 && !hist1) return set_err("forward_multistep_dev: hist2 needs hist1");
+  RunArgs a;
+  a.in = x; a.t = t; a.noise = z; a.coef_dev = coef_dev; a.x_out = x_out; a.hist1 = hist1; a.hist2 = hist2;
+  return run_plan(h, a, (cudaStream_t)stream);
+}
+// Without history the kernel reads only the leading b200ad_step_coef of *coef_dev, so a plain one may stand in for it.
 extern "C" int b200ad_unet_forward_step_dev(b200ad_unet* h, const float* x, const float* t, const float* z,
                                             const b200ad_step_coef* coef_dev, float* x_out, void* stream) {
-  if (!coef_dev || !x_out) return set_err("coef_dev and x_out are required");
-  RunArgs a;
-  a.in = x; a.t = t; a.noise = z; a.coef_dev = coef_dev; a.x_out = x_out;
-  return run_plan(h, a, (cudaStream_t)stream);
+  return b200ad_unet_forward_multistep_dev(h, x, t, z, reinterpret_cast<const b200ad_multistep_coef*>(coef_dev), nullptr,
+                                           nullptr, x_out, stream);
 }
 extern "C" int b200ad_unet_last_launch_count(const b200ad_unet* h) { return h->last_launches; }
 

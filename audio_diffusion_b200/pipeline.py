@@ -7,8 +7,8 @@ the engine's pipeline, organised as four stages with the reference's observable 
 
   1. `_start_state`      initial noise, drawn with the caller's generator exactly as :120-130 does;
   2. `_condition`        optional audio conditioning / in-painting columns (:134-157);
-  3. `_denoise`          the loop (:159-185) on `UNet2DModel.forward_step` — U-Net forward with the DDPM/DDIM update fused
-                         into the output kernel (the reference makes two calls, :163 and :165-179);
+  3. `_denoise`          the loop (:159-185) on `UNet2DModel.forward_step` — U-Net forward with the DDPM/DDIM/DPM-Solver++
+                         update fused into the output kernel (the reference makes two calls, :163 and :165-179);
   4. `_deliver`          optional VAE decode (:187-190), float -> uint8 on the GPU, bit-exact with :192-194, PIL images,
                          and `Mel.images_to_audio` batched on the GPU instead of one image at a time on the CPU (:201).
 
@@ -29,7 +29,7 @@ from PIL import Image
 from . import _lib
 from .hub_io import DIFFUSERS_VERSION, save_model
 from .mel import Mel
-from .schedulers import DDIMScheduler, DDPMScheduler, randn_tensor
+from .schedulers import DDIMScheduler, DDPMScheduler, DPMSolverMultistepScheduler, randn_tensor
 from .unet import UNet2DModel
 from .vae import AutoencoderKL
 
@@ -40,7 +40,8 @@ GRAPH_MAX_BATCH = 8               # batches up to this size run the denoising st
 # reference / in diffusers, and directories pushed by the reference's train_unet.py load here.
 _UPSTREAM = {
     "UNet2DModel": "diffusers", "UNet2DConditionModel": "diffusers", "AutoencoderKL": "diffusers",
-    "DDPMScheduler": "diffusers", "DDIMScheduler": "diffusers", "Mel": "audio_diffusion",
+    "DDPMScheduler": "diffusers", "DDIMScheduler": "diffusers", "DPMSolverMultistepScheduler": "diffusers",
+    "Mel": "audio_diffusion",
 }
 
 
@@ -127,7 +128,7 @@ class DiffusionPipeline:
         with open(os.path.join(path, cls.config_name)) as f:
             index = json.load(f)
         own = {"UNet2DModel": UNet2DModel, "AutoencoderKL": AutoencoderKL, "DDPMScheduler": DDPMScheduler,
-               "DDIMScheduler": DDIMScheduler, "Mel": Mel}
+               "DDIMScheduler": DDIMScheduler, "DPMSolverMultistepScheduler": DPMSolverMultistepScheduler, "Mel": Mel}
         mods = {}
         for k, v in index.items():
             if k.startswith("_") or not isinstance(v, list):
@@ -170,7 +171,7 @@ def image_to_unit_range(image) -> np.ndarray:
 class AudioDiffusionPipeline(DiffusionPipeline):
     _optional_components = ["vqvae"]
 
-    def __init__(self, vqvae, unet, mel: Mel, scheduler: Union[DDIMScheduler, DDPMScheduler]):
+    def __init__(self, vqvae, unet, mel: Mel, scheduler: Union[DDIMScheduler, DDPMScheduler, DPMSolverMultistepScheduler]):
         super().__init__()
         self.register_modules(unet=unet, scheduler=scheduler, mel=mel, vqvae=vqvae)
 
@@ -211,14 +212,20 @@ class AudioDiffusionPipeline(DiffusionPipeline):
         fused = hasattr(unet, "forward_step") and hasattr(sch, "step_coef")
         extra = {"eta": eta} if isinstance(sch, DDIMScheduler) else {}
         cond = () if encoding is None else (encoding,)
+        # A multistep scheduler's fused step keeps the x0 of its previous steps in history planes on the device, zeroed
+        # here so that a coefficient of 0 (the warm-up steps) never meets a stale value.
+        nhist = sch.history_len if fused and isinstance(sch, DPMSolverMultistepScheduler) else None
+        hist = None
         # Small batches (the facade's batch_size=1, audiodiffusion/__init__.py:59) are bound by the host enqueueing ~120
         # launches per step: replay the step as one CUDA graph (same kernels, bit-identical results).
         stepper = None
         if (fused and encoding is None and inpaint is None and images.shape[0] <= GRAPH_MAX_BATCH
                 and hasattr(unet, "graph_stepper") and not getattr(unet, "is_conditional", False)
                 and os.environ.get("B200AD_CUDA_GRAPH", "1") != "0"):
-            stepper = unet.graph_stepper(images)
+            stepper = unet.graph_stepper(images, history=nhist)
             images = stepper.x                    # the stepper's own buffer, initialised from the start state
+        elif nhist:
+            hist = torch.zeros((nhist,) + tuple(images.shape), dtype=torch.float32, device=images.device)
         for k, t in enumerate(self.progress_bar(sch.timesteps[start_step:])):
             if fused:
                 z = None
@@ -227,7 +234,7 @@ class AudioDiffusionPipeline(DiffusionPipeline):
                 if stepper is not None:
                     images = stepper.step(t, sch.step_coef(t, eta), z)
                     continue
-                images = unet.forward_step(images, t, sch.step_coef(t, eta), *cond, noise=z, out=images)
+                images = unet.forward_step(images, t, sch.step_coef(t, eta), *cond, noise=z, out=images, history=hist)
             else:                                     # any model / scheduler pair with the reference's duck type
                 eps = unet(images, t, *cond)["sample"]
                 images = sch.step(model_output=eps, timestep=t, sample=images, generator=step_generator,

@@ -17,7 +17,7 @@ import torch
 from torch.autograd.function import once_differentiable
 
 from . import _lib
-from ._lib import MAX_BLOCKS, StepCoefC, UNetConfigC
+from ._lib import MAX_BLOCKS, MultistepCoefC, StepCoefC, UNetConfigC
 from .engine import EngineModel, _Cfg
 
 
@@ -265,17 +265,39 @@ class UNet2DModel(EngineModel):
         return ctx()
 
     # ------------------------------------------------------------------ sampling
-    def forward_step(self, sample: torch.Tensor, timestep, coef: StepCoefC, noise: Optional[torch.Tensor] = None,
-                     out: Optional[torch.Tensor] = None, want_eps: bool = False):
-        """Fused `scheduler.step(unet(sample, t), t, sample)["prev_sample"]` (pipeline_audio_diffusion.py:163-179)."""
-        return self._forward_step(sample, timestep, coef, None, noise, out, want_eps)
+    def forward_step(self, sample: torch.Tensor, timestep, coef: Union[StepCoefC, MultistepCoefC],
+                     noise: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None, want_eps: bool = False,
+                     history: Optional[torch.Tensor] = None):
+        """Fused `scheduler.step(unet(sample, t), t, sample)["prev_sample"]` (pipeline_audio_diffusion.py:163-179).  A multistep
+        scheduler (`DPMSolverMultistepScheduler.step_coef` gives `MultistepCoefC`) also passes `history`: fp32 (k, *sample.shape),
+        k = 1 or 2, the x0 of the previous k steps, which the step reads and rotates in place (zero-filled at the start)."""
+        return self._forward_step(sample, timestep, coef, None, noise, out, want_eps, history)
+
+    def _check_history(self, x: torch.Tensor, coef, history: Optional[torch.Tensor]) -> int:
+        """Number of history planes the step reads; refuses a history the coefficients do not match."""
+        multi = isinstance(coef, MultistepCoefC)
+        if history is None:
+            if multi and (coef.c_h1 != 0.0 or coef.c_h2 != 0.0):
+                raise ValueError(f"{type(self).__name__}(b200): multistep coefficients need a history tensor")
+            return 0
+        if not multi:
+            raise ValueError(f"{type(self).__name__}(b200): a history tensor needs multistep coefficients (MultistepCoefC)")
+        if (history.dim() != 5 or history.shape[0] not in (1, 2) or history.shape[1:] != x.shape
+                or history.dtype != torch.float32 or not history.is_contiguous() or history.device != x.device):
+            raise ValueError(f"{type(self).__name__}(b200): history must be a contiguous fp32 tensor (k, "
+                             f"{', '.join(map(str, x.shape))}) with k in (1, 2) on {x.device}, got {tuple(history.shape)} "
+                             f"{history.dtype} on {history.device}")
+        if history.shape[0] == 1 and coef.c_h2 != 0.0:
+            raise ValueError(f"{type(self).__name__}(b200): a third-order step needs two history planes")
+        return history.shape[0]
 
     @torch.no_grad()
-    def _forward_step(self, sample: torch.Tensor, timestep, coef: StepCoefC, enc, noise: Optional[torch.Tensor],
-                      out: Optional[torch.Tensor], want_eps: bool):
+    def _forward_step(self, sample: torch.Tensor, timestep, coef, enc, noise: Optional[torch.Tensor],
+                      out: Optional[torch.Tensor], want_eps: bool, history: Optional[torch.Tensor] = None):
         x = self._check_input(sample)
         self._check_step(x, "noise", noise)
         self._check_step(x, "out", out)
+        k = self._check_history(x, coef, history)
         n, _, hh, ww = x.shape
         with torch.cuda.device(x.device):
             self._fwd_gen[0] += 1
@@ -287,86 +309,124 @@ class UNet2DModel(EngineModel):
             eps = torch.empty_like(x) if want_eps else None
             z = noise.to(torch.float32).contiguous() if noise is not None else None
             self._set_encoding(e)
-            _lib.check(self._fn("forward_step")(
-                self._h, x.data_ptr(), t.data_ptr(), z.data_ptr() if z is not None else None, C.byref(coef),
-                out.data_ptr(), eps.data_ptr() if eps is not None else None, _lib.stream_ptr()))
+            zp, ep = z.data_ptr() if z is not None else None, eps.data_ptr() if eps is not None else None
+            if isinstance(coef, MultistepCoefC):
+                h1 = history[0].data_ptr() if k >= 1 else None
+                h2 = history[1].data_ptr() if k == 2 else None
+                _lib.check(self._fn("forward_multistep")(self._h, x.data_ptr(), t.data_ptr(), zp, C.byref(coef), h1, h2, out.data_ptr(),
+                                                         ep, _lib.stream_ptr()))
+            else:
+                _lib.check(self._fn("forward_step")(self._h, x.data_ptr(), t.data_ptr(), zp, C.byref(coef), out.data_ptr(),
+                                                    ep, _lib.stream_ptr()))
         return (out, eps) if want_eps else out
 
-    def graph_stepper(self, sample: torch.Tensor) -> "GraphStepper":
+    def graph_stepper(self, sample: torch.Tensor, history: Optional[int] = None) -> "GraphStepper":
         """CUDA-graph replay of `forward_step`: see `GraphStepper`.  The stepper owns its sample buffer (`stepper.x`, initialised
-        from `sample`) and is cached per shape, so repeated pipeline calls re-use one captured graph as long as the model
-        stays bound the same way (weights, batch, mode)."""
+        from `sample`) and is cached per shape and kind, so repeated pipeline calls re-use one captured graph as long as the
+        model stays bound the same way (weights, batch, mode).  `history`: None for DDPM / DDIM coefficients (`StepCoefC`),
+        else the number of history planes (0-2) of a multistep scheduler's steps (`MultistepCoefC`); they start zeroed."""
         x = self._check_input(sample)
         self._check_step(x, "sample", None)
+        if history not in (None, 0, 1, 2):
+            raise ValueError(f"graph_stepper: history must be None, 0, 1 or 2, got {history!r}")
         n, _, hh, ww = x.shape
         cache = self.__dict__.setdefault("_steppers", {})
-        key = (tuple(x.shape), x.device)
+        key = (tuple(x.shape), x.device, history)
         st = cache.get(key)
         if st is not None:
             with torch.cuda.device(x.device):
                 self._bind(n, hh, ww, False, x.device)
             if st._bound == (self._packed_key, self._ws_key):
                 st.x.copy_(x)
+                if st.hist is not None:
+                    st.hist.zero_()
                 return st
-        st = GraphStepper(self, x.clone())
+        st = GraphStepper(self, x.clone(), history)
         cache[key] = st
         return st
 
 
 class GraphStepper:
     """The denoising loop's step as ONE `cudaGraphLaunch`: `x <- scheduler.step(unet(x, t), t, x)` with everything that changes
-    from step to step (timestep, scheduler coefficients, noise) in fixed device buffers (`b200ad_unet_forward_step_dev`).
+    from step to step (timestep, scheduler coefficients, noise) in fixed device buffers (`b200ad_unet_forward_step_dev`, or
+    `b200ad_unet_forward_multistep_dev` with the history buffers `hist` of a multistep scheduler).
 
     Small batches are bound by the host, not by the GPU: at batch 1 and 256x256 the ~120 launches of a step take longer to
     enqueue than to execute (bench.py `configs.B1_latency`), which is the path the reference facade takes
     (audiodiffusion/__init__.py:59 hard-codes batch_size=1).  The kernels and their order are those of `forward_step`, so the
     results are bit-identical to the eager path (tests/test_gpu_pipeline.py::test_graph_stepper_equals_eager)."""
 
-    def __init__(self, model: UNet2DModel, sample: torch.Tensor):
+    def __init__(self, model: UNet2DModel, sample: torch.Tensor, history: Optional[int] = None):
         if getattr(model, "is_conditional", False):
             raise NotImplementedError("GraphStepper: unconditional U-Net only")
         if sample.dtype != torch.float32 or not sample.is_contiguous() or sample.device.type != "cuda":
             raise ValueError("GraphStepper: the sample buffer must be a contiguous fp32 CUDA tensor (it is updated in place)")
         self.model, self.x = model, sample
+        self.multistep = history is not None
         n, _, hh, ww = sample.shape
         dev = sample.device
         self.t = torch.zeros(n, dtype=torch.float32, device=dev)
         self.z = torch.zeros_like(sample)
-        self.coef = torch.zeros(32, dtype=torch.uint8, device=dev)          # one b200ad_step_coef
+        ctype = MultistepCoefC if self.multistep else StepCoefC
+        self.coef = torch.zeros(C.sizeof(ctype), dtype=torch.uint8, device=dev)    # one b200ad_(multi)step_coef
+        self.hist = torch.zeros((history,) + tuple(sample.shape), dtype=torch.float32, device=dev) if history else None
+        h1 = self.hist[0].data_ptr() if history else None
+        h2 = self.hist[1].data_ptr() if history == 2 else None
         L = _lib.lib()
         with torch.cuda.device(dev), torch.no_grad():
             model._fwd_gen[0] += 1
             model._bind(n, hh, ww, False, dev)
             scratch = torch.empty_like(sample)
+            scratch_hist = torch.zeros_like(self.hist) if history else None
 
-            def enqueue(out):
-                _lib.check(L.b200ad_unet_forward_step_dev(model._h, self.x.data_ptr(), self.t.data_ptr(), self.z.data_ptr(),
-                                                          self.coef.data_ptr(), out.data_ptr(), _lib.stream_ptr()))
+            def enqueue(out, hist1, hist2):
+                if self.multistep:
+                    _lib.check(L.b200ad_unet_forward_multistep_dev(model._h, self.x.data_ptr(), self.t.data_ptr(),
+                                                                   self.z.data_ptr(), self.coef.data_ptr(), hist1, hist2,
+                                                                   out.data_ptr(), _lib.stream_ptr()))
+                else:
+                    _lib.check(L.b200ad_unet_forward_step_dev(model._h, self.x.data_ptr(), self.t.data_ptr(), self.z.data_ptr(),
+                                                              self.coef.data_ptr(), out.data_ptr(), _lib.stream_ptr()))
+            sh1 = scratch_hist[0].data_ptr() if history else None
+            sh2 = scratch_hist[1].data_ptr() if history == 2 else None
             side = torch.cuda.Stream(device=dev)
             side.wait_stream(torch.cuda.current_stream(dev))
             with torch.cuda.stream(side):
-                enqueue(scratch)             # warm-up outside the capture (function attributes, lazy module loading);
-                enqueue(scratch)             # writes to a scratch tensor: the sample is untouched
+                enqueue(scratch, sh1, sh2)   # warm-up outside the capture (function attributes, lazy module loading);
+                enqueue(scratch, sh1, sh2)   # writes to scratch tensors: the sample and the history are untouched
             torch.cuda.current_stream(dev).wait_stream(side)
             torch.cuda.synchronize(dev)
             self.graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(self.graph):
-                enqueue(self.x)
-            del scratch
+                enqueue(self.x, h1, h2)
+            del scratch, scratch_hist
         self._bound = (model._packed_key, model._ws_key)
 
-    def step(self, timestep, coef: StepCoefC, noise: Optional[torch.Tensor] = None) -> torch.Tensor:
+    def step(self, timestep, coef: Union[StepCoefC, MultistepCoefC], noise: Optional[torch.Tensor] = None) -> torch.Tensor:
         m = self.model
         if (m._packed_key, m._ws_key) != self._bound:
             raise _lib.B200ADError("GraphStepper: the model was re-bound (weights, batch or mode changed) after the capture")
+        if isinstance(coef, MultistepCoefC) != self.multistep:
+            raise ValueError(f"GraphStepper: captured for {'MultistepCoefC' if self.multistep else 'StepCoefC'} coefficients, "
+                             f"got {type(coef).__name__}")
         if noise is not None and noise.shape != self.x.shape:     # copy_ would broadcast it
             raise ValueError(f"GraphStepper: noise must have the sample's shape {tuple(self.x.shape)}, "
                              f"got {tuple(noise.shape)}")
-        c = StepCoefC(coef.sqrt_1m_at, coef.inv_sqrt_at, coef.clip, coef.c_x0, coef.c_xt, coef.c_eps,
-                      coef.c_z if noise is not None else 0.0, coef.do_clip)
+        if self.multistep:
+            k = 0 if self.hist is None else self.hist.shape[0]
+            if (k < 1 and coef.c_h1 != 0.0) or (k < 2 and coef.c_h2 != 0.0):
+                raise ValueError(f"GraphStepper: captured with {k} history planes, the coefficients need more")
+            s = coef.step
+            c = MultistepCoefC(StepCoefC(s.sqrt_1m_at, s.inv_sqrt_at, s.clip, s.c_x0, s.c_xt, s.c_eps,
+                                         s.c_z if noise is not None else 0.0, s.do_clip), coef.c_h1, coef.c_h2)
+            upload = _lib.lib().b200ad_multistep_scalars_upload
+        else:
+            c = StepCoefC(coef.sqrt_1m_at, coef.inv_sqrt_at, coef.clip, coef.c_x0, coef.c_xt, coef.c_eps,
+                          coef.c_z if noise is not None else 0.0, coef.do_clip)
+            upload = _lib.lib().b200ad_step_scalars_upload
         with torch.cuda.device(self.x.device):
-            _lib.check(_lib.lib().b200ad_step_scalars_upload(C.byref(c), float(timestep), self.coef.data_ptr(), self.t.data_ptr(),
-                                                             self.t.numel(), _lib.stream_ptr()))
+            _lib.check(upload(C.byref(c), float(timestep), self.coef.data_ptr(), self.t.data_ptr(), self.t.numel(),
+                              _lib.stream_ptr()))
         if noise is not None:
             self.z.copy_(noise)
         m._fwd_gen[0] += 1

@@ -26,7 +26,7 @@ from typing import Optional, Sequence, Tuple, Union
 
 import torch
 
-from ._lib import MAX_BLOCKS, StepCoefC
+from ._lib import MAX_BLOCKS, MultistepCoefC, StepCoefC
 from .engine import _Cfg
 from .unet import UNet2DModel, _unet_config
 
@@ -119,10 +119,12 @@ class UNet2DConditionModel(UNet2DModel):
                                           "(pass precomputed encodings, e.g. .detach())")
         return self._forward(sample, timestep, encoder_hidden_states, return_dict)
 
-    def forward_step(self, sample: torch.Tensor, timestep, coef: StepCoefC, encoder_hidden_states: torch.Tensor = None,
-                     noise: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None, want_eps: bool = False):
-        """Fused `scheduler.step(unet(sample, t, encoding), t, sample)["prev_sample"]` (pipeline_audio_diffusion.py:161-179)."""
-        return self._forward_step(sample, timestep, coef, encoder_hidden_states, noise, out, want_eps)
+    def forward_step(self, sample: torch.Tensor, timestep, coef: Union[StepCoefC, MultistepCoefC],
+                     encoder_hidden_states: torch.Tensor = None, noise: Optional[torch.Tensor] = None,
+                     out: Optional[torch.Tensor] = None, want_eps: bool = False, history: Optional[torch.Tensor] = None):
+        """Fused `scheduler.step(unet(sample, t, encoding), t, sample)["prev_sample"]` (pipeline_audio_diffusion.py:161-179);
+        `history` as for `UNet2DModel.forward_step`."""
+        return self._forward_step(sample, timestep, coef, encoder_hidden_states, noise, out, want_eps, history)
 
 
 def load_cond_unet(sub: str) -> UNet2DConditionModel:

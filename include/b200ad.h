@@ -105,6 +105,31 @@ int b200ad_unet_forward_step_dev(b200ad_unet* h, const float* x, const float* t,
 int b200ad_step_scalars_upload(const b200ad_step_coef* coef, float t, b200ad_step_coef* coef_dev, float* t_dev, int n,
                                void* stream);
 
+/* Multistep scheduler update (DPMSolverMultistepScheduler, DPM-Solver++): the step also reads the data predictions x0 of
+ * the previous one or two steps from history buffers and writes this step's x0 there.  Per element:
+ *   x0  = (x - step.sqrt_1m_at * eps) * step.inv_sqrt_at          (clamped only if step.do_clip)
+ *   out = step.c_x0 * x0 + step.c_xt * x + step.c_eps * eps + c_h1 * hist1 + c_h2 * hist2 + step.c_z * z
+ *   hist2 = hist1 (if hist2 != NULL);  hist1 = x0
+ * hist1 / hist2 are fp32 buffers shaped like x (NULL: none; hist2 needs hist1).  Each element is read and written by one
+ * thread, so the buffers keep their roles from step to step (no pointer swap) and the call can be captured into a CUDA
+ * graph.  Start a run with zero-filled buffers: a zero coefficient then never meets a stale value (NaN * 0).  With both
+ * NULL this is b200ad_unet_forward_step / _dev (c_h1, c_h2 unread). */
+typedef struct {
+  b200ad_step_coef step;
+  float c_h1, c_h2;
+} b200ad_multistep_coef;
+int b200ad_unet_forward_multistep(b200ad_unet* h, const float* x, const float* t, const float* z,
+                                  const b200ad_multistep_coef* coef, float* hist1, float* hist2, float* x_out,
+                                  float* eps_out, void* stream);
+/* The multistep step with the coefficients in DEVICE memory (one b200ad_multistep_coef), for CUDA-graph capture as
+ * b200ad_unet_forward_step_dev; z must be non-NULL. */
+int b200ad_unet_forward_multistep_dev(b200ad_unet* h, const float* x, const float* t, const float* z,
+                                      const b200ad_multistep_coef* coef_dev, float* hist1, float* hist2, float* x_out,
+                                      void* stream);
+/* b200ad_step_scalars_upload for the multistep coefficients. */
+int b200ad_multistep_scalars_upload(const b200ad_multistep_coef* coef, float t, b200ad_multistep_coef* coef_dev,
+                                    float* t_dev, int n, void* stream);
+
 /* Debug / parity: copy a named internal activation of the last forward to fp32 NCHW.
  * Names follow the oracle taps (e.g. "conv_in", "down_blocks.0.resnets.0", "mid_block.attentions.0").
  * Returns the number of channels, or negative. dst may be NULL to query (dims[0..2] = C, H, W). */
